@@ -6,7 +6,6 @@
 #include <emmintrin.h>
 
 #include <algorithm>
-#include <chrono>
 #include <thread>
 #include <vector>
 
@@ -238,14 +237,9 @@ static int d2h_copy_sync(pixo_b200_ctx *ctx, void *dst, const void *src, size_t 
         PIXO_CUDA(ctx, cudaStreamSynchronize(st));
         return 0;
     }
-    const bool dbg = getenv("PIXO_B200_TIMING") != nullptr;
-    auto now = [] { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    const double t0 = dbg ? now() : 0;
     PIXO_TRY(ensure_pinned(ctx, ctx->h_out, bytes));
-    const double t1 = dbg ? now() : 0;
     PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_out.ptr, src, bytes, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaStreamSynchronize(st));
-    if (dbg) fprintf(stderr, "  d2h: ensure %.0f us, dma of %zu B %.0f us\n", t1 - t0, bytes, now() - t1);
     const int n = (int)((bytes + PIECE - 1) / PIECE);
     host_pool(ctx)->run(n, [&](int j) {
         const size_t off = (size_t)j * PIECE, len = std::min(PIECE, bytes - off);
@@ -433,6 +427,56 @@ int pixo_b200_download(pixo_b200_ctx *ctx, void *dst_host, const void *src_dev, 
 
 // ---- JPEG ---------------------------------------------------------------------------------
 
+// encode_into validation order, src/jpeg/mod.rs:333-373: quality, then the restart interval
+static int validate_options(pixo_b200_ctx *ctx, uint32_t quality, uint32_t restart_interval)
+{
+    if (quality == 0 || quality > 100)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
+    if (restart_interval > 65535)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_RESTART, "Invalid restart interval %u", restart_interval);
+    return 0;
+}
+
+static void tables_from(const uint64_t *hist, bool has_chroma, HuffTables &t)
+{
+    // build_optimized_huffman_tables(..).unwrap_or_default(), src/jpeg/mod.rs:379-392
+    if (!(hist && huff_from_histogram(hist, has_chroma, t))) huff_standard(t);
+}
+
+// need: bytes of headers, scan and EOI marker
+static int check_room(pixo_b200_ctx *ctx, size_t out_cap, size_t need)
+{
+    if (need > out_cap)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)", out_cap, need);
+    return 0;
+}
+
+// Ends a frame whose `body` scan bytes follow its `hdr` header bytes in out: checks that the EOI marker
+// fits too, writes it and stores the frame's length.  body == (size_t)-1: the host coder ran out of room.
+static int finish_frame(pixo_b200_ctx *ctx, uint8_t *out, size_t out_cap, size_t hdr, size_t body, size_t *out_len)
+{
+    if (body == (size_t)-1)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
+    PIXO_TRY(check_room(ctx, out_cap, hdr + body + 2));
+    out[hdr + body] = 0xFF;
+    out[hdr + body + 1] = 0xD9;
+    *out_len = hdr + body + 2;
+    return 0;
+}
+
+// Coefficient arrays of consecutive frames in one buffer: per frame Y, then Cb, then Cr, each array
+// 256-byte aligned, so one stride steps each array to the next frame's.
+struct CoefLayout {
+    size_t yb, cbb, each;  // bytes of the Y array, of one chroma array, of a frame
+    explicit CoefLayout(const FrameGeometry &g)
+        : yb(align_up(g.ny * 64 * sizeof(int16_t), 256)), cbb(align_up(g.nc * 64 * sizeof(int16_t), 256)),
+          each(yb + 2 * cbb) {}
+    size_t stride() const { return each / sizeof(int16_t); }
+    int16_t *y(void *frame) const { return reinterpret_cast<int16_t *>(frame); }
+    int16_t *cb(void *frame) const { return reinterpret_cast<int16_t *>(static_cast<uint8_t *>(frame) + yb); }
+    int16_t *cr(void *frame) const { return reinterpret_cast<int16_t *>(static_cast<uint8_t *>(frame) + yb + cbb); }
+};
+
 void pixo_b200_quant_tables(int quality, uint8_t lum_zz[64], uint8_t chr_zz[64], float lum[64],
                             float chr[64])
 {
@@ -480,14 +524,18 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
     return 0;
 }
 
-// shared by the host-buffer entry points: upload, transform (+hist), download coefficients
-static int transform_host(pixo_b200_ctx *ctx, const uint8_t *pixels, const FrameGeometry &g,
-                          const float lum_q[64], const float chr_q[64], uint32_t flags,
-                          uint32_t restart_interval, bool want_hist, int16_t *y, int16_t *cb,
-                          int16_t *cr, uint64_t *hist)
+// upload, transform (+ histogram), download the coefficients
+int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t width,
+                                uint32_t height, uint32_t color_type, uint32_t subsampling,
+                                const float lum_q[64], const float chr_q[64], int16_t *y,
+                                int16_t *cb, int16_t *cr, uint32_t flags, uint64_t *hist)
 {
-    const size_t bpp = g.color_type == PIXO_B200_GRAY ? 1 : 3;
-    const size_t in_bytes = (size_t)g.width * g.height * bpp;
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
+    if (!pixels || !y || !lum_q || !chr_q || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    const size_t in_bytes = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t yb = g.ny * 64 * sizeof(int16_t), cbb = g.nc * 64 * sizeof(int16_t);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
@@ -501,13 +549,12 @@ static int transform_host(pixo_b200_ctx *ctx, const uint8_t *pixels, const Frame
     auto *dcb = reinterpret_cast<int16_t *>(ctx->d_cb.ptr);
     auto *dcr = reinterpret_cast<int16_t *>(ctx->d_cr.ptr);
     PIXO_TRY(launch_jpeg_transform(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
-                                   g.width, g.height, g.color_type, g.subsampling, lum_q, chr_q,
+                                   width, height, color_type, subsampling, lum_q, chr_q,
                                    dy, g.ny * 64, dcb, dcr, g.nc * 64, flags));
-    if (want_hist) {
+    if (hist) {
         PIXO_TRY(ensure_dev(ctx, ctx->d_out, kHistWords * sizeof(uint64_t)));
         PIXO_TRY(launch_jpeg_histogram(ctx, dy, g.ny * 64, dcb, dcr, g.nc * 64, 1, g.ny, g.nc,
-                                       g.y_per_mcu, restart_interval,
-                                       (flags & PIXO_B200_COEF_ZIGZAG) != 0,
+                                       g.y_per_mcu, 0, (flags & PIXO_B200_COEF_ZIGZAG) != 0,
                                        reinterpret_cast<uint64_t *>(ctx->d_out.ptr)));
         PIXO_CUDA(ctx, cudaMemcpyAsync(hist, ctx->d_out.ptr, kHistWords * sizeof(uint64_t),
                                        cudaMemcpyDeviceToHost, ctx->stream));
@@ -521,53 +568,11 @@ static int transform_host(pixo_b200_ctx *ctx, const uint8_t *pixels, const Frame
     return 0;
 }
 
-int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t width,
-                                uint32_t height, uint32_t color_type, uint32_t subsampling,
-                                const float lum_q[64], const float chr_q[64], int16_t *y,
-                                int16_t *cb, int16_t *cr, uint32_t flags, uint64_t *hist)
-{
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
-    if (!pixels || !y || !lum_q || !chr_q || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    return transform_host(ctx, pixels, g, lum_q, chr_q, flags, 0, hist != nullptr, y, cb, cr, hist);
-}
-
-static int entropy_from_host_arrays(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb,
-                                    const int16_t *cr, const FrameGeometry &g, uint32_t quality,
-                                    uint32_t restart_interval, const uint64_t *hist,
-                                    uint8_t *out, size_t out_cap, size_t *out_len, int threads)
-{
-    uint8_t lum_zz[64], chr_zz[64];
-    quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
-    HuffTables t;
-    // build_optimized_huffman_tables(..).unwrap_or_default(), src/jpeg/mod.rs:379-392
-    if (!(hist && huff_from_histogram(hist, g.has_chroma, t))) huff_standard(t);
-    if (out_cap < 1024 + 2)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
-    size_t n = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
-    const size_t body = entropy_encode_scan(y, cb, cr, g, t, restart_interval, false, out + n,
-                                            out_cap - n - 2, threads);
-    if (body == (size_t)-1)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
-    n += body;
-    out[n++] = 0xFF;
-    out[n++] = 0xD9;
-    *out_len = n;
-    return 0;
-}
-
 static int validate_encode(pixo_b200_ctx *ctx, size_t pixels_len, uint32_t width, uint32_t height,
                            uint32_t color_type, uint32_t quality, uint32_t subsampling,
-                           uint32_t restart_interval, bool restart_given_zero)
+                           uint32_t restart_interval)
 {
-    // encode_into validation order, src/jpeg/mod.rs:333-373
-    if (quality == 0 || quality > 100)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
-    (void)restart_given_zero;
-    if (restart_interval > 65535)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_RESTART, "Invalid restart interval %u", restart_interval);
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     const size_t bpp = color_type == PIXO_B200_GRAY ? 1 : 3;
     const size_t expected = (size_t)width * height * bpp;
@@ -601,6 +606,48 @@ static uint64_t default_scan_cap(const pixo_b200_ctx *ctx, size_t raw_bytes)
     return align_up(want < 1024 ? 1024 : want, 256);
 }
 
+constexpr int kGaveUp = -1;  // recode_scan: the device stage did not finish the scan
+
+// Codes one frame's scan on the device until it fits, in ctx->d_retry: the scan, then the entropy
+// stage's scratch.  The first pass may be cut into segments and has `cap` bytes.  After a pass
+// that did not finish, its flags decide: bit 1 (a look-back chain timed out) gives up; bit 2 (a
+// segment outgrew its share) runs again unsegmented; bit 0 (the scan did not fit, and the length is
+// the size it needs) runs again with room for that size, unless headers, scan and EOI would no
+// longer fit out_cap.  Three passes at most.  Returns 0 with the scan at the start of d_retry and
+// its length in *len, kGaveUp, or an error.  It touches no other scratch of the context but
+// d_raw (segmented passes), so encode_frames can use it while the next group's work is queued.
+static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                       const FrameGeometry &g, const HuffTables &t, uint32_t restart_interval, bool segments,
+                       size_t cap, size_t hdr, size_t out_cap, size_t *len)
+{
+    const size_t ent = entropy_scratch_bytes(1, g, restart_interval);
+    for (int pass = 0;; ++pass) {
+        const size_t scan_bytes = align_up(cap, 256);
+        PIXO_TRY(ensure_dev(ctx, ctx->d_retry, scan_bytes + ent + 256));
+        auto *buf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
+        uint64_t *d_len = nullptr;
+        uint32_t *d_ovf = nullptr;
+        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments,
+                                     buf + scan_bytes, buf, cap, &d_len, &d_ovf));
+        uint64_t n = 0;
+        uint32_t ovf = 0;
+        PIXO_CUDA(ctx, cudaMemcpyAsync(&n, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(&ovf, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (!ovf) {
+            *len = (size_t)n;
+            return 0;
+        }
+        if ((ovf & 2u) || pass == 2) return kGaveUp;
+        if (ovf & 4u) {
+            segments = false;
+            continue;
+        }
+        PIXO_TRY(check_room(ctx, out_cap, hdr + (size_t)n + 2));
+        cap = align_up((size_t)n + 64, 256);
+    }
+}
+
 // Encode n frames of identical geometry and options.  GPU: colour/DCT/quantise (K1/K2), symbol
 // statistics when optimize_huffman (K3), Huffman bit packing + 0xFF stuffing + restart markers
 // (k_huff); host: headers, optimised-table construction, EOI.  Frames are processed in groups of
@@ -620,9 +667,8 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     float lum[64], chr[64];
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, lum, chr);
-    const size_t yb = align_up(g.ny * 64 * sizeof(int16_t), 256);
-    const size_t cbb = align_up(g.nc * 64 * sizeof(int16_t), 256);
-    const size_t coef_each = yb + 2 * cbb;
+    const CoefLayout L(g);
+    const size_t cs = L.stride();
     const size_t in_stride = align_up(len_each, 256);
     const uint64_t scan_cap = default_scan_cap(ctx, len_each);
     const size_t ent_one = entropy_scratch_bytes(1, g, restart_interval);
@@ -637,14 +683,14 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         return optimize ? (size_t)k * ent_one : entropy_scratch_bytes(k, g, restart_interval);
     };
     auto group_bytes = [&](uint32_t k) {
-        return 2 * (size_t)k * in_stride + 2 * (size_t)k * coef_each + ent_bytes(k) + 2 * (size_t)k * scan_cap;
+        return 2 * (size_t)k * in_stride + 2 * (size_t)k * L.each + ent_bytes(k) + 2 * (size_t)k * scan_cap;
     };
     while (G > 1 && group_bytes(G) > budget) --G;
     const uint32_t ngroups = (n_images + G - 1) / G;
 
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ensure_dev(ctx, ctx->d_in, 2 * (size_t)G * in_stride));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, 2 * (size_t)G * coef_each));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, 2 * (size_t)G * L.each));
     PIXO_TRY(ensure_dev(ctx, ctx->d_ent, ent_bytes(G)));
     PIXO_TRY(ensure_dev(ctx, ctx->d_out, 2 * (size_t)G * scan_cap));
     PIXO_TRY(ensure_dev(ctx, ctx->d_misc, (size_t)G * kHistWords * sizeof(uint64_t) + 256));
@@ -665,18 +711,10 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto *h_hist = reinterpret_cast<uint64_t *>(h_meta + 2 * meta_slot);
     auto h_len_of = [&](int slot) { return reinterpret_cast<uint64_t *>(h_meta + (size_t)slot * meta_slot); };
     auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
-    struct Coef { int16_t *y, *cb, *cr; };
-    const size_t cstride = coef_each / 2;
-    auto coef_of = [&](int slot) {
-        uint8_t *base = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * coef_each;
-        return Coef{reinterpret_cast<int16_t *>(base), reinterpret_cast<int16_t *>(base + yb),
-                    reinterpret_cast<int16_t *>(base + yb + cbb)};
-    };
+    auto coef_of = [&](int slot) { return reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * L.each; };
     std::vector<HuffTables> tables[2];
     const bool out_locked = is_page_locked(out);
     DrainOnError drain(ctx);
-    const bool dbg = getenv("PIXO_B200_TIMING") != nullptr;
-    auto now = [] { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
 
     auto upload = [&](uint32_t gi) -> int {
         const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
@@ -693,25 +731,24 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto compute = [&](uint32_t gi) -> int {
         const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
         const int slot = (int)(gi & 1);
-        const Coef c = coef_of(slot);
+        uint8_t *c = coef_of(slot);
         PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_in[slot], 0));
         PIXO_TRY(launch_jpeg_transform(ctx, d_in + (size_t)slot * G * in_stride, in_stride, cnt, g.width,
-                                       g.height, g.color_type, g.subsampling, lum, chr, c.y, cstride,
-                                       g.has_chroma ? c.cb : nullptr, g.has_chroma ? c.cr : nullptr, cstride, 0));
+                                       g.height, g.color_type, g.subsampling, lum, chr, L.y(c), cs,
+                                       g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr, cs, 0));
         PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
         std::vector<HuffTables> &tb = tables[slot];
         tb.resize(optimize ? cnt : 1);
         if (optimize) {
             auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-            PIXO_TRY(launch_jpeg_histogram(ctx, c.y, cstride, c.cb, c.cr, cstride, cnt, g.ny, g.nc, g.y_per_mcu,
+            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g.ny, g.nc, g.y_per_mcu,
                                            restart_interval, false, d_hist));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t),
                                            cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the table build needs the statistics
-            for (uint32_t k = 0; k < cnt; ++k)  // unwrap_or_default, src/jpeg/mod.rs:379-392
-                if (!huff_from_histogram(h_hist + (size_t)k * kHistWords, g.has_chroma, tb[k])) huff_standard(tb[k]);
+            for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, g.has_chroma, tb[k]);
         } else {
-            huff_standard(tb[0]);
+            tables_from(nullptr, g.has_chroma, tb[0]);
         }
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
         if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_out[slot], 0));  // slot's previous D2H drained
@@ -721,14 +758,14 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         uint64_t *h_len = h_len_of(slot);
         uint32_t *h_ovf = h_ovf_of(slot);
         if (!optimize) {
-            PIXO_TRY(launch_jpeg_entropy(ctx, c.y, cstride, c.cb, c.cr, cstride, cnt, g, tb[0], restart_interval, true,
+            PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g, tb[0], restart_interval, true,
                                          ent, scan, scan_cap, &d_len, &d_ovf));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, d_len, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
         } else {
             for (uint32_t k = 0; k < cnt; ++k) {  // per-image tables: one pass per image, each in its own scratch
-                PIXO_TRY(launch_jpeg_entropy(ctx, c.y + (size_t)k * cstride, cstride, c.cb + (size_t)k * cstride,
-                                             c.cr + (size_t)k * cstride, cstride, 1, g, tb[k], restart_interval, true,
+                uint8_t *f = c + (size_t)k * L.each;
+                PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, 1, g, tb[k], restart_interval, true,
                                              ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
                                              &d_ovf));
                 PIXO_CUDA(ctx, cudaMemcpyAsync(h_len + k, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -743,14 +780,12 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto finish = [&](uint32_t gi) -> int {
         const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
         const int slot = (int)(gi & 1);
-        const Coef c = coef_of(slot);
+        uint8_t *c = coef_of(slot);
         const std::vector<HuffTables> &tb = tables[slot];
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
         const uint64_t *h_len = h_len_of(slot);
         const uint32_t *h_ovf = h_ovf_of(slot);
-        const double tf0 = dbg ? now() : 0;
         PIXO_CUDA(ctx, cudaEventSynchronize(ev_len[slot]));
-        if (dbg) fprintf(stderr, "  finish: waited %.0f us for the group's kernels\n", now() - tf0);
         std::vector<size_t> hdr(cnt);
         bool redo = false;
         for (uint32_t k = 0; k < cnt; ++k) {
@@ -759,17 +794,12 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             hdr[k] = write_headers(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
             if (h_ovf[k]) { redo = true; continue; }
             const size_t body = (size_t)h_len[k];
-            if (hdr[k] + body + 2 > out_cap_each)
-                return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)",
-                                 out_cap_each, hdr[k] + body + 2);
+            PIXO_TRY(finish_frame(ctx, o, out_cap_each, hdr[k], body, &out_lens[img]));
             if (out_locked)
                 PIXO_CUDA(ctx, cudaMemcpyAsync(o + hdr[k], scan + (size_t)k * scan_cap, body, cudaMemcpyDeviceToHost,
                                                ctx->d2h_stream));
             else   // ordinary caller memory: through the pinned ring, copied out by the host pool
                 PIXO_TRY(d2h_copy_sync(ctx, o + hdr[k], scan + (size_t)k * scan_cap, body, ctx->d2h_stream));
-            o[hdr[k] + body] = 0xFF;
-            o[hdr[k] + body + 1] = 0xD9;
-            out_lens[img] = hdr[k] + body + 2;
         }
         PIXO_CUDA(ctx, cudaEventRecord(ev_out[slot], ctx->d2h_stream));
         if (!redo) return 0;
@@ -779,59 +809,35 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             if (!h_ovf[k]) continue;
             const uint32_t img = first + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
+            uint8_t *f = c + (size_t)k * L.each;
             const HuffTables &t = tb[optimize ? k : 0];
-            bool done = false;
             // bit 0: the scan did not fit (the kernel reported the size it needs); bit 2: a segment's raw
             // string did not fit its share - either way code the frame again on the GPU, unsegmented, with
             // enough room.  Bit 1 (a faulted chain) goes to the host coder.
+            int rc = kGaveUp;
+            size_t body = 0;
             if (!(h_ovf[k] & 2u) && ctx->gpu_retry) {
-                size_t need = (h_ovf[k] & 4u) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
-                for (int attempt = 0; attempt < 3 && !done; ++attempt) {
-                    if (hdr[k] + need + 2 > out_cap_each && !(h_ovf[k] & 4u))
-                        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)",
-                                         out_cap_each, hdr[k] + need + 2);
-                    const uint64_t cap2 = align_up(need + 64, 256);
-                    PIXO_TRY(ensure_dev(ctx, ctx->d_retry, cap2 + ent_one + 256));
-                    auto *rbuf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
-                    uint64_t *d_len = nullptr;
-                    uint32_t *d_ovf = nullptr;
-                    PIXO_TRY(launch_jpeg_entropy(ctx, c.y + (size_t)k * cstride, cstride, c.cb + (size_t)k * cstride,
-                                                 c.cr + (size_t)k * cstride, cstride, 1, g, t, restart_interval, false,
-                                                 rbuf + cap2, rbuf, cap2, &d_len, &d_ovf));
-                    uint64_t len2 = 0;
-                    uint32_t ovf2 = 0;
-                    PIXO_CUDA(ctx, cudaMemcpyAsync(&len2, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
-                    PIXO_CUDA(ctx, cudaMemcpyAsync(&ovf2, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
-                    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-                    if (ovf2 & 2u) break;
-                    if (ovf2) { need = (size_t)len2; continue; }
-                    if (hdr[k] + (size_t)len2 + 2 > out_cap_each)
-                        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)",
-                                         out_cap_each, hdr[k] + (size_t)len2 + 2);
-                    PIXO_CUDA(ctx, cudaMemcpyAsync(o + hdr[k], rbuf, (size_t)len2, cudaMemcpyDeviceToHost, ctx->stream));
-                    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-                    o[hdr[k] + len2] = 0xFF;
-                    o[hdr[k] + len2 + 1] = 0xD9;
-                    out_lens[img] = hdr[k] + (size_t)len2 + 2;
-                    done = true;
-                }
+                const size_t need = (h_ovf[k] & 4u) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
+                if (!(h_ovf[k] & 4u)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
+                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), g, t, restart_interval, false, align_up(need + 64, 256),
+                                 hdr[k], out_cap_each, &body);
+                if (rc != 0 && rc != kGaveUp) return rc;
             }
-            if (done) continue;
+            if (rc == 0) {
+                PIXO_TRY(finish_frame(ctx, o, out_cap_each, hdr[k], body, &out_lens[img]));
+                PIXO_CUDA(ctx, cudaMemcpyAsync(o + hdr[k], ctx->d_retry.ptr, body, cudaMemcpyDeviceToHost, ctx->stream));
+                PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+                continue;
+            }
             // last resort: the host entropy coder on the GPU's coefficient arrays
             ctx->host_fallbacks += 1;
-            PIXO_TRY(ensure_pinned(ctx, ctx->h_out, coef_each));
+            PIXO_TRY(ensure_pinned(ctx, ctx->h_out, L.each));
             auto *hc = reinterpret_cast<uint8_t *>(ctx->h_out.ptr);
-            PIXO_CUDA(ctx, cudaMemcpyAsync(hc, reinterpret_cast<const uint8_t *>(c.y) + (size_t)k * coef_each, coef_each,
-                                           cudaMemcpyDeviceToHost, ctx->stream));
+            PIXO_CUDA(ctx, cudaMemcpyAsync(hc, f, L.each, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            const size_t body = entropy_encode_scan(reinterpret_cast<int16_t *>(hc), reinterpret_cast<int16_t *>(hc + yb),
-                                                    reinterpret_cast<int16_t *>(hc + yb + cbb), g, t, restart_interval,
-                                                    false, o + hdr[k], out_cap_each - hdr[k] - 2, ctx->host_threads);
-            if (body == (size_t)-1)
-                return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap_each);
-            o[hdr[k] + body] = 0xFF;
-            o[hdr[k] + body + 1] = 0xD9;
-            out_lens[img] = hdr[k] + body + 2;
+            body = entropy_encode_scan(L.y(hc), L.cb(hc), L.cr(hc), g, t, restart_interval, false, o + hdr[k],
+                                       out_cap_each - hdr[k] - 2, ctx->host_threads);
+            PIXO_TRY(finish_frame(ctx, o, out_cap_each, hdr[k], body, &out_lens[img]));
         }
         return 0;
     };
@@ -840,22 +846,15 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     PIXO_CUDA(ctx, cudaEventRecord(ev_out[0], ctx->stream));
     PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ev_out[0], 0));
     PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->d2h_stream, ev_out[0], 0));
-    const double t0 = dbg ? now() : 0;
     PIXO_TRY(upload(0));
-    const double t1 = dbg ? now() : 0;
     for (uint32_t gi = 0; gi < ngroups; ++gi) {
         if (gi + 1 < ngroups) PIXO_TRY(upload(gi + 1));
         PIXO_TRY(compute(gi));
         if (gi > 0) PIXO_TRY(finish(gi - 1));
     }
-    const double t2 = dbg ? now() : 0;
     PIXO_TRY(finish(ngroups - 1));
-    const double t3 = dbg ? now() : 0;
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (dbg)
-        fprintf(stderr, "encode_frames n=%u: upload(0) queued %.0f us, compute queued %.0f us, last finish %.0f us, drain %.0f us\n",
-                n_images, t1 - t0, t2 - t1, t3 - t2, now() - t3);
     drain.armed = false;
     return 0;
 }
@@ -867,8 +866,7 @@ int pixo_b200_jpeg_encode(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixe
                           uint8_t *out, size_t out_cap, size_t *out_len)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len, width, height, color_type, quality, subsampling,
-                             restart_interval, false));
+    PIXO_TRY(validate_encode(ctx, pixels_len, width, height, color_type, quality, subsampling, restart_interval));
     if (!pixels || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (progressive)
         return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED,
@@ -886,8 +884,8 @@ int pixo_b200_jpeg_encode_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_
                                 uint8_t *out, size_t out_cap_each, size_t *out_lens)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len_each, width, height, color_type, quality,
-                             subsampling, restart_interval, false));
+    PIXO_TRY(validate_encode(ctx, pixels_len_each, width, height, color_type, quality, subsampling,
+                             restart_interval));
     if (!pixels || !out || !out_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (n_images == 0) return 0;
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
@@ -902,8 +900,7 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
                               uint32_t *d_overflow)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    if (quality == 0 || quality > 100)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
+    PIXO_TRY(validate_options(ctx, quality, 0));
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     if (!d_pixels || !d_scan || !d_scan_len || !d_overflow)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
@@ -914,24 +911,19 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     float lum[64], chr[64];
     quant_tables((int)quality, nullptr, nullptr, lum, chr);
-    const size_t yb = align_up(g.ny * 64 * sizeof(int16_t), 256);
-    const size_t cbb = align_up(g.nc * 64 * sizeof(int16_t), 256);
-    const size_t coef_each = yb + 2 * cbb;
+    const CoefLayout L(g);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, (size_t)n_images * coef_each));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, (size_t)n_images * L.each));
     PIXO_TRY(ensure_dev(ctx, ctx->d_ent, entropy_scratch_bytes(n_images, g, 0)));
-    auto *d_coef = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
-    auto *dy = reinterpret_cast<int16_t *>(d_coef);
-    auto *dcb = reinterpret_cast<int16_t *>(d_coef + yb);
-    auto *dcr = reinterpret_cast<int16_t *>(d_coef + yb + cbb);
+    void *c = ctx->d_coef.ptr;
     PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
-                                   lum, chr, dy, coef_each / 2, g.has_chroma ? dcb : nullptr,
-                                   g.has_chroma ? dcr : nullptr, coef_each / 2, 0));
+                                   lum, chr, L.y(c), L.stride(), g.has_chroma ? L.cb(c) : nullptr,
+                                   g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0));
     HuffTables t;
     huff_standard(t);
     uint64_t *len_src = nullptr;
     uint32_t *ovf_src = nullptr;
-    PIXO_TRY(launch_jpeg_entropy(ctx, dy, coef_each / 2, dcb, dcr, coef_each / 2, n_images, g, t, 0, true,
+    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true,
                                  reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan, scan_cap_each,
                                  &len_src, &ovf_src));
     PIXO_CUDA(ctx, cudaMemcpyAsync(d_scan_len, len_src, (size_t)n_images * 8, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -945,10 +937,7 @@ int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const in
                                   uint32_t restart_interval, uint32_t optimize_huffman,
                                   uint8_t *out, size_t out_cap, size_t *out_len)
 {
-    if (quality == 0 || quality > 100)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
-    if (restart_interval > 65535)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_RESTART, "Invalid restart interval %u", restart_interval);
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     if (!y || !out || !out_len || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
@@ -960,12 +949,19 @@ int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const in
                           !coefficients_in_range(cr, g.nc, restart_interval, 1))))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
                          "coefficient out of the baseline range (|AC| <= 1023, |DC difference| <= 2047)");
+    if (out_cap < 1024 + 2)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
     uint64_t hist[536];
     if (optimize_huffman) host_histogram(y, cb, cr, g, restart_interval, hist);
+    HuffTables t;
+    tables_from(optimize_huffman ? hist : nullptr, g.has_chroma, t);
+    uint8_t lum_zz[64], chr_zz[64];
+    quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
+    const size_t hdr = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
     int threads = ctx ? ctx->host_threads : (int)std::thread::hardware_concurrency();
-    return entropy_from_host_arrays(ctx, y, cb, cr, g, quality, restart_interval,
-                                    optimize_huffman ? hist : nullptr, out, out_cap, out_len,
-                                    threads < 1 ? 1 : threads);
+    const size_t body = entropy_encode_scan(y, cb, cr, g, t, restart_interval, false, out + hdr, out_cap - hdr - 2,
+                                            threads < 1 ? 1 : threads);
+    return finish_frame(ctx, out, out_cap, hdr, body, out_len);
 }
 
 int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
@@ -975,10 +971,7 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
                                       uint8_t *out, size_t out_cap, size_t *out_len)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    if (quality == 0 || quality > 100)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
-    if (restart_interval > 65535)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_RESTART, "Invalid restart interval %u", restart_interval);
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     if (!d_y || !out || !out_len || (color_type != PIXO_B200_GRAY && (!d_cb || !d_cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
@@ -988,67 +981,36 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, kHistWords * sizeof(uint64_t) + 256));
-    auto *h_meta = reinterpret_cast<uint8_t *>(ctx->h_misc.ptr);
-    HuffTables t;
-    huff_standard(t);
+    uint64_t *h_hist = nullptr;
     if (optimize_huffman) {
         PIXO_TRY(ensure_dev(ctx, ctx->d_misc, kHistWords * sizeof(uint64_t) + 256));
+        PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, kHistWords * sizeof(uint64_t) + 256));
         auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-        auto *h_hist = reinterpret_cast<uint64_t *>(h_meta + 256);
+        h_hist = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, restart_interval,
                                        false, d_hist));
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, kHistWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (!huff_from_histogram(h_hist, g.has_chroma, t)) huff_standard(t);  // unwrap_or_default
     }
+    HuffTables t;
+    tables_from(h_hist, g.has_chroma, t);
     const size_t hdr = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
     // The device scan buffer follows the size a JPEG of this geometry normally has, not the caller's
     // worst-case capacity (tens of GB for a gigapixel frame); a scan that needs more is coded again
     // with the exact size the kernel reported.
     const size_t raw = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
-    size_t scan_cap = std::min<size_t>((out_cap - hdr - 2) & ~(size_t)15, (size_t)default_scan_cap(ctx, raw));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_ent, entropy_scratch_bytes(1, g, restart_interval)));
-    auto *h_len = reinterpret_cast<uint64_t *>(h_meta);
-    auto *h_ovf = reinterpret_cast<uint32_t *>(h_meta + 8);
-    uint8_t *d_scan = nullptr;
-    bool segments = true;
-    for (int attempt = 0;; ++attempt) {
-        PIXO_TRY(ensure_dev(ctx, ctx->d_out, scan_cap + 16));
-        uint64_t *d_len = nullptr;
-        uint32_t *d_ovf = nullptr;
-        d_scan = reinterpret_cast<uint8_t *>(ctx->d_out.ptr);
-        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments,
-                                     reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan, scan_cap, &d_len, &d_ovf));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (!*h_ovf) break;
-        if ((*h_ovf & 2u) || attempt >= 2)
-            return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish (flags %u)", *h_ovf);
-        segments = !(*h_ovf & 4u);   // a segment outgrew its share: once more, unsegmented
-        if (!segments) continue;
-        if (hdr + (size_t)*h_len + 2 > out_cap)
-            return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)", out_cap,
-                             hdr + (size_t)*h_len + 2);
-        scan_cap = align_up((size_t)*h_len + 64, 256);
-    }
-    const size_t body = (size_t)*h_len;
-    PIXO_CUDA(ctx, cudaMemcpyAsync(out + hdr, d_scan, body, cudaMemcpyDeviceToHost, ctx->stream));
+    const size_t scan_cap = std::min<size_t>((out_cap - hdr - 2) & ~(size_t)15, (size_t)default_scan_cap(ctx, raw));
+    size_t body = 0;
+    const int rc = recode_scan(ctx, d_y, d_cb, d_cr, g, t, restart_interval, true, scan_cap, hdr, out_cap, &body);
+    if (rc == kGaveUp) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish");
+    PIXO_TRY(rc);
+    PIXO_TRY(finish_frame(ctx, out, out_cap, hdr, body, out_len));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(out + hdr, ctx->d_retry.ptr, body, cudaMemcpyDeviceToHost, ctx->stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    out[hdr + body] = 0xFF;
-    out[hdr + body + 1] = 0xD9;
-    *out_len = hdr + body + 2;
     return 0;
 }
 
 // ---- one frame tiled over several GPUs -----------------------------------------------------------
-
-static void tables_from(const uint64_t *hist, bool has_chroma, HuffTables &t)
-{
-    // build_optimized_huffman_tables(..).unwrap_or_default(), src/jpeg/mod.rs:379-392
-    if (!(hist && huff_from_histogram(hist, has_chroma, t))) huff_standard(t);
-}
 
 int pixo_b200_jpeg_band_last_dc(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
                                 const int16_t *d_cr, size_t ny, size_t nc, int32_t last_dc[3])
@@ -1215,10 +1177,7 @@ int pixo_b200_jpeg_write_headers(uint32_t width, uint32_t height, uint32_t color
                                  uint32_t subsampling, uint32_t restart_interval, const uint64_t *hist,
                                  uint8_t *out, size_t out_cap, size_t *out_len)
 {
-    if (quality == 0 || quality > 100)
-        return set_error(nullptr, PIXO_B200_ERR_INVALID_QUALITY, "Invalid quality %u: must be 1-100", quality);
-    if (restart_interval > 65535)
-        return set_error(nullptr, PIXO_B200_ERR_INVALID_RESTART, "Invalid restart interval %u", restart_interval);
+    PIXO_TRY(validate_options(nullptr, quality, restart_interval));
     PIXO_TRY(validate_jpeg(nullptr, width, height, color_type, subsampling));
     if (!out || !out_len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (out_cap < 1024) return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);

@@ -283,6 +283,63 @@ def test_encode_dev_device_resident(po, gpu_ctx):
                 assert ovf[k] != 0
 
 
+def _upload_coefficients(po, img, w, h, ct, ss, q):
+    """The oracle's coefficients, and the same arrays as int16 device tensors (None for absent chroma)."""
+    import torch
+    host = po.jpeg_coefficients(img, w, h, ct, ss, q)
+    dev = [torch.from_numpy(a).cuda() if len(a) else None for a in host]
+    torch.cuda.synchronize()
+    return host, dev
+
+
+@pytest.mark.parametrize("w,h,ct,ss", [(333, 222, 2, 1), (333, 222, 2, 0), (257, 129, 0, 0)])
+def test_entropy_encode_dev_matches_oracle(po, gpu_ctx, w, h, ct, ss):
+    """pixo_b200_jpeg_entropy_encode_dev on device coefficients: standard and optimised tables,
+    with and without a restart interval, 4:2:0 / 4:4:4 / gray."""
+    grad = po.gen_gradient_rgb(w, h)
+    for img in (po.gen_noise(w, h, 3 if ct == 2 else 1, 4), grad if ct == 2 else grad[::3].copy()):
+        (y, cb, cr), d = _upload_coefficients(po, img, w, h, ct, ss, 80)
+        for ri in (0, 7):
+            for opt in (False, True):
+                o = JpegOptions(w, h, ColorType(ct), 80, Subsampling(ss), ri or None, opt)
+                ref = po.jpeg_encode_from_coefficients(y, cb, cr, w, h, ct, 80, ss, ri, opt)
+                assert jpeg.entropy_encode_dev(*d, o, ctx=gpu_ctx) == ref, (ri, opt)
+
+
+def test_entropy_encode_dev_recodes_on_the_gpu(po, monkeypatch):
+    """A scan that outgrows the first pass's device buffer is coded again with the size the kernel
+    reported: unsegmented (q=100 noise beyond the heuristic), after a segmented first pass, and after
+    a segmented first pass into a tiny buffer.  An output that holds the headers but not the scan is
+    reported as too small, and nothing is written past it."""
+    import ctypes as C
+    from pixo_b200 import _lib
+    w, h = 640, 480
+    img = po.gen_noise(w, h, 3, 7)
+    with pixo_b200.Context(0) as ctx:
+        for q, segments, cap in ((100, None, 0), (80, "5", 0), (80, "5", 4096)):
+            if segments:
+                monkeypatch.setenv("PIXO_B200_SEGMENTS", segments)
+            ctx.set_scan_capacity(cap)
+            (y, cb, cr), d = _upload_coefficients(po, img, w, h, 2, 1, q)
+            ref = po.jpeg_encode_from_coefficients(y, cb, cr, w, h, 2, q, 1)
+            if q == 100:
+                assert len(ref) > (w * h * 3 // 2 + 65536) * 9 // 8   # really beyond the heuristic
+            l0 = ctx.launch_count
+            assert jpeg.entropy_encode_dev(*d, JpegOptions(w, h, ColorType.Rgb, q, Subsampling.S420), ctx=ctx) == ref
+            # two k_huff passes unsegmented; one k_huff<RAW> + four splice kernels per segmented pass
+            assert ctx.launch_count - l0 >= (2 if not segments else 5 if not cap else 10), (q, segments, cap)
+        ctx.set_scan_capacity(0)
+        monkeypatch.delenv("PIXO_B200_SEGMENTS")
+        out_cap = 4096
+        buf = np.full(out_cap + 256, 0xA5, np.uint8)
+        n = C.c_size_t(0)
+        rc = _lib.load().pixo_b200_jpeg_entropy_encode_dev(
+            ctx.handle, d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(), w, h, 2, 80, 1, 0, 0,
+            buf.ctypes.data, out_cap, C.byref(n))
+        assert rc == _lib.ERR_OUTPUT_TOO_SMALL
+        assert (buf[out_cap:] == 0xA5).all()
+
+
 def test_large_pageable_input_takes_the_staged_copy(po, gpu_ctx):
     """Sources of 64 MB and more (ordinary, pageable memory) are pushed through the pinned slot
     ring by several host threads; the pieces must land exactly where a single copy would put them."""
