@@ -179,7 +179,11 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
 
 /* Entropy-code caller-provided coefficient arrays (host) into a baseline JPEG: the host half of
  * pixo_b200_jpeg_encode on its own (src/jpeg/mod.rs:395-447,1408-1563 consuming arrays shaped
- * like compute_all_coefficients' result).  Host-only, no device needed. */
+ * like compute_all_coefficients' result).  Host-only, no device needed.
+ * Coefficients outside the baseline range - an AC value with |v| > 1023, or a DC difference (int16
+ * wrapping, against the previous block of the component, 0 after a restart) with |d| > 2047 - have no
+ * Huffman code: every entry point that takes caller coefficients returns
+ * PIXO_B200_ERR_INVALID_ARGUMENT for them (the stream-ordered ones set bit 3 of d_flags). */
 int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb,
                                   const int16_t *cr, uint32_t width, uint32_t height,
                                   uint32_t color_type, uint32_t quality, uint32_t subsampling,
@@ -224,13 +228,18 @@ int pixo_b200_jpeg_band_histogram_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
                                       const int16_t *d_cr, uint32_t width, uint32_t band_height,
                                       uint32_t color_type, uint32_t subsampling,
                                       const int32_t dc_seed[3], uint64_t *d_hist /* 536, device */);
+/* (pixo_b200_jpeg_band_histogram_dev does not wait for the device, so it cannot report coefficients
+ * outside the baseline range: it counts them in the nearest category, and the band's
+ * pixo_b200_jpeg_band_entropy_dev(_async) rejects them.) */
 /* hist (host, optional): the frame's summed statistics -> optimised tables (standard when NULL or
  * when they cannot be built, as the reference's unwrap_or_default does).  d_raw: 16-byte aligned,
  * raw_cap a multiple of 4; it must stay untouched until the band has been spliced.  A raw_cap of at
  * least the band's pixel bytes + 1 MiB lets a long band be coded as several independent segments
  * (shorter look-back chains); with less room the band is coded as one string, in what raw_cap leaves
- * after 512 bytes for its bit count and tail.  A string that does not fit returns
- * PIXO_B200_ERR_OUTPUT_TOO_SMALL with *nbits = the bits it needs. */
+ * after 512 bytes for its bit count and tail.  A segment gets about its pixel bytes; a dense band
+ * whose segments outgrow that is coded again as one string in the same call.  A string that does not
+ * fit returns PIXO_B200_ERR_OUTPUT_TOO_SMALL with *nbits = the bits it needs; a second call whose
+ * raw_cap holds those bits' bytes rounded up to a multiple of 256, plus the 512, succeeds. */
 int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
                                     const int16_t *d_cr, uint32_t width, uint32_t band_height,
                                     uint32_t color_type, uint32_t subsampling,
@@ -248,8 +257,10 @@ int pixo_b200_jpeg_band_splice_dev(pixo_b200_ctx *ctx, const uint8_t *d_raw, uin
  *   d_dc_seed:   int32[3] in device memory (written by an earlier operation on the stream)
  *   d_bits_tail: uint64[2] out, {bit count, last 7 bits}
  *   d_offset:    uint64[3] in, {start_bit, the last 7 bits of the stream before this band, is_last_band}
- *   d_flags:     uint32, OR-ed: bit 0 a capacity was too small, bit 1 device fault (caller zeroes it)
- * raw_cap must be at least the band's pixel bytes + 1 MiB. */
+ *   d_flags:     uint32, OR-ed: bit 0 a capacity was too small, bit 1 device fault, bit 3 a coefficient
+ *                outside the baseline range (caller zeroes it)
+ * raw_cap must be at least the band's pixel bytes + 1 MiB.  A dense band coded in segments can set bit 0
+ * with that room (see pixo_b200_jpeg_band_entropy_dev, which recodes it as one string). */
 int pixo_b200_jpeg_band_entropy_dev_async(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
                                           const int16_t *d_cr, uint32_t width, uint32_t band_height,
                                           uint32_t color_type, uint32_t subsampling,

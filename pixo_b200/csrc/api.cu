@@ -607,18 +607,21 @@ static uint64_t default_scan_cap(const pixo_b200_ctx *ctx, size_t raw_bytes)
 }
 
 constexpr int kGaveUp = -1;  // recode_scan: the device stage did not finish the scan
+static const char kOutOfRange[] = "coefficient out of the baseline range (|AC| <= 1023, |DC difference| <= 2047)";
 
 // Codes one frame's scan on the device until it fits, in ctx->d_retry: the scan, then the entropy
 // stage's scratch.  The first pass may be cut into segments and has `cap` bytes.  After a pass
-// that did not finish, its flags decide: bit 1 (a look-back chain timed out) gives up; bit 2 (a
+// that did not finish, its flags decide: bit 3 (a coefficient outside the baseline range) is
+// ERR_INVALID_ARGUMENT; bit 1 (a look-back chain timed out) gives up; bit 2 (a
 // segment outgrew its share) runs again unsegmented; bit 0 (the scan did not fit, and the length is
 // the size it needs) runs again with room for that size, unless headers, scan and EOI would no
 // longer fit out_cap.  Three passes at most.  Returns 0 with the scan at the start of d_retry and
 // its length in *len, kGaveUp, or an error.  It touches no other scratch of the context but
 // d_raw (segmented passes), so encode_frames can use it while the next group's work is queued.
+// check: the arrays are the caller's (launch_jpeg_entropy); the transform's are always in range.
 static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                        const FrameGeometry &g, const HuffTables &t, uint32_t restart_interval, bool segments,
-                       size_t cap, size_t hdr, size_t out_cap, size_t *len)
+                       bool check, size_t cap, size_t hdr, size_t out_cap, size_t *len)
 {
     const size_t ent = entropy_scratch_bytes(1, g, restart_interval);
     for (int pass = 0;; ++pass) {
@@ -627,7 +630,7 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
         auto *buf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
         uint64_t *d_len = nullptr;
         uint32_t *d_ovf = nullptr;
-        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments,
+        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments, check,
                                      buf + scan_bytes, buf, cap, &d_len, &d_ovf));
         uint64_t n = 0;
         uint32_t ovf = 0;
@@ -638,6 +641,7 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
             *len = (size_t)n;
             return 0;
         }
+        if (ovf & 8u) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
         if ((ovf & 2u) || pass == 2) return kGaveUp;
         if (ovf & 4u) {
             segments = false;
@@ -759,14 +763,14 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         uint32_t *h_ovf = h_ovf_of(slot);
         if (!optimize) {
             PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g, tb[0], restart_interval, true,
-                                         ent, scan, scan_cap, &d_len, &d_ovf));
+                                         false, ent, scan, scan_cap, &d_len, &d_ovf));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, d_len, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
         } else {
             for (uint32_t k = 0; k < cnt; ++k) {  // per-image tables: one pass per image, each in its own scratch
                 uint8_t *f = c + (size_t)k * L.each;
                 PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, 1, g, tb[k], restart_interval, true,
-                                             ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
+                                             false, ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
                                              &d_ovf));
                 PIXO_CUDA(ctx, cudaMemcpyAsync(h_len + k, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
                 PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf + k, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -819,7 +823,7 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             if (!(h_ovf[k] & 2u) && ctx->gpu_retry) {
                 const size_t need = (h_ovf[k] & 4u) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
                 if (!(h_ovf[k] & 4u)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
-                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), g, t, restart_interval, false, align_up(need + 64, 256),
+                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), g, t, restart_interval, false, false, align_up(need + 64, 256),
                                  hdr[k], out_cap_each, &body);
                 if (rc != 0 && rc != kGaveUp) return rc;
             }
@@ -923,11 +927,24 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     huff_standard(t);
     uint64_t *len_src = nullptr;
     uint32_t *ovf_src = nullptr;
-    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true,
+    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true, false,
                                  reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan, scan_cap_each,
                                  &len_src, &ovf_src));
     PIXO_CUDA(ctx, cudaMemcpyAsync(d_scan_len, len_src, (size_t)n_images * 8, cudaMemcpyDeviceToDevice, ctx->stream));
     PIXO_CUDA(ctx, cudaMemcpyAsync(d_overflow, ovf_src, (size_t)n_images * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    return 0;
+}
+
+// Host coefficient arrays: baseline Huffman tables code DC differences of category <= 11 and AC values
+// of category <= 10 (what an 8-bit forward DCT can produce); anything else has no code.  seed: the DC
+// predictors before block 0 (a band of a tiled frame), or null.
+static int check_range(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb, const int16_t *cr,
+                       const FrameGeometry &g, uint32_t restart_interval, const int32_t *seed)
+{
+    if (!coefficients_in_range(y, g.ny, restart_interval, g.y_per_mcu, seed ? seed[0] : 0) ||
+        (g.has_chroma && (!coefficients_in_range(cb, g.nc, restart_interval, 1, seed ? seed[1] : 0) ||
+                          !coefficients_in_range(cr, g.nc, restart_interval, 1, seed ? seed[2] : 0))))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
     return 0;
 }
 
@@ -942,13 +959,7 @@ int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const in
     if (!y || !out || !out_len || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    // baseline Huffman tables code DC differences of category <= 11 and AC values of category <= 10
-    // (what an 8-bit forward DCT can produce); anything else has no code
-    if (!coefficients_in_range(y, g.ny, restart_interval, g.y_per_mcu) ||
-        (g.has_chroma && (!coefficients_in_range(cb, g.nc, restart_interval, 1) ||
-                          !coefficients_in_range(cr, g.nc, restart_interval, 1))))
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
-                         "coefficient out of the baseline range (|AC| <= 1023, |DC difference| <= 2047)");
+    PIXO_TRY(check_range(ctx, y, cb, cr, g, restart_interval, nullptr));
     if (out_cap < 1024 + 2)
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
     uint64_t hist[536];
@@ -1001,7 +1012,7 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     const size_t raw = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t scan_cap = std::min<size_t>((out_cap - hdr - 2) & ~(size_t)15, (size_t)default_scan_cap(ctx, raw));
     size_t body = 0;
-    const int rc = recode_scan(ctx, d_y, d_cb, d_cr, g, t, restart_interval, true, scan_cap, hdr, out_cap, &body);
+    const int rc = recode_scan(ctx, d_y, d_cb, d_cr, g, t, restart_interval, true, true, scan_cap, hdr, out_cap, &body);
     if (rc == kGaveUp) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish");
     PIXO_TRY(rc);
     PIXO_TRY(finish_frame(ctx, out, out_cap, hdr, body, out_len));
@@ -1060,15 +1071,21 @@ int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, cons
     PIXO_TRY(ensure_dev(ctx, ctx->d_misc, 256));
     PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, 256));
     auto *d = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    PIXO_CUDA(ctx, cudaMemsetAsync(d + 2, 0, 4, ctx->stream));
-    PIXO_TRY(launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, dc_seed, nullptr, d_raw, raw_cap, d,
-                                 reinterpret_cast<uint32_t *>(d + 2)));
     auto *h = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, 20, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    const uint32_t ovf = *reinterpret_cast<uint32_t *>(h + 2);
+    uint32_t ovf = 0;
+    // a segment that outgrew its share (bit 0 of a segmented pass): the band again, as one string
+    for (bool segments = true;; segments = false) {
+        PIXO_CUDA(ctx, cudaMemsetAsync(d + 2, 0, 4, ctx->stream));
+        PIXO_TRY(launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, dc_seed, nullptr, segments, d_raw, raw_cap, d,
+                                     reinterpret_cast<uint32_t *>(d + 2)));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, 20, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        ovf = *reinterpret_cast<uint32_t *>(h + 2);
+        if (!(segments && ovf == 1u && ctx->bands[d_raw].S > 1)) break;
+    }
     *nbits = h[0];
     *tail7 = (uint32_t)h[1];
+    if (ovf & 8) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
     if (ovf & 2) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish (flags %u)", ovf);
     if (ovf) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %zu too small (need %llu)", raw_cap,
                               (unsigned long long)((h[0] + 7) / 8));
@@ -1121,7 +1138,8 @@ int pixo_b200_jpeg_band_entropy_dev_async(pixo_b200_ctx *ctx, const int16_t *d_y
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %zu too small (need %zu)", raw_cap,
                          band_raw_bytes(g));
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    return launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, nullptr, d_dc_seed, d_raw, raw_cap, d_bits_tail, d_flags);
+    return launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, nullptr, d_dc_seed, true, d_raw, raw_cap, d_bits_tail,
+                               d_flags);
 }
 
 int pixo_b200_jpeg_band_splice_dev_async(pixo_b200_ctx *ctx, const uint8_t *d_raw, const uint64_t *d_offset,
@@ -1143,6 +1161,7 @@ int pixo_b200_jpeg_band_entropy(const int16_t *y, const int16_t *cb, const int16
     if (!y || !raw || !nbits || !tail7 || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
         return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
+    PIXO_TRY(check_range(nullptr, y, cb, cr, g, 0, dc_seed));
     HuffTables t;
     tables_from(hist, g.has_chroma, t);
     const uint64_t n = band_encode_raw(y, cb, cr, g, t, dc_seed, raw, raw_cap, tail7);
@@ -1159,6 +1178,7 @@ int pixo_b200_jpeg_band_histogram(const int16_t *y, const int16_t *cb, const int
     if (!y || !hist || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
         return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
+    PIXO_TRY(check_range(nullptr, y, cb, cr, g, 0, dc_seed));
     host_histogram(y, cb, cr, g, 0, hist, dc_seed);
     return 0;
 }

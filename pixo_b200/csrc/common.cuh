@@ -145,11 +145,13 @@ struct HuffTables;
 size_t entropy_scratch_bytes(uint32_t n, const FrameGeometry &g, uint32_t restart_interval);
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, uint8_t *d_scratch,
-                        uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len, uint32_t **d_overflow);
+                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, bool check,
+                        uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len,
+                        uint32_t **d_overflow);
 int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                         const FrameGeometry &g, const HuffTables &t, const int dc_seed[3], const int *d_dc_seed,
-                        uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail, uint32_t *d_flags);
+                        bool allow_segments, uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail,
+                        uint32_t *d_flags);
 int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_bit, uint32_t base_tail, bool last,
                        const uint64_t *d_base, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
                        uint32_t *d_flags);

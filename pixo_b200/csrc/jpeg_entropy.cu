@@ -84,7 +84,8 @@ struct EntParams {
     int dc_seed[3];                // DC predictors (Y, Cb, Cr) before block 0: 0 for a whole image, the previous
                                    // band's last DCs when the arrays are one band of a frame tiled over several GPUs
     unsigned long long *out_tail;  // RAW only: [n] the stream's last 7 bits
-    uint32_t *overflow;            // [n] bit 0: out_cap was exceeded (out_len = the size needed); bit 1: a chain timed out
+    uint32_t *overflow;            // [n] bit 0: out_cap was exceeded (out_len = the size needed); bit 1: a chain timed out;
+                                   // bit 3: a coefficient outside the baseline range (see code_block)
 };
 
 constexpr int CB = 32;             // blocks per chunk == one warp
@@ -221,10 +222,14 @@ __device__ __forceinline__ uint32_t msb_index(uint32_t v)  // FLO: 31 - clz, v !
 //   !SPILL: later words are dropped (the caller sees the length and runs the SPILL variant).
 // Pending bits are kept left-aligned in `acc`; a symbol arrives left-aligned too (vl, n bits).
 // Returns the block's length in bits; *acc_out = the last, partial word (left-aligned).
-template <bool SPILL>
+// CHECK (caller coefficients; pixels cannot produce anything else): a DC difference of category > 11
+// or an AC value of category > 10 has no baseline code, so its category is clamped (no table is read
+// outside its entries, the length stays <= MAX_W words) and *bad is set; the caller reports the block
+// instead of using its bits.  Off, the loop is a few instructions per symbol shorter.
+template <bool SPILL, bool CHECK>
 __device__ __forceinline__ uint32_t code_block(uint32_t M0, uint32_t M1, int diff, const uint32_t *dctab,
                                                uint32_t sa_ac, uint32_t sa_stage, uint32_t sa_slot,
-                                               uint32_t *spill, uint32_t *acc_out)
+                                               uint32_t *spill, uint32_t *acc_out, bool *bad)
 {
     uint32_t acc = 0, filled = 0;
     uint32_t sp = sa_slot;
@@ -265,7 +270,7 @@ __device__ __forceinline__ uint32_t code_block(uint32_t M0, uint32_t M1, int dif
     };
     {   // DC difference
         const uint32_t a = (uint32_t)abs(diff);
-        const uint32_t cat = 32u - (uint32_t)__clz(a);
+        const uint32_t cat = CHECK ? min(32u - (uint32_t)__clz(a), 11u) : 32u - (uint32_t)__clz(a);
         const uint32_t e = dctab[cat];
         const uint32_t amp = a ^ (((1u << cat) - 1u) & (uint32_t)(diff >> 31));
         const uint32_t n = e & 31u;
@@ -273,6 +278,7 @@ __device__ __forceinline__ uint32_t code_block(uint32_t M0, uint32_t M1, int dif
     }
     const uint32_t zrl = lds_u32(sa_ac + AC_ZRL * 4), eob = lds_u32(sa_ac + AC_EOB * 4);
     uint32_t nprev = ~0u;  // -(previous position) - 1
+    uint32_t amax = CHECK ? (uint32_t)abs(diff) >> 11 : 0u;   // non-zero: a value has no code (DC > 2047, AC > 1023)
     // (no constants live across the loop: at 80 registers ptxas re-materialises them every
     // iteration - the single-bit mask comes from BMSK, the amplitude mask from a shifted sign)
     const uint32_t sa_ac_top = sa_ac + 31u * 4u;   // entry of (run, cat) = sa_ac_top + run*48 - clz(|c|)*4
@@ -297,7 +303,8 @@ __device__ __forceinline__ uint32_t code_block(uint32_t M0, uint32_t M1, int dif
 #pragma unroll 1
             while (run >= 16u) { put(zrl & 0xFFFF0000u, zrl & 31u); run -= 16u; }  // rare: keep it small
             const uint32_t a = (uint32_t)abs(c);
-            const uint32_t lz = (uint32_t)__clz((int)a);   // 32 - cat
+            if (CHECK) amax |= a >> 10;
+            const uint32_t lz = CHECK ? max((uint32_t)__clz((int)a), 22u) : (uint32_t)__clz((int)a);   // 32 - cat
             const uint32_t e = lds_u32(sa_ac_top + run * (AC_STRIDE * 4u) - lz * 4u);
             const uint32_t amp = a ^ ((uint32_t)(c >> 31) >> lz);     // c >= 0: c; c < 0: (c - 1) masked to cat bits
             const uint32_t n = e & 31u;
@@ -306,6 +313,7 @@ __device__ __forceinline__ uint32_t code_block(uint32_t M0, uint32_t M1, int dif
     }
     if (nprev != ~63u) put(eob & 0xFFFF0000u, eob & 31u);
     *acc_out = acc;
+    *bad = amax != 0;
     return ((sp - sa_slot) / (CB * 4)) * 32u + filled;
 }
 
@@ -371,7 +379,8 @@ struct ChunkState {
 // assembled windows, phase B and chain 2 do not exist, and the final chunk reports the string's
 // bit count and its last 7 bits.  k_seg_* below splice such strings into scan bytes once their
 // bit offsets are known.
-template <bool RAW>
+// CHECK: see code_block; a block with a coefficient outside the baseline range sets overflow bit 3.
+template <bool RAW, bool CHECK>
 __global__ void __launch_bounds__(32 * HUFF_WARPS, HUFF_CTAS_PER_SM)
 k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
 {
@@ -483,9 +492,11 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             const uint32_t sa_ac = (uint32_t)__cvta_generic_to_shared(&T.ac[tbl][0]);
             const uint32_t sa_slot = (uint32_t)__cvta_generic_to_shared(slot) + 4u * lane;
             uint32_t acc;
-            L = code_block<false>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc);
+            bool bad;
+            L = code_block<false, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc, &bad);
             if (L > SLOT_W * 32u)  // long block: run again, keeping the words past the slot in local memory
-                L = code_block<true>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc);
+                L = code_block<true, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc, &bad);
+            if (CHECK && bad) atomicOr(&P.overflow[C.img], 8u);
             asm volatile("" ::: "memory");  // slot words were written through st.shared
             const int nw = (int)(L >> 5), filled = (int)(L & 31u);
             nwt = nw;
@@ -972,8 +983,10 @@ __global__ void __launch_bounds__(SPL_THREADS) k_seg_prefix(const __grid_constan
     __shared__ unsigned long long sh64[SPL_THREADS / 32];
     __shared__ uint32_t sh32[SPL_THREADS / 32];
     __shared__ int shmax[SPL_THREADS / 32];
+    __shared__ uint32_t shbad;   // the OR of the segments' flags
     const uint32_t i = blockIdx.x, s = threadIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (s == 0) shbad = 0;       // (the scans' barriers below order this before the atomicOr)
     unsigned long long base = P.base_bit;
     uint32_t base_tail = P.base_tail, last_band = P.last_band;
     if (P.base_dev) { base = P.base_dev[0]; base_tail = (uint32_t)P.base_dev[1]; last_band = (uint32_t)P.base_dev[2]; }
@@ -1007,11 +1020,15 @@ __global__ void __launch_bounds__(SPL_THREADS) k_seg_prefix(const __grid_constan
     const uint32_t tail_prev = prev >= 0 ? (uint32_t)P.tails[i * P.S + prev] : base_tail;
     r.tail_in = tail_prev & ((1u << r.phase) - 1u);
     if (live) P.rec[q] = r;
-    const uint32_t bad = (uint32_t)__syncthreads_or((int)bad_here);
+    const uint32_t wbad = __reduce_or_sync(0xffffffffu, bad_here);
+    if (lane == 0 && wbad) atomicOr(&shbad, wbad);
+    __syncthreads();
+    const uint32_t bad = shbad;
     if (s == 0) {
         P.ntiles[i] = total_tiles;
-        // a raw segment that did not fit (or a faulted chain): the caller codes the image again unsegmented
-        if (bad || total_tiles > P.max_tiles) { P.overflow[i] = 4u | (bad & 2u); P.ntiles[i] = 0; P.out_len[i] = 0; }
+        // a raw segment that did not fit (or a faulted chain): the caller codes the image again unsegmented;
+        // a coefficient outside the baseline range (bit 3) is passed on, the caller does not retry it
+        if (bad || total_tiles > P.max_tiles) { P.overflow[i] = 4u | (bad & 10u); P.ntiles[i] = 0; P.out_len[i] = 0; }
         else if (total_tiles == 0) P.out_len[i] = 0;
     }
 }
@@ -1253,9 +1270,10 @@ static uint64_t mcu_raw_bytes(const FrameGeometry &g) { return (uint64_t)g.y_per
 
 // k_huff<RAW> over the n * S segments of sp (P: the coefficient arrays and DC predictors).  The strings go
 // to raw_area, each segment's bit count and tail after them (off_bits / off_tails: a band's travel with its
-// strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).
+// strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).  check: see
+// code_block.
 static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint32_t n, const FrameGeometry &g,
-                         const SegPlan &sp, uint8_t *seg_scratch, uint8_t *raw_area)
+                         const SegPlan &sp, bool check, uint8_t *seg_scratch, uint8_t *raw_area)
 {
     cudaStream_t st = ctx->stream;
     const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
@@ -1279,7 +1297,8 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint
     PIXO_CUDA(ctx, cudaMemsetAsync(ent, 0, sp.ent.zero_bytes, st));
     const size_t want = ((size_t)P.nimages * P.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    k_huff<true><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
+    if (check) k_huff<true, true><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
+    else k_huff<true, false><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
     ctx->launches += 1;
     PIXO_CUDA(ctx, cudaGetLastError());
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_bits, P.out_len, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
@@ -1323,10 +1342,13 @@ static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, ui
 // Enqueue the entropy stage for n whole images (natural-order coefficient arrays) on ctx->stream.
 // d_scratch: entropy_scratch_bytes.  d_out: n * out_cap bytes of scan data; *d_out_len /
 // *d_overflow point into the scratch.  allow_segments: few long images may be cut into segments.
+// check: the arrays are the caller's, not the transform's - reject coefficients outside the baseline
+// range (overflow bit 3, see code_block).
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, uint8_t *d_scratch,
-                        uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len, uint32_t **d_overflow)
+                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, bool check,
+                        uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len,
+                        uint32_t **d_overflow)
 {
     const uint64_t nblocks = g.ny + 2 * g.nc;
     const uint64_t bpm_ = g.y_per_mcu + (g.has_chroma ? 2 : 0);
@@ -1369,14 +1391,15 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
         PIXO_TRY(ensure_dev(ctx, ctx->d_raw, sp.total + sp.raw_total));
         auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
         uint8_t *raw_area = seg_scratch + sp.total;
-        PIXO_TRY(code_segments(ctx, P, T, n, g, sp, seg_scratch, raw_area));
+        PIXO_TRY(code_segments(ctx, P, T, n, g, sp, check, seg_scratch, raw_area));
         return splice_segments(ctx, n, sp, seg_scratch, raw_area,
                                reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), 0, 0, true,
                                nullptr, d_out, out_cap, P.out_len, P.overflow);
     }
     const size_t want = ((size_t)n * pl.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    k_huff<false><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
+    if (check) k_huff<false, true><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
+    else k_huff<false, false><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
     ctx->launches += 1;
     PIXO_CUDA(ctx, cudaGetLastError());
     return 0;
@@ -1390,16 +1413,20 @@ size_t band_raw_bytes(const FrameGeometry &g)
 // Code one band of a frame tiled over several GPUs into the caller's buffer d_raw (k_huff<RAW> over S >= 1
 // segments, see code_segments), then k_band_totals: the band's {bit count, last 7 bits} to d_bits_tail, its
 // flags OR-ed into *d_flags.  DC predictors: d_dc_seed (device memory) when it is not null, else dc_seed.
-// A long band is cut into segments when their strings fit raw_cap; otherwise the band is one string, in
-// whatever raw_cap leaves after the trailer of bit count and tail.
+// A long band is cut into segments when allow_segments is set and their strings fit raw_cap; otherwise the
+// band is one string, in whatever raw_cap leaves after the trailer of bit count and tail.  A segment's
+// share is its pixel bytes + 4 KiB, so a dense band (large coefficients) can outgrow it (bit 0) although
+// the band as one string fits raw_cap: the caller then codes it again without segments.
 int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                         const FrameGeometry &g, const HuffTables &t, const int dc_seed[3], const int *d_dc_seed,
-                        uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail, uint32_t *d_flags)
+                        bool allow_segments, uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail,
+                        uint32_t *d_flags)
 {
     if ((g.ny + 2 * g.nc) > 0xFFFFFFFFull)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "entropy stage: too many blocks per call");
     const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
-    SegPlan sp = plan_segments(1, segments_for(1, g.total_mcus(), bpm), g.total_mcus(), bpm, mcu_raw_bytes(g));
+    SegPlan sp = plan_segments(1, allow_segments ? segments_for(1, g.total_mcus(), bpm) : 1, g.total_mcus(), bpm,
+                               mcu_raw_bytes(g));
     if (sp.S == 1 || sp.raw_total > raw_cap) {
         sp = plan_segments(1, 1, g.total_mcus(), bpm, mcu_raw_bytes(g));
         const size_t trailer = sp.raw_total - sp.raw_bytes;
@@ -1419,7 +1446,7 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     HuffDev T;
     make_huff_dev(t, &T);
     ctx->bands[d_raw] = sp;
-    PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, seg_scratch, d_raw));
+    PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, true, seg_scratch, d_raw));   // a band's arrays are the caller's
     k_band_totals<<<1, 32, 0, ctx->stream>>>(reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
                                              reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
                                              reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,

@@ -376,9 +376,10 @@ struct StuffWriter {
 
 }  // namespace
 
-bool coefficients_in_range(const int16_t *blocks, size_t nblocks, uint32_t restart_interval, uint32_t per_mcu)
+bool coefficients_in_range(const int16_t *blocks, size_t nblocks, uint32_t restart_interval, uint32_t per_mcu,
+                           int seed)
 {
-    int prev = 0;
+    int prev = seed;
     for (size_t b = 0; b < nblocks; ++b) {
         const int16_t *blk = blocks + b * 64;
         if (restart_interval && b % per_mcu == 0 && (b / per_mcu) % restart_interval == 0) prev = 0;

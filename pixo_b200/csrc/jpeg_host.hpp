@@ -62,8 +62,9 @@ size_t band_splice(const uint8_t *raw, uint64_t nbits, uint32_t phase, uint32_t 
                    uint8_t *out, size_t cap);
 
 // true when every AC coefficient has category <= 10 and every DC difference (previous block of
-// the same component, reset at restart boundaries) category <= 11
-bool coefficients_in_range(const int16_t *blocks, size_t nblocks, uint32_t restart_interval, uint32_t per_mcu);
+// the same component, reset at restart boundaries; `seed` before block 0) category <= 11
+bool coefficients_in_range(const int16_t *blocks, size_t nblocks, uint32_t restart_interval, uint32_t per_mcu,
+                           int seed = 0);
 
 // run fn(job) for job in [0, n) on up to `threads` std::threads
 void parallel_jobs(int n, int threads, void (*fn)(int, void *), void *arg);

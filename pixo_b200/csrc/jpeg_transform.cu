@@ -1014,7 +1014,9 @@ k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *_
         const int prev = reset ? 0 : (idx ? (int)arr[(idx - 1) * 64] : seed);
         const int dc = (int)(int16_t)(wv[0] & 0xFFFF);
         const int diff = (int)(int16_t)(dc - prev);
-        atomicAdd(&sh[(lum ? 0 : 12) + category16(diff)], 1u);
+        // categories past the baseline tables (DC > 11, AC > 10) are clamped to stay inside their
+        // bins; such input is rejected by the entropy stage that follows (overflow bit 3)
+        atomicAdd(&sh[(lum ? 0 : 12) + min(category16(diff), 11)], 1u);
         // AC: walk coefficients in zig-zag order
         uint32_t *ac = sh + (lum ? 24 : 280);
         int run = 0;
@@ -1027,7 +1029,7 @@ k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *_
                 ++run;
             } else {
                 if (run >= 16) { atomicAdd(&ac[0xF0], (uint32_t)(run >> 4)); run &= 15; }
-                atomicAdd(&ac[(run << 4) | category16(c)], 1u);
+                atomicAdd(&ac[(run << 4) | min(category16(c), 10)], 1u);
                 run = 0;
             }
         }

@@ -93,3 +93,46 @@ def test_entropy_rejects_uncodable_coefficients_and_bad_restart():
         with pytest.raises(pixo_b200.PixoError) as e:
             fn()
         assert e.value.code == E.ERR_INVALID_RESTART
+    # -32768 after 15 zeros in Cr (its category would index one past the chroma AC statistics), and a
+    # DC difference that is out of range only because the restart interval resets the predictor
+    c = np.zeros((1, 64), np.int16)
+    cr = c.copy(); cr[0, 12] = -32768          # natural 12 = zig-zag 16: 15 zeros before it
+    y2 = np.zeros((2, 64), np.int16); y2[:, 0] = (2047, 4000)
+    for args, opts in (((c, c, cr), JpegOptions(8, 8, ColorType.Rgb, 80, Subsampling.S444)),
+                       ((y2, z, z), JpegOptions(16, 8, ColorType.Gray, 80, Subsampling.S444, 1))):
+        with pytest.raises(pixo_b200.PixoError) as e:
+            entropy_encode(*args, opts)
+        assert e.value.code == E.ERR_INVALID_ARGUMENT
+    assert entropy_encode(y2, z, z, JpegOptions(16, 8, ColorType.Gray, 80, Subsampling.S444))[:2] == b"\xff\xd8"
+    # the band twins check the same rules, with the seed as the first predictor
+    _band_twins_reject_out_of_range()
+
+
+def _band_twins_reject_out_of_range():
+    import ctypes as C
+    E = pixo_b200._lib
+    lib = E.load()
+    z = np.zeros((1, 64), np.int16)
+
+    def both(y, cb, cr, ct, seed):
+        s = (C.c_int32 * 3)(*seed)
+        hist = np.full(537, 7, np.uint64)
+        raw = np.zeros(1 << 16, np.uint8)
+        nbits, tail = C.c_uint64(), C.c_uint32()
+        rh = lib.pixo_b200_jpeg_band_histogram(y.ctypes.data, cb.ctypes.data, cr.ctypes.data, 8, 8, ct, 0, s,
+                                               hist.ctypes.data_as(E.u64p))
+        assert hist[536] == 7
+        re = lib.pixo_b200_jpeg_band_entropy(y.ctypes.data, cb.ctypes.data, cr.ctypes.data, 8, 8, ct, 0, s, None,
+                                             raw.ctypes.data, raw.size, C.byref(nbits), C.byref(tail))
+        return rh, re
+
+    ac = z.copy(); ac[0, 1] = 1024
+    assert both(ac, z, z, 0, (0, 0, 0)) == (E.ERR_INVALID_ARGUMENT,) * 2
+    ok = z.copy(); ok[0, 0] = -1
+    assert both(ok, z, z, 0, (2047, 0, 0)) == (E.ERR_INVALID_ARGUMENT,) * 2     # -1 - 2047: the seed counts
+    assert both(ok, z, z, 0, (2046, 0, 0)) == (0, 0)
+    assert both(z, z, ok, 2, (0, 0, 2047)) == (E.ERR_INVALID_ARGUMENT,) * 2      # Cr's own seed
+    assert both(z, z, ok, 2, (0, 2047, 0)) == (0, 0)
+    for nat in (12, 63):                                                          # run 15 / run 62
+        cr = z.copy(); cr[0, nat] = -32768
+        assert both(z, z, cr, 2, (0, 0, 0)) == (E.ERR_INVALID_ARGUMENT,) * 2
