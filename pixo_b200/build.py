@@ -39,17 +39,6 @@ def needs_build() -> bool:
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_variant(out: str, defines: list[str]) -> str:
-    """Development aid: build an A/B variant (-D flags) next to the real library."""
-    cmd = [_nvcc()] + NVCC_FLAGS + [f"-D{d}" for d in defines] + \
-          [os.path.join(CSRC, s) for s in SOURCES] + ["-o", out, "-lpthread"]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0:
-        sys.stderr.write(proc.stdout + proc.stderr)
-        raise RuntimeError("nvcc failed")
-    return out
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return SO

@@ -1236,8 +1236,8 @@ int pixo_b200_png_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t i
     if (!d_data || !d_out) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    return launch_png_filter(ctx, d_data, in_stride, n_images, width, height, row_bytes,
-                             bytes_per_pixel, strategy, d_out, out_stride, d_adler);
+    return launch_png_filter_rows(ctx, d_data, in_stride, n_images, width, height, row_bytes,
+                                  bytes_per_pixel, strategy, d_out, out_stride, d_adler, nullptr, height);
 }
 
 int pixo_b200_png_filter(pixo_b200_ctx *ctx, const uint8_t *data, uint32_t width,
@@ -1254,9 +1254,10 @@ int pixo_b200_png_filter(pixo_b200_ctx *ctx, const uint8_t *data, uint32_t width
     PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
     uint32_t *d_adler = adler32_out ? reinterpret_cast<uint32_t *>(ctx->d_y.ptr) : nullptr;
-    PIXO_TRY(launch_png_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
-                               width, height, row_bytes, bytes_per_pixel, strategy,
-                               reinterpret_cast<uint8_t *>(ctx->d_out.ptr), out_bytes, d_adler));
+    PIXO_TRY(launch_png_filter_rows(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
+                                    width, height, row_bytes, bytes_per_pixel, strategy,
+                                    reinterpret_cast<uint8_t *>(ctx->d_out.ptr), out_bytes, d_adler, nullptr,
+                                    height));
     PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     if (adler32_out)
         PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));

@@ -20,13 +20,16 @@ namespace pixo {
 
 constexpr int kHistWords = 536;  // dc_lum[12] dc_chrom[12] ac_lum[256] ac_chrom[256]
 
-// Per-table divisor / reciprocal pairs, passed by value as a __grid_constant__ kernel
-// parameter so that every use is a constant-bank operand with a static offset.
-// r[i] = RN(1/d[i]); q = fma(fma(-x*r, d, x), r, x*r) == RN(x/d) for every d in 1..255 and
-// every binary32 x (proved exhaustively by tools/verify_div.c).
-struct QuantTab {
-    float lum_d[64], lum_r[64], chr_d[64], chr_r[64];
-};
+// natural index of zig-zag position i (src/jpeg/quantize.rs:18-22); with a compile-time i the
+// kernels' reorders are static register renaming
+__host__ __device__ constexpr int zz_nat(int i)
+{
+    constexpr int t[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
+                           12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
+                           35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
+                           58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+    return t[i];
+}
 
 struct Scratch {
     void *ptr = nullptr;
@@ -130,10 +133,6 @@ int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_strid
                           uint32_t n_images, size_t ny, size_t nc, uint32_t blocks_y_per_mcu,
                           uint32_t restart_interval, bool zigzag_in, uint64_t *d_hist,
                           const int *dc_seed = nullptr);
-int launch_png_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
-                      uint32_t n_images, uint32_t width, uint32_t height, size_t row_bytes,
-                      uint32_t bpp, uint32_t strategy, uint8_t *d_out, size_t out_stride,
-                      uint32_t *d_adler);
 int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
                            uint32_t width, uint32_t height, size_t row_bytes, uint32_t bpp, uint32_t strategy,
                            uint8_t *d_out, size_t out_stride, uint32_t *d_adler, const uint8_t *d_above,

@@ -33,16 +33,6 @@
 namespace pixo {
 namespace {
 
-// natural index of zig-zag position i (src/jpeg/quantize.rs:18-22)
-__host__ __device__ constexpr int zz_nat(int i)
-{
-    constexpr int t[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
-                           12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
-                           35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
-                           58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
-    return t[i];
-}
-
 // Huffman tables as the symbol loop wants them: one word per symbol,
 //   entry = (code << (32 - len)) | (len + cat),   cat = symbol & 15 (AC) or the DC category
 // i.e. the code left-aligned in the upper half-word and the total field width (code + amplitude
@@ -91,14 +81,8 @@ struct EntParams {
 constexpr int CB = 32;             // blocks per chunk == one warp
 static_assert(CB * 4 == 128, "the slot word stride is spelled out in code_block's PTX");
 constexpr int HUFF_WARPS = 4;      // warps per CTA (they only share the tables)
-#ifndef HUFF_CTAS_N
-#define HUFF_CTAS_N 6
-#endif
-constexpr int HUFF_CTAS_PER_SM = HUFF_CTAS_N;
-#ifndef HUFF_SLOT_W
-#define HUFF_SLOT_W 16
-#endif
-constexpr int SLOT_W = HUFF_SLOT_W;  // words of a block's code kept in shared memory (16: 512 bits)
+constexpr int HUFF_CTAS_PER_SM = 6;
+constexpr int SLOT_W = 16;         // words of a block's code kept in shared memory (16: 512 bits)
 constexpr int MAX_W = 54;          // worst case: 27 + 63 * 26 = 1665 bits
 constexpr int WIN_W = 256;         // stream words assembled per round (32 bytes per lane)
 constexpr int WIN_B = WIN_W * 4;

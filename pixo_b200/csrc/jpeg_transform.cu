@@ -18,23 +18,11 @@
 #include <string.h>
 
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 
 #include "common.cuh"
 
 namespace pixo {
 namespace {
-
-// zig-zag order (src/jpeg/quantize.rs:18-22) as a compile-time table: static register renaming
-__host__ __device__ constexpr int zz(int i)
-{
-    constexpr int t[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
-                           12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
-                           35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
-                           58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
-    return t[i];
-}
 
 // ---- strict binary32 arithmetic: one rounding per op, never contracted ------------------
 #define FADD(a, b) __fadd_rn((a), (b))
@@ -257,10 +245,8 @@ struct __align__(16) QPair {
     float nd_lo, nd_hi, r_lo, r_hi;
 };
 
-// The quantiser's table as a KERNEL PARAMETER (constant bank): 32 entries per component table, one
-// per output word.  With K_QMODE 1 / 2 (below) it is indexed with compile-time offsets plus a
-// warp-uniform table selector, so ptxas can fetch the entries into uniform registers; the default
-// (K_QMODE 0) copies it to shared memory once per CTA.
+// The quantiser's table, passed as a kernel parameter and copied to shared memory once per CTA:
+// 32 entries per component table, one per output word.
 struct QPairTab {
     QPair t[2][32];  // [0] luminance, [1] chrominance (x4 folded in for 4:2:0, see fill_qpair_tab)
 };
@@ -274,21 +260,9 @@ struct QPairTab {
 // `out` is the block's 128-byte slot in a warp-private shared-memory stage; its eight 16-byte
 // chunks are written at chunk index (k ^ swz) so that the lanes of a quarter warp hit distinct
 // banks (the caller then copies the stage out with fully coalesced 512-byte warp stores).
-//
-// Where the quantiser's table lives is a build-time choice (K_QMODE):
-//   0  shared memory, one copy of the transform: 32 LDS.128 per block
-//   1  constant bank with STATIC offsets (uniform-register operands, no LDS) - but static offsets
-//      mean one copy of the transform PER TABLE, which costs instruction-cache room
-//   2  as 1, but only the column pass + quantiser exists per table; the row pass (which reads no
-//      table) is shared
-// (A warp-uniform run-time index into the constant bank is no alternative: ptxas then emits
-// per-thread constant loads into vector registers, even when the index comes from a vote.)
-#ifndef K_QMODE
-#define K_QMODE 0
-#endif
-struct QuantSmem {
-    QPair t[2][32];
-};
+// The table is read from shared memory (32 LDS.128 per block) because constant-bank tables with
+// static offsets would need one copy of the transform per table, and a run-time index into the
+// constant bank gives per-thread loads.
 
 // row pass on row pairs; the post-scale is done lane by lane so the results land in the
 // column-pair layout C[r][j] = (V[r][2j], V[r][2j+1]) without transposes
@@ -357,7 +331,7 @@ __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab
 #pragma unroll
         for (int m = 0; m < 4; ++m) {
             if (ZIGZAG) {
-                const int i0 = zz(k * 8 + m * 2), i1 = zz(k * 8 + m * 2 + 1);
+                const int i0 = zz_nat(k * 8 + m * 2), i1 = zz_nat(k * 8 + m * 2 + 1);
                 w[m] = __byte_perm(W[i0 >> 1], W[i1 >> 1],
                                    ((i0 & 1) ? 0x0032 : 0x0010) | ((i1 & 1) ? 0x7600 : 0x5400));
             } else {
@@ -370,31 +344,13 @@ __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab
 
 // chroma_u MUST be warp-uniform (the callers derive it from a warp vote, so the branch is one).
 template <bool ZIGZAG>
-__device__ __forceinline__ void dct_quant_store_x2(f2 (&R)[4][8], const QPairTab &qp, const QuantSmem *qs,
-                                                   const bool chroma_u, uint4 *__restrict__ out, const int swz)
+__device__ __forceinline__ void dct_quant_store_x2(f2 (&R)[4][8], const QPairTab *qs, const bool chroma_u,
+                                                   uint4 *__restrict__ out, const int swz)
 {
-#if K_QMODE == 0
     f2 C[8][4];
     dct_rows_x2(R, C);
     const QPair *t = qs->t[chroma_u ? 1 : 0];
     dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return t[i]; }, out, swz);
-#elif K_QMODE == 1
-    if (chroma_u) {
-        f2 C[8][4];
-        dct_rows_x2(R, C);
-        dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return qp.t[1][i]; }, out, swz);
-    } else {
-        f2 C[8][4];
-        dct_rows_x2(R, C);
-        dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return qp.t[0][i]; }, out, swz);
-    }
-#else
-    f2 C[8][4];
-    dct_rows_x2(R, C);
-    if (chroma_u) dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return qp.t[1][i]; }, out, swz);
-    else dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return qp.t[0][i]; }, out, swz);
-    (void)qs;
-#endif
 }
 
 // Copy a warp's 32-slot stage (4 KB, swizzled as above) to global memory: instruction j moves
@@ -462,16 +418,11 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const void *tmap, int x, 
 // 16-byte-pitched images arrive by one 3-D cp.async.bulk.tensor (TMA); bottom-edge units
 // (row replication) and unaligned images use the warp-cooperative clamped loader.
 // =========================================================================================
-#ifndef K1_WARPS_N
-#define K1_WARPS_N 4
-#endif
-constexpr int K1_WARPS = K1_WARPS_N;
+constexpr int K1_WARPS = 4;
 constexpr int K1_THREADS = K1_WARPS * 32;
 // 2, not 3: on the H100 the 255-register build does not spill and runs 32 4K frames in 0.58 ms against
 // 0.61 ms at 3 CTAs per SM (168 registers, spills); the grid follows the occupancy query.
-#ifndef K1_MIN_BLOCKS
-#define K1_MIN_BLOCKS 2
-#endif
+constexpr int K1_MIN_BLOCKS = 2;
 constexpr int K1_MCUS = 16;             // MCUs per unit, staged as two half tiles of 8 MCUs
 constexpr int K1_HB = 8 * 16 * 3;        // 384 bytes per half-tile row
 constexpr int K1_HALF_BYTES = 16 * K1_HB;  // 6 KB; also hosts that half's 4 KB output stage
@@ -494,10 +445,21 @@ struct __align__(128) K1WarpSmem {
 
 struct __align__(128) K1Smem {
     K1WarpSmem w[K1_WARPS];
-#if K_QMODE == 0
-    QuantSmem q;
-#endif
+    QPairTab q;
 };
+
+// 8 RGB pixels in six words -> the eight raw 4-byte windows (r,g,b,next r) the dot products read
+__device__ __forceinline__ void rgb_windows8(const uint32_t (&w)[6], uint32_t (&win)[8])
+{
+    win[0] = w[0];
+    win[1] = __funnelshift_r(w[0], w[1], 24);
+    win[2] = __funnelshift_r(w[1], w[2], 16);
+    win[3] = w[2] >> 8;
+    win[4] = w[3];
+    win[5] = __funnelshift_r(w[3], w[4], 24);
+    win[6] = __funnelshift_r(w[4], w[5], 16);
+    win[7] = w[5] >> 8;
+}
 
 // One RGB row of a Y block (8 px in six words): Y - 128 as float for each pixel and the packed
 // chroma terms P = [(256 - cb) | 0xFF00, (256 - cr) | 0xFF00] clamped per colour.rs.
@@ -508,14 +470,7 @@ struct __align__(128) K1Smem {
 __device__ __forceinline__ void ycc_row8(const uint32_t (&w)[6], float (&yv)[8], uint32_t (&hs)[4])
 {
     uint32_t win[8];
-    win[0] = w[0];
-    win[1] = __funnelshift_r(w[0], w[1], 24);
-    win[2] = __funnelshift_r(w[1], w[2], 16);
-    win[3] = w[2] >> 8;
-    win[4] = w[3];
-    win[5] = __funnelshift_r(w[3], w[4], 24);
-    win[6] = __funnelshift_r(w[4], w[5], 16);
-    win[7] = w[5] >> 8;
+    rgb_windows8(w, win);
     uint32_t pp[8];
 #pragma unroll
     for (int x = 0; x < 8; ++x) {
@@ -550,12 +505,8 @@ k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
     K1WarpSmem &WS = S.w[warp];
-#if K_QMODE == 0
     for (int i = tid; i < 64; i += K1_THREADS) S.q.t[i >> 5][i & 31] = qp.t[i >> 5][i & 31];
-    const QuantSmem *QS = &S.q;
-#else
-    const QuantSmem *QS = nullptr;
-#endif
+    const QPairTab *QS = &S.q;
 
     if (lane == 0) {
         mbar_init(&WS.bar, 1);
@@ -704,7 +655,7 @@ k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
             // The transform runs in every lane (edge lanes work on garbage and their slots are never
             // flushed): the quantiser's table reads are uniform-datapath loads, which exist only in
             // warp-convergent code.
-            dct_quant_store_x2<ZIGZAG>(R, qp, QS, chroma_u, stage + slot * 8, swz);
+            dct_quant_store_x2<ZIGZAG>(R, QS, chroma_u, stage + slot * 8, swz);
             if (!chroma_u) {
                 uint4 *ybase = reinterpret_cast<uint4 *>(P.y + (size_t)img * P.y_stride +
                                                          (mcu_base + job * 8) * 4 * 64);
@@ -731,21 +682,9 @@ k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
 // row; every warp owns 32 consecutive blocks, runs the same packed block pipeline as K1 and
 // flushes its 4 KB stage with coalesced stores).
 // =========================================================================================
-constexpr int K2_BLOCKS = 64;
+constexpr int GRAY_BLOCKS = 64;
 
-// 8 RGB pixels in six words -> the eight raw 4-byte windows (r,g,b,next r) the dot products read
-__device__ __forceinline__ void rgb_windows8(const uint32_t (&w)[6], uint32_t (&win)[8])
-{
-    win[0] = w[0];
-    win[1] = __funnelshift_r(w[0], w[1], 24);
-    win[2] = __funnelshift_r(w[1], w[2], 16);
-    win[3] = w[2] >> 8;
-    win[4] = w[3];
-    win[5] = __funnelshift_r(w[3], w[4], 24);
-    win[6] = __funnelshift_r(w[4], w[5], 16);
-    win[7] = w[5] >> 8;
-}
-// ... -> Y - 128 as float
+// 8 RGB pixels in six words (see rgb_windows8) -> Y - 128 as float
 __device__ __forceinline__ void y_row8(const uint32_t (&w)[6], float (&v)[8])
 {
     uint32_t win[8];
@@ -773,45 +712,37 @@ __device__ __forceinline__ void c_row8(const uint32_t (&w)[6], uint32_t wgt, flo
 // three component passes read the same RGB tile, so it cannot double as the output stage the way
 // K1's half tiles do).  Lane = block; pass c converts the lane's 8x8 pixels to component c and
 // runs the packed DCT/quantiser; the warp's 4 KB stage goes out as 512-byte coalesced stores.
-constexpr int K4_WARPS = 4;
-constexpr int K4_THREADS = K4_WARPS * 32;
-constexpr int K4_ROW_B = 32 * 8 * 3;           // 768 bytes per tile row
-constexpr int K4_TILE_BYTES = 8 * K4_ROW_B;    // 6 KB
+constexpr int K444_WARPS = 4;
+constexpr int K444_THREADS = K444_WARPS * 32;
+constexpr int K444_ROW_B = 32 * 8 * 3;           // 768 bytes per tile row
+constexpr int K444_TILE_BYTES = 8 * K444_ROW_B;  // 6 KB
+// 2, not 3: at 168 registers ptxas demotes a block array to local memory; on the H100 the 4:4:4
+// kernel takes 0.93 ms per 32 4K frames at 2 CTAs per SM against 0.99-1.00 ms at 3.
+constexpr int K444_MIN_BLOCKS = 2;
 
-struct __align__(128) K4WarpSmem {
-    uint8_t tile[2][K4_TILE_BYTES];
+struct __align__(128) K444WarpSmem {
+    uint8_t tile[2][K444_TILE_BYTES];
     uint4 stage[256];
     uint64_t bar[2];
 };
 
-struct __align__(128) K4Smem {
-    K4WarpSmem w[K4_WARPS];
-#if K_QMODE == 0
-    QuantSmem q;
-#endif
+struct __align__(128) K444Smem {
+    K444WarpSmem w[K444_WARPS];
+    QPairTab q;
 };
 
 // K1Params with mcus_x / mcus_y = blocks per row / block rows, units_x = units per block row
-// 2, not 3: at 168 registers ptxas demotes a block array to local memory; on the H100 the 4:4:4
-// kernel takes 0.93 ms per 32 4K frames at 2 CTAs per SM against 0.99-1.00 ms at 3.
-#ifndef K4_MIN_BLOCKS
-#define K4_MIN_BLOCKS 2
-#endif
 template <bool ZIGZAG>
-__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS)
+__global__ void __launch_bounds__(K444_THREADS, K444_MIN_BLOCKS)
 k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab qp,
            const __grid_constant__ CUtensorMap tmap)
 {
     extern __shared__ __align__(128) uint8_t smem_raw[];
-    K4Smem &S = *reinterpret_cast<K4Smem *>(smem_raw);
+    K444Smem &S = *reinterpret_cast<K444Smem *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    K4WarpSmem &WS = S.w[warp];
-#if K_QMODE == 0
-    for (int i = tid; i < 64; i += K4_THREADS) S.q.t[i >> 5][i & 31] = qp.t[i >> 5][i & 31];
-    const QuantSmem *QS = &S.q;
-#else
-    const QuantSmem *QS = nullptr;
-#endif
+    K444WarpSmem &WS = S.w[warp];
+    for (int i = tid; i < 64; i += K444_THREADS) S.q.t[i >> 5][i & 31] = qp.t[i >> 5][i & 31];
+    const QPairTab *QS = &S.q;
     if (lane == 0) {
         mbar_init(&WS.bar[0], 1);
         mbar_init(&WS.bar[1], 1);
@@ -821,7 +752,7 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
 
     const uint32_t units_per_img = P.mcus_y * P.units_x;   // no division in the loop: see k_jpeg_420
     const uint64_t nunits = (uint64_t)units_per_img * P.n_images;
-    const uint32_t stride = gridDim.x * K4_WARPS;
+    const uint32_t stride = gridDim.x * K444_WARPS;
     const uint32_t d_ux = stride % P.units_x, d_t = stride / P.units_x;
     const uint32_t d_by = d_t % P.mcus_y, d_img = d_t / P.mcus_y;
     uint32_t phase = 0;  // bit b = parity to wait for on bar[b]
@@ -837,15 +768,15 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
     auto issue_tma = [&](uint32_t img_, uint32_t by_, uint32_t ux_, int b) {
         if (unit_by_tma(by_)) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(&WS.bar[b], K4_TILE_BYTES);
-            tma_load_3d(WS.tile[b], &tmap, (int)(ux_ * (K4_ROW_B / 8)), (int)(by_ * 8), (int)img_, &WS.bar[b]);
+            mbar_expect_tx(&WS.bar[b], K444_TILE_BYTES);
+            tma_load_3d(WS.tile[b], &tmap, (int)(ux_ * (K444_ROW_B / 8)), (int)(by_ * 8), (int)img_, &WS.bar[b]);
         }
     };
 
-    uint64_t u = (uint64_t)blockIdx.x * K4_WARPS + warp;
+    uint64_t u = (uint64_t)blockIdx.x * K444_WARPS + warp;
     uint32_t img, by, ux;
     {
-        const uint32_t u0 = blockIdx.x * K4_WARPS + warp;
+        const uint32_t u0 = blockIdx.x * K444_WARPS + warp;
         img = u0 / units_per_img;
         const uint32_t rem = u0 - img * units_per_img;
         by = rem / P.units_x;
@@ -871,7 +802,7 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
         // warp-convergent, which the quantiser's uniform-datapath table reads need.
         const uint8_t *base = WS.tile[b] + lane * 24;
         auto row_words = [&](int r, uint32_t (&wds)[6]) {
-            const uint2 *p = reinterpret_cast<const uint2 *>(base + r * K4_ROW_B);
+            const uint2 *p = reinterpret_cast<const uint2 *>(base + r * K444_ROW_B);
             const uint2 a = p[0], c1 = p[1], c2 = p[2];
             wds[0] = a.x; wds[1] = a.y; wds[2] = c1.x; wds[3] = c1.y; wds[4] = c2.x; wds[5] = c2.y;
         };
@@ -908,7 +839,7 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
                     for (int x = 0; x < 8; ++x) R[rp][x] = pk(v0[x], v1[x]);
                 }
             }
-            dct_quant_store_x2<ZIGZAG>(R, qp, QS, chroma_u, WS.stage + lane * 8, lane & 7);
+            dct_quant_store_x2<ZIGZAG>(R, QS, chroma_u, WS.stage + lane * 8, lane & 7);
             flush(comp == 0 ? P.y + (size_t)img * P.y_stride : (comp == 1 ? P.cb : P.cr) + (size_t)img * P.c_stride);
         }
         __syncwarp();  // every lane is done with tile[b]: the TMA issued next iteration may refill it
@@ -922,25 +853,21 @@ k_jpeg_gray(const uint8_t *__restrict__ pixels, size_t pixel_stride, uint32_t w,
             uint32_t blocks_x, uint32_t tiles_x, int16_t *__restrict__ yout, size_t y_stride,
             const __grid_constant__ QPairTab qp)
 {
-    constexpr int TB = K2_BLOCKS * 8;  // 512
+    constexpr int TB = GRAY_BLOCKS * 8;  // 512
     __shared__ __align__(16) uint8_t tile[8 * TB];
     __shared__ __align__(16) uint4 stage[2][256];
-#if K_QMODE == 0
-    __shared__ QuantSmem qsm;
+    __shared__ QPairTab qsm;
     for (int i = threadIdx.x; i < 64; i += 64) qsm.t[i >> 5][i & 31] = qp.t[i >> 5][i & 31];
-    const QuantSmem *QS = &qsm;
-#else
-    const QuantSmem *QS = nullptr;
-#endif
+    const QPairTab *QS = &qsm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tx = blockIdx.x % tiles_x;
     const uint32_t brow = blockIdx.x / tiles_x;
     const uint32_t img = blockIdx.y;
     const uint8_t *image = pixels + (size_t)img * pixel_stride;
-    load_tile<1, 8, K2_BLOCKS * 8, 64>(tile, image, w, h, tx * (K2_BLOCKS * 8), brow * 8, tid);
+    load_tile<1, 8, GRAY_BLOCKS * 8, 64>(tile, image, w, h, tx * (GRAY_BLOCKS * 8), brow * 8, tid);
     __syncthreads();
     const int j = tid;
-    const uint32_t b0 = tx * K2_BLOCKS;
+    const uint32_t b0 = tx * GRAY_BLOCKS;
     {   // every lane (the tile is fully defined: load_tile replicates past the right edge; the flush drops them)
         f2 R[4][8];
 #pragma unroll
@@ -956,7 +883,7 @@ k_jpeg_gray(const uint8_t *__restrict__ pixels, size_t pixel_stride, uint32_t w,
                 R[rp][x] = sub2(pk(f0, f1), K2(8388736.0f));
             }
         }
-        dct_quant_store_x2<ZIGZAG>(R, qp, QS, false, stage[warp] + lane * 8, lane & 7);
+        dct_quant_store_x2<ZIGZAG>(R, QS, false, stage[warp] + lane * 8, lane & 7);
     }
     const uint32_t first = b0 + warp * 32;
     uint4 *dbase = reinterpret_cast<uint4 *>(yout + (size_t)img * y_stride + ((size_t)brow * blocks_x + first) * 64);
@@ -1022,7 +949,7 @@ k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *_
         int run = 0;
 #pragma unroll
         for (int i = 1; i < 64; ++i) {
-            const int nat = ZIGZAG_IN ? i : zz(i);
+            const int nat = ZIGZAG_IN ? i : zz_nat(i);
             const uint32_t word = wv[nat >> 1];
             const int c = (int)(int16_t)((nat & 1) ? (word >> 16) : (word & 0xFFFF));
             if (c == 0) {
@@ -1103,68 +1030,38 @@ bool make_rgb_tensor_map(CUtensorMap *tm, const uint8_t *pixels, size_t pixel_st
                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int launch_k1(pixo_b200_ctx *ctx, const uint8_t *px, size_t pixel_stride, uint32_t n, uint32_t w,
-              uint32_t h, int16_t *y, size_t y_stride, int16_t *cb, int16_t *cr, size_t c_stride,
-              const QPairTab &qt, bool zigzag)
+// k_jpeg_420, or k_jpeg_444 when `s444`: persistent kernels with one unit per warp in flight, so the
+// grid is as many CTAs as fit on the device (the occupancy query, asked once per device, kernel and
+// zigzag flag) and no more than the units need.  Only enqueues: the caller counts the launch.
+int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, bool zigzag, const uint8_t *px, size_t pixel_stride,
+                         uint32_t n, uint32_t w, uint32_t h, int16_t *y, size_t y_stride, int16_t *cb,
+                         int16_t *cr, size_t c_stride, const QPairTab &qt)
 {
+    // 4:2:0 walks MCUs of 16x16 px, 16 to a unit; 4:4:4 walks 8x8 blocks, 32 to a unit
+    const uint32_t px_per = s444 ? 8 : 16, per_unit = s444 ? 32 : K1_MCUS;
     K1Params P;
     P.pixels = px; P.pixel_stride = pixel_stride; P.w = w; P.h = h;
-    P.mcus_x = (w + 15) / 16; P.mcus_y = (h + 15) / 16;
-    P.units_x = (P.mcus_x + K1_MCUS - 1) / K1_MCUS;
+    P.mcus_x = (w + px_per - 1) / px_per; P.mcus_y = (h + px_per - 1) / px_per;
+    P.units_x = (P.mcus_x + per_unit - 1) / per_unit;
     P.n_images = n; P.y = y; P.cb = cb; P.cr = cr; P.y_stride = y_stride; P.c_stride = c_stride;
     alignas(64) CUtensorMap tm;
     memset(&tm, 0, sizeof tm);
-    P.use_tma = make_rgb_tensor_map(&tm, px, pixel_stride, n, w, h, K1_HB / 8, 16) ? 1u : 0u;
-    static int blocks_per_sm[64][2];  // function attributes are per device
-    const size_t smem = sizeof(K1Smem);
-    auto kern = zigzag ? k_jpeg_420<true> : k_jpeg_420<false>;
-    int &bps = blocks_per_sm[ctx->device & 63][zigzag];
+    // one TMA box: half a 4:2:0 unit (8 MCUs) or a whole 4:4:4 unit, px_per rows
+    P.use_tma = make_rgb_tensor_map(&tm, px, pixel_stride, n, w, h, (s444 ? K444_ROW_B : K1_HB) / 8, px_per) ? 1u : 0u;
+    const int warps = s444 ? K444_WARPS : K1_WARPS;
+    const size_t smem = s444 ? sizeof(K444Smem) : sizeof(K1Smem);
+    auto kern = !s444 ? (zigzag ? k_jpeg_420<true> : k_jpeg_420<false>) : (zigzag ? k_jpeg_444<true> : k_jpeg_444<false>);
+    static int blocks_per_sm[64][2][2];  // [device][s444][zigzag]: function attributes are per device
+    int &bps = blocks_per_sm[ctx->device & 63][s444][zigzag];
     if (!bps) {
         PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int nb = 0;
-        PIXO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, K1_THREADS, smem));
+        PIXO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, warps * 32, smem));
         bps = nb > 0 ? nb : 1;
     }
     const uint64_t nunits = (uint64_t)P.mcus_y * P.units_x * n;
-    uint64_t grid = (uint64_t)ctx->sm_count * bps;
-    if (grid > (nunits + K1_WARPS - 1) / K1_WARPS) grid = (nunits + K1_WARPS - 1) / K1_WARPS;
-    kern<<<(unsigned)grid, K1_THREADS, smem, ctx->stream>>>(P, qt, tm);
-    ctx->launches++;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
-}
-
-int launch_k444(pixo_b200_ctx *ctx, const uint8_t *px, size_t pixel_stride, uint32_t n, uint32_t w,
-                uint32_t h, int16_t *y, size_t y_stride, int16_t *cb, int16_t *cr, size_t c_stride,
-                const QPairTab &qt, bool zigzag)
-{
-    K1Params P;
-    P.pixels = px; P.pixel_stride = pixel_stride; P.w = w; P.h = h;
-    P.mcus_x = (w + 7) / 8; P.mcus_y = (h + 7) / 8;     // blocks
-    P.units_x = (P.mcus_x + 31) / 32;
-    P.n_images = n; P.y = y; P.cb = cb; P.cr = cr; P.y_stride = y_stride; P.c_stride = c_stride;
-    alignas(64) CUtensorMap tm;
-    memset(&tm, 0, sizeof tm);
-    P.use_tma = make_rgb_tensor_map(&tm, px, pixel_stride, n, w, h, K4_ROW_B / 8, 8) ? 1u : 0u;
-    static int blocks_per_sm[64][2];  // function attributes are per device
-    const size_t smem = sizeof(K4Smem);
-    auto kern = zigzag ? k_jpeg_444<true> : k_jpeg_444<false>;
-    int &bps = blocks_per_sm[ctx->device & 63][zigzag];
-    if (!bps) {
-        PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int nb = 0;
-        PIXO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, K4_THREADS, smem));
-        bps = nb > 0 ? nb : 1;
-    }
-    const uint64_t nunits = (uint64_t)P.mcus_y * P.units_x * n;
-    uint64_t grid = (uint64_t)ctx->sm_count * bps;
-    if (grid > (nunits + K4_WARPS - 1) / K4_WARPS) grid = (nunits + K4_WARPS - 1) / K4_WARPS;
-    if (getenv("PIXO_B200_DEBUG"))
-        fprintf(stderr, "k_jpeg_444: use_tma=%u blocks/SM=%d grid=%llu units=%llu\n", P.use_tma, bps,
-                (unsigned long long)grid, (unsigned long long)nunits);
-    kern<<<(unsigned)grid, K4_THREADS, smem, ctx->stream>>>(P, qt, tm);
-    ctx->launches++;
-    PIXO_CUDA(ctx, cudaGetLastError());
+    const uint64_t grid = std::min<uint64_t>((uint64_t)ctx->sm_count * bps, (nunits + warps - 1) / warps);
+    kern<<<(unsigned)grid, warps * 32, smem, ctx->stream>>>(P, qt, tm);
     return 0;
 }
 
@@ -1199,16 +1096,13 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
         int16_t *cr = d_cr ? d_cr + (size_t)i0 * c_stride : nullptr;
         if (color_type == PIXO_B200_GRAY) {
             const uint32_t bx = (w + 7) / 8, by = (h + 7) / 8;
-            const uint32_t tiles_x = (bx + K2_BLOCKS - 1) / K2_BLOCKS;
+            const uint32_t tiles_x = (bx + GRAY_BLOCKS - 1) / GRAY_BLOCKS;
             dim3 grid(tiles_x * by, nb);
             if (zigzag) k_jpeg_gray<true><<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, qt);
             else k_jpeg_gray<false><<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, qt);
-        } else if (subsampling == PIXO_B200_S444) {
-            PIXO_TRY(launch_k444(ctx, px, pixel_stride, nb, w, h, y, y_stride, cb, cr, c_stride, qt, zigzag));
-            continue;
         } else {
-            PIXO_TRY(launch_k1(ctx, px, pixel_stride, nb, w, h, y, y_stride, cb, cr, c_stride, qt, zigzag));
-            continue;
+            PIXO_TRY(launch_rgb_transform(ctx, subsampling == PIXO_B200_S444, zigzag, px, pixel_stride, nb, w, h, y,
+                                          y_stride, cb, cr, c_stride, qt));
         }
         ctx->launches++;
         PIXO_CUDA(ctx, cudaGetLastError());

@@ -90,13 +90,46 @@ __device__ __forceinline__ uint32_t paeth_pred4(uint32_t a, uint32_t b, uint32_t
     return sel4(cw, c, near);
 }
 
-__device__ __forceinline__ uint32_t paeth4(uint32_t a, uint32_t b, uint32_t c) { return paeth_pred4(a, b, c); }
-
 __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v)
 {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// The reference's decision ladders over a row's score_filter sums s[] (sum |i8|), up to Paeth:
+// adaptive_filter (src/png/filter.rs:302-393) goes through None, Sub, Up, Average and
+// adaptive_filter_fast (:474-527) through Sub, Up.  A candidate replaces the best on a strict <,
+// and the ladder ends early once the best scores <= early.  When it has not ended, Paeth then
+// replaces the best on a strict < (the callers decide when to score Paeth).
+struct LadderPick {
+    int filter;
+    unsigned long long score;
+    bool done;   // the ladder ended early: Paeth is out
+};
+template <typename Scores>
+__device__ __forceinline__ LadderPick cheap_ladder(Scores s, bool fast, uint32_t row_bytes)
+{
+    LadderPick p;
+    if (fast) {
+        const unsigned long long early = (unsigned long long)row_bytes / 8 + 1;
+        p.filter = 1; p.score = s[1];
+        p.done = p.score <= early;
+        if (!p.done) {
+            if (s[2] < p.score) { p.score = s[2]; p.filter = 2; }
+            p.done = p.score <= early;
+        }
+    } else {
+        const unsigned long long early = (unsigned long long)row_bytes / 4 + 1;
+        p.filter = 0; p.score = s[0];
+        p.done = p.score <= early;
+        for (int f = 1; f < 4 && !p.done; ++f)
+            if (s[f] < p.score) {
+                p.score = s[f]; p.filter = f;
+                if (p.score == 0 || p.score <= early) p.done = true;
+            }
+    }
+    return p;
 }
 
 // Copy `len` bytes src[0..len) to dst (shared, 16-byte aligned) with the widest loads the
@@ -191,9 +224,22 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
     const uint32_t bpp = P.bpp;
     const uint32_t ashift = (4 - bpp) * 8;
     const int nseg = (int)((rb + segcap - 1) / segcap);
-    // optimize_alpha: rewrite the staged words (halo included; segments start on 16-byte
-    // multiples, so words never straddle pixels) before anyone reads them
-    auto fix_alpha = [&](int slen) {
+    // Stage bytes [s0, s0 + slen) of the row and of the row above into cur / prev; callers first
+    // wait at a barrier for the previous segment's readers.  A 16-byte front halo holds the bytes
+    // left of the segment (zeros at row start), and the tail of the last word is zeroed so masked
+    // lanes read defined data.  Then optimize_alpha rewrites the staged words (halo included;
+    // segments start on 16-byte multiples, so words never straddle pixels) before anyone reads them.
+    auto stage_segment = [&](size_t s0, int slen) {
+        if (tid < 16) {
+            const long long gi = (long long)s0 - 16 + tid;
+            cur[tid] = gi >= 0 ? row[gi] : 0;
+            prev[tid] = (gi >= 0 && prow) ? prow[gi] : 0;
+        }
+        stage_bytes(cur + 16, row + s0, slen, lo_b, hi_b, tid);
+        if (prow) stage_bytes(prev + 16, prow + s0, slen, plo_b, phi_b, tid);
+        else for (int i = tid; i < slen; i += PNG_THREADS) prev[16 + i] = 0;
+        for (int i = slen + tid; i < ((slen + 3) & ~3); i += PNG_THREADS) { cur[16 + i] = 0; prev[16 + i] = 0; }
+        __syncthreads();
         if (!P.opt_alpha) return;
         const int nwords = (16 + slen + 3) >> 2;
         for (int k = tid; k < nwords; k += PNG_THREADS) {
@@ -228,20 +274,7 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                 const size_t s0 = (size_t)seg * segcap;
                 const int slen = (int)min((size_t)segcap, rb - s0);
                 __syncthreads();
-                if (nseg > 1 || f == 0) {
-                    if (tid < 16) {
-                        const long long gi = (long long)s0 - 16 + tid;
-                        cur[tid] = gi >= 0 ? row[gi] : 0;
-                        prev[tid] = (gi >= 0 && prow) ? prow[gi] : 0;
-                    }
-                    stage_bytes(cur + 16, row + s0, slen, lo_b, hi_b, tid);
-                    if (prow) stage_bytes(prev + 16, prow + s0, slen, plo_b, phi_b, tid);
-                    else for (int i = tid; i < slen; i += PNG_THREADS) prev[16 + i] = 0;
-                    // zero the tail of the last word (defined data for the word-wise passes)
-                    for (int i = slen + tid; i < ((slen + 3) & ~3); i += PNG_THREADS) { cur[16 + i] = 0; prev[16 + i] = 0; }
-                    __syncthreads();
-                    fix_alpha(slen);
-                }
+                if (nseg > 1 || f == 0) stage_segment(s0, slen);
                 const uint32_t *c32 = reinterpret_cast<const uint32_t *>(cur) + 4;
                 const uint32_t *p32 = reinterpret_cast<const uint32_t *>(prev) + 4;
                 const int nw = (slen + 3) >> 2;
@@ -255,7 +288,7 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                     case 1: v = __vsub4(x, a); break;
                     case 2: v = __vsub4(x, b); break;
                     case 3: v = __vsub4(x, __vhaddu4(a, b)); break;
-                    default: v = __vsub4(x, paeth4(a, b, c)); break;
+                    default: v = __vsub4(x, paeth_pred4(a, b, c)); break;
                     }
                     reinterpret_cast<uint32_t *>(sbuf)[k] = v;
                 }
@@ -298,19 +331,7 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                                  (nseg > 1);
             if (restage) {
                 __syncthreads();
-                // 16-byte front halo: the bpp bytes left of the segment (zeros at row start)
-                if (tid < 16) {
-                    const long long gi = (long long)s0 - 16 + tid;
-                    cur[tid] = gi >= 0 ? row[gi] : 0;
-                    prev[tid] = (gi >= 0 && prow) ? prow[gi] : 0;
-                }
-                stage_bytes(cur + 16, row + s0, slen, lo_b, hi_b, tid);
-                if (prow) stage_bytes(prev + 16, prow + s0, slen, plo_b, phi_b, tid);
-                else for (int i = tid; i < slen; i += PNG_THREADS) prev[16 + i] = 0;
-                // zero the tail of the last word so masked lanes read defined data
-                for (int i = slen + tid; i < ((slen + 3) & ~3); i += PNG_THREADS) { cur[16 + i] = 0; prev[16 + i] = 0; }
-                __syncthreads();
-                fix_alpha(slen);
+                stage_segment(s0, slen);
             }
             const uint32_t *c32 = reinterpret_cast<const uint32_t *>(cur) + 4;
             const uint32_t *p32 = reinterpret_cast<const uint32_t *>(prev) + 4;
@@ -327,7 +348,7 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                     sc[1] += sum_abs_s8x4(__vsub4(x, a) & mask);
                     sc[2] += sum_abs_s8x4(__vsub4(x, b) & mask);
                     if (!fast) sc[3] += sum_abs_s8x4(__vsub4(x, __vhaddu4(a, b)) & mask);
-                    sc[4] += sum_abs_s8x4(__vsub4(x, paeth4(a, b, c)) & mask);
+                    sc[4] += sum_abs_s8x4(__vsub4(x, paeth_pred4(a, b, c)) & mask);
                 } else {
                     uint32_t f;
                     switch (filter) {
@@ -335,7 +356,7 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                     case 1: f = __vsub4(x, a); break;
                     case 2: f = __vsub4(x, b); break;
                     case 3: f = __vsub4(x, __vhaddu4(a, b)); break;
-                    default: f = __vsub4(x, paeth4(a, b, c)); break;
+                    default: f = __vsub4(x, paeth_pred4(a, b, c)); break;
                     }
                     f &= mask;
                     // Adler terms: stream index q = 1 + s0 + 4k + j, weight (n_out - q)
@@ -385,33 +406,8 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
                     for (int w = 0; w < PNG_THREADS / 32; ++w) t += red[f][w];
                     s[f] = t;
                 }
-                int best;
-                if (P.strategy == PIXO_B200_FILTER_ADAPTIVE_FAST) {
-                    // adaptive_filter_fast, src/png/filter.rs:474-527
-                    const unsigned long long early = (unsigned long long)rb / 8 + 1;
-                    best = 1;
-                    unsigned long long bs = s[1];
-                    if (bs > early) {
-                        if (s[2] < bs) { bs = s[2]; best = 2; }
-                        if (bs > early && s[4] < bs) best = 4;
-                    }
-                } else {
-                    // adaptive_filter, src/png/filter.rs:302-393: first candidate (None, Sub, Up,
-                    // Average in order) that becomes the best with a score <= early wins
-                    // outright; otherwise strict-< argmin, Paeth last.
-                    const unsigned long long early = (unsigned long long)rb / 4 + 1;
-                    best = 0;
-                    unsigned long long bs = s[0];
-                    bool done = bs <= early;  // covers the score == 0 exit as well
-                    for (int f = 1; f < 5 && !done; ++f) {
-                        if (s[f] < bs) {
-                            bs = s[f];
-                            best = f;
-                            if (f < 4 && (bs == 0 || bs <= early)) done = true;
-                        }
-                    }
-                }
-                s_filter = best;
+                const LadderPick p = cheap_ladder(s, P.strategy == PIXO_B200_FILTER_ADAPTIVE_FAST, P.row_bytes_lo);
+                s_filter = !p.done && s[4] < p.score ? 4 : p.filter;   // Paeth replaces on strict <
             }
             __syncthreads();
             filter = s_filter;
@@ -466,13 +462,8 @@ __global__ void __launch_bounds__(PNG_THREADS) k_png_filter(const PngParams P)
 // =========================================================================================
 // 3, not 4: at 64 registers k_png_band<0> spills; on the H100 64 4K RGBA frames take 2.32-2.34 ms
 // (Adaptive) / 2.19-2.20 ms (AdaptiveFast) at 80 registers against 2.61-2.62 / 2.49 ms at 64.
-#ifndef PNG_BAND_MIN_BLOCKS
-#define PNG_BAND_MIN_BLOCKS 3
-#endif
-#ifndef PNG_BAND_ROWS
-#define PNG_BAND_ROWS 16
-#endif
-constexpr int BAND_ROWS = PNG_BAND_ROWS;
+constexpr int PNG_BAND_MIN_BLOCKS = 3;
+constexpr int BAND_ROWS = 16;
 
 struct BandParams {
     const uint8_t *data;
@@ -538,7 +529,7 @@ __global__ void __launch_bounds__(PNG_THREADS, PNG_BAND_MIN_BLOCKS) k_png_band(c
     const uint32_t chunk = (((nj + 7) / 8) + 31) & ~31u;
     const uint32_t j_lo = warp * chunk, j_hi = min(nj, j_lo + chunk);
 
-    auto load_row = [&](uint32_t r, uint8_t *buf, bool async) {
+    auto load_row = [&](uint32_t r, uint8_t *buf) {
         const uint8_t *src = image + (size_t)r * rb;
         if (P.async16) {
             const uint32_t nv = rb >> 4;
@@ -547,7 +538,6 @@ __global__ void __launch_bounds__(PNG_THREADS, PNG_BAND_MIN_BLOCKS) k_png_band(c
         } else {
             stage_bytes(buf + 16, src, (int)rb, lo_b, hi_b, tid);
         }
-        (void)async;
     };
     // halos are zero for the whole band ("left" of the first pixel is 0)
     if (tid < 12) reinterpret_cast<uint32_t *>(bufs[tid >> 2])[tid & 3] = 0;
@@ -560,9 +550,9 @@ __global__ void __launch_bounds__(PNG_THREADS, PNG_BAND_MIN_BLOCKS) k_png_band(c
             stage_bytes(bufs[(r0 + 2) % 3] + 16, P.above, (int)rb, P.above, P.above + rb, tid);
         }
     } else {
-        load_row(r0 - 1, bufs[(r0 + 2) % 3], false);
+        load_row(r0 - 1, bufs[(r0 + 2) % 3]);
     }
-    load_row(r0, bufs[r0 % 3], false);
+    load_row(r0, bufs[r0 % 3]);
     asm volatile("cp.async.commit_group;" ::: "memory");
 
     unsigned long long accA = 0, accBpos = 0, accBneg = 0;
@@ -570,7 +560,7 @@ __global__ void __launch_bounds__(PNG_THREADS, PNG_BAND_MIN_BLOCKS) k_png_band(c
 
     bool prev_needed_paeth = false;   // the band's first row takes the two-phase route
     for (uint32_t r = r0; r < r1; ++r) {
-        if (r + 1 < r1) load_row(r + 1, bufs[(r + 1) % 3], true);
+        if (r + 1 < r1) load_row(r + 1, bufs[(r + 1) % 3]);
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 1;" ::: "memory");   // everything but the newest group
         __syncthreads();
@@ -689,31 +679,12 @@ __global__ void __launch_bounds__(PNG_THREADS, PNG_BAND_MIN_BLOCKS) k_png_band(c
             else { score_row(std::integral_constant<int, 0>{}); reduce_scores(0, 4); }
             if (tid == 0) {
                 const volatile unsigned long long *sc = s_score;
-                int best;
-                bool done;
-                unsigned long long bs;
-                if (fast) {   // adaptive_filter_fast, src/png/filter.rs:474-527
-                    const unsigned long long early = (unsigned long long)rb / 8 + 1;
-                    best = 1; bs = sc[1];
-                    done = bs <= early;
-                    if (!done) {
-                        if (sc[2] < bs) { bs = sc[2]; best = 2; }
-                        done = bs <= early;
-                    }
-                } else {      // adaptive_filter, src/png/filter.rs:302-393
-                    const unsigned long long early = (unsigned long long)rb / 4 + 1;
-                    best = 0; bs = sc[0];
-                    done = bs <= early;
-                    for (int f = 1; f < 4 && !done; ++f)
-                        if (sc[f] < bs) {
-                            bs = sc[f]; best = f;
-                            if (bs == 0 || bs <= early) done = true;
-                        }
-                }
-                if (fused && !done && sc[4] < bs) best = 4;   // Paeth replaces on strict <
+                const LadderPick p = cheap_ladder(sc, fast, rb);
+                int best = p.filter;
+                if (fused && !p.done && sc[4] < p.score) best = 4;   // Paeth replaces on strict <
                 s_filter = best;
-                s_best = bs;
-                s_need_paeth = done ? 0 : 1;
+                s_best = p.score;
+                s_need_paeth = p.done ? 0 : 1;
             }
             __syncthreads();
             prev_needed_paeth = s_need_paeth != 0;
@@ -990,20 +961,6 @@ k_adler32(const uint8_t *__restrict__ data, size_t len, unsigned long long *acc,
 }
 
 }  // namespace
-
-int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
-                           uint32_t n_images, uint32_t width, uint32_t height, size_t row_bytes,
-                           uint32_t bpp, uint32_t strategy, uint8_t *d_out, size_t out_stride,
-                           uint32_t *d_adler, const uint8_t *d_above, uint32_t rule_height);
-
-int launch_png_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
-                      uint32_t n_images, uint32_t width, uint32_t height, size_t row_bytes,
-                      uint32_t bpp, uint32_t strategy, uint8_t *d_out, size_t out_stride,
-                      uint32_t *d_adler)
-{
-    return launch_png_filter_rows(ctx, d_data, in_stride, n_images, width, height, row_bytes, bpp, strategy, d_out,
-                                  out_stride, d_adler, nullptr, height);
-}
 
 // `height` rows starting at d_data; d_above (single image only): the raw row above them when they
 // are a band of an image of `rule_height` rows (the strategy pre-rules look at the whole image).
