@@ -464,18 +464,39 @@ static int finish_frame(pixo_b200_ctx *ctx, uint8_t *out, size_t out_cap, size_t
     return 0;
 }
 
-// Coefficient arrays of consecutive frames in one buffer: per frame Y, then Cb, then Cr, each array
-// 256-byte aligned, so one stride steps each array to the next frame's.
+// Coefficient records (common.cuh) of consecutive frames in one buffer: per frame the Y, Cb and Cr
+// coefficient arrays, then their three extent arrays, each array 256-byte aligned, so one stride steps
+// each array to the next frame's.
 struct CoefLayout {
-    size_t yb, cbb, each;  // bytes of the Y array, of one chroma array, of a frame
+    size_t yb, cbb, yeb, ceb, each;  // bytes of the Y array, of one chroma array, of their extents, of a frame
     explicit CoefLayout(const FrameGeometry &g)
         : yb(align_up(g.ny * 64 * sizeof(int16_t), 256)), cbb(align_up(g.nc * 64 * sizeof(int16_t), 256)),
-          each(yb + 2 * cbb) {}
+          yeb(align_up(g.ny, 256)), ceb(align_up(g.nc, 256)), each(yb + 2 * cbb + yeb + 2 * ceb) {}
     size_t stride() const { return each / sizeof(int16_t); }
     int16_t *y(void *frame) const { return reinterpret_cast<int16_t *>(frame); }
     int16_t *cb(void *frame) const { return reinterpret_cast<int16_t *>(static_cast<uint8_t *>(frame) + yb); }
     int16_t *cr(void *frame) const { return reinterpret_cast<int16_t *>(static_cast<uint8_t *>(frame) + yb + cbb); }
+    CoefExtents extents(void *frame) const
+    {
+        uint8_t *e = static_cast<uint8_t *>(frame) + yb + 2 * cbb;
+        return CoefExtents{e, e + yeb, e + yeb + ceb, each};
+    }
 };
+
+// A frame's coefficient records as dense zig-zag arrays, in place (host memory): the sectors past each
+// block's record become zeros.
+static void expand_records(const CoefLayout &L, const FrameGeometry &g, void *frame)
+{
+    const CoefExtents e = L.extents(frame);
+    int16_t *arr[3] = {L.y(frame), L.cb(frame), L.cr(frame)};
+    const uint8_t *ext[3] = {e.y, e.cb, e.cr};
+    const size_t nb[3] = {g.ny, g.nc, g.nc};
+    for (int c = 0; c < (g.has_chroma ? 3 : 1); ++c)
+        for (size_t b = 0; b < nb[c]; ++b) {
+            const int sectors = ext[c][b];   // 1..4 sectors of 16 coefficients
+            memset(arr[c] + b * 64 + sectors * 16, 0, (size_t)(4 - sectors) * 32);
+        }
+}
 
 void pixo_b200_quant_tables(int quality, uint8_t lum_zz[64], uint8_t chr_zz[64], float lum[64],
                             float chr[64])
@@ -519,7 +540,7 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
         const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, y_stride, d_cb, d_cr, c_stride, n_images, g.ny,
                                        g.nc, g.y_per_mcu, 0, (flags & PIXO_B200_COEF_ZIGZAG) != 0,
-                                       d_hist));
+                                       nullptr, d_hist));
     }
     return 0;
 }
@@ -554,7 +575,7 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     if (hist) {
         PIXO_TRY(ensure_dev(ctx, ctx->d_out, kHistWords * sizeof(uint64_t)));
         PIXO_TRY(launch_jpeg_histogram(ctx, dy, g.ny * 64, dcb, dcr, g.nc * 64, 1, g.ny, g.nc,
-                                       g.y_per_mcu, 0, (flags & PIXO_B200_COEF_ZIGZAG) != 0,
+                                       g.y_per_mcu, 0, (flags & PIXO_B200_COEF_ZIGZAG) != 0, nullptr,
                                        reinterpret_cast<uint64_t *>(ctx->d_out.ptr)));
         PIXO_CUDA(ctx, cudaMemcpyAsync(hist, ctx->d_out.ptr, kHistWords * sizeof(uint64_t),
                                        cudaMemcpyDeviceToHost, ctx->stream));
@@ -618,10 +639,11 @@ static const char kOutOfRange[] = "coefficient out of the baseline range (|AC| <
 // longer fit out_cap.  Three passes at most.  Returns 0 with the scan at the start of d_retry and
 // its length in *len, kGaveUp, or an error.  It touches no other scratch of the context but
 // d_raw (segmented passes), so encode_frames can use it while the next group's work is queued.
-// check: the arrays are the caller's (launch_jpeg_entropy); the transform's are always in range.
+// ext: the transform's coefficient records (always in range); null: the caller's arrays, checked
+// (launch_jpeg_entropy).
 static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
-                       const FrameGeometry &g, const HuffTables &t, uint32_t restart_interval, bool segments,
-                       bool check, size_t cap, size_t hdr, size_t out_cap, size_t *len)
+                       const CoefExtents *ext, const FrameGeometry &g, const HuffTables &t, uint32_t restart_interval,
+                       bool segments, size_t cap, size_t hdr, size_t out_cap, size_t *len)
 {
     const size_t ent = entropy_scratch_bytes(1, g, restart_interval);
     for (int pass = 0;; ++pass) {
@@ -630,7 +652,7 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
         auto *buf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
         uint64_t *d_len = nullptr;
         uint32_t *d_ovf = nullptr;
-        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments, check,
+        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments, ext,
                                      buf + scan_bytes, buf, cap, &d_len, &d_ovf));
         uint64_t n = 0;
         uint32_t ovf = 0;
@@ -736,17 +758,18 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
         const int slot = (int)(gi & 1);
         uint8_t *c = coef_of(slot);
+        const CoefExtents ec = L.extents(c);
         PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_in[slot], 0));
         PIXO_TRY(launch_jpeg_transform(ctx, d_in + (size_t)slot * G * in_stride, in_stride, cnt, g.width,
                                        g.height, g.color_type, g.subsampling, lum, chr, L.y(c), cs,
-                                       g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr, cs, 0));
+                                       g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr, cs, 0, &ec));
         PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
         std::vector<HuffTables> &tb = tables[slot];
         tb.resize(optimize ? cnt : 1);
         if (optimize) {
             auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g.ny, g.nc, g.y_per_mcu,
-                                           restart_interval, false, d_hist));
+                                           restart_interval, false, &ec, d_hist));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t),
                                            cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the table build needs the statistics
@@ -763,14 +786,15 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         uint32_t *h_ovf = h_ovf_of(slot);
         if (!optimize) {
             PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g, tb[0], restart_interval, true,
-                                         false, ent, scan, scan_cap, &d_len, &d_ovf));
+                                         &ec, ent, scan, scan_cap, &d_len, &d_ovf));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, d_len, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
         } else {
             for (uint32_t k = 0; k < cnt; ++k) {  // per-image tables: one pass per image, each in its own scratch
                 uint8_t *f = c + (size_t)k * L.each;
+                const CoefExtents ef = L.extents(f);
                 PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, 1, g, tb[k], restart_interval, true,
-                                             false, ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
+                                             &ef, ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
                                              &d_ovf));
                 PIXO_CUDA(ctx, cudaMemcpyAsync(h_len + k, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
                 PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf + k, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -823,7 +847,8 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             if (!(h_ovf[k] & 2u) && ctx->gpu_retry) {
                 const size_t need = (h_ovf[k] & 4u) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
                 if (!(h_ovf[k] & 4u)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
-                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), g, t, restart_interval, false, false, align_up(need + 64, 256),
+                const CoefExtents ef = L.extents(f);
+                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), &ef, g, t, restart_interval, false, align_up(need + 64, 256),
                                  hdr[k], out_cap_each, &body);
                 if (rc != 0 && rc != kGaveUp) return rc;
             }
@@ -833,13 +858,14 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
                 PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
                 continue;
             }
-            // last resort: the host entropy coder on the GPU's coefficient arrays
+            // last resort: the host entropy coder on the GPU's coefficient records, made dense
             ctx->host_fallbacks += 1;
             PIXO_TRY(ensure_pinned(ctx, ctx->h_out, L.each));
             auto *hc = reinterpret_cast<uint8_t *>(ctx->h_out.ptr);
             PIXO_CUDA(ctx, cudaMemcpyAsync(hc, f, L.each, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            body = entropy_encode_scan(L.y(hc), L.cb(hc), L.cr(hc), g, t, restart_interval, false, o + hdr[k],
+            expand_records(L, g, hc);
+            body = entropy_encode_scan(L.y(hc), L.cb(hc), L.cr(hc), g, t, restart_interval, true, o + hdr[k],
                                        out_cap_each - hdr[k] - 2, ctx->host_threads);
             PIXO_TRY(finish_frame(ctx, o, out_cap_each, hdr[k], body, &out_lens[img]));
         }
@@ -920,14 +946,15 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     PIXO_TRY(ensure_dev(ctx, ctx->d_coef, (size_t)n_images * L.each));
     PIXO_TRY(ensure_dev(ctx, ctx->d_ent, entropy_scratch_bytes(n_images, g, 0)));
     void *c = ctx->d_coef.ptr;
+    const CoefExtents ec = L.extents(c);
     PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
                                    lum, chr, L.y(c), L.stride(), g.has_chroma ? L.cb(c) : nullptr,
-                                   g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0));
+                                   g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0, &ec));
     HuffTables t;
     huff_standard(t);
     uint64_t *len_src = nullptr;
     uint32_t *ovf_src = nullptr;
-    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true, false,
+    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true, &ec,
                                  reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan, scan_cap_each,
                                  &len_src, &ovf_src));
     PIXO_CUDA(ctx, cudaMemcpyAsync(d_scan_len, len_src, (size_t)n_images * 8, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -999,7 +1026,7 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
         auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
         h_hist = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                       false, d_hist));
+                                       false, nullptr, d_hist));
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, kHistWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
@@ -1012,7 +1039,7 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     const size_t raw = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t scan_cap = std::min<size_t>((out_cap - hdr - 2) & ~(size_t)15, (size_t)default_scan_cap(ctx, raw));
     size_t body = 0;
-    const int rc = recode_scan(ctx, d_y, d_cb, d_cr, g, t, restart_interval, true, true, scan_cap, hdr, out_cap, &body);
+    const int rc = recode_scan(ctx, d_y, d_cb, d_cr, nullptr, g, t, restart_interval, true, scan_cap, hdr, out_cap, &body);
     if (rc == kGaveUp) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish");
     PIXO_TRY(rc);
     PIXO_TRY(finish_frame(ctx, out, out_cap, hdr, body, out_len));
@@ -1048,7 +1075,8 @@ int pixo_b200_jpeg_band_histogram_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    return launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, 0, false, d_hist, dc_seed);
+    return launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, 0, false, nullptr, d_hist,
+                                 dc_seed);
 }
 
 int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,

@@ -31,6 +31,18 @@ __host__ __device__ constexpr int zz_nat(int i)
     return t[i];
 }
 
+// Coefficient records, the format the transform hands the encode paths' K3 and k_huff: a block's 64
+// coefficients in zig-zag order in its 128-byte slot, of which only the 32-byte sectors up to the one
+// holding the last non-zero coefficient are written (sector 0, with the DC that the next block predicts
+// from, always), plus one byte per block in an extent array: the number of sectors written, 1..4.
+// Bytes past the last written sector are undefined; a reader loads the record's 2 * sectors 16-byte
+// pieces and takes the rest as zeros.  Extent arrays of the Y, Cb and Cr coefficient arrays, `stride`
+// bytes between images:
+struct CoefExtents {
+    uint8_t *y, *cb, *cr;
+    size_t stride;
+};
+
 struct Scratch {
     void *ptr = nullptr;
     size_t cap = 0;
@@ -123,15 +135,17 @@ int ensure_pinned(pixo_b200_ctx *ctx, Scratch &s, size_t bytes);
     } while (0)
 
 // ---- launchers implemented in the .cu files ----
+// ext: write coefficient records and their extents (flags is then ignored)
 int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
                           uint32_t n_images, uint32_t w, uint32_t h, uint32_t color_type,
                           uint32_t subsampling, const float *lum_q, const float *chr_q,
                           int16_t *d_y, size_t y_stride, int16_t *d_cb, int16_t *d_cr,
-                          size_t c_stride, uint32_t flags);
+                          size_t c_stride, uint32_t flags, const CoefExtents *ext = nullptr);
+// ext: the arrays are coefficient records (zigzag_in is then ignored)
 int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                           const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
                           uint32_t n_images, size_t ny, size_t nc, uint32_t blocks_y_per_mcu,
-                          uint32_t restart_interval, bool zigzag_in, uint64_t *d_hist,
+                          uint32_t restart_interval, bool zigzag_in, const CoefExtents *ext, uint64_t *d_hist,
                           const int *dc_seed = nullptr);
 int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
                            uint32_t width, uint32_t height, size_t row_bytes, uint32_t bpp, uint32_t strategy,
@@ -142,11 +156,13 @@ int launch_adler32(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32
 struct FrameGeometry;
 struct HuffTables;
 size_t entropy_scratch_bytes(uint32_t n, const FrameGeometry &g, uint32_t restart_interval);
+// ext: the arrays are the transform's coefficient records; null: the caller's dense natural-order
+// arrays, whose coefficients are checked against the baseline range
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, bool check,
-                        uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len,
-                        uint32_t **d_overflow);
+                        const HuffTables &t, uint32_t restart_interval, bool allow_segments,
+                        const CoefExtents *ext, uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap,
+                        uint64_t **d_out_len, uint32_t **d_overflow);
 int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                         const FrameGeometry &g, const HuffTables &t, const int dc_seed[3], const int *d_dc_seed,
                         bool allow_segments, uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail,

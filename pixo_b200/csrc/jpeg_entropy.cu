@@ -12,9 +12,13 @@
 // independent of the others; only its POSITION in the stream is not.  The kernel is persistent
 // and every warp works alone (warp-level synchronisation only): it draws a chunk of 32
 // consecutive blocks (scan order) of one image from a ticket counter, then
-//   1. each lane codes its block once into a private shared-memory slot (the zig-zag reorder
-//      happens in registers on the way in; a 64-bit non-zero mask drives the symbol loop, so the loop runs once per
-//      non-zero coefficient and there is a single, small copy of the symbol code);
+//   1. each lane codes its block once into a private shared-memory slot; a 64-bit non-zero mask
+//      drives the symbol loop, so the loop runs once per non-zero coefficient and there is a single,
+//      small copy of the symbol code.  The encode paths hand over the transform's coefficient records
+//      (CoefExtents, common.cuh): the lane loads the block's extent, then only the 32-byte sectors
+//      the transform wrote, already in zig-zag order.  Caller arrays (the CHECK instantiations) are
+//      dense and in natural order: the zig-zag reorder happens in registers on the way in.  Either
+//      way the mask is computed from the words;
 //   2. the block bit lengths are scanned in the warp; the chunk total enters a decoupled
 //      look-back chain (one status word per chunk: bit count + the chunk's last 7 bits), which
 //      yields the chunk's bit offset in the image's stream and the partial byte it inherits;
@@ -48,8 +52,10 @@ struct HuffDev {
 };
 
 struct EntParams {
-    const int16_t *y, *cb, *cr;    // blocks in natural order, as compute_all_coefficients returns them
+    const int16_t *y, *cb, *cr;    // CHECK: blocks in natural order, as compute_all_coefficients returns them;
+                                   // else the transform's coefficient records, with their extents in e
     size_t y_stride, c_stride;     // int16 elements between images
+    CoefExtents e;
     uint32_t bpm;                  // blocks per MCU in scan order: 6 (4:2:0), 3 (4:4:4), 1 (gray)
     uint32_t y_per_mcu;            // 4, 1, 1
     uint32_t nblocks;              // per image, scan order
@@ -395,11 +401,14 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         uint32_t s0, iend, interval = 0;
         uint32_t nblk = P.nblocks;
         size_t y_off = (size_t)C.img * P.y_stride, c_off = (size_t)C.img * P.c_stride;
+        size_t ey_off = (size_t)C.img * P.e.stride, ec_off = ey_off;   // the same blocks' extents
         bool seg_prev = false;     // block 0 continues the previous segment's DC chain
         if (RAW && P.seg_per_img > 1) {
             const uint32_t ii = C.img / P.seg_per_img, seg = C.img - ii * P.seg_per_img;
             y_off = (size_t)ii * P.y_stride + (size_t)seg * P.seg_y_stride;
             c_off = (size_t)ii * P.c_stride + (size_t)seg * P.seg_c_stride;
+            ey_off = (size_t)ii * P.e.stride + (size_t)seg * (P.seg_y_stride / 64);
+            ec_off = (size_t)ii * P.e.stride + (size_t)seg * (P.seg_c_stride / 64);
             if (seg == P.seg_per_img - 1) nblk = P.nblocks_last;
             seg_prev = seg != 0;
         }
@@ -430,21 +439,22 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             const uint32_t m = s / P.bpm;
             const uint32_t k = s - m * P.bpm;
             const int16_t *arr;
-            size_t idx;
+            const uint8_t *earr;   // !CHECK: the array's extents (P.e is null otherwise)
+            size_t idx, eidx;
             int seed;
-            if (k < P.y_per_mcu) { arr = P.y + y_off; idx = (size_t)m * P.y_per_mcu + k; tbl = 0; seed = P.dc_seed[0]; }
-            else if (k == P.y_per_mcu) { arr = P.cb + c_off; idx = m; tbl = 1; seed = P.dc_seed[1]; }
-            else { arr = P.cr + c_off; idx = m; tbl = 1; seed = P.dc_seed[2]; }
+            if (k < P.y_per_mcu) { arr = P.y + y_off; earr = P.e.y; idx = (size_t)m * P.y_per_mcu + k; eidx = ey_off + idx; tbl = 0; seed = P.dc_seed[0]; }
+            else if (k == P.y_per_mcu) { arr = P.cb + c_off; earr = P.e.cb; idx = m; eidx = ec_off + idx; tbl = 1; seed = P.dc_seed[1]; }
+            else { arr = P.cr + c_off; earr = P.e.cr; idx = m; eidx = ec_off + idx; tbl = 1; seed = P.dc_seed[2]; }
             // DC predictors restart with the interval (src/jpeg/mod.rs:1433-1443)
             const bool dc_reset = P.rst_mcus && m % P.rst_mcus == 0 && (k == 0 || k >= P.y_per_mcu);
             // (a later segment's first block follows the previous segment's last one in the same array)
             if (P.dc_seed_dev && idx == 0 && !seg_prev) seed = P.dc_seed_dev[k < P.y_per_mcu ? 0 : (k == P.y_per_mcu ? 1 : 2)];
             const int prev_dc = dc_reset ? 0 : ((idx || seg_prev) ? arr[((long long)idx - 1) * 64] : seed);
             const uint4 *src = reinterpret_cast<const uint4 *>(arr + idx * 64);
-            uint32_t e0 = 0, e1 = 0;
             int dc;
-            {
-                uint32_t n[32];  // the block as K1 wrote it: natural order, two coefficients per word
+            uint32_t w[32];  // the block in zig-zag order: word j = coefficients zz(2j), zz(2j+1)
+            if (CHECK) {
+                uint32_t n[32];  // the caller's block: natural order, two coefficients per word
 #pragma unroll
                 for (int q = 0; q < 8; ++q) {
                     const uint4 v = __ldg(src + q);
@@ -452,8 +462,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                 }
                 dc = (int)(int16_t)(n[0] & 0xFFFF);
                 // zig-zag reorder (zigzag_reorder, src/jpeg/quantize.rs:107-113) on the way into the
-                // stage: word j = coefficients zz(2j), zz(2j+1); all indices are compile-time
-                uint32_t w[32];
+                // stage; all indices are compile-time
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
                     const int i0 = zz_nat(2 * j), i1 = zz_nat(2 * j + 1);
@@ -462,14 +471,36 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                 }
 #pragma unroll
                 for (int j = 0; j < 32; ++j) M.stage[j * CB + lane] = w[j];
+            } else {
+                // the transform's record, already in zig-zag order: its written sectors (sector 0 is
+                // always there, so its load does not wait for the extent), zeros for the rest.  The
+                // symbol loop reads only the stage words of non-zero coefficients, so only the
+                // record's words are staged.
+                const int np = 2 * __ldg(earr + eidx);
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const uint4 v = (q < 2 || q < np) ? __ldg(src + q) : make_uint4(0, 0, 0, 0);
+                    w[q * 4] = v.x; w[q * 4 + 1] = v.y; w[q * 4 + 2] = v.z; w[q * 4 + 3] = v.w;
+                }
+                dc = (int)(int16_t)(w[0] & 0xFFFF);
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    if (q < 2 || q < np) {
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) M.stage[(q * 4 + t) * CB + lane] = w[q * 4 + t];
+                    }
+                }
+            }
+            asm volatile("" ::: "memory");  // the stage is read back through ld.shared below
+            {   // bit i = zig-zag coefficient i != 0
+                uint32_t e0 = 0, e1 = 0;
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     e0 += __vminu2(w[j], 0x00010001u) * (1u << j);       // disjoint bits: + is |
                     e1 += __vminu2(w[16 + j], 0x00010001u) * (1u << j);
                 }
+                M0 = interleave16(e0); M1 = interleave16(e1);
             }
-            asm volatile("" ::: "memory");  // the stage is read back through ld.shared below
-            M0 = interleave16(e0); M1 = interleave16(e1);  // bit i = coefficient i != 0
             diff = (int)(int16_t)(dc - prev_dc);
         }
         if (s < iend) {
@@ -1254,11 +1285,12 @@ static uint64_t mcu_raw_bytes(const FrameGeometry &g) { return (uint64_t)g.y_per
 
 // k_huff<RAW> over the n * S segments of sp (P: the coefficient arrays and DC predictors).  The strings go
 // to raw_area, each segment's bit count and tail after them (off_bits / off_tails: a band's travel with its
-// strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).  check: see
-// code_block.
+// strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).  Arrays
+// without extents are the caller's: checked, see code_block.
 static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint32_t n, const FrameGeometry &g,
-                         const SegPlan &sp, bool check, uint8_t *seg_scratch, uint8_t *raw_area)
+                         const SegPlan &sp, uint8_t *seg_scratch, uint8_t *raw_area)
 {
+    const bool check = P.e.y == nullptr;
     cudaStream_t st = ctx->stream;
     const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     uint8_t *ent = seg_scratch + sp.off_ent;
@@ -1323,17 +1355,18 @@ static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, ui
     return 0;
 }
 
-// Enqueue the entropy stage for n whole images (natural-order coefficient arrays) on ctx->stream.
-// d_scratch: entropy_scratch_bytes.  d_out: n * out_cap bytes of scan data; *d_out_len /
-// *d_overflow point into the scratch.  allow_segments: few long images may be cut into segments.
-// check: the arrays are the caller's, not the transform's - reject coefficients outside the baseline
-// range (overflow bit 3, see code_block).
+// Enqueue the entropy stage for n whole images on ctx->stream.  d_scratch: entropy_scratch_bytes.
+// d_out: n * out_cap bytes of scan data; *d_out_len / *d_overflow point into the scratch.
+// allow_segments: few long images may be cut into segments.  ext: the arrays are the transform's
+// coefficient records; null: they are the caller's natural-order arrays, and coefficients outside the
+// baseline range are rejected (overflow bit 3, see code_block).
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                        const HuffTables &t, uint32_t restart_interval, bool allow_segments, bool check,
-                        uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap, uint64_t **d_out_len,
-                        uint32_t **d_overflow)
+                        const HuffTables &t, uint32_t restart_interval, bool allow_segments,
+                        const CoefExtents *ext, uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap,
+                        uint64_t **d_out_len, uint32_t **d_overflow)
 {
+    const bool check = ext == nullptr;
     const uint64_t nblocks = g.ny + 2 * g.nc;
     const uint64_t bpm_ = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     uint64_t rst_blocks = (uint64_t)restart_interval * bpm_;
@@ -1343,6 +1376,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "entropy stage: too many blocks per call");
     EntParams P;
     P.y = d_y; P.cb = d_cb; P.cr = d_cr; P.y_stride = y_stride; P.c_stride = c_stride;
+    P.e = ext ? *ext : CoefExtents{nullptr, nullptr, nullptr, 0};
     P.bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     P.y_per_mcu = g.y_per_mcu;
     P.nblocks = (uint32_t)nblocks;
@@ -1375,7 +1409,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
         PIXO_TRY(ensure_dev(ctx, ctx->d_raw, sp.total + sp.raw_total));
         auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
         uint8_t *raw_area = seg_scratch + sp.total;
-        PIXO_TRY(code_segments(ctx, P, T, n, g, sp, check, seg_scratch, raw_area));
+        PIXO_TRY(code_segments(ctx, P, T, n, g, sp, seg_scratch, raw_area));
         return splice_segments(ctx, n, sp, seg_scratch, raw_area,
                                reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), 0, 0, true,
                                nullptr, d_out, out_cap, P.out_len, P.overflow);
@@ -1430,7 +1464,7 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     HuffDev T;
     make_huff_dev(t, &T);
     ctx->bands[d_raw] = sp;
-    PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, true, seg_scratch, d_raw));   // a band's arrays are the caller's
+    PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, seg_scratch, d_raw));   // a band's arrays are the caller's (no extents)
     k_band_totals<<<1, 32, 0, ctx->stream>>>(reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
                                              reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
                                              reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,

@@ -284,12 +284,19 @@ __device__ __forceinline__ void dct_rows_x2(f2 (&R)[4][8], f2 (&C)[8][4])
     }
 }
 
+// What the transform writes per block: natural order, zig-zag order (both all 64 coefficients), or
+// a coefficient record (zig-zag order, cut after the sector of the last non-zero coefficient, plus
+// its extent: see CoefExtents in common.cuh).
+enum CoefOut { kNatural, kZigzag, kRecords };
+
 // column pass on column pairs, quantising each pair of columns as soon as it is transformed;
-// tab(i) returns table entry i (one per output word)
-template <bool ZIGZAG, typename TabFn>
+// tab(i) returns table entry i (one per output word).  kRecords: *eout = the block's record extent
+// (32-byte sectors up to the last non-zero one: an OR over each sector's words, a few instructions).
+template <int OUT, typename TabFn>
 __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab, uint4 *__restrict__ out,
-                                                        const int swz)
+                                                        const int swz, uint8_t *eout)
 {
+    constexpr bool ZIGZAG = OUT != kNatural;
     constexpr float SK[8] = {AAN_S0, AAN_S1, AAN_S2, AAN_S3, AAN_S4, AAN_S5, AAN_S6, AAN_S7};
     uint32_t W[32];
     const f2 half2 = K2(0.5f), magic2 = K2(12582912.0f);  // 1.5 * 2^23
@@ -325,47 +332,74 @@ __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab
             W[r * 4 + j] = __byte_perm(tl, th, 0x5410) ^ neg;
         }
     }
+    uint32_t Z[32];   // the output words in the order they are stored
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-        uint32_t w[4];
 #pragma unroll
         for (int m = 0; m < 4; ++m) {
             if (ZIGZAG) {
                 const int i0 = zz_nat(k * 8 + m * 2), i1 = zz_nat(k * 8 + m * 2 + 1);
-                w[m] = __byte_perm(W[i0 >> 1], W[i1 >> 1],
-                                   ((i0 & 1) ? 0x0032 : 0x0010) | ((i1 & 1) ? 0x7600 : 0x5400));
+                Z[k * 4 + m] = __byte_perm(W[i0 >> 1], W[i1 >> 1],
+                                           ((i0 & 1) ? 0x0032 : 0x0010) | ((i1 & 1) ? 0x7600 : 0x5400));
             } else {
-                w[m] = W[k * 4 + m];
+                Z[k * 4 + m] = W[k * 4 + m];
             }
         }
-        out[k ^ swz] = make_uint4(w[0], w[1], w[2], w[3]);
+        out[k ^ swz] = make_uint4(Z[k * 4], Z[k * 4 + 1], Z[k * 4 + 2], Z[k * 4 + 3]);
+    }
+    if (OUT == kRecords) {
+        uint32_t o[4] = {0, 0, 0, 0};   // OR of sector 1..3's words
+#pragma unroll
+        for (int i = 8; i < 32; ++i) o[i >> 3] |= Z[i];
+        *eout = (uint8_t)(o[3] ? 4 : o[2] ? 3 : o[1] ? 2 : 1);
     }
 }
 
 // chroma_u MUST be warp-uniform (the callers derive it from a warp vote, so the branch is one).
-template <bool ZIGZAG>
+template <int OUT>
 __device__ __forceinline__ void dct_quant_store_x2(f2 (&R)[4][8], const QPairTab *qs, const bool chroma_u,
-                                                   uint4 *__restrict__ out, const int swz)
+                                                   uint4 *__restrict__ out, const int swz, uint8_t *eout)
 {
     f2 C[8][4];
     dct_rows_x2(R, C);
     const QPair *t = qs->t[chroma_u ? 1 : 0];
-    dct_cols_quant_store_x2<ZIGZAG>(C, [&](int i) { return t[i]; }, out, swz);
+    dct_cols_quant_store_x2<OUT>(C, [&](int i) { return t[i]; }, out, swz, eout);
 }
 
 // Copy a warp's 32-slot stage (4 KB, swizzled as above) to global memory: instruction j moves
-// slots 4j..4j+3, i.e. 512 contiguous bytes per warp store.
-template <typename SwzFn, typename DstFn>
-__device__ __forceinline__ void flush_stage(const uint4 *__restrict__ stage, int lane, SwzFn swz_of,
-                                            DstFn dst_of)
+// slots 4j..4j+3, i.e. 512 contiguous bytes per warp store.  dst_of(s): slot s's destination, or
+// null when it has none.  kRecords: ext[s] is slot s's record extent in sectors (the warp's 32
+// extents, 4-byte aligned in shared memory); only the sectors of a slot's record are written, and the
+// extents go out as one 32-byte warp store to edst_of(s) (null: none).
+template <int OUT, typename SwzFn, typename DstFn, typename EDstFn>
+__device__ __forceinline__ void flush_stage(const uint4 *__restrict__ stage, const uint8_t *ext, int lane,
+                                            SwzFn swz_of, DstFn dst_of, EDstFn edst_of)
 {
     __syncwarp();
+    uint32_t e[8];   // kRecords: word j holds the extents of slots 4j..4j+3; this lane's is byte lane >> 3
+    if (OUT == kRecords) {
+        const uint4 a = reinterpret_cast<const uint4 *>(ext)[0], b = reinterpret_cast<const uint4 *>(ext)[1];
+        e[0] = a.x; e[1] = a.y; e[2] = a.z; e[3] = a.w; e[4] = b.x; e[5] = b.y; e[6] = b.z; e[7] = b.w;
+    }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int s = j * 4 + (lane >> 3), k = lane & 7;
         const uint4 v = stage[s * 8 + (k ^ swz_of(s))];
         uint4 *d = dst_of(s);
-        if (d) d[k] = v;
+        if (OUT != kRecords) {
+            if (d) d[k] = v;
+        } else {
+            // piece k lies in sector k >> 1.  A predicated store: left to itself, ptxas branches around
+            // the stage read and the address arithmetic of every skipped piece.
+            const uint32_t keep = (d != nullptr) & ((uint32_t)(k >> 1) < __byte_perm(e[j], 0, 0x4440 + (lane >> 3)));
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %5, 0;\n\t"
+                         "@p st.global.v4.u32 [%0], {%1, %2, %3, %4};\n\t}"
+                         :: "l"(d + k), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(keep) : "memory");
+        }
+    }
+    if (OUT == kRecords) {
+        uint8_t *ed = edst_of(lane);
+        if (ed) *ed = ext[lane];
     }
     __syncwarp();
 }
@@ -434,12 +468,14 @@ struct K1Params {
     uint32_t w, h, mcus_x, mcus_y, units_x, n_images;
     int16_t *y, *cb, *cr;
     size_t y_stride, c_stride;
+    CoefExtents e;                   // kRecords only
     uint32_t use_tma;
 };
 
 struct __align__(128) K1WarpSmem {
     uint8_t tile[2][K1_HALF_BYTES];  // pixels of MCUs 0-7 / 8-15; reused as output stage once read
     uint32_t csum[K1_MCUS * 64];     // chroma quad sums; reused as the chroma pass's output stage
+    __align__(16) uint8_t ext[32];   // kRecords: the stage's record extents, by slot
     uint64_t bar;
 };
 
@@ -495,7 +531,7 @@ __device__ __noinline__ void warp_load_tile_rgb(uint8_t *__restrict__ smem,
     load_tile<3, ROWS, TILE_PX, 32>(smem, img, w, h, x0, y0, lane);
 }
 
-template <bool ZIGZAG>
+template <int OUT>
 __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
 k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab qp,
            const __grid_constant__ CUtensorMap tmap)
@@ -655,21 +691,29 @@ k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
             // The transform runs in every lane (edge lanes work on garbage and their slots are never
             // flushed): the quantiser's table reads are uniform-datapath loads, which exist only in
             // warp-convergent code.
-            dct_quant_store_x2<ZIGZAG>(R, QS, chroma_u, stage + slot * 8, swz);
+            dct_quant_store_x2<OUT>(R, QS, chroma_u, stage + slot * 8, swz, &WS.ext[slot]);
             if (!chroma_u) {
-                uint4 *ybase = reinterpret_cast<uint4 *>(P.y + (size_t)img * P.y_stride +
-                                                         (mcu_base + job * 8) * 4 * 64);
+                const size_t b0 = (mcu_base + job * 8) * 4;   // the job's first Y block
+                uint4 *ybase = reinterpret_cast<uint4 *>(P.y + (size_t)img * P.y_stride + b0 * 64);
                 const uint32_t first = job * 8;
-                flush_stage(
-                    stage, lane, [](int s) { return ((s >> 3) << 1) | (s & 1); },
-                    [&](int s) -> uint4 * { return first + (s >> 2) < n_mcu ? ybase + s * 8 : nullptr; });
+                flush_stage<OUT>(
+                    stage, WS.ext, lane, [](int s) { return ((s >> 3) << 1) | (s & 1); },
+                    [&](int s) -> uint4 * { return first + (s >> 2) < n_mcu ? ybase + s * 8 : nullptr; },
+                    [&](int s) -> uint8_t * {   // called for kRecords only: P.e is set
+                        return first + (s >> 2) < n_mcu ? P.e.y + ((size_t)img * P.e.stride + b0 + s) : nullptr;
+                    });
             } else {
                 uint4 *cbb = reinterpret_cast<uint4 *>(P.cb + (size_t)img * P.c_stride + mcu_base * 64);
                 uint4 *crb = reinterpret_cast<uint4 *>(P.cr + (size_t)img * P.c_stride + mcu_base * 64);
-                flush_stage(
-                    stage, lane, [](int s) { return s & 7; },
+                flush_stage<OUT>(
+                    stage, WS.ext, lane, [](int s) { return s & 7; },
                     [&](int s) -> uint4 * {
                         return (uint32_t)(s & 15) < n_mcu ? (s < 16 ? cbb : crb) + (s & 15) * 8 : nullptr;
+                    },
+                    [&](int s) -> uint8_t * {   // kRecords only
+                        return (uint32_t)(s & 15) < n_mcu
+                                   ? (s < 16 ? P.e.cb : P.e.cr) + ((size_t)img * P.e.stride + mcu_base + (s & 15))
+                                   : nullptr;
                     });
             }
         }
@@ -723,6 +767,7 @@ constexpr int K444_MIN_BLOCKS = 2;
 struct __align__(128) K444WarpSmem {
     uint8_t tile[2][K444_TILE_BYTES];
     uint4 stage[256];
+    __align__(16) uint8_t ext[32];   // kRecords: the stage's record extents
     uint64_t bar[2];
 };
 
@@ -732,7 +777,7 @@ struct __align__(128) K444Smem {
 };
 
 // K1Params with mcus_x / mcus_y = blocks per row / block rows, units_x = units per block row
-template <bool ZIGZAG>
+template <int OUT>
 __global__ void __launch_bounds__(K444_THREADS, K444_MIN_BLOCKS)
 k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab qp,
            const __grid_constant__ CUtensorMap tmap)
@@ -806,11 +851,13 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
             const uint2 a = p[0], c1 = p[1], c2 = p[2];
             wds[0] = a.x; wds[1] = a.y; wds[2] = c1.x; wds[3] = c1.y; wds[4] = c2.x; wds[5] = c2.y;
         };
-        auto flush = [&](int16_t *arr) {
-            uint4 *dbase = reinterpret_cast<uint4 *>(arr + ((size_t)by * P.mcus_x + bx0) * 64);
-            flush_stage(
-                WS.stage, lane, [](int s) { return s & 7; },
-                [&](int s) -> uint4 * { return bx0 + s < P.mcus_x ? dbase + s * 8 : nullptr; });
+        const size_t b0 = (size_t)by * P.mcus_x + bx0;   // the unit's first block
+        auto flush = [&](int16_t *arr, uint8_t *earr) {   // earr: the extents (kRecords only)
+            uint4 *dbase = reinterpret_cast<uint4 *>(arr + b0 * 64);
+            flush_stage<OUT>(
+                WS.stage, WS.ext, lane, [](int s) { return s & 7; },
+                [&](int s) -> uint4 * { return bx0 + s < P.mcus_x ? dbase + s * 8 : nullptr; },
+                [&](int s) -> uint8_t * { return bx0 + s < P.mcus_x ? earr + s : nullptr; });
         };
 #pragma unroll 1
         for (int comp = 0; comp < 3; ++comp) {
@@ -839,23 +886,27 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
                     for (int x = 0; x < 8; ++x) R[rp][x] = pk(v0[x], v1[x]);
                 }
             }
-            dct_quant_store_x2<ZIGZAG>(R, QS, chroma_u, WS.stage + lane * 8, lane & 7);
-            flush(comp == 0 ? P.y + (size_t)img * P.y_stride : (comp == 1 ? P.cb : P.cr) + (size_t)img * P.c_stride);
+            dct_quant_store_x2<OUT>(R, QS, chroma_u, WS.stage + lane * 8, lane & 7, &WS.ext[lane]);
+            uint8_t *earr = nullptr;
+            if (OUT == kRecords)
+                earr = (comp == 0 ? P.e.y : (comp == 1 ? P.e.cb : P.e.cr)) + ((size_t)img * P.e.stride + b0);
+            flush(comp == 0 ? P.y + (size_t)img * P.y_stride : (comp == 1 ? P.cb : P.cr) + (size_t)img * P.c_stride, earr);
         }
         __syncwarp();  // every lane is done with tile[b]: the TMA issued next iteration may refill it
         img = img_n; by = by_n; ux = ux_n;
     }
 }
 
-template <bool ZIGZAG>
+template <int OUT>
 __global__ void __launch_bounds__(64)
 k_jpeg_gray(const uint8_t *__restrict__ pixels, size_t pixel_stride, uint32_t w, uint32_t h,
             uint32_t blocks_x, uint32_t tiles_x, int16_t *__restrict__ yout, size_t y_stride,
-            const __grid_constant__ QPairTab qp)
+            uint8_t *__restrict__ yext, size_t e_stride, const __grid_constant__ QPairTab qp)
 {
     constexpr int TB = GRAY_BLOCKS * 8;  // 512
     __shared__ __align__(16) uint8_t tile[8 * TB];
     __shared__ __align__(16) uint4 stage[2][256];
+    __shared__ __align__(16) uint8_t ext[2][32];   // kRecords: the stages' record extents
     __shared__ QPairTab qsm;
     for (int i = threadIdx.x; i < 64; i += 64) qsm.t[i >> 5][i & 31] = qp.t[i >> 5][i & 31];
     const QPairTab *QS = &qsm;
@@ -883,13 +934,17 @@ k_jpeg_gray(const uint8_t *__restrict__ pixels, size_t pixel_stride, uint32_t w,
                 R[rp][x] = sub2(pk(f0, f1), K2(8388736.0f));
             }
         }
-        dct_quant_store_x2<ZIGZAG>(R, QS, false, stage[warp] + lane * 8, lane & 7);
+        dct_quant_store_x2<OUT>(R, QS, false, stage[warp] + lane * 8, lane & 7, &ext[warp][lane]);
     }
     const uint32_t first = b0 + warp * 32;
-    uint4 *dbase = reinterpret_cast<uint4 *>(yout + (size_t)img * y_stride + ((size_t)brow * blocks_x + first) * 64);
-    flush_stage(
-        stage[warp], lane, [](int s) { return s & 7; },
-        [&](int s) -> uint4 * { return first + s < blocks_x ? dbase + s * 8 : nullptr; });
+    const size_t bfirst = (size_t)brow * blocks_x + first;
+    uint4 *dbase = reinterpret_cast<uint4 *>(yout + (size_t)img * y_stride + bfirst * 64);
+    flush_stage<OUT>(
+        stage[warp], ext[warp], lane, [](int s) { return s & 7; },
+        [&](int s) -> uint4 * { return first + s < blocks_x ? dbase + s * 8 : nullptr; },
+        [&](int s) -> uint8_t * {   // kRecords only
+            return first + s < blocks_x ? yext + ((size_t)img * e_stride + bfirst + s) : nullptr;
+        });
 }
 
 // =========================================================================================
@@ -905,10 +960,11 @@ __device__ __forceinline__ int category16(int v)
     return 32 - __clz(a);  // 0 for 0
 }
 
-template <bool ZIGZAG_IN>
+// IN: the arrays' CoefOut format; kRecords reads the extents in E.
+template <int IN>
 __global__ void __launch_bounds__(256)
 k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *__restrict__ cbcoef,
-            const int16_t *__restrict__ crcoef, size_t c_stride, size_t ny, size_t nc,
+            const int16_t *__restrict__ crcoef, size_t c_stride, const CoefExtents E, size_t ny, size_t nc,
             uint32_t blocks_y_per_mcu, uint32_t restart_interval,
             unsigned long long *__restrict__ hist, const int seed_y, const int seed_cb, const int seed_cr)
 {
@@ -920,18 +976,21 @@ k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *_
     for (size_t b = (size_t)blockIdx.x * blockDim.x + threadIdx.x; b < total;
          b += (size_t)gridDim.x * blockDim.x) {
         const int16_t *arr;
+        const uint8_t *earr;
         size_t idx;
         bool lum;
         uint32_t per_mcu;
         int seed;  // predictor before block 0: non-zero only for a band of a tiled frame
-        if (b < ny) { arr = ycoef + (size_t)img * y_stride; idx = b; lum = true; per_mcu = blocks_y_per_mcu; seed = seed_y; }
-        else if (b < ny + nc) { arr = cbcoef + (size_t)img * c_stride; idx = b - ny; lum = false; per_mcu = 1; seed = seed_cb; }
-        else { arr = crcoef + (size_t)img * c_stride; idx = b - ny - nc; lum = false; per_mcu = 1; seed = seed_cr; }
+        if (b < ny) { arr = ycoef + (size_t)img * y_stride; earr = E.y; idx = b; lum = true; per_mcu = blocks_y_per_mcu; seed = seed_y; }
+        else if (b < ny + nc) { arr = cbcoef + (size_t)img * c_stride; earr = E.cb; idx = b - ny; lum = false; per_mcu = 1; seed = seed_cb; }
+        else { arr = crcoef + (size_t)img * c_stride; earr = E.cr; idx = b - ny - nc; lum = false; per_mcu = 1; seed = seed_cr; }
         const uint4 *src = reinterpret_cast<const uint4 *>(arr + idx * 64);
+        // a record's pieces past its last written sector are undefined: zeros instead
+        const int np = IN == kRecords ? 2 * __ldg(earr + ((size_t)img * E.stride + idx)) : 8;
         uint32_t wv[32];
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-            const uint4 t = __ldg(src + k);
+            const uint4 t = k < np ? __ldg(src + k) : make_uint4(0, 0, 0, 0);
             wv[k * 4] = t.x; wv[k * 4 + 1] = t.y; wv[k * 4 + 2] = t.z; wv[k * 4 + 3] = t.w;
         }
         // DC difference against the previous block of this component
@@ -949,7 +1008,7 @@ k_jpeg_hist(const int16_t *__restrict__ ycoef, size_t y_stride, const int16_t *_
         int run = 0;
 #pragma unroll
         for (int i = 1; i < 64; ++i) {
-            const int nat = ZIGZAG_IN ? i : zz_nat(i);
+            const int nat = IN != kNatural ? i : zz_nat(i);
             const uint32_t word = wv[nat >> 1];
             const int c = (int)(int16_t)((nat & 1) ? (word >> 16) : (word & 0xFFFF));
             if (c == 0) {
@@ -1032,10 +1091,10 @@ bool make_rgb_tensor_map(CUtensorMap *tm, const uint8_t *pixels, size_t pixel_st
 
 // k_jpeg_420, or k_jpeg_444 when `s444`: persistent kernels with one unit per warp in flight, so the
 // grid is as many CTAs as fit on the device (the occupancy query, asked once per device, kernel and
-// zigzag flag) and no more than the units need.  Only enqueues: the caller counts the launch.
-int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, bool zigzag, const uint8_t *px, size_t pixel_stride,
+// output format) and no more than the units need.  Only enqueues: the caller counts the launch.
+int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, int out, const uint8_t *px, size_t pixel_stride,
                          uint32_t n, uint32_t w, uint32_t h, int16_t *y, size_t y_stride, int16_t *cb,
-                         int16_t *cr, size_t c_stride, const QPairTab &qt)
+                         int16_t *cr, size_t c_stride, const CoefExtents &e, const QPairTab &qt)
 {
     // 4:2:0 walks MCUs of 16x16 px, 16 to a unit; 4:4:4 walks 8x8 blocks, 32 to a unit
     const uint32_t px_per = s444 ? 8 : 16, per_unit = s444 ? 32 : K1_MCUS;
@@ -1043,16 +1102,20 @@ int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, bool zigzag, const uint8
     P.pixels = px; P.pixel_stride = pixel_stride; P.w = w; P.h = h;
     P.mcus_x = (w + px_per - 1) / px_per; P.mcus_y = (h + px_per - 1) / px_per;
     P.units_x = (P.mcus_x + per_unit - 1) / per_unit;
-    P.n_images = n; P.y = y; P.cb = cb; P.cr = cr; P.y_stride = y_stride; P.c_stride = c_stride;
+    P.n_images = n; P.y = y; P.cb = cb; P.cr = cr; P.y_stride = y_stride; P.c_stride = c_stride; P.e = e;
     alignas(64) CUtensorMap tm;
     memset(&tm, 0, sizeof tm);
     // one TMA box: half a 4:2:0 unit (8 MCUs) or a whole 4:4:4 unit, px_per rows
     P.use_tma = make_rgb_tensor_map(&tm, px, pixel_stride, n, w, h, (s444 ? K444_ROW_B : K1_HB) / 8, px_per) ? 1u : 0u;
     const int warps = s444 ? K444_WARPS : K1_WARPS;
     const size_t smem = s444 ? sizeof(K444Smem) : sizeof(K1Smem);
-    auto kern = !s444 ? (zigzag ? k_jpeg_420<true> : k_jpeg_420<false>) : (zigzag ? k_jpeg_444<true> : k_jpeg_444<false>);
-    static int blocks_per_sm[64][2][2];  // [device][s444][zigzag]: function attributes are per device
-    int &bps = blocks_per_sm[ctx->device & 63][s444][zigzag];
+    void (*const k420[3])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_420<kNatural>, k_jpeg_420<kZigzag>,
+                                                               k_jpeg_420<kRecords>};
+    void (*const k444[3])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_444<kNatural>, k_jpeg_444<kZigzag>,
+                                                               k_jpeg_444<kRecords>};
+    auto kern = s444 ? k444[out] : k420[out];
+    static int blocks_per_sm[64][2][3];  // [device][s444][out]: function attributes are per device
+    int &bps = blocks_per_sm[ctx->device & 63][s444][out];
     if (!bps) {
         PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int nb = 0;
@@ -1065,17 +1128,25 @@ int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, bool zigzag, const uint8
     return 0;
 }
 
+// The extents of the frames from image i0 on (none: dense arrays)
+CoefExtents extents_from(const CoefExtents *e, size_t i0)
+{
+    if (!e) return CoefExtents{nullptr, nullptr, nullptr, 0};
+    const size_t o = i0 * e->stride;
+    return CoefExtents{e->y + o, e->cb ? e->cb + o : nullptr, e->cr ? e->cr + o : nullptr, e->stride};
+}
+
 }  // namespace
 
 int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
                           uint32_t n_images, uint32_t w, uint32_t h, uint32_t color_type,
                           uint32_t subsampling, const float *lum_q, const float *chr_q,
                           int16_t *d_y, size_t y_stride, int16_t *d_cb, int16_t *d_cr,
-                          size_t c_stride, uint32_t flags)
+                          size_t c_stride, uint32_t flags, const CoefExtents *ext)
 {
     QPairTab qt;
     fill_qpair_tab(lum_q, chr_q, (color_type != PIXO_B200_GRAY && subsampling == PIXO_B200_S420) ? 4.0f : 1.0f, &qt);
-    const bool zigzag = (flags & PIXO_B200_COEF_ZIGZAG) != 0;
+    const int out = ext ? kRecords : (flags & PIXO_B200_COEF_ZIGZAG) ? kZigzag : kNatural;
     // the exact-division identity is proved for integer divisors 1..255 only
     for (int i = 0; i < 64; ++i) {
         const float a = lum_q[i], b = chr_q[i];
@@ -1094,15 +1165,18 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
         int16_t *y = d_y + (size_t)i0 * y_stride;
         int16_t *cb = d_cb ? d_cb + (size_t)i0 * c_stride : nullptr;
         int16_t *cr = d_cr ? d_cr + (size_t)i0 * c_stride : nullptr;
+        const CoefExtents e = extents_from(ext, i0);
         if (color_type == PIXO_B200_GRAY) {
             const uint32_t bx = (w + 7) / 8, by = (h + 7) / 8;
             const uint32_t tiles_x = (bx + GRAY_BLOCKS - 1) / GRAY_BLOCKS;
             dim3 grid(tiles_x * by, nb);
-            if (zigzag) k_jpeg_gray<true><<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, qt);
-            else k_jpeg_gray<false><<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, qt);
+            void (*const kg[3])(const uint8_t *, size_t, uint32_t, uint32_t, uint32_t, uint32_t, int16_t *, size_t,
+                                uint8_t *, size_t, QPairTab) = {k_jpeg_gray<kNatural>, k_jpeg_gray<kZigzag>,
+                                                                 k_jpeg_gray<kRecords>};
+            kg[out]<<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, e.y, e.stride, qt);
         } else {
-            PIXO_TRY(launch_rgb_transform(ctx, subsampling == PIXO_B200_S444, zigzag, px, pixel_stride, nb, w, h, y,
-                                          y_stride, cb, cr, c_stride, qt));
+            PIXO_TRY(launch_rgb_transform(ctx, subsampling == PIXO_B200_S444, out, px, pixel_stride, nb, w, h, y,
+                                          y_stride, cb, cr, c_stride, e, qt));
         }
         ctx->launches++;
         PIXO_CUDA(ctx, cudaGetLastError());
@@ -1113,7 +1187,8 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
 int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                           const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
                           uint32_t n_images, size_t ny, size_t nc, uint32_t blocks_y_per_mcu,
-                          uint32_t restart_interval, bool zigzag_in, uint64_t *d_hist, const int *dc_seed)
+                          uint32_t restart_interval, bool zigzag_in, const CoefExtents *ext, uint64_t *d_hist,
+                          const int *dc_seed)
 {
     const int s0 = dc_seed ? dc_seed[0] : 0, s1 = dc_seed ? dc_seed[1] : 0, s2 = dc_seed ? dc_seed[2] : 0;
     PIXO_CUDA(ctx, cudaMemsetAsync(d_hist, 0, (size_t)n_images * kHistWords * sizeof(uint64_t),
@@ -1130,10 +1205,13 @@ int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_strid
         const int16_t *y = d_y + (size_t)i0 * y_stride;
         const int16_t *cb = d_cb ? d_cb + (size_t)i0 * c_stride : nullptr;
         const int16_t *cr = d_cr ? d_cr + (size_t)i0 * c_stride : nullptr;
-        if (zigzag_in)
-            k_jpeg_hist<true><<<grid, 256, 0, ctx->stream>>>(y, y_stride, cb, cr, c_stride, ny, nc, blocks_y_per_mcu, restart_interval, hist, s0, s1, s2);
-        else
-            k_jpeg_hist<false><<<grid, 256, 0, ctx->stream>>>(y, y_stride, cb, cr, c_stride, ny, nc, blocks_y_per_mcu, restart_interval, hist, s0, s1, s2);
+        const CoefExtents e = extents_from(ext, i0);
+        void (*const kh[3])(const int16_t *, size_t, const int16_t *, const int16_t *, size_t, CoefExtents, size_t, size_t,
+                            uint32_t, uint32_t, unsigned long long *, int, int, int) = {
+            k_jpeg_hist<kNatural>, k_jpeg_hist<kZigzag>, k_jpeg_hist<kRecords>};
+        const int in = ext ? kRecords : zigzag_in ? kZigzag : kNatural;
+        kh[in]<<<grid, 256, 0, ctx->stream>>>(y, y_stride, cb, cr, c_stride, e, ny, nc, blocks_y_per_mcu, restart_interval,
+                                              hist, s0, s1, s2);
         ctx->launches++;
         PIXO_CUDA(ctx, cudaGetLastError());
     }
