@@ -324,6 +324,53 @@ int pixo_b200_png_filter_rows_dev(pixo_b200_ctx *ctx, const uint8_t *d_rows, con
 /* Adler-32 of A ++ B from adler32(A), adler32(B) and len(B).  Host-only. */
 uint32_t pixo_b200_adler32_combine(uint32_t adler_a, uint32_t adler_b, uint64_t len_b);
 
+/* Lossless colour-type and palette reduction ahead of the filter: what pixo's balanced and max presets
+ * do in encode_into before DEFLATE (src/png/mod.rs:521-568).  Flags for the strategy word of
+ * pixo_b200_png_reduce_filter* only (pixo_b200_png_filter* keep rejecting them):
+ *   REDUCE_COLOR_TYPE  PngOptions::reduce_color_type  RGB/RGBA -> Gray (1/2/4/8 bits), RGB, GrayAlpha
+ *   REDUCE_PALETTE     PngOptions::reduce_palette     RGB/RGBA with <= 256 colours -> indexed */
+#define PIXO_B200_PNG_REDUCE_COLOR_TYPE 0x200u
+#define PIXO_B200_PNG_REDUCE_PALETTE 0x400u
+
+/* The reduced image (ReducedImage, src/png/mod.rs:673-680): what write_ihdr, PLTE and tRNS need. */
+typedef struct {
+    uint8_t color_type_byte;       /* IHDR colour type: 0 Gray, 2 RGB, 3 indexed, 4 GrayAlpha, 6 RGBA */
+    uint8_t bit_depth;             /* IHDR bit depth: 1, 2, 4 or 8 */
+    uint8_t effective_color_type;  /* PIXO_B200_GRAY..RGBA as maybe_optimize_alpha sees it (indexed: RGB) */
+    uint8_t bytes_per_pixel;       /* of the filter (1 for indexed and sub-byte gray) */
+    uint32_t palette_len;          /* PLTE entries, 0 = no PLTE */
+    uint32_t trns_len;             /* tRNS entries: palette_len when some alpha is below 255, else 0
+                                      (src/png/mod.rs:535-545) */
+    uint32_t reserved;
+    uint64_t row_bytes;            /* bytes of a reduced row; the filtered stream has height*(row_bytes+1) */
+    uint8_t palette[256][4];       /* RGBA, PLTE order (the modified Zeng order) */
+} pixo_b200_png_reduced;
+
+/* Replaces maybe_reduce_color_type -> maybe_optimize_alpha -> filter::apply_filters_with_row_bytes in
+ * encode_into (src/png/mod.rs:521-568): maybe_reduce_color_type :683-836, build_palette :838-900,
+ * optimize_palette_order / mzeng_reindex / apply_most_popular_first :909-1120, all_gray_rgb /
+ * analyze_rgba :1122-1147, reduce_gray_bit_depth / palette_bit_depth / pack_bits_rows
+ * (src/png/bit_depth.rs).  The GPU finds the colours, the gray / opaque properties and the palette
+ * statistics, packs the reduced rows and filters them with the same kernels as pixo_b200_png_filter;
+ * the host orders the <= 256 palette entries.  strategy_and_flags: a filter strategy OR-ed with
+ * PIXO_B200_PNG_OPTIMIZE_ALPHA (applied to the REDUCED rows when their effective colour type is RGBA
+ * or GrayAlpha) and the two REDUCE flags.  Validation as encode_into (src/png/mod.rs:442-467).
+ * out: height*(info->row_bytes+1) bytes (PIXO_B200_ERR_OUTPUT_TOO_SMALL with *out_len = the size
+ * needed otherwise); adler32_out (optional): Adler-32 of the filtered stream. */
+int pixo_b200_png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width,
+                                uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                pixo_b200_png_reduced *info, uint8_t *out, size_t out_cap, size_t *out_len,
+                                uint32_t *adler32_out);
+/* Batch of device-resident frames of one input geometry: frame i at d_data + i*in_stride, its filtered
+ * stream (height*(info[i].row_bytes+1) bytes) at d_out + i*out_stride, out_stride >= height*(width*bpp+1);
+ * d_adler (optional): n_images u32.  Frames of one batch may reduce differently.  Returns once info[] is
+ * valid (the palette ordering is host work between GPU passes); the filter and its Adler-32 are still
+ * asynchronous on the context's stream. */
+int pixo_b200_png_reduce_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
+                                    uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                    uint32_t strategy_and_flags, pixo_b200_png_reduced *info, uint8_t *d_out,
+                                    size_t out_stride, uint32_t *d_adler);
+
 /* Replaces compress::adler32::adler32 — src/compress/adler32.rs:11-47 (dispatch
  * src/simd/mod.rs:72-90).  Host buffer in, checksum out. */
 int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t *out);

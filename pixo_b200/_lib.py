@@ -90,6 +90,10 @@ SYMBOLS = {
                                        C.c_uint32, vp, u32p]),
     "pixo_b200_png_filter_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                            C.c_size_t, C.c_uint32, C.c_uint32, vp, C.c_size_t, vp]),
+    "pixo_b200_png_reduce_filter": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                              vp, vp, C.c_size_t, szp, u32p]),
+    "pixo_b200_png_reduce_filter_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                  C.c_uint32, C.c_uint32, vp, vp, C.c_size_t, vp]),
     "pixo_b200_adler32": (C.c_int, [vp, vp, C.c_size_t, u32p]),
     "pixo_b200_adler32_dev": (C.c_int, [vp, vp, C.c_size_t, vp]),
 }

@@ -327,9 +327,10 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw};
+    Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
+                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
-    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc};
+    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red};
     for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->stage_events) cudaEventDestroy(ev);
@@ -1307,6 +1308,77 @@ int pixo_b200_png_filter_rows_dev(pixo_b200_ctx *ctx, const uint8_t *d_rows, con
     return launch_png_filter_rows(ctx, d_rows, row_bytes * band_rows, 1, width, band_rows, row_bytes, bytes_per_pixel,
                                   strategy, d_out, (row_bytes + 1) * (size_t)band_rows, d_adler, d_row_above,
                                   image_height);
+}
+
+// encode_into's checks (src/png/mod.rs:442-467) plus the strategy word of the reduce entry points
+static int validate_png_reduce(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, uint32_t color_type,
+                               uint32_t strategy_and_flags)
+{
+    if (width == 0 || height == 0)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", width, height);
+    if (width > (1u << 24) || height > (1u << 24))  // src/png/mod.rs:21
+        return set_error(ctx, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Image dimensions %ux%u exceed maximum %u", width, height, 1u << 24);
+    if (color_type > PIXO_B200_RGBA)
+        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED_COLOR, "Unsupported color type: %u", color_type);
+    const uint32_t known = 0xFFu | PIXO_B200_PNG_OPTIMIZE_ALPHA | PIXO_B200_PNG_REDUCE_COLOR_TYPE | PIXO_B200_PNG_REDUCE_PALETTE;
+    if ((strategy_and_flags & ~known) || (strategy_and_flags & 0xFFu) > PIXO_B200_FILTER_BIGRAMS)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "unknown filter strategy or flags %#x", strategy_and_flags);
+    return 0;
+}
+
+int pixo_b200_png_reduce_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
+                                    uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                    uint32_t strategy_and_flags, pixo_b200_png_reduced *info, uint8_t *d_out,
+                                    size_t out_stride, uint32_t *d_adler)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_png_reduce(ctx, width, height, color_type, strategy_and_flags));
+    if (!d_data || !d_out || !info) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const size_t raw = (size_t)width * height * (color_type + 1);
+    if (n_images > 1 && in_stride < raw)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
+    const size_t need = (size_t)height * ((size_t)width * (color_type + 1) + 1);
+    if (n_images > 1 && out_stride < need)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
+    if (n_images == 0) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return png_reduce_filter(ctx, d_data, in_stride, n_images, width, height, color_type, strategy_and_flags, info,
+                             d_out, out_stride, d_adler);
+}
+
+int pixo_b200_png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width,
+                                uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                pixo_b200_png_reduced *info, uint8_t *out, size_t out_cap, size_t *out_len,
+                                uint32_t *adler32_out)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_png_reduce(ctx, width, height, color_type, strategy_and_flags));
+    if (!data || !out || !info || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const size_t in_bytes = (size_t)width * height * (color_type + 1);
+    if (data_len != in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, data_len);
+    const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes + 16));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
+    PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
+    uint32_t *d_adler = reinterpret_cast<uint32_t *>(ctx->d_y.ptr);
+    PIXO_TRY(png_reduce_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
+                               color_type, strategy_and_flags, info, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
+                               out_bytes, d_adler));
+    const size_t got = (size_t)height * (info->row_bytes + 1);
+    *out_len = got;
+    if (got > out_cap) {
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
+    }
+    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, got, cudaMemcpyDeviceToHost, ctx->stream));
+    if (adler32_out)
+        PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
 }
 
 uint32_t pixo_b200_adler32_combine(uint32_t adler_a, uint32_t adler_b, uint64_t len_b)

@@ -3,6 +3,8 @@
   apply_filters / apply_filters_with_row_bytes   src/png/filter.rs:52-206
   FilterStrategy                                 src/png/mod.rs:345-364
   adler32                                        src/compress/adler32.rs:11
+  reduce_and_filter[_dev]                        maybe_reduce_color_type -> maybe_optimize_alpha ->
+                                                 apply_filters_with_row_bytes, src/png/mod.rs:521-568,683-1147
 """
 from __future__ import annotations
 
@@ -30,6 +32,8 @@ class FilterStrategy(enum.IntEnum):
 
 
 OPTIMIZE_ALPHA = 0x100  # PIXO_B200_PNG_OPTIMIZE_ALPHA
+REDUCE_COLOR_TYPE = 0x200  # PIXO_B200_PNG_REDUCE_COLOR_TYPE
+REDUCE_PALETTE = 0x400  # PIXO_B200_PNG_REDUCE_PALETTE
 
 
 @dataclasses.dataclass
@@ -40,6 +44,48 @@ class PngOptions:
     color_type: ColorType = ColorType.Rgba
     filter_strategy: FilterStrategy = FilterStrategy.Adaptive
     optimize_alpha: bool = False   # applied on the fly (Rgba / GrayAlpha), src/png/mod.rs:633-671
+    reduce_color_type: bool = False  # reduce_and_filter* only, src/png/mod.rs:683-836
+    reduce_palette: bool = False     # reduce_and_filter* only, src/png/mod.rs:838-900
+
+    @classmethod
+    def from_preset(cls, width: int, height: int, preset: int) -> "PngOptions":
+        """PngOptions::from_preset (src/png/mod.rs:129-197): 0 fast, 2 max, anything else balanced."""
+        if preset == 0:
+            return cls(width, height, ColorType.Rgba, FilterStrategy.AdaptiveFast, False, False, False)
+        st = FilterStrategy.Bigrams if preset == 2 else FilterStrategy.Adaptive
+        return cls(width, height, ColorType.Rgba, st, True, True, True)
+
+    def strategy_word(self) -> int:
+        """The strategy word of pixo_b200_png_reduce_filter*: strategy | flags."""
+        return (int(self.filter_strategy) | (OPTIMIZE_ALPHA if self.optimize_alpha else 0)
+                | (REDUCE_COLOR_TYPE if self.reduce_color_type else 0) | (REDUCE_PALETTE if self.reduce_palette else 0))
+
+
+class _Reduced(C.Structure):
+    """pixo_b200_png_reduced (include/pixo_b200.h)."""
+    _fields_ = [("color_type_byte", C.c_uint8), ("bit_depth", C.c_uint8), ("effective_color_type", C.c_uint8),
+                ("bytes_per_pixel", C.c_uint8), ("palette_len", C.c_uint32), ("trns_len", C.c_uint32),
+                ("reserved", C.c_uint32), ("row_bytes", C.c_uint64), ("palette", (C.c_uint8 * 4) * 256)]
+
+
+@dataclasses.dataclass
+class ReducedImage:
+    """pixo::png's ReducedImage (src/png/mod.rs:673-680) without the rows: what IHDR, PLTE and tRNS need."""
+    color_type_byte: int
+    bit_depth: int
+    effective_color_type: ColorType
+    bytes_per_pixel: int
+    row_bytes: int
+    palette: np.ndarray | None   # (n, 4) uint8 RGBA in PLTE order
+    trns: bytes | None           # tRNS payload, present iff some alpha is below 255
+
+    @classmethod
+    def _from_c(cls, r: _Reduced) -> "ReducedImage":
+        n = int(r.palette_len)
+        pal = np.ctypeslib.as_array(r.palette).reshape(256, 4)[:n].copy() if n else None
+        trns = pal[:, 3].tobytes() if (n and r.trns_len) else None
+        return cls(int(r.color_type_byte), int(r.bit_depth), ColorType(int(r.effective_color_type)),
+                   int(r.bytes_per_pixel), int(r.row_bytes), pal, trns)
 
 
 def _as_u8(data) -> np.ndarray:
@@ -94,6 +140,36 @@ def apply_filters_rows_dev(d_rows, d_row_above, width, image_height, band_rows, 
     _lib.check(ctx.handle, _lib.load().pixo_b200_png_filter_rows_dev(
         ctx.handle, p(d_rows), p(d_row_above), int(width), int(image_height), int(band_rows), int(row_bytes),
         int(bytes_per_pixel), int(strategy) | (OPTIMIZE_ALPHA if optimize_alpha else 0), p(d_out), p(d_adler)))
+
+
+def reduce_and_filter(data, options: PngOptions, ctx: Context | None = None):
+    """maybe_reduce_color_type -> maybe_optimize_alpha -> apply_filters_with_row_bytes as encode_into runs
+    them (src/png/mod.rs:521-568): (ReducedImage, filtered stream, its Adler-32).  See
+    pixo_b200_png_reduce_filter."""
+    ctx = ctx or default_context()
+    d = _as_u8(data)
+    w, h = int(options.width), int(options.height)
+    out = np.empty(max(h * (w * ColorType(options.color_type).bytes_per_pixel() + 1), 1), np.uint8)
+    info, n, ad = _Reduced(), C.c_size_t(), C.c_uint32()
+    rc = _lib.load().pixo_b200_png_reduce_filter(ctx.handle, d.ctypes.data if d.size else None, d.size, w, h,
+                                                 int(options.color_type), options.strategy_word(), C.byref(info),
+                                                 out.ctypes.data, out.size, C.byref(n), C.byref(ad))
+    _lib.check(ctx.handle, rc)
+    return ReducedImage._from_c(info), out[:n.value], ad.value
+
+
+def reduce_and_filter_dev(d_data, in_stride, n_images, options: PngOptions, d_out, out_stride, d_adler=None,
+                          ctx: Context | None = None):
+    """Device-resident batch (anything with .data_ptr()): see pixo_b200_png_reduce_filter_dev.  Returns the
+    n_images ReducedImage descriptions; the filtered streams and checksums are still being written
+    asynchronously on the context's stream."""
+    ctx = ctx or default_context()
+    infos = (_Reduced * max(int(n_images), 1))()
+    p = lambda t: None if t is None else int(t.data_ptr())
+    _lib.check(ctx.handle, _lib.load().pixo_b200_png_reduce_filter_dev(
+        ctx.handle, p(d_data), int(in_stride), int(n_images), int(options.width), int(options.height),
+        int(options.color_type), options.strategy_word(), infos, p(d_out), int(out_stride), p(d_adler)))
+    return [ReducedImage._from_c(infos[i]) for i in range(int(n_images))]
 
 
 def adler32_combine(adler_a: int, adler_b: int, len_b: int) -> int:

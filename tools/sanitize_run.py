@@ -76,4 +76,22 @@ for st in (FilterStrategy.Adaptive, FilterStrategy.AdaptiveFast, FilterStrategy.
                                d_out, d_ad, ctx=ctx)
     ctx.sync()
     assert np.array_equal(d_out.cpu().numpy(), whole.reshape(hh, ww * bpp + 1)[20:50].reshape(-1)), st
+# PNG colour-type / palette reduction: every branch of the analysis, index, pack and filter kernels
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+from reduce_inputs import make_reduce_input  # noqa: E402
+for kind, ch, n, (ww, hh) in (("pal", 3, 2, (9, 5)), ("pal", 4, 3, (7, 6)), ("pal", 4, 17, (65, 9)),
+                              ("palblk", 4, 256, (300, 40)), ("pal", 3, 257, (300, 40)), ("graypal", 3, 4, (33, 7)),
+                              ("graypal", 4, 200, (33, 7)), ("opaque", 4, 0, (70, 33)), ("grayalpha", 4, 0, (70, 33)),
+                              ("noise", 4, 0, (70, 33)), ("noise", 1, 0, (20, 9)), ("noise", 2, 0, (20, 9))):
+    px = make_reduce_input(kind, ww, hh, ch, 1, n)
+    for rct, rpal in ((True, True), (True, False), (False, True)):
+        for st in (FilterStrategy.Adaptive, FilterStrategy.Bigrams):
+            png.reduce_and_filter(px, PngOptions(ww, hh, ColorType(ch - 1), st, True, rct, rpal), ctx=ctx)
+frames = [make_reduce_input(k, 300, 40, 4, 2, n) for k, n in (("pal", 5), ("opaque", 0), ("pal", 300), ("grayalpha", 0))]
+d_in = torch.from_numpy(np.concatenate(frames)).to(dev)
+d_out = torch.empty(4 * 40 * (300 * 4 + 1), dtype=torch.uint8, device=dev)
+d_ad = torch.zeros(4, dtype=torch.int32, device=dev)
+torch.cuda.synchronize(dev)
+png.reduce_and_filter_dev(d_in, 300 * 40 * 4, 4, PngOptions.from_preset(300, 40, 1), d_out, 40 * (300 * 4 + 1), d_ad, ctx=ctx)
+ctx.sync()
 print("tour done")
