@@ -371,6 +371,44 @@ int pixo_b200_png_reduce_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, s
                                     uint32_t strategy_and_flags, pixo_b200_png_reduced *info, uint8_t *d_out,
                                     size_t out_stride, uint32_t *d_adler);
 
+/* Lossy palette quantisation ahead of the filter: what encode_into does when PngOptions::quantization
+ * selects it (src/png/mod.rs:469-511, QuantizationOptions :70-100).  Flags for the strategy word of
+ * pixo_b200_png_quantize_filter* only (every other entry point keeps rejecting them):
+ *   QUANTIZE_AUTO   QuantizationMode::Auto   quantise RGB/RGBA when should_quantize_auto says so
+ *   QUANTIZE_FORCE  QuantizationMode::Force  quantise every RGB/RGBA image
+ *   DITHER          QuantizationOptions::dithering (Floyd-Steinberg on RGB, alpha kept)
+ * Neither mode flag is QuantizationMode::Off; both together are an error. */
+#define PIXO_B200_PNG_QUANTIZE_AUTO 0x800u
+#define PIXO_B200_PNG_QUANTIZE_FORCE 0x1000u
+#define PIXO_B200_PNG_DITHER 0x2000u
+
+/* Replaces encode_into's choice between quantize_image -> encode_indexed_into (src/png/mod.rs:469-511,
+ * 1505-1701, 1814-1886) and the lossless reduction path (pixo_b200_png_reduce_filter, which frames that do
+ * not quantise take with the same OPTIMIZE_ALPHA / REDUCE_* flags).  A quantised frame is described as
+ * colour type 3, bit depth 8, bytes_per_pixel 1, row_bytes = width, effective colour type RGB; palette in
+ * pixo's order (median-cut box order after k-means, or key order when the image has at most max_colors
+ * histogram colours) and trns_len the length maybe_trim_transparency keeps (0: no tRNS).  Its 8-bit index
+ * rows are filtered with the strategy encode_indexed_into uses (Adaptive, AdaptiveFast, MinSum and Bigrams
+ * become None).  max_colors: QuantizationOptions::max_colors (a u16; above 256 acts as 256, 0 is legal).
+ * palette (optional, RGBA, 1..256 entries): the palette pixo's median_cut_palette produced, mapped exactly
+ * as quantize_image maps one (6-6-6 table, then the plain map or the dither).  Without it, an image whose
+ * histogram samples hold more than 8192 colours returns PIXO_B200_ERR_UNSUPPORTED: pixo keeps the 8192
+ * most frequent with an unstable sort whose tie order decides the palette and is not restated here.
+ * out / out_len / adler32_out as pixo_b200_png_reduce_filter. */
+int pixo_b200_png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width,
+                                  uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                  uint32_t max_colors, const uint8_t *palette, uint32_t palette_len,
+                                  pixo_b200_png_reduced *info, uint8_t *out, size_t out_cap, size_t *out_len,
+                                  uint32_t *adler32_out);
+/* Batch of device-resident frames, as pixo_b200_png_reduce_filter_dev; a batch may mix frames that
+ * quantise with frames that do not.  palettes (optional, HOST memory): n_images x 256 x 4 bytes with
+ * palette_lens[i] entries for frame i, 0 = design it.  Returns once info[] is valid. */
+int pixo_b200_png_quantize_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
+                                      uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                      uint32_t strategy_and_flags, uint32_t max_colors, const uint8_t *palettes,
+                                      const uint32_t *palette_lens, pixo_b200_png_reduced *info, uint8_t *d_out,
+                                      size_t out_stride, uint32_t *d_adler);
+
 /* Replaces compress::adler32::adler32 — src/compress/adler32.rs:11-47 (dispatch
  * src/simd/mod.rs:72-90).  Host buffer in, checksum out. */
 int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t *out);

@@ -94,6 +94,11 @@ SYMBOLS = {
                                               vp, vp, C.c_size_t, szp, u32p]),
     "pixo_b200_png_reduce_filter_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                                   C.c_uint32, C.c_uint32, vp, vp, C.c_size_t, vp]),
+    "pixo_b200_png_quantize_filter": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                C.c_uint32, vp, C.c_uint32, vp, vp, C.c_size_t, szp, u32p]),
+    "pixo_b200_png_quantize_filter_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                    C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_size_t,
+                                                    vp]),
     "pixo_b200_adler32": (C.c_int, [vp, vp, C.c_size_t, u32p]),
     "pixo_b200_adler32_dev": (C.c_int, [vp, vp, C.c_size_t, vp]),
 }

@@ -328,9 +328,9 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
-                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img};
+                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
-    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red};
+    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant};
     for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->stage_events) cudaEventDestroy(ev);
@@ -1368,6 +1368,85 @@ int pixo_b200_png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t 
     PIXO_TRY(png_reduce_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
                                color_type, strategy_and_flags, info, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
                                out_bytes, d_adler));
+    const size_t got = (size_t)height * (info->row_bytes + 1);
+    *out_len = got;
+    if (got > out_cap) {
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
+    }
+    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, got, cudaMemcpyDeviceToHost, ctx->stream));
+    if (adler32_out)
+        PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+// the reduce entry points' checks, the quantisation flags and QuantizationOptions::max_colors (a u16)
+static int validate_png_quantize(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, uint32_t color_type,
+                                 uint32_t strategy_and_flags, uint32_t max_colors)
+{
+    const uint32_t qflags = PIXO_B200_PNG_QUANTIZE_AUTO | PIXO_B200_PNG_QUANTIZE_FORCE | PIXO_B200_PNG_DITHER;
+    PIXO_TRY(validate_png_reduce(ctx, width, height, color_type, strategy_and_flags & ~qflags));
+    if ((strategy_and_flags & PIXO_B200_PNG_QUANTIZE_AUTO) && (strategy_and_flags & PIXO_B200_PNG_QUANTIZE_FORCE))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "QUANTIZE_AUTO and QUANTIZE_FORCE are exclusive");
+    if (max_colors > 65535)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "max_colors %u is not a u16", max_colors);
+    return 0;
+}
+
+int pixo_b200_png_quantize_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
+                                      uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                      uint32_t strategy_and_flags, uint32_t max_colors, const uint8_t *palettes,
+                                      const uint32_t *palette_lens, pixo_b200_png_reduced *info, uint8_t *d_out,
+                                      size_t out_stride, uint32_t *d_adler)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_png_quantize(ctx, width, height, color_type, strategy_and_flags, max_colors));
+    if (!d_data || !d_out || !info) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (palettes && !palette_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "palettes without palette_lens");
+    for (uint32_t i = 0; palettes && i < n_images; ++i)
+        if (palette_lens[i] > 256)
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "palette_lens[%u] = %u not in 0..256", i, palette_lens[i]);
+    const size_t raw = (size_t)width * height * (color_type + 1);
+    if (n_images > 1 && in_stride < raw)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
+    const size_t need = (size_t)height * ((size_t)width * (color_type + 1) + 1);
+    if (n_images > 1 && out_stride < need)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
+    if (n_images == 0) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return png_quantize_filter(ctx, d_data, in_stride, n_images, width, height, color_type, strategy_and_flags,
+                               max_colors, palettes, palettes ? palette_lens : nullptr, info, d_out, out_stride, d_adler);
+}
+
+int pixo_b200_png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width,
+                                  uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                  uint32_t max_colors, const uint8_t *palette, uint32_t palette_len,
+                                  pixo_b200_png_reduced *info, uint8_t *out, size_t out_cap, size_t *out_len,
+                                  uint32_t *adler32_out)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_png_quantize(ctx, width, height, color_type, strategy_and_flags, max_colors));
+    if (!data || !out || !info || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if ((palette == nullptr) != (palette_len == 0) || palette_len > 256)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "a given palette has 1..256 entries (palette_len %u)", palette_len);
+    const size_t in_bytes = (size_t)width * height * (color_type + 1);
+    if (data_len != in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, data_len);
+    uint8_t pal256[1024];
+    if (palette) memcpy(pal256, palette, (size_t)palette_len * 4);
+    const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes + 16));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
+    PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
+    uint32_t *d_adler = reinterpret_cast<uint32_t *>(ctx->d_y.ptr);
+    PIXO_TRY(png_quantize_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
+                                 color_type, strategy_and_flags, max_colors, palette ? pal256 : nullptr,
+                                 palette ? &palette_len : nullptr, info, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
+                                 out_bytes, d_adler));
     const size_t got = (size_t)height * (info->row_bytes + 1);
     *out_len = got;
     if (got > out_cap) {

@@ -107,7 +107,8 @@ struct pixo_b200_ctx {
     // reusable scratch (device + pinned host)
     pixo::Scratch d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
     pixo::Scratch d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
-    pixo::Scratch h_in, h_out, h_misc, h_red;
+    pixo::Scratch d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
+    pixo::Scratch h_in, h_out, h_misc, h_red, h_quant;
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
     pixo::HostPool *pool = nullptr;         // see HostPool
@@ -157,6 +158,12 @@ int launch_adler32(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32
 int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
                       uint32_t width, uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
                       pixo_b200_png_reduced *info, uint8_t *d_out, size_t out_stride, uint32_t *d_adler);
+// pixo_b200_png_quantize_filter_dev after validation (png_quantize.cu); palettes / palette_lens are host
+// memory and may be null
+int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
+                        uint32_t width, uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                        uint32_t max_colors, const uint8_t *palettes, const uint32_t *palette_lens,
+                        pixo_b200_png_reduced *info, uint8_t *d_out, size_t out_stride, uint32_t *d_adler);
 
 struct FrameGeometry;
 struct HuffTables;

@@ -76,4 +76,92 @@ void palette_order(uint32_t n, const uint32_t *counts, const uint32_t *tri, uint
     for (uint32_t k = 0; k < n; ++k) order[k] = (uint8_t)remap[k];
 }
 
+namespace {
+
+struct ColorCount {
+    uint32_t key, count;
+};
+
+uint32_t channel_of(uint32_t key, int ch) { return (key >> (24 - 8 * ch)) & 255u; }
+
+// ColorBox::range: (channel, score) with weights r 2, g 4, b 1, a 3; a later channel wins only when
+// strictly larger
+void box_range(const std::vector<ColorCount> &c, int &channel, uint32_t &score)
+{
+    uint32_t lo[4] = {255, 255, 255, 255}, hi[4] = {0, 0, 0, 0};
+    for (const ColorCount &e : c)
+        for (int ch = 0; ch < 4; ++ch) {
+            lo[ch] = std::min(lo[ch], channel_of(e.key, ch));
+            hi[ch] = std::max(hi[ch], channel_of(e.key, ch));
+        }
+    static const uint32_t weight[4] = {2, 4, 1, 3};
+    channel = 0;
+    score = (hi[0] - lo[0]) * weight[0];
+    for (int ch = 1; ch < 4; ++ch)
+        if ((hi[ch] - lo[ch]) * weight[ch] > score) { score = (hi[ch] - lo[ch]) * weight[ch]; channel = ch; }
+}
+
+}  // namespace
+
+std::vector<uint32_t> median_cut_palette(const std::vector<uint32_t> &keys, const std::vector<uint32_t> &counts,
+                                         uint32_t max_colors)
+{
+    std::vector<std::vector<ColorCount>> boxes(1);
+    std::vector<std::pair<int, uint32_t>> range(1);   // each box's (channel, score)
+    for (size_t i = 0; i < keys.size(); ++i) boxes[0].push_back({keys[i], counts[i]});
+    if (boxes[0].empty()) return {255u};
+    box_range(boxes[0], range[0].first, range[0].second);
+    while (boxes.size() < max_colors) {
+        // max_by_key: the LAST box of the largest score
+        size_t idx = 0;
+        for (size_t b = 1; b < boxes.size(); ++b)
+            if (range[b].second >= range[idx].second) idx = b;
+        if (boxes[idx].size() <= 1) break;
+        std::vector<ColorCount> c = std::move(boxes[idx]);
+        const int ch = range[idx].first;
+        boxes.erase(boxes.begin() + (ptrdiff_t)idx);
+        range.erase(range.begin() + (ptrdiff_t)idx);
+        std::stable_sort(c.begin(), c.end(), [ch](const ColorCount &a, const ColorCount &b) {
+            return channel_of(a.key, ch) < channel_of(b.key, ch);
+        });
+        // u32 arithmetic as pixo's release build does it (wrapping)
+        uint32_t total = 0, acc = 0;
+        for (const ColorCount &e : c) total += e.count;
+        size_t split = 0;
+        for (size_t i = 0; i < c.size(); ++i) {
+            acc += c[i].count;
+            if (acc >= total / 2) { split = i; break; }
+        }
+        split = std::min(split, c.size() - 2);
+        boxes.emplace_back(c.begin(), c.begin() + (ptrdiff_t)split + 1);
+        boxes.emplace_back(c.begin() + (ptrdiff_t)split + 1, c.end());
+        for (size_t b = boxes.size() - 2; b < boxes.size(); ++b) {
+            range.emplace_back();
+            box_range(boxes[b], range.back().first, range.back().second);
+        }
+    }
+    // make_palette_entry: u64 integer mean of each box
+    std::vector<uint32_t> pal;
+    for (const auto &b : boxes) {
+        uint64_t sum[4] = {0, 0, 0, 0}, total = 0;
+        for (const ColorCount &e : b) {
+            for (int ch = 0; ch < 4; ++ch) sum[ch] += (uint64_t)channel_of(e.key, ch) * e.count;
+            total += e.count;
+        }
+        if (!total) { pal.push_back(255u); continue; }
+        uint32_t key = 0;
+        for (int ch = 0; ch < 4; ++ch) key |= (uint32_t)(sum[ch] / total) << (24 - 8 * ch);
+        pal.push_back(key);
+    }
+    return pal;
+}
+
+uint32_t trimmed_trns_len(const uint32_t *alpha, uint32_t n)
+{
+    uint32_t len = 0;
+    for (uint32_t i = 0; i < n; ++i)
+        if (alpha[i] != 255u) len = i + 1;
+    return len;
+}
+
 }  // namespace pixo

@@ -5,6 +5,8 @@
   adler32                                        src/compress/adler32.rs:11
   reduce_and_filter[_dev]                        maybe_reduce_color_type -> maybe_optimize_alpha ->
                                                  apply_filters_with_row_bytes, src/png/mod.rs:521-568,683-1147
+  quantize_and_filter[_dev]                      encode_into's quantisation branch (quantize_image ->
+                                                 encode_indexed_into) or the above, src/png/mod.rs:469-511
 """
 from __future__ import annotations
 
@@ -34,6 +36,16 @@ class FilterStrategy(enum.IntEnum):
 OPTIMIZE_ALPHA = 0x100  # PIXO_B200_PNG_OPTIMIZE_ALPHA
 REDUCE_COLOR_TYPE = 0x200  # PIXO_B200_PNG_REDUCE_COLOR_TYPE
 REDUCE_PALETTE = 0x400  # PIXO_B200_PNG_REDUCE_PALETTE
+QUANTIZE_AUTO = 0x800  # PIXO_B200_PNG_QUANTIZE_AUTO
+QUANTIZE_FORCE = 0x1000  # PIXO_B200_PNG_QUANTIZE_FORCE
+DITHER = 0x2000  # PIXO_B200_PNG_DITHER
+
+
+class QuantizationMode(enum.IntEnum):
+    """pixo::png::QuantizationMode (src/png/mod.rs:70-79)."""
+    Off = 0
+    Auto = 1
+    Force = 2
 
 
 @dataclasses.dataclass
@@ -46,6 +58,10 @@ class PngOptions:
     optimize_alpha: bool = False   # applied on the fly (Rgba / GrayAlpha), src/png/mod.rs:633-671
     reduce_color_type: bool = False  # reduce_and_filter* only, src/png/mod.rs:683-836
     reduce_palette: bool = False     # reduce_and_filter* only, src/png/mod.rs:838-900
+    # QuantizationOptions (src/png/mod.rs:81-100), quantize_and_filter* only
+    quantization_mode: QuantizationMode = QuantizationMode.Off
+    max_colors: int = 256
+    dithering: bool = False
 
     @classmethod
     def from_preset(cls, width: int, height: int, preset: int) -> "PngOptions":
@@ -55,10 +71,25 @@ class PngOptions:
         st = FilterStrategy.Bigrams if preset == 2 else FilterStrategy.Adaptive
         return cls(width, height, ColorType.Rgba, st, True, True, True)
 
+    @classmethod
+    def from_preset_with_lossless(cls, width: int, height: int, preset: int, lossless: bool) -> "PngOptions":
+        """PngOptions::from_preset_with_lossless (src/png/mod.rs:203-213): lossy selects Auto quantisation with
+        dithering and 256 colours, as PngOptionsBuilder::lossy does."""
+        o = cls.from_preset(width, height, preset)
+        if not lossless:
+            o.quantization_mode, o.max_colors, o.dithering = QuantizationMode.Auto, 256, True
+        return o
+
     def strategy_word(self) -> int:
-        """The strategy word of pixo_b200_png_reduce_filter*: strategy | flags."""
-        return (int(self.filter_strategy) | (OPTIMIZE_ALPHA if self.optimize_alpha else 0)
-                | (REDUCE_COLOR_TYPE if self.reduce_color_type else 0) | (REDUCE_PALETTE if self.reduce_palette else 0))
+        """The strategy word of pixo_b200_png_reduce_filter* / quantize_filter*: strategy | flags (the
+        quantisation flags only when quantisation is selected)."""
+        w = (int(self.filter_strategy) | (OPTIMIZE_ALPHA if self.optimize_alpha else 0)
+             | (REDUCE_COLOR_TYPE if self.reduce_color_type else 0) | (REDUCE_PALETTE if self.reduce_palette else 0))
+        if self.quantization_mode == QuantizationMode.Auto:
+            w |= QUANTIZE_AUTO
+        elif self.quantization_mode == QuantizationMode.Force:
+            w |= QUANTIZE_FORCE
+        return w | (DITHER if self.dithering and self.quantization_mode != QuantizationMode.Off else 0)
 
 
 class _Reduced(C.Structure):
@@ -77,13 +108,13 @@ class ReducedImage:
     bytes_per_pixel: int
     row_bytes: int
     palette: np.ndarray | None   # (n, 4) uint8 RGBA in PLTE order
-    trns: bytes | None           # tRNS payload, present iff some alpha is below 255
+    trns: bytes | None           # tRNS payload (a quantised image's is trimmed after its last alpha below 255)
 
     @classmethod
     def _from_c(cls, r: _Reduced) -> "ReducedImage":
         n = int(r.palette_len)
         pal = np.ctypeslib.as_array(r.palette).reshape(256, 4)[:n].copy() if n else None
-        trns = pal[:, 3].tobytes() if (n and r.trns_len) else None
+        trns = pal[:int(r.trns_len), 3].tobytes() if (n and r.trns_len) else None
         return cls(int(r.color_type_byte), int(r.bit_depth), ColorType(int(r.effective_color_type)),
                    int(r.bytes_per_pixel), int(r.row_bytes), pal, trns)
 
@@ -170,6 +201,52 @@ def reduce_and_filter_dev(d_data, in_stride, n_images, options: PngOptions, d_ou
         ctx.handle, p(d_data), int(in_stride), int(n_images), int(options.width), int(options.height),
         int(options.color_type), options.strategy_word(), infos, p(d_out), int(out_stride), p(d_adler)))
     return [ReducedImage._from_c(infos[i]) for i in range(int(n_images))]
+
+
+def quantize_and_filter(data, options: PngOptions, palette=None, ctx: Context | None = None):
+    """What encode_into hands DEFLATE with options.quantization_mode / max_colors / dithering: a quantised
+    image (colour type 3, 8-bit indices) or, when pixo would not quantise, reduce_and_filter's result.
+    palette: optional (n, 4) RGBA median-cut palette to map with (pixo's truncation case).  Returns
+    (ReducedImage, filtered stream, its Adler-32).  See pixo_b200_png_quantize_filter."""
+    ctx = ctx or default_context()
+    d = _as_u8(data)
+    w, h = int(options.width), int(options.height)
+    out = np.empty(max(h * (w * ColorType(options.color_type).bytes_per_pixel() + 1), 1), np.uint8)
+    info, n, ad = _Reduced(), C.c_size_t(), C.c_uint32()
+    pal = None if palette is None else np.ascontiguousarray(palette, np.uint8).reshape(-1, 4)
+    rc = _lib.load().pixo_b200_png_quantize_filter(
+        ctx.handle, d.ctypes.data if d.size else None, d.size, w, h, int(options.color_type), options.strategy_word(),
+        int(options.max_colors), None if pal is None else pal.ctypes.data, 0 if pal is None else len(pal),
+        C.byref(info), out.ctypes.data, out.size, C.byref(n), C.byref(ad))
+    _lib.check(ctx.handle, rc)
+    return ReducedImage._from_c(info), out[:n.value], ad.value
+
+
+def quantize_and_filter_dev(d_data, in_stride, n_images, options: PngOptions, d_out, out_stride, d_adler=None,
+                            palettes=None, ctx: Context | None = None):
+    """Device-resident batch (anything with .data_ptr()): see pixo_b200_png_quantize_filter_dev.  palettes:
+    optional list of n_images entries, each None (design it) or an (n, 4) RGBA palette.  Returns the
+    n_images ReducedImage descriptions; the filtered streams and checksums are still being written
+    asynchronously on the context's stream."""
+    ctx = ctx or default_context()
+    n_images = int(n_images)
+    infos = (_Reduced * max(n_images, 1))()
+    p = lambda t: None if t is None else int(t.data_ptr())
+    pals, lens = None, None
+    if palettes is not None:
+        pals = np.zeros((max(n_images, 1), 256, 4), np.uint8)
+        lens = np.zeros(max(n_images, 1), np.uint32)
+        for i, q in enumerate(palettes):
+            if q is not None:
+                q = np.asarray(q, np.uint8).reshape(-1, 4)
+                pals[i, :len(q)] = q
+                lens[i] = len(q)
+    _lib.check(ctx.handle, _lib.load().pixo_b200_png_quantize_filter_dev(
+        ctx.handle, p(d_data), int(in_stride), n_images, int(options.width), int(options.height),
+        int(options.color_type), options.strategy_word(), int(options.max_colors),
+        None if pals is None else pals.ctypes.data, None if lens is None else lens.ctypes.data, infos, p(d_out),
+        int(out_stride), p(d_adler)))
+    return [ReducedImage._from_c(infos[i]) for i in range(n_images)]
 
 
 def adler32_combine(adler_a: int, adler_b: int, len_b: int) -> int:
