@@ -46,7 +46,7 @@ typedef enum {
     PIXO_B200_ERR_INVALID_RESTART = 6,     /* Error::InvalidRestartInterval */
     PIXO_B200_ERR_INVALID_ARGUMENT = 7,    /* null pointer, unknown enum value ... */
     PIXO_B200_ERR_OUTPUT_TOO_SMALL = 8,    /* caller's output capacity insufficient */
-    PIXO_B200_ERR_UNSUPPORTED = 9,         /* option outside the hot path (progressive, trellis) */
+    PIXO_B200_ERR_UNSUPPORTED = 9,         /* option outside the hot path (progressive) */
     PIXO_B200_ERR_CUDA = 10,               /* CUDA runtime/driver failure (no device, launch) */
     PIXO_B200_ERR_OOM = 11                 /* device or pinned allocation failed */
 } pixo_b200_status;
@@ -63,8 +63,9 @@ enum {
     PIXO_B200_FILTER_BIGRAMS = 8
 };
 
-/* flags for pixo_b200_jpeg_coefficients* */
-#define PIXO_B200_COEF_ZIGZAG 1u /* emit each block in zig-zag order (quantize.rs:107-113) */
+/* flags for pixo_b200_jpeg_coefficients* (ZIGZAG also for pixo_b200_jpeg_trellis_quantize_dev) */
+#define PIXO_B200_COEF_ZIGZAG 1u  /* emit each block in zig-zag order (quantize.rs:107-113) */
+#define PIXO_B200_COEF_TRELLIS 2u /* trellis-quantise: compute_all_coefficients(.., use_trellis = true) */
 
 /* ---- context ---------------------------------------------------------------------------- */
 int pixo_b200_version(void);
@@ -119,11 +120,16 @@ int pixo_b200_jpeg_block_counts(uint32_t width, uint32_t height, uint32_t color_
 /* Replaces compute_all_coefficients — src/jpeg/mod.rs:932-966 (and the per-MCU transform
  * work inlined in encode_scan :1408-1563 and build_optimized_huffman_tables :684-824):
  * extract_block/extract_mcu_420 (:1565-1656) -> color::rgb_to_ycbcr (src/color.rs:60-77) ->
- * dct::dct_2d (src/jpeg/dct.rs:614-700) -> quantize_block (src/jpeg/quantize.rs:99-105).
+ * dct::dct_2d (src/jpeg/dct.rs:614-700) -> quantize_dct (:970): quantize_block
+ * (src/jpeg/quantize.rs:99-105), or with PIXO_B200_COEF_TRELLIS trellis::trellis_quantize
+ * (src/jpeg/trellis.rs:67-208, lambda None) as use_trellis = true selects (pixo's max preset).
  * y: ny*64, cb/cr: nc*64 int16 (cb/cr ignored for Gray), natural order unless
  * PIXO_B200_COEF_ZIGZAG, blocks in the reference's MCU order (4:2:0: Y TL,TR,BL,BR per MCU).
  * hist (optional, may be NULL): 536 u64 = dc_lum[12] dc_chrom[12] ac_lum[256] ac_chrom[256],
- * the count_block statistics of src/jpeg/mod.rs:826-860 with no restart interval. */
+ * the count_block statistics of src/jpeg/mod.rs:826-860 with no restart interval.  hist must be
+ * NULL with PIXO_B200_COEF_TRELLIS (PIXO_B200_ERR_INVALID_ARGUMENT): pixo builds its tables from
+ * plain-rounded coefficients, which a call without the flag returns.  Other flag bits are ignored.
+ * With PIXO_B200_COEF_TRELLIS the _dev variant waits for the device before it returns. */
 int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t width,
                                 uint32_t height, uint32_t color_type, uint32_t subsampling,
                                 const float lum_q[64], const float chr_q[64], int16_t *y,
@@ -138,6 +144,19 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
                                     const float lum_q[64], const float chr_q[64], int16_t *d_y,
                                     size_t y_stride, int16_t *d_cb, int16_t *d_cr,
                                     size_t c_stride, uint32_t flags, uint64_t *d_hist);
+
+/* Replaces trellis::trellis_quantize (src/jpeg/trellis.rs:67-208) for a batch of blocks, with the
+ * same kernel PIXO_B200_COEF_TRELLIS runs.  d_dct: n_blocks x 64 f32 DCT coefficients (natural order,
+ * device, 16-byte aligned); q: 64 f32 quantiser entries (natural order, host; integers 1..255);
+ * lambda: pixo's Option<f32>, 1.0f for None (trellis_quantize_adaptive's formula, trellis.rs:304-321,
+ * picks it from the quality).  d_out: n_blocks x 64 int16 (device, 16-byte aligned), natural order
+ * unless PIXO_B200_COEF_ZIGZAG.  Waits for the device.  PIXO_B200_ERR_INVALID_ARGUMENT for input
+ * this kernel does not carry: a non-finite coefficient or cost, a non-zero |dct| below 2^-100, or
+ * |dct / q| above 32766 (where the reference's i16 candidates saturate or overflow); the output is
+ * then unspecified. */
+int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, size_t n_blocks,
+                                        const float q[64], float lambda, int16_t *d_out,
+                                        uint32_t flags);
 
 /* Replaces pixo::jpeg::encode_into — src/jpeg/mod.rs:328-447 (baseline: encode_scan :1408).
  * GPU: colour/subsample/DCT/quantise, symbol statistics when optimize_huffman, Huffman bit

@@ -52,6 +52,7 @@ SYMBOLS = {
     "pixo_b200_jpeg_coefficients_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                                   C.c_uint32, C.c_uint32, f32p, f32p, vp, C.c_size_t,
                                                   vp, vp, C.c_size_t, C.c_uint32, vp]),
+    "pixo_b200_jpeg_trellis_quantize_dev": (C.c_int, [vp, vp, C.c_size_t, f32p, C.c_float, vp, C.c_uint32]),
     "pixo_b200_jpeg_encode": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                         C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                         C.c_uint32, vp, C.c_size_t, szp]),

@@ -6,6 +6,7 @@
 #include <emmintrin.h>
 
 #include <algorithm>
+#include <cmath>
 #include <thread>
 #include <vector>
 
@@ -328,9 +329,9 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
-                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img};
+                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
-    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant};
+    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant, &ctx->h_trellis};
     for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->stage_events) cudaEventDestroy(ev);
@@ -515,6 +516,75 @@ int pixo_b200_jpeg_block_counts(uint32_t width, uint32_t height, uint32_t color_
     return 0;
 }
 
+// Bit 0 of the trellis status word, read back after the context's stream has drained
+static int trellis_status(pixo_b200_ctx *ctx, const uint32_t *d_status)
+{
+    PIXO_TRY(ensure_pinned(ctx, ctx->h_trellis, sizeof(uint32_t)));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_trellis.ptr, d_status, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (*static_cast<const uint32_t *>(ctx->h_trellis.ptr))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "trellis input out of range: a non-finite value or cost, a non-zero |dct| below 2^-100, or |dct / q| above 32766");
+    return 0;
+}
+
+// f32 DCT scratch per piece of work: whole frames in groups that stay within kTrellisScratch (a 4K 4:2:0
+// frame is ~50 MB), and a frame larger than that in bands of whole MCU rows that do.  A band's MCUs lie
+// entirely inside it (only the frame's own last MCU row replicates edge rows), so a band's blocks are
+// exactly the frame's, and its coefficients land at the band's first MCU in the frame's arrays.
+static constexpr size_t kTrellisScratch = (size_t)256 << 20;
+
+// COEF_TRELLIS: compute_all_coefficients(.., use_trellis = true).  Per piece the transform writes each
+// block's f32 DCT to the context's scratch, then k_trellis quantises each component's blocks into the
+// caller's arrays.  Waits for the device (the input check is reported by the call).
+static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
+                                uint32_t width, uint32_t height, uint32_t color_type, uint32_t subsampling,
+                                const float lum_q[64], const float chr_q[64], int16_t *d_y, size_t y_stride,
+                                int16_t *d_cb, int16_t *d_cr, size_t c_stride, bool zigzag)
+{
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    const bool chroma = g.has_chroma;
+    const size_t row_bytes = (size_t)g.mcus_x * (g.y_per_mcu + (chroma ? 2 : 0)) * 64 * sizeof(float);  // per MCU row
+    const size_t frame_bytes = row_bytes * g.mcus_y;
+    const uint32_t mcu_px = g.y_per_mcu == 4 ? 16 : 8, bpp = color_type == PIXO_B200_GRAY ? 1 : 3;
+    // whole frames per group, or MCU rows per band
+    const uint32_t group = (uint32_t)std::max<size_t>(1, std::min<size_t>(n_images, kTrellisScratch / frame_bytes));
+    const uint32_t band = frame_bytes <= kTrellisScratch
+                              ? g.mcus_y
+                              : (uint32_t)std::max<size_t>(1, std::min<size_t>(g.mcus_y, kTrellisScratch / row_bytes));
+    const size_t piece_bytes = band < g.mcus_y ? row_bytes * band : frame_bytes * group;
+    PIXO_TRY(ensure_dev(ctx, ctx->d_trellis, 256 + piece_bytes));
+    auto *status = static_cast<uint32_t *>(ctx->d_trellis.ptr);
+    float *fy = reinterpret_cast<float *>(static_cast<uint8_t *>(ctx->d_trellis.ptr) + 256);
+    PIXO_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(uint32_t), ctx->stream));
+    // frames [i0, i0 + nb) from MCU row m0 on, `rows` MCU rows each
+    auto piece = [&](uint32_t i0, uint32_t nb, uint32_t m0, uint32_t rows) -> int {
+        const uint32_t h = std::min(rows * mcu_px, height - m0 * mcu_px);
+        const FrameGeometry p = make_geometry(width, h, color_type, subsampling);
+        const size_t nc = chroma ? p.nc : 0;
+        float *fcb = nc ? fy + (size_t)nb * p.ny * 64 : nullptr;
+        float *fcr = nc ? fcb + (size_t)nb * nc * 64 : nullptr;
+        const size_t y0 = (size_t)i0 * y_stride + (size_t)m0 * g.mcus_x * g.y_per_mcu * 64;
+        const size_t c0 = (size_t)i0 * c_stride + (size_t)m0 * g.mcus_x * 64;
+        PIXO_TRY(launch_jpeg_transform_dct(ctx, d_pixels + (size_t)i0 * pixel_stride + (size_t)m0 * mcu_px * width * bpp,
+                                           pixel_stride, nb, width, h, color_type, subsampling, lum_q, chr_q, fy,
+                                           p.ny * 64, fcb, fcr, nc * 64));
+        PIXO_TRY(launch_trellis(ctx, fy, p.ny * 64, d_y + y0, y_stride, p.ny, nb, lum_q, 1.0f, zigzag, status));
+        if (nc) {
+            PIXO_TRY(launch_trellis(ctx, fcb, nc * 64, d_cb + c0, c_stride, nc, nb, chr_q, 1.0f, zigzag, status));
+            PIXO_TRY(launch_trellis(ctx, fcr, nc * 64, d_cr + c0, c_stride, nc, nb, chr_q, 1.0f, zigzag, status));
+        }
+        return 0;
+    };
+    if (band == g.mcus_y) {
+        for (uint32_t i0 = 0; i0 < n_images; i0 += group) PIXO_TRY(piece(i0, std::min(group, n_images - i0), 0, band));
+    } else {
+        for (uint32_t i = 0; i < n_images; ++i)
+            for (uint32_t m0 = 0; m0 < g.mcus_y; m0 += band) PIXO_TRY(piece(i, 1, m0, band));
+    }
+    return trellis_status(ctx, status);
+}
+
 int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
                                     size_t pixel_stride, uint32_t n_images, uint32_t width,
                                     uint32_t height, uint32_t color_type, uint32_t subsampling,
@@ -528,12 +598,20 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (color_type != PIXO_B200_GRAY && (!d_cb || !d_cr))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null chroma buffer");
+    if ((flags & PIXO_B200_COEF_TRELLIS) && d_hist)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "COEF_TRELLIS takes no histogram (pixo's tables come from plain-rounded coefficients)");
     if (n_images == 0) return 0;
     if ((reinterpret_cast<uintptr_t>(d_y) & 15) || (y_stride & 7) ||
         (d_cb && ((reinterpret_cast<uintptr_t>(d_cb) & 15) || (reinterpret_cast<uintptr_t>(d_cr) & 15) || (c_stride & 7))))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
                          "coefficient buffers must be 16-byte aligned with strides multiple of 8");
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (flags & PIXO_B200_COEF_TRELLIS)
+        return trellis_coefficients(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
+                                    lum_q, chr_q, d_y, y_stride, color_type == PIXO_B200_GRAY ? nullptr : d_cb,
+                                    color_type == PIXO_B200_GRAY ? nullptr : d_cr, c_stride,
+                                    (flags & PIXO_B200_COEF_ZIGZAG) != 0);
     PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height,
                                    color_type, subsampling, lum_q, chr_q, d_y, y_stride, d_cb,
                                    d_cr, c_stride, flags));
@@ -556,6 +634,9 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     if (!pixels || !y || !lum_q || !chr_q || (color_type != PIXO_B200_GRAY && (!cb || !cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if ((flags & PIXO_B200_COEF_TRELLIS) && hist)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "COEF_TRELLIS takes no histogram (pixo's tables come from plain-rounded coefficients)");
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     const size_t in_bytes = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t yb = g.ny * 64 * sizeof(int16_t), cbb = g.nc * 64 * sizeof(int16_t);
@@ -570,9 +651,15 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     auto *dy = reinterpret_cast<int16_t *>(ctx->d_y.ptr);
     auto *dcb = reinterpret_cast<int16_t *>(ctx->d_cb.ptr);
     auto *dcr = reinterpret_cast<int16_t *>(ctx->d_cr.ptr);
-    PIXO_TRY(launch_jpeg_transform(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
-                                   width, height, color_type, subsampling, lum_q, chr_q,
-                                   dy, g.ny * 64, dcb, dcr, g.nc * 64, flags));
+    if (flags & PIXO_B200_COEF_TRELLIS)
+        PIXO_TRY(trellis_coefficients(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
+                                      height, color_type, subsampling, lum_q, chr_q, dy, g.ny * 64,
+                                      cbb ? dcb : nullptr, cbb ? dcr : nullptr, g.nc * 64,
+                                      (flags & PIXO_B200_COEF_ZIGZAG) != 0));
+    else
+        PIXO_TRY(launch_jpeg_transform(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
+                                       width, height, color_type, subsampling, lum_q, chr_q,
+                                       dy, g.ny * 64, dcb, dcr, g.nc * 64, flags));
     if (hist) {
         PIXO_TRY(ensure_dev(ctx, ctx->d_out, kHistWords * sizeof(uint64_t)));
         PIXO_TRY(launch_jpeg_histogram(ctx, dy, g.ny * 64, dcb, dcr, g.nc * 64, 1, g.ny, g.nc,
@@ -588,6 +675,27 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     }
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;
+}
+
+int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, size_t n_blocks, const float q[64],
+                                        float lambda, int16_t *d_out, uint32_t flags)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (!d_dct || !q || !d_out) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    for (int k = 0; k < 64; ++k)   // every table pixo builds; the exact division is proved for these
+        if (!(q[k] >= 1.0f && q[k] <= 255.0f && q[k] == (float)(int)q[k]))
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "quantisation table entries must be integers in 1..255");
+    if (!std::isfinite(lambda)) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "lambda is not finite");
+    if ((reinterpret_cast<uintptr_t>(d_dct) & 15) || (reinterpret_cast<uintptr_t>(d_out) & 15))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "block buffers must be 16-byte aligned");
+    if (n_blocks == 0) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_trellis, 256));
+    auto *status = static_cast<uint32_t *>(ctx->d_trellis.ptr);
+    PIXO_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(uint32_t), ctx->stream));
+    PIXO_TRY(launch_trellis(ctx, d_dct, 0, d_out, 0, n_blocks, 1, q, lambda, (flags & PIXO_B200_COEF_ZIGZAG) != 0,
+                            status));
+    return trellis_status(ctx, status);
 }
 
 static int validate_encode(pixo_b200_ctx *ctx, size_t pixels_len, uint32_t width, uint32_t height,

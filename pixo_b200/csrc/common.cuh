@@ -108,6 +108,7 @@ struct pixo_b200_ctx {
     pixo::Scratch d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
     pixo::Scratch d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
     pixo::Scratch d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
+    pixo::Scratch d_trellis, h_trellis;          // JPEG trellis: status word + f32 DCT blocks; its status on the host
     pixo::Scratch h_in, h_out, h_misc, h_red, h_quant;
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
@@ -143,6 +144,16 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
                           uint32_t subsampling, const float *lum_q, const float *chr_q,
                           int16_t *d_y, size_t y_stride, int16_t *d_cb, int16_t *d_cr,
                           size_t c_stride, uint32_t flags, const CoefExtents *ext = nullptr);
+// the same transform writing each block's unquantised f32 DCT (natural order, 64 floats; 4:2:0 chroma:
+// the DCT of the averaged block), strides in floats: the input of launch_trellis
+int launch_jpeg_transform_dct(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
+                              uint32_t w, uint32_t h, uint32_t color_type, uint32_t subsampling,
+                              const float *lum_q, const float *chr_q, float *d_y, size_t y_stride, float *d_cb,
+                              float *d_cr, size_t c_stride);
+// k_trellis (jpeg_trellis.cu) on nb blocks of each of n_frames frames (strides in elements); q: host table,
+// natural order.  Sets bit 0 of *d_status for input it rejects (see jpeg_trellis.cu).
+int launch_trellis(pixo_b200_ctx *ctx, const float *d_src, size_t src_stride, int16_t *d_dst, size_t dst_stride,
+                   uint64_t nb, uint32_t n_frames, const float q[64], float lambda, bool zigzag, uint32_t *d_status);
 // ext: the arrays are coefficient records (zigzag_in is then ignored)
 int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                           const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,

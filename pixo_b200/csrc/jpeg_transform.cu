@@ -286,18 +286,34 @@ __device__ __forceinline__ void dct_rows_x2(f2 (&R)[4][8], f2 (&C)[8][4])
 
 // What the transform writes per block: natural order, zig-zag order (both all 64 coefficients), or
 // a coefficient record (zig-zag order, cut after the sector of the last non-zero coefficient, plus
-// its extent: see CoefExtents in common.cuh).
-enum CoefOut { kNatural, kZigzag, kRecords };
+// its extent: see CoefExtents in common.cuh), or - kDct, the trellis quantiser's input - the block's
+// unquantised f32 DCT in natural order (256 bytes), written straight from registers to global memory.
+enum CoefOut { kNatural, kZigzag, kRecords, kDct };
 
 // column pass on column pairs, quantising each pair of columns as soon as it is transformed;
 // tab(i) returns table entry i (one per output word).  kRecords: *eout = the block's record extent
 // (32-byte sectors up to the last non-zero one: an OR over each sector's words, a few instructions).
+// kDct: no quantiser; the DCT times `dscale` (a power of two, so exact) goes to dout (null: nowhere).
 template <int OUT, typename TabFn>
 __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab, uint4 *__restrict__ out,
-                                                        const int swz, uint8_t *eout)
+                                                        const int swz, uint8_t *eout, float *dout, float dscale)
 {
     constexpr bool ZIGZAG = OUT != kNatural;
     constexpr float SK[8] = {AAN_S0, AAN_S1, AAN_S2, AAN_S3, AAN_S4, AAN_S5, AAN_S6, AAN_S7};
+    if constexpr (OUT == kDct) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const f2 in[8] = {C[0][j], C[1][j], C[2][j], C[3][j], C[4][j], C[5][j], C[6][j], C[7][j]};
+            f2 o[8];
+            aan_1d_x2_core(in, o);
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+                const f2 x = mul2(mul2(o[r], K2(SK[r])), K2(dscale));
+                if (dout) *reinterpret_cast<float2 *>(dout + r * 8 + 2 * j) = make_float2(x.lo, x.hi);
+            }
+        }
+        return;
+    }
     uint32_t W[32];
     const f2 half2 = K2(0.5f), magic2 = K2(12582912.0f);  // 1.5 * 2^23
     uint32_t kSign, kOne;  // in registers so copysign(1.0, q) is ONE lop3: (q & sign) | one
@@ -358,12 +374,13 @@ __device__ __forceinline__ void dct_cols_quant_store_x2(f2 (&C)[8][4], TabFn tab
 // chroma_u MUST be warp-uniform (the callers derive it from a warp vote, so the branch is one).
 template <int OUT>
 __device__ __forceinline__ void dct_quant_store_x2(f2 (&R)[4][8], const QPairTab *qs, const bool chroma_u,
-                                                   uint4 *__restrict__ out, const int swz, uint8_t *eout)
+                                                   uint4 *__restrict__ out, const int swz, uint8_t *eout,
+                                                   float *dout = nullptr, float dscale = 1.0f)
 {
     f2 C[8][4];
     dct_rows_x2(R, C);
     const QPair *t = qs->t[chroma_u ? 1 : 0];
-    dct_cols_quant_store_x2<OUT>(C, [&](int i) { return t[i]; }, out, swz, eout);
+    dct_cols_quant_store_x2<OUT>(C, [&](int i) { return t[i]; }, out, swz, eout, dout, dscale);
 }
 
 // Copy a warp's 32-slot stage (4 KB, swizzled as above) to global memory: instruction j moves
@@ -466,7 +483,7 @@ struct K1Params {
     const uint8_t *pixels;
     size_t pixel_stride;
     uint32_t w, h, mcus_x, mcus_y, units_x, n_images;
-    int16_t *y, *cb, *cr;
+    int16_t *y, *cb, *cr;            // kDct: float arrays (and the strides count floats)
     size_t y_stride, c_stride;
     CoefExtents e;                   // kRecords only
     uint32_t use_tma;
@@ -691,6 +708,21 @@ k_jpeg_420(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
             // The transform runs in every lane (edge lanes work on garbage and their slots are never
             // flushed): the quantiser's table reads are uniform-datapath loads, which exist only in
             // warp-convergent code.
+            if constexpr (OUT == kDct) {
+                // the block's f32 DCT straight to its slot; the chroma block holds 4x the averaged
+                // block (quad sums), so its DCT is scaled by 0.25, exactly
+                float *dout = nullptr;
+                if (!chroma_u) {
+                    if (job * 8u + (slot >> 2) < n_mcu)
+                        dout = reinterpret_cast<float *>(P.y) + (size_t)img * P.y_stride + ((mcu_base + job * 8) * 4 + slot) * 64;
+                } else if ((uint32_t)(lane & 15) < n_mcu) {
+                    dout = reinterpret_cast<float *>(lane < 16 ? P.cb : P.cr) + (size_t)img * P.c_stride +
+                           (mcu_base + (lane & 15)) * 64;
+                }
+                dct_quant_store_x2<OUT>(R, QS, chroma_u, stage + slot * 8, swz, &WS.ext[slot], dout,
+                                        chroma_u ? 0.25f : 1.0f);
+                continue;
+            }
             dct_quant_store_x2<OUT>(R, QS, chroma_u, stage + slot * 8, swz, &WS.ext[slot]);
             if (!chroma_u) {
                 const size_t b0 = (mcu_base + job * 8) * 4;   // the job's first Y block
@@ -886,6 +918,13 @@ k_jpeg_444(const __grid_constant__ K1Params P, const __grid_constant__ QPairTab 
                     for (int x = 0; x < 8; ++x) R[rp][x] = pk(v0[x], v1[x]);
                 }
             }
+            if constexpr (OUT == kDct) {   // the block's f32 DCT straight to its slot
+                float *arr = reinterpret_cast<float *>(comp == 0 ? P.y : (comp == 1 ? P.cb : P.cr)) +
+                             (size_t)img * (comp == 0 ? P.y_stride : P.c_stride);
+                dct_quant_store_x2<OUT>(R, QS, chroma_u, WS.stage + lane * 8, lane & 7, &WS.ext[lane],
+                                        bx0 + lane < P.mcus_x ? arr + (b0 + lane) * 64 : nullptr);
+                continue;
+            }
             dct_quant_store_x2<OUT>(R, QS, chroma_u, WS.stage + lane * 8, lane & 7, &WS.ext[lane]);
             uint8_t *earr = nullptr;
             if (OUT == kRecords)
@@ -933,6 +972,14 @@ k_jpeg_gray(const uint8_t *__restrict__ pixels, size_t pixel_stride, uint32_t w,
                 const float f1 = __uint_as_float(__byte_perm(wb[x >> 2], 0x4B000000u, 0x7650 + (x & 3)));
                 R[rp][x] = sub2(pk(f0, f1), K2(8388736.0f));
             }
+        }
+        if constexpr (OUT == kDct) {   // the block's f32 DCT straight to its slot (yout is a float array)
+            const uint32_t blk = b0 + j;
+            dct_quant_store_x2<OUT>(R, QS, false, stage[warp] + lane * 8, lane & 7, &ext[warp][lane],
+                                    blk < blocks_x ? reinterpret_cast<float *>(yout) + (size_t)img * y_stride +
+                                                         ((size_t)brow * blocks_x + blk) * 64
+                                                   : nullptr);
+            return;
         }
         dct_quant_store_x2<OUT>(R, QS, false, stage[warp] + lane * 8, lane & 7, &ext[warp][lane]);
     }
@@ -1109,12 +1156,12 @@ int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, int out, const uint8_t *
     P.use_tma = make_rgb_tensor_map(&tm, px, pixel_stride, n, w, h, (s444 ? K444_ROW_B : K1_HB) / 8, px_per) ? 1u : 0u;
     const int warps = s444 ? K444_WARPS : K1_WARPS;
     const size_t smem = s444 ? sizeof(K444Smem) : sizeof(K1Smem);
-    void (*const k420[3])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_420<kNatural>, k_jpeg_420<kZigzag>,
-                                                               k_jpeg_420<kRecords>};
-    void (*const k444[3])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_444<kNatural>, k_jpeg_444<kZigzag>,
-                                                               k_jpeg_444<kRecords>};
+    void (*const k420[4])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_420<kNatural>, k_jpeg_420<kZigzag>,
+                                                               k_jpeg_420<kRecords>, k_jpeg_420<kDct>};
+    void (*const k444[4])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_444<kNatural>, k_jpeg_444<kZigzag>,
+                                                               k_jpeg_444<kRecords>, k_jpeg_444<kDct>};
     auto kern = s444 ? k444[out] : k420[out];
-    static int blocks_per_sm[64][2][3];  // [device][s444][out]: function attributes are per device
+    static int blocks_per_sm[64][2][4];  // [device][s444][out]: function attributes are per device
     int &bps = blocks_per_sm[ctx->device & 63][s444][out];
     if (!bps) {
         PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1136,17 +1183,18 @@ CoefExtents extents_from(const CoefExtents *e, size_t i0)
     return CoefExtents{e->y + o, e->cb ? e->cb + o : nullptr, e->cr ? e->cr + o : nullptr, e->stride};
 }
 
-}  // namespace
-
-int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
-                          uint32_t n_images, uint32_t w, uint32_t h, uint32_t color_type,
-                          uint32_t subsampling, const float *lum_q, const float *chr_q,
-                          int16_t *d_y, size_t y_stride, int16_t *d_cb, int16_t *d_cr,
-                          size_t c_stride, uint32_t flags, const CoefExtents *ext)
+// launch_jpeg_transform / launch_jpeg_transform_dct: `out` is the CoefOut format; the arrays hold int16
+// coefficients, or floats for kDct (strides in elements either way)
+int transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images, uint32_t w,
+              uint32_t h, uint32_t color_type, uint32_t subsampling, const float *lum_q, const float *chr_q,
+              int out, void *d_y_, size_t y_stride, void *d_cb_, void *d_cr_, size_t c_stride, const CoefExtents *ext)
 {
     QPairTab qt;
     fill_qpair_tab(lum_q, chr_q, (color_type != PIXO_B200_GRAY && subsampling == PIXO_B200_S420) ? 4.0f : 1.0f, &qt);
-    const int out = ext ? kRecords : (flags & PIXO_B200_COEF_ZIGZAG) ? kZigzag : kNatural;
+    const size_t esz = out == kDct ? sizeof(float) : sizeof(int16_t);
+    auto at = [esz](void *base, size_t elems) -> int16_t * {   // element offset in the arrays' own type
+        return base ? reinterpret_cast<int16_t *>(static_cast<uint8_t *>(base) + elems * esz) : nullptr;
+    };
     // the exact-division identity is proved for integer divisors 1..255 only
     for (int i = 0; i < 64; ++i) {
         const float a = lum_q[i], b = chr_q[i];
@@ -1162,17 +1210,17 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
     for (uint32_t i0 = 0; i0 < n_images; i0 += per_launch) {
         const uint32_t nb = n_images - i0 < per_launch ? n_images - i0 : per_launch;
         const uint8_t *px = d_pixels + (size_t)i0 * pixel_stride;
-        int16_t *y = d_y + (size_t)i0 * y_stride;
-        int16_t *cb = d_cb ? d_cb + (size_t)i0 * c_stride : nullptr;
-        int16_t *cr = d_cr ? d_cr + (size_t)i0 * c_stride : nullptr;
+        int16_t *y = at(d_y_, (size_t)i0 * y_stride);
+        int16_t *cb = at(d_cb_, (size_t)i0 * c_stride);
+        int16_t *cr = at(d_cr_, (size_t)i0 * c_stride);
         const CoefExtents e = extents_from(ext, i0);
         if (color_type == PIXO_B200_GRAY) {
             const uint32_t bx = (w + 7) / 8, by = (h + 7) / 8;
             const uint32_t tiles_x = (bx + GRAY_BLOCKS - 1) / GRAY_BLOCKS;
             dim3 grid(tiles_x * by, nb);
-            void (*const kg[3])(const uint8_t *, size_t, uint32_t, uint32_t, uint32_t, uint32_t, int16_t *, size_t,
+            void (*const kg[4])(const uint8_t *, size_t, uint32_t, uint32_t, uint32_t, uint32_t, int16_t *, size_t,
                                 uint8_t *, size_t, QPairTab) = {k_jpeg_gray<kNatural>, k_jpeg_gray<kZigzag>,
-                                                                 k_jpeg_gray<kRecords>};
+                                                                 k_jpeg_gray<kRecords>, k_jpeg_gray<kDct>};
             kg[out]<<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, e.y, e.stride, qt);
         } else {
             PIXO_TRY(launch_rgb_transform(ctx, subsampling == PIXO_B200_S444, out, px, pixel_stride, nb, w, h, y,
@@ -1182,6 +1230,28 @@ int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
         PIXO_CUDA(ctx, cudaGetLastError());
     }
     return 0;
+}
+
+}  // namespace
+
+int launch_jpeg_transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                          uint32_t n_images, uint32_t w, uint32_t h, uint32_t color_type,
+                          uint32_t subsampling, const float *lum_q, const float *chr_q,
+                          int16_t *d_y, size_t y_stride, int16_t *d_cb, int16_t *d_cr,
+                          size_t c_stride, uint32_t flags, const CoefExtents *ext)
+{
+    const int out = ext ? kRecords : (flags & PIXO_B200_COEF_ZIGZAG) ? kZigzag : kNatural;
+    return transform(ctx, d_pixels, pixel_stride, n_images, w, h, color_type, subsampling, lum_q, chr_q, out, d_y,
+                     y_stride, d_cb, d_cr, c_stride, ext);
+}
+
+int launch_jpeg_transform_dct(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
+                              uint32_t w, uint32_t h, uint32_t color_type, uint32_t subsampling,
+                              const float *lum_q, const float *chr_q, float *d_y, size_t y_stride, float *d_cb,
+                              float *d_cr, size_t c_stride)
+{
+    return transform(ctx, d_pixels, pixel_stride, n_images, w, h, color_type, subsampling, lum_q, chr_q, kDct, d_y,
+                     y_stride, d_cb, d_cr, c_stride, nullptr);
 }
 
 int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,

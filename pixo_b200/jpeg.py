@@ -90,10 +90,15 @@ def block_counts(width, height, color_type=ColorType.Rgb, subsampling=Subsamplin
     return ny.value, nc.value
 
 
+COEF_ZIGZAG, COEF_TRELLIS = 1, 2   # flags of pixo_b200_jpeg_coefficients* (include/pixo_b200.h)
+
+
 def compute_all_coefficients(data, width, height, color_type=ColorType.Rgb,
                              subsampling=Subsampling.S420, quality=None, lum_q=None, chr_q=None,
-                             zigzag=False, histograms=False, ctx: Context | None = None):
-    """compute_all_coefficients (src/jpeg/mod.rs:932-966) -> (y, cb, cr[, hist]) int16 [n,64]."""
+                             zigzag=False, histograms=False, ctx: Context | None = None, use_trellis=False):
+    """compute_all_coefficients (src/jpeg/mod.rs:932-966) -> (y, cb, cr[, hist]) int16 [n,64].
+    use_trellis: trellis-quantise every block, as pixo's max preset does (no histograms then: pixo's
+    tables come from the plain-rounded coefficients)."""
     ctx = ctx or default_context()
     d = _as_u8(data)
     bpp = 1 if int(color_type) == ColorType.Gray else 3
@@ -111,10 +116,54 @@ def compute_all_coefficients(data, width, height, color_type=ColorType.Rgb,
     rc = _lib.load().pixo_b200_jpeg_coefficients(
         ctx.handle, d.ctypes.data, width, height, int(color_type), int(subsampling),
         lum_q.ctypes.data_as(_lib.f32p), chr_q.ctypes.data_as(_lib.f32p), y.ctypes.data,
-        cb.ctypes.data, cr.ctypes.data, 1 if zigzag else 0, hist.ctypes.data if histograms else None)
+        cb.ctypes.data, cr.ctypes.data, (COEF_ZIGZAG if zigzag else 0) | (COEF_TRELLIS if use_trellis else 0),
+        hist.ctypes.data if histograms else None)
     _lib.check(ctx.handle, rc)
     out = (y, cb[:nc], cr[:nc])
     return out + (hist,) if histograms else out
+
+
+def trellis_lambda(quality: int) -> float:
+    """trellis_quantize_adaptive's lambda (src/jpeg/trellis.rs:304-321), in binary32 as pixo computes it."""
+    q = int(quality)
+    f = np.float32
+    if q >= 80:
+        return float(f(f(0.5) + f(100 - q) * f(0.025)))
+    if q >= 50:
+        return float(f(f(1.0) + f(80 - q) * f(0.033)))
+    return float(f(f(2.0) + f(50 - q) * f(0.04)))
+
+
+def trellis_quantize_dev(d_dct, quant_table, lam=None, d_out=None, zigzag=False, ctx: Context | None = None):
+    """trellis::trellis_quantize (src/jpeg/trellis.rs:67-208) for a batch of blocks on the device:
+    d_dct float32 [n, 64] (natural order, anything with .data_ptr()), quant_table 64 natural-order
+    entries, lam None for pixo's default 1.0.  Writes / returns d_out int16 [n, 64] (a new torch tensor
+    on the same device when None)."""
+    ctx = ctx or default_context()
+    if d_out is None:
+        import torch
+        d_out = torch.empty(d_dct.shape, dtype=torch.int16, device=d_dct.device)
+    q = np.ascontiguousarray(quant_table, np.float32).reshape(64)
+    n = int(d_dct.numel()) // 64
+    rc = _lib.load().pixo_b200_jpeg_trellis_quantize_dev(
+        ctx.handle, int(d_dct.data_ptr()), n, q.ctypes.data_as(_lib.f32p), 1.0 if lam is None else float(lam),
+        int(d_out.data_ptr()), COEF_ZIGZAG if zigzag else 0)
+    _lib.check(ctx.handle, rc)
+    return d_out
+
+
+def trellis_quantize(dct, quant_table, lam=None, ctx: Context | None = None) -> np.ndarray:
+    """trellis::trellis_quantize on host blocks: dct float32 [64] or [n, 64] -> int16 of the same shape."""
+    import torch
+    a = np.ascontiguousarray(dct, np.float32)
+    dev = torch.device("cuda", (ctx or default_context()).device)
+    out = trellis_quantize_dev(torch.from_numpy(a.reshape(-1, 64)).to(dev), quant_table, lam, ctx=ctx)
+    return out.cpu().numpy().reshape(a.shape)
+
+
+def trellis_quantize_adaptive(dct, quant_table, quality, ctx: Context | None = None) -> np.ndarray:
+    """trellis::trellis_quantize_adaptive (src/jpeg/trellis.rs:304-321)."""
+    return trellis_quantize(dct, quant_table, trellis_lambda(quality), ctx=ctx)
 
 
 def encode_into(output: bytearray, data, options: JpegOptions, ctx: Context | None = None) -> None:
