@@ -213,7 +213,10 @@ int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const in
  * pixo_b200_jpeg_coefficients_dev writes): optimised-table statistics (K3) and the Huffman /
  * stuffing / restart stage (k_huff) run on the GPU, only the scan bytes come back; out receives
  * the complete JPEG.  This is what a frame tiled over several GPUs uses once its bands'
- * coefficients have been gathered on one of them (SURVEY.md section 8e). */
+ * coefficients have been gathered on one of them (SURVEY.md section 8e).
+ * d_y, and d_cb / d_cr unless Gray, must be 16-byte aligned (the kernels load whole blocks as
+ * 16-byte vectors): PIXO_B200_ERR_INVALID_ARGUMENT otherwise, before anything is launched.  The
+ * same holds for pixo_b200_jpeg_band_histogram_dev and pixo_b200_jpeg_band_entropy_dev(_async). */
 int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
                                       const int16_t *d_cr, uint32_t width, uint32_t height,
                                       uint32_t color_type, uint32_t quality, uint32_t subsampling,
@@ -322,7 +325,9 @@ int pixo_b200_png_filter(pixo_b200_ctx *ctx, const uint8_t *data, uint32_t width
                          uint32_t strategy, uint8_t *out, uint32_t *adler32_out);
 
 /* Device-pointer, batched variant (asynchronous).  Frame i: d_data + i*in_stride ->
- * d_out + i*out_stride; d_adler (optional): n_images u32. */
+ * d_out + i*out_stride; d_adler (optional): n_images u32.  Frames must not overlap: with
+ * n_images > 1, in_stride < height*row_bytes returns PIXO_B200_ERR_INVALID_DATA_LENGTH and
+ * out_stride < height*(row_bytes+1) returns PIXO_B200_ERR_OUTPUT_TOO_SMALL.  Any alignment. */
 int pixo_b200_png_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
                              uint32_t n_images, uint32_t width, uint32_t height,
                              size_t row_bytes, uint32_t bytes_per_pixel, uint32_t strategy,

@@ -1084,6 +1084,17 @@ static int check_range(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb, 
     return 0;
 }
 
+// Caller coefficient arrays on the device: the statistics and Huffman kernels load each block as
+// 16-byte vectors, so an array that is not 16-byte aligned is refused before anything is launched.
+static int check_coef_alignment(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                                bool has_chroma)
+{
+    auto mis = [](const int16_t *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
+    if (mis(d_y) || (has_chroma && (mis(d_cb) || mis(d_cr))))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient arrays must be 16-byte aligned");
+    return 0;
+}
+
 int pixo_b200_jpeg_entropy_encode(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb,
                                   const int16_t *cr, uint32_t width, uint32_t height,
                                   uint32_t color_type, uint32_t quality, uint32_t subsampling,
@@ -1125,6 +1136,7 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     if (out_cap < 1024 + 2)
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    PIXO_TRY(check_coef_alignment(ctx, d_y, d_cb, d_cr, g.has_chroma));
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1183,6 +1195,7 @@ int pixo_b200_jpeg_band_histogram_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     if (!d_y || !d_hist || (color_type != PIXO_B200_GRAY && (!d_cb || !d_cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
+    PIXO_TRY(check_coef_alignment(ctx, d_y, d_cb, d_cr, g.has_chroma));
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, 0, false, nullptr, d_hist,
                                  dc_seed);
@@ -1201,6 +1214,7 @@ int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, cons
     if ((raw_cap & 3) || (reinterpret_cast<uintptr_t>(d_raw) & 15))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "raw buffer must be 16-byte aligned, capacity multiple of 4");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
+    PIXO_TRY(check_coef_alignment(ctx, d_y, d_cb, d_cr, g.has_chroma));
     HuffTables t;
     tables_from(hist, g.has_chroma, t);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1269,6 +1283,7 @@ int pixo_b200_jpeg_band_entropy_dev_async(pixo_b200_ctx *ctx, const int16_t *d_y
     if ((raw_cap & 3) || (reinterpret_cast<uintptr_t>(d_raw) & 15))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "raw buffer must be 16-byte aligned, capacity multiple of 4");
     const FrameGeometry g = make_geometry(width, band_height, color_type, subsampling);
+    PIXO_TRY(check_coef_alignment(ctx, d_y, d_cb, d_cr, g.has_chroma));
     HuffTables t;
     tables_from(hist, g.has_chroma, t);
     if (raw_cap < band_raw_bytes(g))
@@ -1371,6 +1386,13 @@ int pixo_b200_png_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t i
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     PIXO_TRY(validate_png(ctx, width, height, row_bytes, bytes_per_pixel, strategy));
     if (!d_data || !d_out) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    // frames of a batch must not overlap: every image's rows are read whole, and its CTAs write
+    // its filtered stream while other images' CTAs write theirs
+    const size_t raw = row_bytes * height, need = (row_bytes + 1) * (size_t)height;
+    if (n_images > 1 && in_stride < raw)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
+    if (n_images > 1 && out_stride < need)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return launch_png_filter_rows(ctx, d_data, in_stride, n_images, width, height, row_bytes,

@@ -232,8 +232,8 @@ def entropy_encode(y, cb, cr, options: JpegOptions, ctx: Context | None = None) 
 
 def entropy_encode_dev(d_y, d_cb, d_cr, options: JpegOptions, ctx: Context | None = None) -> bytes:
     """Entropy-code coefficient arrays that live on the device (anything with .data_ptr(), e.g.
-    int16 torch tensors in compute_all_coefficients' layout) into a complete JPEG: Huffman
-    statistics, bit packing, stuffing and restart markers run on the GPU."""
+    int16 torch tensors in compute_all_coefficients' layout, 16-byte aligned) into a complete JPEG:
+    Huffman statistics, bit packing, stuffing and restart markers run on the GPU."""
     ctx = ctx or default_context()
     cap = output_capacity(options.width, options.height)
     buf = np.empty(cap, np.uint8)
