@@ -426,7 +426,9 @@ int pixo_b200_png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_
                                   uint32_t *adler32_out);
 /* Batch of device-resident frames, as pixo_b200_png_reduce_filter_dev; a batch may mix frames that
  * quantise with frames that do not.  palettes (optional, HOST memory): n_images x 256 x 4 bytes with
- * palette_lens[i] entries for frame i, 0 = design it.  Returns once info[] is valid. */
+ * palette_lens[i] entries for frame i, 0 = design it.  Any n_images: the quantised frames are mapped and
+ * filtered in passes of a few thousand, so the context's scratch does not grow with the batch.  Returns
+ * once info[] is valid. */
 int pixo_b200_png_quantize_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride,
                                       uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
                                       uint32_t strategy_and_flags, uint32_t max_colors, const uint8_t *palettes,

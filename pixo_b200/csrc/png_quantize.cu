@@ -41,6 +41,7 @@ constexpr uint32_t LUT_CELLS = 64 * 64 * 64;
 constexpr uint32_t SAMPLE_CHUNK = 64;            // images per sort (6 bits of the key)
 constexpr int DITHER_WARPS = 4;                  // warps per CTA of k_quant_dither
 constexpr uint32_t SPIN_LIMIT = 1u << 22;        // polls (with back-off) before a wait is a fault
+constexpr size_t QUANT_PASS = 4096;              // quantised images per pass of k-means, tables, map and filter
 
 __device__ __forceinline__ uint32_t redmean(uint32_t c, uint32_t p)
 {
@@ -466,11 +467,14 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         }
     }
 
-    std::vector<uint32_t> qids;
-    for (uint32_t i = 0; i < n_images; ++i) if (kind[i] != LOSSLESS) qids.push_back(i);
-    const size_t nq = qids.size();
+    std::vector<uint32_t> qall;
+    for (uint32_t i = 0; i < n_images; ++i) if (kind[i] != LOSSLESS) qall.push_back(i);
     const size_t idx_stride = al256(npix);
-    if (nq) {
+    // steps 3-5 in passes of at most QUANT_PASS quantised images: every grid.y stays within CUDA's limit
+    // and the scratch (about 330 KB per image besides its indices) does not grow with the batch
+    for (size_t q0 = 0; q0 < qall.size(); q0 += QUANT_PASS) {
+        const std::vector<uint32_t> qids(qall.begin() + q0, qall.begin() + std::min(qall.size(), q0 + QUANT_PASS));
+        const size_t nq = qids.size();
         // 3. k-means, tables, map / dither on the device
         const size_t o_jobs = 0, jobs_bytes = al256(nq * (sizeof(KmeansJob) + sizeof(LutJob) + sizeof(MapJob) + sizeof(DitherJob)) + 1024);
         const size_t o_pal = jobs_bytes, o_acc = o_pal + al256(nq * 256 * 4), o_col = o_acc + al256(nq * 256 * 5 * 8);
@@ -483,7 +487,8 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         auto *d_acc = reinterpret_cast<unsigned long long *>(base + o_acc);
         auto *d_col = reinterpret_cast<uint32_t *>(base + o_col);
         uint8_t *d_idx = base + o_idx;
-        std::vector<uint32_t> h_pal(nq * 256, 0), h_col(nq * MAX_HIST_COLORS * 2, 0);
+        std::vector<uint32_t> h_pal(nq * 256, 0);
+        std::vector<uint32_t> h_col;   // each k-means job's histogram colours then counts, packed
         std::vector<KmeansJob> km;
         std::vector<LutJob> lj;
         std::vector<MapJob> mj;
@@ -494,10 +499,10 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
             std::copy(pal[i].begin(), pal[i].end(), h_pal.begin() + k * 256);
             uint32_t *dp = d_pal + k * 256;
             if (!hcol[i].empty()) {   // median cut ran: two k-means passes over its histogram
-                std::copy(hcol[i].begin(), hcol[i].end(), h_col.begin() + k * MAX_HIST_COLORS * 2);
-                std::copy(hcnt[i].begin(), hcnt[i].end(), h_col.begin() + k * MAX_HIST_COLORS * 2 + MAX_HIST_COLORS);
-                const uint32_t *cc = d_col + k * MAX_HIST_COLORS * 2;
-                km.push_back({cc, cc + MAX_HIST_COLORS, (uint32_t)hcol[i].size(), (uint32_t)pal[i].size(), dp, d_acc + k * 256 * 5});
+                const uint32_t *cc = d_col + h_col.size();
+                h_col.insert(h_col.end(), hcol[i].begin(), hcol[i].end());
+                h_col.insert(h_col.end(), hcnt[i].begin(), hcnt[i].end());
+                km.push_back({cc, cc + hcol[i].size(), (uint32_t)hcol[i].size(), (uint32_t)pal[i].size(), dp, d_acc + k * 256 * 5});
                 max_cols = std::max(max_cols, (uint32_t)hcol[i].size());
             }
             uint8_t *lut = base + o_lut + k * LUT_CELLS;
@@ -524,7 +529,7 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         PIXO_CUDA(ctx, cudaMemcpyAsync(base, jobs.data(), o, cudaMemcpyHostToDevice, ctx->stream));
         PIXO_CUDA(ctx, cudaMemcpyAsync(d_pal, h_pal.data(), nq * 256 * 4, cudaMemcpyHostToDevice, ctx->stream));
         if (!km.empty()) {
-            PIXO_CUDA(ctx, cudaMemcpyAsync(d_col, h_col.data(), nq * MAX_HIST_COLORS * 8, cudaMemcpyHostToDevice, ctx->stream));
+            PIXO_CUDA(ctx, cudaMemcpyAsync(d_col, h_col.data(), h_col.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
             PIXO_CUDA(ctx, cudaMemsetAsync(d_acc, 0, nq * 256 * 5 * 8, ctx->stream));
             for (int pass = 0; pass < 2; ++pass) {
                 k_quant_kmeans<<<dim3((max_cols + Q_THREADS - 1) / Q_THREADS, (uint32_t)km.size()), Q_THREADS, 0, ctx->stream>>>(d_km);
