@@ -164,7 +164,8 @@ int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, 
  * mod.rs:1423-1445); host: headers (:449-648) and Huffman table construction
  * (src/jpeg/huffman.rs:100-391).  Byte-identical to the reference.  Only the scan bytes come
  * back over PCIe.  restart_interval 0 = None.  progressive is outside this path
- * (PIXO_B200_ERR_UNSUPPORTED when non-zero); trellis_quant is accepted and ignored, exactly as
+ * (PIXO_B200_ERR_UNSUPPORTED when non-zero: progressive files come from
+ * pixo_b200_jpeg_encode_progressive); trellis_quant is accepted and ignored, exactly as
  * the reference's baseline encode_scan ignores use_trellis (src/jpeg/mod.rs:1408-1563 always
  * calls quantize_block). */
 int pixo_b200_jpeg_encode(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len,
@@ -181,6 +182,45 @@ int pixo_b200_jpeg_encode_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_
                                 uint32_t color_type, uint32_t quality, uint32_t subsampling,
                                 uint32_t restart_interval, uint32_t optimize_huffman,
                                 uint8_t *out, size_t out_cap_each, size_t *out_lens);
+
+/* pixo::jpeg::encode_into with options.progressive (src/jpeg/mod.rs:395-410, encode_progressive
+ * :872-927): the same file pixo writes - SOI, APP0, DQT, SOF2, DHT, DRI when restart_interval != 0,
+ * then the 7 scans of simple_progressive_script (Y DC, Cb DC, Cr DC, Y 1-10, Y 11-63, Cb 1-63,
+ * Cr 1-63, Ah = Al = 0), each an SOS and its entropy-coded segment, then EOI.  pixo's quirks are kept:
+ * every scan walks its component's array in compute_all_coefficients order (MCU order for 4:2:0 Y),
+ * DC predictors are never reset, DRI is written but no RST marker, the optimised tables come from the
+ * plain-rounded baseline statistics (restart interval included) also under trellis_quant, EOB runs
+ * whose symbol a table lacks get the (0, 4) fallback code, and a gray frame still gets the (empty)
+ * chroma scans.  These files are pixo's, not always conformant JPEGs.  GPU: transform, statistics,
+ * COEF_TRELLIS when trellis_quant, and the progressive scan stage (stuffed segments); host: headers and
+ * tables.  Same errors as pixo_b200_jpeg_encode; PIXO_B200_ERR_CUDA for a device fault (no host twin). */
+int pixo_b200_jpeg_encode_progressive(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len,
+                                      uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                      uint32_t subsampling, uint32_t restart_interval, uint32_t optimize_huffman,
+                                      uint32_t trellis_quant, uint8_t *out, size_t out_cap, size_t *out_len);
+int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len_each,
+                                            uint32_t n_images, uint32_t width, uint32_t height,
+                                            uint32_t color_type, uint32_t quality, uint32_t subsampling,
+                                            uint32_t restart_interval, uint32_t optimize_huffman,
+                                            uint32_t trellis_quant, uint8_t *out, size_t out_cap_each,
+                                            size_t *out_lens);
+
+/* The progressive scan stage on caller coefficient arrays (device memory, compute_all_coefficients'
+ * layout: natural order, frame i at d_y + i*y_stride, d_cb/d_cr + i*c_stride, strides in int16
+ * elements, multiples of 8 and at least a frame's blocks when n_frames > 1; arrays 16-byte aligned;
+ * d_cb/d_cr ignored for gray).  Per frame the 7 stuffed, 1-padded segments back to back at
+ * d_out + i*out_cap_each, lengths in d_scan_len[i*7 + s] (the size needed, also when it did not fit);
+ * d_overflow[i] bit 0: they did not fit out_cap_each and nothing was written for that frame.
+ * dht: 4 x (16 counts + 256 values), order dc_lum, dc_chrom, ac_lum, ac_chrom (the file's DHT), NULL =
+ * the standard tables.  PIXO_B200_ERR_INVALID_ARGUMENT, with nothing written, for a coefficient outside
+ * -16383..16383 (every DC difference then fits int16 and every category is <= 15), a table with more
+ * than 256 values or a code that does not fit its length, or a layout above.  Waits for the device to
+ * measure the scans; the final copy into d_out is queued on the context's stream. */
+int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
+                                         const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
+                                         uint32_t n_frames, uint32_t width, uint32_t height, uint32_t color_type,
+                                         uint32_t subsampling, const uint8_t *dht, uint8_t *d_out,
+                                         size_t out_cap_each, uint64_t *d_scan_len, uint32_t *d_overflow);
 
 /* Device-resident variant of the whole hot path (asynchronous on the context's stream):
  * frame i at d_pixels + i*pixel_stride -> entropy-coded scan bytes (what encode_scan appends

@@ -59,6 +59,15 @@ SYMBOLS = {
     "pixo_b200_jpeg_encode_batch": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                               C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                               C.c_uint32, vp, C.c_size_t, szp]),
+    "pixo_b200_jpeg_encode_progressive": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                    C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                    vp, C.c_size_t, szp]),
+    "pixo_b200_jpeg_encode_progressive_batch": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                          C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                          C.c_uint32, C.c_uint32, vp, C.c_size_t, szp]),
+    "pixo_b200_jpeg_progressive_scans_dev": (C.c_int, [vp, vp, C.c_size_t, vp, vp, C.c_size_t, C.c_uint32,
+                                                       C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp,
+                                                       C.c_size_t, vp, vp]),
     "pixo_b200_jpeg_encode_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                             C.c_uint32, C.c_uint32, vp, C.c_size_t, vp, vp]),
     "pixo_b200_jpeg_entropy_encode": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32,

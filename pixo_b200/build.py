@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libpixo_b200.so")
-SOURCES = ["api.cu", "jpeg_transform.cu", "jpeg_trellis.cu", "jpeg_entropy.cu", "png_filter.cu", "png_reduce.cu", "png_quantize.cu",
+SOURCES = ["api.cu", "jpeg_transform.cu", "jpeg_trellis.cu", "jpeg_entropy.cu", "jpeg_progressive.cu", "png_filter.cu", "png_reduce.cu", "png_quantize.cu",
            "jpeg_host.cpp", "png_host.cpp"]
 HEADERS = ["common.cuh", "jpeg_host.hpp", "png_host.hpp", os.path.join("..", "..", "include", "pixo_b200.h")]
 

@@ -329,9 +329,10 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
-                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis};
+                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis,
+                       &ctx->d_prog, &ctx->d_prog_raw, &ctx->d_prog_out};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
-    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant, &ctx->h_trellis};
+    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant, &ctx->h_trellis, &ctx->h_prog};
     for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->stage_events) cudaEventDestroy(ev);
@@ -793,9 +794,16 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
 // PCIe.  A frame whose scan outgrows the device buffer is coded again on the GPU with the exact
 // size; the host entropy coder (same GPU coefficient arrays) is the last resort for a faulted
 // device stage and is counted in ctx->host_fallbacks.
+// progressive (encode_progressive, src/jpeg/mod.rs:872-927): the transform writes dense natural-order
+// arrays instead of records (K3 reads them for the optimised tables, which pixo builds from the
+// plain-rounded coefficients, restart interval included); with trellis the arrays are then overwritten by
+// COEF_TRELLIS (the plain transform is skipped when no table needs it); the progressive stage codes the 7
+// scans, and the host writes SOF2, the SOS of each scan and copies the segments in between.  A group is
+// finished before the next one is computed (the stage's buffers are the context's).
 static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_each, uint32_t n_images,
                          const FrameGeometry &g, uint32_t quality, uint32_t restart_interval,
-                         bool optimize, uint8_t *out, size_t out_cap_each, size_t *out_lens)
+                         bool optimize, uint8_t *out, size_t out_cap_each, size_t *out_lens,
+                         bool progressive = false, bool trellis = false)
 {
     if (out_cap_each < 1024 + 2)  // before any GPU work is queued
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap_each);
@@ -848,6 +856,7 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
     auto coef_of = [&](int slot) { return reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * L.each; };
     std::vector<HuffTables> tables[2];
+    ProgResult prog;
     const bool out_locked = is_page_locked(out);
     DrainOnError drain(ctx);
 
@@ -859,6 +868,66 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             PIXO_TRY(h2d_copy(ctx, d_in + ((size_t)slot * G + k) * in_stride,
                               pixels + (size_t)(first + k) * len_each, len_each, ctx->copy_stream));
         PIXO_CUDA(ctx, cudaEventRecord(ev_in[slot], ctx->copy_stream));
+        return 0;
+    };
+
+    // progressive: coefficients, tables and the 7 segments of every frame of group gi (waits for the device)
+    auto compute_progressive = [&](uint32_t gi) -> int {
+        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
+        const int slot = (int)(gi & 1);
+        uint8_t *c = coef_of(slot);
+        const uint8_t *px = d_in + (size_t)slot * G * in_stride;
+        int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
+        PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_in[slot], 0));
+        if (optimize || !trellis)
+            PIXO_TRY(launch_jpeg_transform(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
+                                           chr, L.y(c), cs, cb, cr, cs, 0));
+        std::vector<HuffTables> &tb = tables[slot];
+        tb.resize(optimize ? cnt : 1);
+        if (optimize) {
+            auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
+            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
+                                           false, nullptr, d_hist));
+            PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t),
+                                           cudaMemcpyDeviceToHost, ctx->stream));
+            PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+            for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, g.has_chroma, tb[k]);
+        } else {
+            tables_from(nullptr, g.has_chroma, tb[0]);
+        }
+        if (trellis)
+            PIXO_TRY(trellis_coefficients(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
+                                          chr, L.y(c), cs, cb, cr, cs, false));
+        PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
+        std::vector<ProgTables> pt(tb.size());
+        for (size_t k = 0; k < tb.size(); ++k) {
+            const uint8_t *vals[4] = {tb[k].vals[0], tb[k].vals[1], tb[k].vals[2], tb[k].vals[3]};
+            prog_tables(tb[k].bits, vals, &pt[k]);
+        }
+        return launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, pt.data(), optimize, false, &prog);
+    };
+
+    // progressive: SOF2 headers, then per scan its SOS and its segment (from the device), EOI
+    auto finish_progressive = [&](uint32_t gi) -> int {
+        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
+        const std::vector<HuffTables> &tb = tables[(int)(gi & 1)];
+        for (uint32_t k = 0; k < cnt; ++k) {
+            const uint32_t img = first + k;
+            uint8_t *o = out + (size_t)img * out_cap_each;
+            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
+            size_t need = pos + 2;
+            for (int s = 0; s < 7; ++s) need += 10 + (size_t)prog.len[(size_t)k * 7 + s];
+            PIXO_TRY(check_room(ctx, out_cap_each, need));
+            for (int s = 0; s < 7; ++s) {
+                pos += write_sos_progressive(o + pos, s);
+                const size_t n = (size_t)prog.len[(size_t)k * 7 + s];
+                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, prog.stage + ((size_t)k * 7 + s) * prog.stage_cap, n, ctx->stream));
+                pos += n;
+            }
+            o[pos] = 0xFF;
+            o[pos + 1] = 0xD9;
+            out_lens[img] = pos + 2;
+        }
         return 0;
     };
 
@@ -988,10 +1057,15 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     PIXO_TRY(upload(0));
     for (uint32_t gi = 0; gi < ngroups; ++gi) {
         if (gi + 1 < ngroups) PIXO_TRY(upload(gi + 1));
+        if (progressive) {
+            PIXO_TRY(compute_progressive(gi));
+            PIXO_TRY(finish_progressive(gi));
+            continue;
+        }
         PIXO_TRY(compute(gi));
         if (gi > 0) PIXO_TRY(finish(gi - 1));
     }
-    PIXO_TRY(finish(ngroups - 1));
+    if (!progressive) PIXO_TRY(finish(ngroups - 1));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     drain.armed = false;
@@ -1009,7 +1083,7 @@ int pixo_b200_jpeg_encode(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixe
     if (!pixels || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     if (progressive)
         return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED,
-                         "progressive scans are outside the accelerated path (sequential entropy stage)");
+                         "progressive JPEGs are encoded by pixo_b200_jpeg_encode_progressive");
     (void)trellis_quant;  // baseline encode_scan ignores use_trellis (src/jpeg/mod.rs:1408-1563)
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     return encode_frames(ctx, pixels, pixels_len, 1, g, quality, restart_interval, optimize_huffman != 0, out,
@@ -1030,6 +1104,99 @@ int pixo_b200_jpeg_encode_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     return encode_frames(ctx, pixels, pixels_len_each, n_images, g, quality, restart_interval,
                          optimize_huffman != 0, out, out_cap_each, out_lens);
+}
+
+int pixo_b200_jpeg_encode_progressive(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len,
+                                      uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                      uint32_t subsampling, uint32_t restart_interval, uint32_t optimize_huffman,
+                                      uint32_t trellis_quant, uint8_t *out, size_t out_cap, size_t *out_len)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_encode(ctx, pixels_len, width, height, color_type, quality, subsampling, restart_interval));
+    if (!pixels || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    return encode_frames(ctx, pixels, pixels_len, 1, g, quality, restart_interval, optimize_huffman != 0, out,
+                         out_cap, out_len, true, trellis_quant != 0);
+}
+
+int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len_each,
+                                            uint32_t n_images, uint32_t width, uint32_t height,
+                                            uint32_t color_type, uint32_t quality, uint32_t subsampling,
+                                            uint32_t restart_interval, uint32_t optimize_huffman,
+                                            uint32_t trellis_quant, uint8_t *out, size_t out_cap_each,
+                                            size_t *out_lens)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_encode(ctx, pixels_len_each, width, height, color_type, quality, subsampling,
+                             restart_interval));
+    if (!pixels || !out || !out_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (n_images == 0) return 0;
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    return encode_frames(ctx, pixels, pixels_len_each, n_images, g, quality, restart_interval,
+                         optimize_huffman != 0, out, out_cap_each, out_lens, true, trellis_quant != 0);
+}
+
+int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
+                                         const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
+                                         uint32_t n_frames, uint32_t width, uint32_t height, uint32_t color_type,
+                                         uint32_t subsampling, const uint8_t *dht, uint8_t *d_out,
+                                         size_t out_cap_each, uint64_t *d_scan_len, uint32_t *d_overflow)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
+    const bool chroma = color_type != PIXO_B200_GRAY;
+    if (!d_y || !d_out || !d_scan_len || !d_overflow || (chroma && (!d_cb || !d_cr)))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    auto mis = [](const int16_t *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
+    if (mis(d_y) || (chroma && (mis(d_cb) || mis(d_cr))))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient arrays must be 16-byte aligned");
+    if ((y_stride & 7) || (chroma && (c_stride & 7)))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient strides must be multiples of 8 elements");
+    if (n_frames > 1 && (y_stride < g.ny * 64 || (chroma && c_stride < g.nc * 64)))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "coefficient strides must hold a frame's blocks (%zu / %zu elements)", g.ny * 64, g.nc * 64);
+    ProgTables T;
+    {
+        HuffTables std_t;
+        uint8_t bits[4][16];
+        const uint8_t *vals[4];
+        if (dht) {
+            for (int k = 0; k < 4; ++k) {
+                memcpy(bits[k], dht + k * 272, 16);
+                vals[k] = dht + k * 272 + 16;
+            }
+        } else {
+            huff_standard(std_t);
+            for (int k = 0; k < 4; ++k) {
+                memcpy(bits[k], std_t.bits[k], 16);
+                vals[k] = std_t.vals[k];
+            }
+        }
+        if (!prog_tables(bits, vals, &T))
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                             "Huffman table: more than 256 values, or a code that does not fit its length");
+    }
+    if (n_frames == 0) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    // The splice kernels take one grid row per segment: at most 8192 frames (57 344 segments) per pass.
+    // More frames are checked first, so that a rejected coefficient leaves every output untouched.
+    constexpr uint32_t kPass = 8192;
+    const int16_t *cb = chroma ? d_cb : nullptr, *cr = chroma ? d_cr : nullptr;
+    auto at = [](const int16_t *a, size_t stride, uint32_t i0) { return a ? a + (size_t)i0 * stride : nullptr; };
+    ProgResult res;
+    if (n_frames > kPass)
+        for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass)
+            PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
+                                        c_stride, std::min(kPass, n_frames - i0), g, &T, false, true, &res));
+    for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass) {
+        const uint32_t cnt = std::min(kPass, n_frames - i0);
+        PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
+                                    c_stride, cnt, g, &T, false, false, &res));
+        PIXO_TRY(launch_progressive_pack(ctx, res, cnt, d_out + (size_t)i0 * out_cap_each, out_cap_each,
+                                         d_scan_len + (size_t)i0 * 7, d_overflow + i0));
+    }
+    return 0;
 }
 
 int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,

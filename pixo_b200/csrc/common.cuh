@@ -89,6 +89,30 @@ struct SegPlan {
     size_t raw_bytes, off_bits, off_tails, raw_total;      // layout of the raw area: strings, then the segments' bit counts and tails
 };
 
+// Huffman tables of the progressive scans as get_code_from_table sees them: (code << 8) | length per
+// symbol, pixo's fallback (0, 4) for a symbol the table does not hold.  DC categories 0..15.
+struct ProgTables {
+    uint32_t dc[2][16];
+    uint32_t ac[2][256];
+};
+
+// Device scratch of the progressive stage for n frames (jpeg_progressive.cu), offsets in bytes
+struct ProgLayout {
+    uint64_t nb[7];
+    uint32_t tile_base[8];
+    uint64_t blk_base[8];
+    size_t off_status, off_blen, off_flag, off_tile_last, off_tile_carry, off_tile_bits, off_tile_off, off_bits, off_tables, total;
+};
+
+// The 7 stuffed segments of each of n frames: segment q = frame * 7 + scan at stage + q * stage_cap, its
+// length in len[q] (host) and d_len[q] (device)
+struct ProgResult {
+    uint8_t *stage = nullptr;
+    size_t stage_cap = 0;
+    uint64_t *d_len = nullptr;
+    std::vector<uint64_t> len;
+};
+
 }  // namespace pixo
 
 struct pixo_b200_ctx {
@@ -109,6 +133,8 @@ struct pixo_b200_ctx {
     pixo::Scratch d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
     pixo::Scratch d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
     pixo::Scratch d_trellis, h_trellis;          // JPEG trellis: status word + f32 DCT blocks; its status on the host
+    pixo::Scratch d_prog, d_prog_raw, d_prog_out, h_prog;   // JPEG progressive scans: per-block state, raw strings,
+                                                            // stuffed segments; bit counts / lengths on the host
     pixo::Scratch h_in, h_out, h_misc, h_red, h_quant;
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
@@ -195,5 +221,19 @@ int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_b
                        uint32_t *d_flags);
 // bytes a band's raw buffer needs for the band as one string of the usual size, with its trailer
 size_t band_raw_bytes(const FrameGeometry &g);
+// n whole raw strings of raw_cap bytes each, spliced on their own (no segments): the raw area holds the
+// strings, then their bit counts (off_bits) and tails (off_tails); the splice scratch is `total` bytes
+SegPlan splice_plan(uint32_t n, size_t raw_cap);
+int launch_splice(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
+                  uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow);
+
+// progressive scans (jpeg_progressive.cu)
+bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
+ProgLayout prog_layout(const FrameGeometry &g, uint32_t n);
+int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
+                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
+                       const ProgTables *T, bool per_frame, bool check_only, ProgResult *res);
+int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
+                            uint64_t *d_scan_len, uint32_t *d_overflow);
 
 }  // namespace pixo

@@ -1490,4 +1490,21 @@ int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_b
                            last, d_base, d_out, out_cap, d_out_len, d_flags);
 }
 
+SegPlan splice_plan(uint32_t n, size_t raw_cap)
+{
+    SegPlan p;
+    p.S = 1;
+    p.seg_mcus = p.last_mcus = 0;
+    lay_out(p, n, 1, raw_cap);
+    return p;
+}
+
+// The progressive scans' strings: each a whole stream of its own (base bit 0, 1-padded at its end)
+int launch_splice(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
+                  uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow)
+{
+    return splice_segments(ctx, n, sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap, d_out_len,
+                           d_overflow);
+}
+
 }  // namespace pixo

@@ -451,8 +451,11 @@ bool huff_from_histogram(const uint64_t hist[536], bool has_chroma, HuffTables &
     return true;
 }
 
-size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
-                     const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval)
+// SOI..DRI with the frame header `sof` (0xFFC0 baseline, 0xFFC2 progressive: write_sof_marker,
+// src/jpeg/mod.rs:498-560)
+static size_t write_frame_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
+                                  const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval,
+                                  unsigned sof)
 {
     uint8_t *p = out;
     auto u8 = [&](unsigned v) { *p++ = (uint8_t)v; };
@@ -464,7 +467,7 @@ size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[
     u16(0xFFDB); u16(67); u8(0); memcpy(p, lum_zz, 64); p += 64;
     u16(0xFFDB); u16(67); u8(1); memcpy(p, chr_zz, 64); p += 64;
     const int ncomp = g.has_chroma ? 3 : 1;
-    u16(0xFFC0); u16(8 + 3 * ncomp); u8(8); u16(g.height & 0xFFFF); u16(g.width & 0xFFFF); u8(ncomp);
+    u16(sof); u16(8 + 3 * ncomp); u8(8); u16(g.height & 0xFFFF); u16(g.width & 0xFFFF); u8(ncomp);
     if (ncomp == 1) { u8(1); u8(0x11); u8(0); }
     else {
         u8(1); u8(g.subsampling == PIXO_B200_S420 ? 0x22 : 0x11); u8(0);
@@ -478,11 +481,36 @@ size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[
         memcpy(p, t.vals[k], (size_t)t.nvals[k]); p += t.nvals[k];
     }
     if (restart_interval) { u16(0xFFDD); u16(4); u16(restart_interval & 0xFFFF); }
+    return (size_t)(p - out);
+}
+
+size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
+                     const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval)
+{
+    uint8_t *p = out + write_frame_headers(out, g, lum_zz, chr_zz, t, restart_interval, 0xFFC0);
+    auto u8 = [&](unsigned v) { *p++ = (uint8_t)v; };
+    auto u16 = [&](unsigned v) { *p++ = (uint8_t)(v >> 8); *p++ = (uint8_t)v; };
+    const int ncomp = g.has_chroma ? 3 : 1;
     u16(0xFFDA); u16(6 + 2 * ncomp); u8(ncomp);
     if (ncomp == 1) { u8(1); u8(0x00); }
     else { u8(1); u8(0x00); u8(2); u8(0x11); u8(3); u8(0x11); }
     u8(0); u8(63); u8(0);
     return (size_t)(p - out);
+}
+
+size_t write_headers_progressive(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
+                                 const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval)
+{
+    return write_frame_headers(out, g, lum_zz, chr_zz, t, restart_interval, 0xFFC2);
+}
+
+size_t write_sos_progressive(uint8_t *out, int scan)
+{
+    static const uint8_t comp[7] = {0, 1, 2, 0, 0, 1, 2}, ss[7] = {0, 0, 0, 1, 11, 1, 1}, se[7] = {0, 0, 0, 10, 63, 63, 63};
+    const uint8_t sos[10] = {0xFF, 0xDA, 0, 8, 1, (uint8_t)(comp[scan] + 1), (uint8_t)(comp[scan] ? 0x11 : 0x00),
+                             ss[scan], se[scan], 0};
+    memcpy(out, sos, sizeof sos);
+    return sizeof sos;
 }
 
 void parallel_jobs(int n, int threads, void (*fn)(int, void *), void *arg)

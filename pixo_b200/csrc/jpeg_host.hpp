@@ -41,6 +41,13 @@ bool huff_from_histogram(const uint64_t hist[536], bool has_chroma, HuffTables &
 size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
                      const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval);
 
+// Progressive files (encode_into with options.progressive, src/jpeg/mod.rs:395-410): SOI..DRI with SOF2,
+// and the SOS of scan 0..6 of simple_progressive_script (write_sos_progressive, :650-683: one component,
+// table selector 0x00 for Y and 0x11 for chroma, Ah = Al = 0; gray frames get the chroma SOS too).
+size_t write_headers_progressive(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],
+                                 const uint8_t chr_zz[64], const HuffTables &t, uint32_t restart_interval);
+size_t write_sos_progressive(uint8_t *out, int scan);   // 10 bytes
+
 // encode_scan (src/jpeg/mod.rs:1408-1563) over precomputed coefficient arrays (natural or
 // zig-zag order), multi-threaded over MCU segments; byte-identical to the sequential
 // reference.  Returns bytes written, or (size_t)-1 when `cap` is too small.

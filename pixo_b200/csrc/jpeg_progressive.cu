@@ -1,0 +1,578 @@
+// jpeg_progressive.cu — the progressive scans of pixo's max preset ON the GPU: the 7 scans of
+// simple_progressive_script, each coded into a stuffed, 1-padded entropy-coded segment of its own.
+//
+// Restates, bit for bit (quirks included):
+//   encode_progressive                  src/jpeg/mod.rs:872-927
+//   encode_dc_scan / encode_ac_first_scan src/jpeg/mod.rs:1248-1365
+//   simple_progressive_script           src/jpeg/progressive.rs:98-110
+//   encode_ac_first / flush_eob_run     src/jpeg/progressive.rs:141-210, 313-345
+//   get_code_from_table                 src/jpeg/progressive.rs:363-380 (a missing symbol is (0, 4))
+//   BitWriterMsb                        src/bits.rs:195-278
+//
+// A scan is one bit stream over ONE component's blocks, in the order of its coefficient array (MCU
+// order for 4:2:0 Y, as pixo writes it).  DC scans code each block's DC against the previous block of
+// the array (never reset).  AC scans (Ss > 0) carry one dependency across blocks, the EOB run: with p the
+// previous non-empty block (in the band [Ss, Se]) and init = 1 when p's last non-zero lies below Se,
+// the run pending before block b is (init + empties between p and b) mod 0x7FFF, and an empty block
+// emits a 0x7FFF run exactly where that count reaches a multiple of 0x7FFF.  "p and its init" is a
+// running maximum over (index, init), so every block's bits follow from a prefix over tiles.
+//
+// One thread per block, tiles of PT blocks; a batch of frames is one launch of each kernel:
+//   k_prog_measure  code length of the block's own symbols, its empty / init flags, the tile's last
+//                   non-empty block; coefficients outside +-16383 set status bit 0
+//   k_prog_carry    per stream: exclusive running maximum of the tiles' last non-empty blocks
+//   k_prog_count    per block: the EOB-run flushes it emits, added to its length; tile bit totals
+//   k_prog_offsets  per stream: exclusive prefix of the tile totals (u64) and the stream's bit count
+//   (host)          reads the bit counts back: the raw area is then sized exactly, so no string can
+//                   outgrow it
+//   k_prog_emit     per block: its bit offset (tile prefix + CTA scan), its bits OR-ed into the
+//                   zeroed raw string (MSB first)
+//   k_seg_*         (jpeg_entropy.cu) splice every raw string into stuffed, 1-padded bytes
+//   k_prog_pack     (device entry) the 7 segments of a frame back to back in the caller's slot
+// Nothing spins on another CTA, so no step can hang: a fault is a CUDA error.
+#include <string.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+#include "jpeg_host.hpp"
+
+namespace pixo {
+namespace {
+
+constexpr int PT = 256;              // blocks per tile == threads per CTA
+constexpr int NSCAN = 7;
+constexpr uint32_t EOBRUN_MAX = 0x7FFF;
+constexpr int kComp[NSCAN] = {0, 1, 2, 0, 0, 1, 2};   // (Ss, Se) of the scans: see scan_ss / scan_se
+
+struct ProgParams {
+    const int16_t *arr[3];           // Y, Cb, Cr: natural order, compute_all_coefficients' layout
+    size_t stride[3];                // int16 elements between frames
+    uint64_t nb[NSCAN];              // blocks of each scan's component
+    uint32_t tile_base[NSCAN + 1];   // first tile of each scan inside a frame; [NSCAN] = tiles per frame
+    uint64_t blk_base[NSCAN + 1];    // first block record of each scan inside a frame; [NSCAN] = per frame
+    uint32_t n;                      // frames
+    uint32_t *blen;                  // [n][blocks]: the block's own bits (measure), then with its flushes (count)
+    uint8_t *flag;                   // [n][blocks]: bit 0 non-empty, bit 1 its last non-zero lies below Se
+    uint32_t *tile_last;             // [n][tiles]: encoded last non-empty block of the tile (see enc_of), 0 = none
+    uint32_t *tile_carry;            // [n][tiles]: ... of every earlier tile of the stream
+    uint32_t *tile_bits;             // [n][tiles]
+    unsigned long long *tile_off;    // [n][tiles]: bits of the stream before the tile
+    unsigned long long *bits;        // [n * NSCAN]: bits of each stream
+    uint32_t *raw;                   // [n * NSCAN][raw_cap / 4] big-endian words, zeroed before k_prog_emit
+    unsigned long long raw_words;    // words per stream
+    uint32_t *status;                // bit 0: a coefficient outside -16383..16383
+    const ProgTables *tables;        // [n] per frame, or [1] for every frame
+    uint32_t tables_per_frame;       // 1 or 0
+};
+
+// tile t of the batch -> frame, scan, tile inside the scan
+struct TileId {
+    uint32_t frame, scan, tile;
+};
+__device__ __forceinline__ TileId tile_id(const ProgParams &P, uint32_t t)
+{
+    TileId id;
+    const uint32_t per = P.tile_base[NSCAN];
+    id.frame = t / per;
+    const uint32_t r = t - id.frame * per;
+    id.scan = 0;
+#pragma unroll
+    for (int s = 1; s < NSCAN; ++s)
+        if (r >= P.tile_base[s]) id.scan = s;
+    id.tile = r - P.tile_base[id.scan];
+    return id;
+}
+
+__device__ __forceinline__ int scan_comp(uint32_t s) { return s == 0 || s == 3 || s == 4 ? 0 : (s == 1 || s == 5 ? 1 : 2); }
+__device__ __forceinline__ int scan_ss(uint32_t s) { return s < 3 ? 0 : (s == 4 ? 11 : 1); }
+__device__ __forceinline__ int scan_se(uint32_t s) { return s < 3 ? 0 : (s == 3 ? 10 : 63); }
+
+// (index + 1) << 1 | init of a non-empty block; larger == later, 0 == none
+__device__ __forceinline__ uint32_t enc_of(uint64_t b, uint8_t flag)
+{
+    return (flag & 1u) ? (uint32_t)(((b + 1) << 1) | ((flag >> 1) & 1u)) : 0u;
+}
+
+template <typename T, typename Op>
+__device__ __forceinline__ T cta_scan_excl(T x, T identity, T *sh, T *total, Op op)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T inc = x;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T v = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc = op(inc, v);
+    }
+    T ex = __shfl_up_sync(0xffffffffu, inc, 1);
+    if (lane == 0) ex = identity;
+    __syncthreads();
+    if (lane == 31) sh[warp] = inc;
+    __syncthreads();
+    T before = identity, all = identity;
+    for (int w = 0; w < (int)(blockDim.x / 32); ++w) {
+        const T v = sh[w];
+        if (w < warp) before = op(before, v);
+        all = op(all, v);
+    }
+    *total = all;
+    return op(before, ex);
+}
+
+struct MaxOp {
+    __device__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
+};
+struct AddOp {
+    template <typename T>
+    __device__ T operator()(T a, T b) const { return a + b; }
+};
+
+__device__ __forceinline__ void load_tables(const ProgParams &P, uint32_t frame, ProgTables &T)
+{
+    const uint32_t *src = reinterpret_cast<const uint32_t *>(P.tables + (P.tables_per_frame ? frame : 0));
+    uint32_t *dst = reinterpret_cast<uint32_t *>(&T);
+    for (int k = threadIdx.x; k < (int)(sizeof(ProgTables) / 4); k += blockDim.x) dst[k] = src[k];
+    __syncthreads();
+}
+
+__device__ __forceinline__ uint32_t category(uint32_t a) { return 32u - (uint32_t)__clz((int)a); }
+
+// One block's own symbols (no EOB-run flush), fed to put(value, nbits) with value's nbits <= 31:
+// DC scans the DC difference, AC scans the (run, size) symbols of [ss, last] with their ZRLs.
+// v: the block, natural order, two coefficients per word.  Returns false when a coefficient of the
+// scan's band lies outside -16383..16383.
+template <typename Put>
+__device__ __forceinline__ bool code_own(const uint32_t (&v)[32], int prev_dc, int ss, int last, bool dc_scan,
+                                         const uint32_t *dctab, const uint32_t *actab, Put put)
+{
+    auto coef = [&](int nat) { return (int)(int16_t)(v[nat >> 1] >> (16 * (nat & 1))); };
+    if (dc_scan) {
+        const int dc = coef(0);
+        const int diff = (int)(int16_t)(dc - prev_dc);          // pixo's i16 difference
+        const uint32_t a = (uint32_t)abs(diff), cat = category(a);
+        const uint32_t e = dctab[min(cat, 15u)];   // (16 only for rejected input)
+        const uint32_t amp = (diff < 0 ? (uint32_t)(diff - 1) : (uint32_t)diff) & ((1u << cat) - 1u);
+        put(((e >> 8) << cat) | amp, (e & 0xFFu) + cat);
+        return dc >= -16383 && dc <= 16383;
+    }
+    uint32_t run = 0;
+    bool ok = true;
+#pragma unroll
+    for (int k = 1; k < 64; ++k) {
+        if (k < ss || k > last) continue;
+        const int c = coef(zz_nat(k));
+        if (c == 0) { ++run; continue; }
+        ok &= c >= -16383 && c <= 16383;
+        while (run >= 16u) {
+            const uint32_t z = actab[0xF0];
+            put(z >> 8, z & 0xFFu);
+            run -= 16u;
+        }
+        const uint32_t a = (uint32_t)abs(c), cat = category(a);
+        const uint32_t e = actab[(run << 4) | min(cat, 15u)];
+        const uint32_t amp = (c < 0 ? (uint32_t)(c - 1) : (uint32_t)c) & ((1u << cat) - 1u);
+        put(((e >> 8) << cat) | amp, (e & 0xFFu) + cat);
+        run = 0;
+    }
+    return ok;
+}
+
+// flush_eob_run of a run r (1..0x7FFF): symbol (log2 r) << 4, then the low log2 r bits of r
+template <typename Put>
+__device__ __forceinline__ void code_eobrun(uint32_t r, const uint32_t *actab, Put put)
+{
+    const uint32_t nb = 31u - (uint32_t)__clz((int)r);
+    const uint32_t e = actab[nb << 4];
+    put(((e >> 8) << nb) | (r - (1u << nb)), (e & 0xFFu) + nb);
+}
+
+// The EOB-run flushes block b emits, in order: `before` (a non-empty block: the pending run; an empty
+// one: 0x7FFF when its count reaches it) and `after` (the stream's last block: whatever is still pending).
+// excl: enc_of of the nearest earlier non-empty block of the stream, 0 = none.
+struct Flushes {
+    uint32_t before, after;
+};
+__device__ __forceinline__ Flushes flushes_of(uint64_t b, uint64_t nb, uint8_t flag, uint32_t excl)
+{
+    const uint64_t p1 = excl >> 1;               // index of p + 1, 0 = none
+    const uint64_t init = excl & 1u;
+    const uint64_t empties = b - p1;             // empty blocks between p and b
+    Flushes f{0, 0};
+    uint32_t pending;
+    if (flag & 1u) {
+        f.before = (uint32_t)((init + empties) % EOBRUN_MAX);
+        pending = (flag >> 1) & 1u;
+    } else {
+        const uint64_t cnt = init + empties + 1;
+        pending = (uint32_t)(cnt % EOBRUN_MAX);
+        if (pending == 0) f.before = EOBRUN_MAX;
+    }
+    if (b + 1 == nb) f.after = pending;
+    return f;
+}
+
+// Loads block b (16-byte aligned, natural order) and finds its last non-zero in [ss, se] (ss - 1: none).
+__device__ __forceinline__ int load_block(const int16_t *blk, int ss, int se, bool dc_scan, uint32_t (&v)[32])
+{
+    if (dc_scan) {
+#pragma unroll
+        for (int k = 0; k < 32; ++k) v[k] = 0;
+        v[0] = (uint16_t)blk[0];
+        return 0;
+    }
+    const uint4 *q = reinterpret_cast<const uint4 *>(blk);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint4 w = q[k];
+        v[4 * k] = w.x; v[4 * k + 1] = w.y; v[4 * k + 2] = w.z; v[4 * k + 3] = w.w;
+    }
+    int last = ss - 1;
+#pragma unroll
+    for (int k = 1; k < 64; ++k) {
+        const int nat = zz_nat(k);
+        if (k >= ss && k <= se && (int16_t)(v[nat >> 1] >> (16 * (nat & 1))) != 0) last = k;
+    }
+    return last;
+}
+
+__global__ void __launch_bounds__(PT) k_prog_measure(const __grid_constant__ ProgParams P)
+{
+    __shared__ ProgTables T;
+    __shared__ uint32_t sh[PT / 32];
+    const TileId id = tile_id(P, blockIdx.x);
+    load_tables(P, id.frame, T);
+    const int comp = scan_comp(id.scan), ss = scan_ss(id.scan), se = scan_se(id.scan);
+    const bool dc_scan = ss == 0;
+    const int lum = comp == 0 ? 0 : 1;
+    const uint64_t nb = P.nb[id.scan];
+    const uint64_t b = (uint64_t)id.tile * PT + threadIdx.x;
+    uint32_t len = 0, enc = 0;
+    uint8_t flag = 0;
+    if (b < nb) {
+        const int16_t *blk = P.arr[comp] + (size_t)id.frame * P.stride[comp] + b * 64;
+        uint32_t v[32];
+        const int last = load_block(blk, ss, se, dc_scan, v);
+        const int prev = (dc_scan && b) ? blk[-64] : 0;
+        bool ok = true;
+        if (dc_scan || last >= ss)
+            ok = code_own(v, prev, ss, last, dc_scan, T.dc[lum], T.ac[lum], [&](uint32_t, uint32_t n) { len += n; });
+        if (!dc_scan && last >= ss) flag = (uint8_t)(1u | (last < se ? 2u : 0u));
+        if (!ok) atomicOr(P.status, 1u);
+        const size_t r = (size_t)id.frame * P.blk_base[NSCAN] + P.blk_base[id.scan] + b;
+        P.blen[r] = len;
+        P.flag[r] = flag;
+        enc = enc_of(b, flag);
+    }
+    uint32_t tot;
+    cta_scan_excl<uint32_t>(enc, 0u, sh, &tot, MaxOp());
+    if (threadIdx.x == 0) P.tile_last[(size_t)id.frame * P.tile_base[NSCAN] + P.tile_base[id.scan] + id.tile] = tot;
+}
+
+// One CTA per stream: exclusive running maximum of tile_last over the stream's tiles
+__global__ void __launch_bounds__(PT) k_prog_carry(const __grid_constant__ ProgParams P)
+{
+    __shared__ uint32_t sh[PT / 32];
+    const uint32_t frame = blockIdx.x / NSCAN, s = blockIdx.x % NSCAN;
+    const uint32_t nt = P.tile_base[s + 1] - P.tile_base[s];
+    const size_t base = (size_t)frame * P.tile_base[NSCAN] + P.tile_base[s];
+    uint32_t run = 0;
+    for (uint32_t t0 = 0; t0 < nt; t0 += PT) {
+        const uint32_t t = t0 + threadIdx.x;
+        const uint32_t x = t < nt ? P.tile_last[base + t] : 0u;
+        uint32_t tot;
+        const uint32_t ex = cta_scan_excl<uint32_t>(x, 0u, sh, &tot, MaxOp());
+        if (t < nt) P.tile_carry[base + t] = max(run, ex);
+        run = max(run, tot);
+    }
+}
+
+// Per block: own bits + its flushes (AC scans) -> blen; tile totals
+__global__ void __launch_bounds__(PT) k_prog_count(const __grid_constant__ ProgParams P)
+{
+    __shared__ ProgTables T;
+    __shared__ uint32_t sh[PT / 32];
+    const TileId id = tile_id(P, blockIdx.x);
+    load_tables(P, id.frame, T);
+    const int comp = scan_comp(id.scan);
+    const bool dc_scan = scan_ss(id.scan) == 0;
+    const int lum = comp == 0 ? 0 : 1;
+    const uint64_t nb = P.nb[id.scan];
+    const uint64_t b = (uint64_t)id.tile * PT + threadIdx.x;
+    const size_t tix = (size_t)id.frame * P.tile_base[NSCAN] + P.tile_base[id.scan] + id.tile;
+    const size_t r = (size_t)id.frame * P.blk_base[NSCAN] + P.blk_base[id.scan] + b;
+    const bool live = b < nb;
+    const uint8_t flag = live ? P.flag[r] : 0;
+    uint32_t len = live ? P.blen[r] : 0u, tot;
+    if (!dc_scan) {   // (uniform per CTA)
+        const uint32_t ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(b, flag), 0u, sh, &tot, MaxOp()));
+        if (live) {
+            const Flushes f = flushes_of(b, nb, flag, ex);
+            auto add = [&](uint32_t, uint32_t n) { len += n; };
+            if (f.before) code_eobrun(f.before, T.ac[lum], add);
+            if (f.after) code_eobrun(f.after, T.ac[lum], add);
+            P.blen[r] = len;
+        }
+    }
+    uint32_t sum;
+    cta_scan_excl<uint32_t>(len, 0u, sh, &sum, AddOp());
+    if (threadIdx.x == 0) P.tile_bits[tix] = sum;
+}
+
+// One CTA per stream: exclusive prefix of the tile totals, the stream's bit count
+__global__ void __launch_bounds__(PT) k_prog_offsets(const __grid_constant__ ProgParams P)
+{
+    __shared__ unsigned long long sh[PT / 32];
+    const uint32_t frame = blockIdx.x / NSCAN, s = blockIdx.x % NSCAN;
+    const uint32_t nt = P.tile_base[s + 1] - P.tile_base[s];
+    const size_t base = (size_t)frame * P.tile_base[NSCAN] + P.tile_base[s];
+    unsigned long long run = 0;
+    for (uint32_t t0 = 0; t0 < nt; t0 += PT) {
+        const uint32_t t = t0 + threadIdx.x;
+        const unsigned long long x = t < nt ? P.tile_bits[base + t] : 0ull;
+        unsigned long long tot;
+        const unsigned long long ex = cta_scan_excl<unsigned long long>(x, 0ull, sh, &tot, AddOp());
+        if (t < nt) P.tile_off[base + t] = run + ex;
+        run += tot;
+    }
+    if (threadIdx.x == 0) P.bits[blockIdx.x] = run;
+}
+
+__device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
+
+// Per block: flushes and symbols OR-ed into the stream's zeroed raw words at the block's bit offset
+__global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgParams P)
+{
+    __shared__ ProgTables T;
+    __shared__ uint32_t sh[PT / 32];
+    __shared__ unsigned long long sh64[PT / 32];
+    const TileId id = tile_id(P, blockIdx.x);
+    load_tables(P, id.frame, T);
+    const int comp = scan_comp(id.scan), ss = scan_ss(id.scan), se = scan_se(id.scan);
+    const bool dc_scan = ss == 0;
+    const int lum = comp == 0 ? 0 : 1;
+    const uint64_t nb = P.nb[id.scan];
+    const uint64_t b = (uint64_t)id.tile * PT + threadIdx.x;
+    const size_t tix = (size_t)id.frame * P.tile_base[NSCAN] + P.tile_base[id.scan] + id.tile;
+    const size_t r = (size_t)id.frame * P.blk_base[NSCAN] + P.blk_base[id.scan] + b;
+    const bool live = b < nb;
+    const uint8_t flag = live ? P.flag[r] : 0;
+    uint32_t ex = 0, tot;
+    if (!dc_scan) ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(b, flag), 0u, sh, &tot, MaxOp()));
+    const unsigned long long len = live ? P.blen[r] : 0ull;
+    unsigned long long all;
+    unsigned long long pos = P.tile_off[tix] + cta_scan_excl<unsigned long long>(len, 0ull, sh64, &all, AddOp());
+    if (!live || len == 0) return;
+    uint32_t *words = P.raw + (size_t)(id.frame * NSCAN + id.scan) * P.raw_words;
+    auto put = [&](uint32_t val, uint32_t n) {
+        if (n == 0) return;
+        const uint32_t al = val << (32u - n);
+        const uint64_t w = pos >> 5;
+        const uint32_t o = (uint32_t)(pos & 31u);
+        atomicOr(words + w, bswap32(al >> o));
+        if (o + n > 32u) atomicOr(words + w + 1, bswap32(al << (32u - o)));
+        pos += n;
+    };
+    const int16_t *blk = P.arr[comp] + (size_t)id.frame * P.stride[comp] + b * 64;
+    uint32_t v[32];
+    const int last = load_block(blk, ss, se, dc_scan, v);
+    const int prev = (dc_scan && b) ? blk[-64] : 0;
+    Flushes f{0, 0};
+    if (!dc_scan) f = flushes_of(b, nb, flag, ex);
+    if (f.before) code_eobrun(f.before, T.ac[lum], put);
+    if (dc_scan || last >= ss) code_own(v, prev, ss, last, dc_scan, T.dc[lum], T.ac[lum], put);
+    if (f.after) code_eobrun(f.after, T.ac[lum], put);
+}
+
+// Per frame: the 7 spliced segments back to back at out + frame * out_cap, their lengths, and
+// overflow bit 0 (nothing copied) when they do not fit
+// (ctas CTAs per segment, sized by the host from the longest segment)
+__global__ void __launch_bounds__(PT) k_prog_pack(uint32_t ctas, const uint8_t *stage, unsigned long long stage_cap,
+                                                  const unsigned long long *seg_len, uint8_t *out,
+                                                  unsigned long long out_cap, unsigned long long *scan_len,
+                                                  uint32_t *overflow)
+{
+    const uint32_t frame = blockIdx.y, s = blockIdx.x / ctas, part = blockIdx.x % ctas;
+    const unsigned long long *L = seg_len + (size_t)frame * NSCAN;
+    unsigned long long off = 0, total = 0;
+    for (uint32_t k = 0; k < NSCAN; ++k) {
+        if (k < s) off += L[k];
+        total += L[k];
+    }
+    if (part == 0 && threadIdx.x == 0) {
+        scan_len[(size_t)frame * NSCAN + s] = L[s];
+        if (s == 0) overflow[frame] = total > out_cap ? 1u : 0u;
+    }
+    if (total > out_cap) return;
+    const uint8_t *src = stage + ((size_t)frame * NSCAN + s) * stage_cap;
+    uint8_t *dst = out + (size_t)frame * out_cap + off;
+    for (unsigned long long j = (unsigned long long)part * PT + threadIdx.x; j < L[s]; j += (unsigned long long)ctas * PT)
+        dst[j] = src[j];
+}
+
+}  // namespace
+
+// get_code_from_table over each table: (code << 8) | length per symbol, pixo's (0, 4) for a symbol the
+// table does not hold.  False when a table holds more than 256 values or a code does not fit its length.
+bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T)
+{
+    memset(T, 0, sizeof *T);
+    for (int k = 0; k < 4; ++k) {
+        uint32_t *dst = k < 2 ? T->dc[k] : T->ac[k - 2];
+        const int nsym = k < 2 ? 16 : 256;
+        for (int s = 0; s < nsym; ++s) dst[s] = 4u;
+        int total = 0;
+        for (int l = 0; l < 16; ++l) total += bits[k][l];
+        if (total > 256) return false;
+        uint32_t code = 0;
+        int idx = 0;
+        std::vector<bool> seen(256, false);
+        for (int l = 0; l < 16; ++l) {
+            for (int c = 0; c < bits[k][l]; ++c, ++idx, ++code) {
+                if (code >= (1u << (l + 1))) return false;
+                const uint8_t sym = vals[k][idx];
+                if (seen[sym]) continue;   // the first entry of a symbol wins
+                seen[sym] = true;
+                if (sym < nsym) dst[sym] = (code << 8) | (uint32_t)(l + 1);
+            }
+            code <<= 1;
+        }
+    }
+    return true;
+}
+
+ProgLayout prog_layout(const FrameGeometry &g, uint32_t n)
+{
+    ProgLayout L;
+    uint32_t tb = 0;
+    uint64_t bb = 0;
+    for (int s = 0; s < NSCAN; ++s) {
+        L.nb[s] = kComp[s] == 0 ? g.ny : g.nc;
+        L.tile_base[s] = tb;
+        L.blk_base[s] = bb;
+        tb += (uint32_t)((L.nb[s] + PT - 1) / PT);
+        bb += L.nb[s];
+    }
+    L.tile_base[NSCAN] = tb;
+    L.blk_base[NSCAN] = bb;
+    auto a256 = [](size_t v) { return (v + 255) / 256 * 256; };
+    const size_t tiles = (size_t)n * tb, blocks = (size_t)n * bb;
+    size_t o = 0;
+    L.off_status = o; o += 256;
+    L.off_blen = o; o += a256(blocks * 4);
+    L.off_flag = o; o += a256(blocks);
+    L.off_tile_last = o; o += a256(tiles * 4);
+    L.off_tile_carry = o; o += a256(tiles * 4);
+    L.off_tile_bits = o; o += a256(tiles * 4);
+    L.off_tile_off = o; o += a256(tiles * 8);
+    L.off_bits = o; o += a256((size_t)n * NSCAN * 8);
+    L.off_tables = o; o += a256((size_t)n * sizeof(ProgTables));
+    L.total = o;
+    return L;
+}
+
+// Measure (and with !check_only, code) the 7 scans of n frames.  Waits for the device twice: after the
+// bit counts (to size the raw strings exactly) and after the splice (segment lengths to the host).
+int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
+                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
+                       const ProgTables *T, bool per_frame, bool check_only, ProgResult *res)
+{
+    cudaStream_t st = ctx->stream;
+    const ProgLayout L = prog_layout(g, n);
+    PIXO_TRY(ensure_dev(ctx, ctx->d_prog, L.total));
+    auto *base = static_cast<uint8_t *>(ctx->d_prog.ptr);
+    ProgParams P;
+    memset(&P, 0, sizeof P);
+    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
+    P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
+    for (int s = 0; s < NSCAN; ++s) P.nb[s] = L.nb[s];
+    for (int s = 0; s <= NSCAN; ++s) { P.tile_base[s] = L.tile_base[s]; P.blk_base[s] = L.blk_base[s]; }
+    P.n = n;
+    P.status = reinterpret_cast<uint32_t *>(base + L.off_status);
+    P.blen = reinterpret_cast<uint32_t *>(base + L.off_blen);
+    P.flag = base + L.off_flag;
+    P.tile_last = reinterpret_cast<uint32_t *>(base + L.off_tile_last);
+    P.tile_carry = reinterpret_cast<uint32_t *>(base + L.off_tile_carry);
+    P.tile_bits = reinterpret_cast<uint32_t *>(base + L.off_tile_bits);
+    P.tile_off = reinterpret_cast<unsigned long long *>(base + L.off_tile_off);
+    P.bits = reinterpret_cast<unsigned long long *>(base + L.off_bits);
+    P.tables = reinterpret_cast<const ProgTables *>(base + L.off_tables);
+    P.tables_per_frame = per_frame ? 1u : 0u;
+    const uint64_t tiles = (uint64_t)n * L.tile_base[NSCAN];
+    if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive stage: too many blocks per call");
+    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(base + L.off_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
+    if (tiles) {
+        k_prog_measure<<<(unsigned)tiles, PT, 0, st>>>(P);
+        k_prog_carry<<<n * NSCAN, PT, 0, st>>>(P);
+        k_prog_count<<<(unsigned)tiles, PT, 0, st>>>(P);
+    }
+    k_prog_offsets<<<n * NSCAN, PT, 0, st>>>(P);
+    ctx->launches += tiles ? 4 : 1;
+    PIXO_CUDA(ctx, cudaGetLastError());
+    const size_t nstream = (size_t)n * NSCAN;
+    PIXO_TRY(ensure_pinned(ctx, ctx->h_prog, 256 + nstream * 8));
+    auto *h_status = static_cast<uint32_t *>(ctx->h_prog.ptr);
+    auto *h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, nstream * 8, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+    if (*h_status)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "coefficient out of the progressive range (-16383..16383)");
+    if (check_only) return 0;
+
+    // raw strings, sized by the longest stream
+    uint64_t max_bytes = 0;
+    for (size_t q = 0; q < nstream; ++q) max_bytes = std::max<uint64_t>(max_bytes, (h_bits[q] + 7) / 8);
+    const size_t raw_cap = (size_t)((max_bytes + 16 + 255) / 256 * 256);
+    SegPlan sp = splice_plan(n * NSCAN, raw_cap);
+    const size_t stage_cap = (2 * raw_cap + 256) / 256 * 256;   // every byte 0xFF still fits
+    const size_t off_len = sp.total, off_ovf = off_len + (nstream * 8 + 255) / 256 * 256;
+    const size_t off_stage = off_ovf + (nstream * 4 + 255) / 256 * 256;
+    PIXO_TRY(ensure_dev(ctx, ctx->d_prog_raw, sp.raw_total));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_prog_out, off_stage + nstream * stage_cap));
+    auto *raw = static_cast<uint8_t *>(ctx->d_prog_raw.ptr);
+    auto *outb = static_cast<uint8_t *>(ctx->d_prog_out.ptr);
+    PIXO_CUDA(ctx, cudaMemsetAsync(raw, 0, sp.raw_total, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(raw + sp.off_bits, P.bits, nstream * 8, cudaMemcpyDeviceToDevice, st));
+    PIXO_CUDA(ctx, cudaMemsetAsync(outb + off_ovf, 0, nstream * 4, st));
+    P.raw = reinterpret_cast<uint32_t *>(raw);
+    P.raw_words = raw_cap / 4;
+    if (tiles) {
+        k_prog_emit<<<(unsigned)tiles, PT, 0, st>>>(P);
+        ctx->launches += 1;
+        PIXO_CUDA(ctx, cudaGetLastError());
+    }
+    auto *d_len = reinterpret_cast<uint64_t *>(outb + off_len);
+    auto *d_ovf = reinterpret_cast<uint32_t *>(outb + off_ovf);
+    PIXO_TRY(launch_splice(ctx, n * NSCAN, sp, outb, raw, outb + off_stage, stage_cap, d_len, d_ovf));
+    PIXO_TRY(ensure_pinned(ctx, ctx->h_prog, 256 + nstream * 12));
+    h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
+    auto *h_ovf = reinterpret_cast<uint32_t *>(h_bits + nstream);
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, d_len, nstream * 8, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, nstream * 4, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+    res->len.assign(h_bits, h_bits + nstream);
+    for (size_t q = 0; q < nstream; ++q)
+        if (h_ovf[q]) return set_error(ctx, PIXO_B200_ERR_CUDA, "progressive splice overflowed its exact-size buffer");
+    res->stage = outb + off_stage;
+    res->stage_cap = stage_cap;
+    res->d_len = d_len;
+    return 0;
+}
+
+int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
+                            uint64_t *d_scan_len, uint32_t *d_overflow)
+{
+    uint64_t longest = 0;
+    for (uint64_t l : res.len) longest = std::max(longest, l);
+    const uint32_t ctas = (uint32_t)std::min<uint64_t>(2048, std::max<uint64_t>(1, (longest + PT * 64 - 1) / (PT * 64)));
+    k_prog_pack<<<dim3(NSCAN * ctas, n), PT, 0, ctx->stream>>>(
+        ctas, res.stage, res.stage_cap, reinterpret_cast<const unsigned long long *>(res.d_len), d_out, out_cap,
+        reinterpret_cast<unsigned long long *>(d_scan_len), d_overflow);
+    ctx->launches += 1;
+    PIXO_CUDA(ctx, cudaGetLastError());
+    return 0;
+}
+
+}  // namespace pixo

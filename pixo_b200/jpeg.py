@@ -213,6 +213,106 @@ def encode_batch(frames: np.ndarray, options: JpegOptions, ctx: Context | None =
     return [out[i, : lens[i]].tobytes() for i in range(n)]
 
 
+def progressive_capacity(width: int, height: int) -> int:
+    """Upper bound on a progressive file's size: a coefficient costs at most 31 bits (16-bit code +
+    15 amplitude bits) plus its share of ZRLs and EOB runs, x2 for 0xFF stuffing, three full-resolution
+    components, headers."""
+    nb = ((int(width) + 7) // 8) * ((int(height) + 7) // 8) * 3
+    return nb * 64 * 9 + 4096
+
+
+def encode_progressive_into(output: bytearray, data, options: JpegOptions, ctx: Context | None = None) -> None:
+    """pixo::jpeg::encode_into with progressive scans (src/jpeg/mod.rs:395-410, 872-927) whatever
+    options.progressive says: SOF2 and the 7 scans of pixo's simple_progressive_script, quirks included
+    (include/pixo_b200.h, pixo_b200_jpeg_encode_progressive).  Clears and refills `output`."""
+    ctx = ctx or default_context()
+    d = _as_u8(data)
+    cap = min(progressive_capacity(options.width, options.height), 2 * d.size + 65536)
+    buf = np.empty(cap, np.uint8)
+    n = C.c_size_t()
+    restart = _restart(options)
+    rc = _lib.load().pixo_b200_jpeg_encode_progressive(
+        ctx.handle, d.ctypes.data, d.size, int(options.width), int(options.height),
+        int(options.color_type), int(options.quality), int(options.subsampling), restart,
+        int(bool(options.optimize_huffman)), int(bool(options.trellis_quant)), buf.ctypes.data, cap, C.byref(n))
+    _lib.check(ctx.handle, rc)
+    del output[:]
+    output.extend(buf[: n.value].tobytes())
+
+
+def encode_progressive(data, options: JpegOptions, ctx: Context | None = None) -> bytes:
+    """The progressive file pixo writes for `options` with progressive = true (JpegOptions.max: its
+    max preset)."""
+    out = bytearray()
+    encode_progressive_into(out, data, options, ctx)
+    return bytes(out)
+
+
+def encode_progressive_batch(frames: np.ndarray, options: JpegOptions, ctx: Context | None = None,
+                             capacity_each: int | None = None) -> list[bytes]:
+    """n frames of identical geometry ([n, h*w*bpp] uint8) -> n progressive files."""
+    restart = _restart(options)
+    ctx = ctx or default_context()
+    f = np.ascontiguousarray(frames, np.uint8)
+    n = f.shape[0]
+    each = f.size // max(n, 1)
+    cap = capacity_each or min(progressive_capacity(options.width, options.height), 2 * each + 8192)
+    out = np.empty((n, cap), np.uint8)
+    lens = (C.c_size_t * n)()
+    rc = _lib.load().pixo_b200_jpeg_encode_progressive_batch(
+        ctx.handle, f.ctypes.data, each, n, int(options.width), int(options.height),
+        int(options.color_type), int(options.quality), int(options.subsampling), restart,
+        int(bool(options.optimize_huffman)), int(bool(options.trellis_quant)), out.ctypes.data, cap, lens)
+    _lib.check(ctx.handle, rc)
+    return [out[i, : lens[i]].tobytes() for i in range(n)]
+
+
+def dht_array(tables) -> np.ndarray:
+    """{(class, id): (bits[16], values)} (a file's DHT, e.g. tests' jpeg_progressive_scans.dht) ->
+    the 4 x (16 counts + 256 values) uint8 array progressive_scans_dev takes."""
+    a = np.zeros((4, 272), np.uint8)
+    for k, key in enumerate([(0, 0), (0, 1), (1, 0), (1, 1)]):
+        if key in tables:
+            bits, vals = tables[key]
+            a[k, :16] = bits
+            a[k, 16:16 + len(vals)] = vals
+    return a
+
+
+def progressive_scans_dev(d_y, d_cb, d_cr, width, height, color_type=ColorType.Rgb,
+                          subsampling=Subsampling.S420, tables=None, n_frames=1, y_stride=None, c_stride=None,
+                          d_out=None, out_cap_each=None, d_scan_len=None, d_overflow=None,
+                          ctx: Context | None = None):
+    """The progressive scan stage on device coefficient arrays (int16 torch tensors in
+    compute_all_coefficients' layout, natural order, 16-byte aligned; frame i at i * stride elements).
+    tables: None for the standard tables, a uint8 [4, 272] array (dht_array) or a DHT dict.
+    Returns (d_out, d_scan_len [n, 7], d_overflow [n]) - new tensors when not given."""
+    import torch
+    ctx = ctx or default_context()
+    ny, nc = block_counts(width, height, color_type, subsampling)
+    dev = d_y.device
+    y_stride = ny * 64 if y_stride is None else int(y_stride)
+    c_stride = nc * 64 if c_stride is None else int(c_stride)
+    if out_cap_each is None:
+        out_cap_each = (progressive_capacity(width, height) + 15) // 16 * 16
+    if d_out is None:
+        d_out = torch.empty(n_frames * out_cap_each, dtype=torch.uint8, device=dev)
+    if d_scan_len is None:
+        d_scan_len = torch.empty((n_frames, 7), dtype=torch.int64, device=dev)
+    if d_overflow is None:
+        d_overflow = torch.empty(n_frames, dtype=torch.int32, device=dev)
+    dht = None
+    if tables is not None:
+        dht = np.ascontiguousarray(dht_array(tables) if isinstance(tables, dict) else tables, np.uint8)
+    ptr = lambda t: None if t is None else int(t.data_ptr())
+    rc = _lib.load().pixo_b200_jpeg_progressive_scans_dev(
+        ctx.handle, ptr(d_y), y_stride, ptr(d_cb), ptr(d_cr), c_stride, int(n_frames), int(width), int(height),
+        int(color_type), int(subsampling), None if dht is None else dht.ctypes.data, ptr(d_out), int(out_cap_each),
+        ptr(d_scan_len), ptr(d_overflow))
+    _lib.check(ctx.handle, rc)
+    return d_out, d_scan_len, d_overflow
+
+
 def entropy_encode(y, cb, cr, options: JpegOptions, ctx: Context | None = None) -> bytes:
     """Host entropy stage on its own (no device needed)."""
     y = np.ascontiguousarray(y, np.int16)

@@ -94,4 +94,20 @@ d_ad = torch.zeros(4, dtype=torch.int32, device=dev)
 torch.cuda.synchronize(dev)
 png.reduce_and_filter_dev(d_in, 300 * 40 * 4, 4, PngOptions.from_preset(300, 40, 1), d_out, 40 * (300 * 4 + 1), d_ad, ctx=ctx)
 ctx.sync()
+# JPEG progressive scans: every k_prog_* kernel, the splice and k_prog_pack, with trellis and plain
+# coefficients, optimised and standard tables, gray / 4:4:4 / 4:2:0, a batch and caller arrays
+for (ww, hh) in ((333, 222), (17, 9)):
+    for ct, ss in ((2, Subsampling.S420), (2, Subsampling.S444), (0, Subsampling.S444)):
+        ch = 1 if ct == 0 else 3
+        im = synthetic.noise(ww, hh, ch, 5)
+        for opt, tr, rst in ((True, True, None), (False, False, 3)):
+            jpeg.encode_progressive(im, JpegOptions(ww, hh, ColorType(ct), 80, ss, rst, opt, True, tr), ctx=ctx)
+frames = np.stack([synthetic.noise(200, 120, 3, k) for k in range(3)])
+jpeg.encode_progressive_batch(frames, JpegOptions.max(200, 120, 80), ctx=ctx)
+yb = np.zeros((40000, 64), np.int16)
+yb[::9000, 1] = 5
+yb[7, 63] = -3
+d_yb = torch.from_numpy(yb).to(dev)
+jpeg.progressive_scans_dev(d_yb, None, None, 8 * 400, 8 * 100, ColorType.Gray, Subsampling.S444, ctx=ctx)
+ctx.sync()
 print("tour done")
