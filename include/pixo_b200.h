@@ -475,6 +475,44 @@ int pixo_b200_png_quantize_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data,
                                       const uint32_t *palette_lens, pixo_b200_png_reduced *info, uint8_t *d_out,
                                       size_t out_stride, uint32_t *d_adler);
 
+/* ---- resize ----------------------------------------------------------------------------- */
+
+/* pixo::resize::ResizeAlgorithm, numbered as the wasm binding numbers it (src/wasm.rs:156-166) */
+enum { PIXO_B200_RESIZE_NEAREST = 0, PIXO_B200_RESIZE_BILINEAR = 1, PIXO_B200_RESIZE_LANCZOS3 = 2 };
+
+/* Replaces pixo::resize::resize_into — src/resize.rs:180-602: Nearest (:299-330), Bilinear (:333-389) and
+ * separable Lanczos3 (:391-602, a u8 intermediate of src_height x dst_width pixels between the passes),
+ * byte-identical, for Gray, GrayAlpha, RGB and RGBA (the output has the input's colour type).  Errors in
+ * this order: PIXO_B200_ERR_INVALID_ARGUMENT for an unknown colour type or algorithm (resizeImage's
+ * checks, src/wasm.rs:183-201), then resize_impl's (src/resize.rs:205-250): a zero source, then a zero
+ * destination dimension PIXO_B200_ERR_INVALID_DIMENSIONS; any dimension above 1 << 24
+ * PIXO_B200_ERR_IMAGE_TOO_LARGE; data_len != src_width*src_height*bpp PIXO_B200_ERR_INVALID_DATA_LENGTH.
+ * Then out_cap below dst_width*dst_height*bpp returns PIXO_B200_ERR_OUTPUT_TOO_SMALL with *out_len = the
+ * size needed.  Where f32 rounding makes pixo's Bilinear index one pixel past the source (a side above
+ * 2^23; pixo panics there) the last pixel is read. */
+int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t src_width,
+                     uint32_t src_height, uint32_t dst_width, uint32_t dst_height, uint32_t color_type,
+                     uint32_t algorithm, uint8_t *out, size_t out_cap, size_t *out_len);
+/* Batch of device-resident frames of one geometry, asynchronous on the context's stream: frame i at
+ * d_src + i*src_stride (src_width*src_height*bpp bytes, rows packed) -> d_dst + i*dst_stride.  Any
+ * alignment and any n_images.  Frames must not overlap: with n_images > 1, src_stride below a source
+ * frame returns PIXO_B200_ERR_INVALID_DATA_LENGTH and dst_stride below a destination frame
+ * PIXO_B200_ERR_OUTPUT_TOO_SMALL.  Nothing is launched unless the call is valid.  Lanczos3's weight tables
+ * are uploaded before the call returns; its intermediate stays within 256 MiB of device scratch (larger
+ * frames go in bands of destination rows).  The output is packed pixels, what
+ * pixo_b200_jpeg_encode_dev and pixo_b200_png_filter_dev read. */
+int pixo_b200_resize_dev(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, uint32_t n_images,
+                         uint32_t src_width, uint32_t src_height, uint32_t dst_width, uint32_t dst_height,
+                         uint32_t color_type, uint32_t algorithm, uint8_t *d_dst, size_t dst_stride);
+/* Lanczos3's contribution table for one axis (precompute_contributions, src/resize.rs:416-456), as the
+ * resizers use it: destination index d reads source indices start[d] .. start[d]+count[d]-1 with weights
+ * weights[offset[d] ..], normalised f32 computed with pixo's own sinf (the libm port of musl's, which the
+ * wasm build runs).  *n_weights receives the total; start/count/offset (dst_size entries each) and weights
+ * may be NULL; weights_cap below the total returns PIXO_B200_ERR_OUTPUT_TOO_SMALL after the other
+ * arrays are written.  Host-only, no device needed. */
+int pixo_b200_resize_weights(uint32_t src_size, uint32_t dst_size, uint32_t *start, uint32_t *count,
+                             uint64_t *offset, float *weights, size_t weights_cap, size_t *n_weights);
+
 /* Replaces compress::adler32::adler32 — src/compress/adler32.rs:11-47 (dispatch
  * src/simd/mod.rs:72-90).  Host buffer in, checksum out. */
 int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t *out);

@@ -109,6 +109,11 @@ SYMBOLS = {
     "pixo_b200_png_quantize_filter_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
                                                     C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_size_t,
                                                     vp]),
+    "pixo_b200_resize": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                   C.c_uint32, vp, C.c_size_t, szp]),
+    "pixo_b200_resize_dev": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                       C.c_uint32, C.c_uint32, C.c_uint32, vp, C.c_size_t]),
+    "pixo_b200_resize_weights": (C.c_int, [C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_size_t, szp]),
     "pixo_b200_adler32": (C.c_int, [vp, vp, C.c_size_t, u32p]),
     "pixo_b200_adler32_dev": (C.c_int, [vp, vp, C.c_size_t, vp]),
 }

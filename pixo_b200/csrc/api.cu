@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "jpeg_host.hpp"
+#include "resize_host.hpp"
 
 namespace pixo {
 
@@ -330,7 +331,7 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     cudaStreamSynchronize(ctx->stream);
     Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
                        &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis,
-                       &ctx->d_prog, &ctx->d_prog_raw, &ctx->d_prog_out};
+                       &ctx->d_prog, &ctx->d_prog_raw, &ctx->d_prog_out, &ctx->d_resize, &ctx->d_resize_tmp};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
     Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant, &ctx->h_trellis, &ctx->h_prog};
     for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
@@ -1788,6 +1789,95 @@ int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint3
     PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_y.ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;
+}
+
+// ---- resize --------------------------------------------------------------------------------
+
+// the wasm binding's enum checks (src/wasm.rs:55-67,156-166), then resize_impl's (src/resize.rs:205-250)
+static int validate_resize(pixo_b200_ctx *ctx, uint32_t sw, uint32_t sh, uint32_t dw, uint32_t dh, uint32_t color_type,
+                           uint32_t algorithm)
+{
+    if (color_type > PIXO_B200_RGBA)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "Invalid color type: %u", color_type);
+    if (algorithm > PIXO_B200_RESIZE_LANCZOS3)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "Invalid resize algorithm: %u", algorithm);
+    if (sw == 0 || sh == 0)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", sw, sh);
+    if (dw == 0 || dh == 0)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", dw, dh);
+    const uint32_t mx = 1u << 24;  // src/resize.rs:30
+    if (sw > mx || sh > mx || dw > mx || dh > mx)
+        return set_error(ctx, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Image dimensions %ux%u exceed maximum %u",
+                         std::max(sw, dw), std::max(sh, dh), mx);
+    return 0;
+}
+
+int pixo_b200_resize_weights(uint32_t src_size, uint32_t dst_size, uint32_t *start, uint32_t *count,
+                             uint64_t *offset, float *weights, size_t weights_cap, size_t *n_weights)
+{
+    if (src_size == 0 || dst_size == 0)
+        return set_error(nullptr, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid size: %u -> %u", src_size, dst_size);
+    if (src_size > (1u << 24) || dst_size > (1u << 24))
+        return set_error(nullptr, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Size %u -> %u exceeds maximum %u", src_size, dst_size,
+                         1u << 24);
+    if (!n_weights) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "n_weights is null");
+    ResizeAxis a;
+    resize_axis(src_size, dst_size, false, a);
+    const size_t total = dst_size ? a.offset[dst_size - 1] + a.count[dst_size - 1] : 0;
+    *n_weights = total;
+    if (start) memcpy(start, a.start.data(), 4 * (size_t)dst_size);
+    if (count) memcpy(count, a.count.data(), 4 * (size_t)dst_size);
+    if (offset) memcpy(offset, a.offset.data(), 8 * (size_t)dst_size);
+    if (!weights) return 0;
+    if (weights_cap < total)
+        return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "weights capacity %zu below %zu", weights_cap, total);
+    resize_axis(src_size, dst_size, true, a);
+    memcpy(weights, a.w.data(), 4 * total);
+    return 0;
+}
+
+int pixo_b200_resize_dev(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, uint32_t n_images,
+                         uint32_t src_width, uint32_t src_height, uint32_t dst_width, uint32_t dst_height,
+                         uint32_t color_type, uint32_t algorithm, uint8_t *d_dst, size_t dst_stride)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_resize(ctx, src_width, src_height, dst_width, dst_height, color_type, algorithm));
+    if (!d_src || !d_dst) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    // frames of a batch must not overlap: a frame's threads write its output while others read theirs
+    const size_t bpp = color_type + 1, raw = (size_t)src_width * src_height * bpp, need = (size_t)dst_width * dst_height * bpp;
+    if (n_images > 1 && src_stride < raw)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, src_stride);
+    if (n_images > 1 && dst_stride < need)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "dst_stride %zu below %zu", dst_stride, need);
+    if (n_images == 0) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return launch_resize(ctx, d_src, src_stride, n_images, src_width, src_height, dst_width, dst_height,
+                         (uint32_t)bpp, algorithm, d_dst, dst_stride);
+}
+
+int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t src_width,
+                     uint32_t src_height, uint32_t dst_width, uint32_t dst_height, uint32_t color_type,
+                     uint32_t algorithm, uint8_t *out, size_t out_cap, size_t *out_len)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_resize(ctx, src_width, src_height, dst_width, dst_height, color_type, algorithm));
+    if (!data || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const size_t bpp = color_type + 1, in_bytes = (size_t)src_width * src_height * bpp;
+    if (data_len != in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, data_len);
+    const size_t out_bytes = (size_t)dst_width * dst_height * bpp;
+    *out_len = out_bytes;
+    if (out_cap < out_bytes)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, out_bytes);
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
+    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes));
+    PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
+    PIXO_TRY(launch_resize(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, src_width, src_height,
+                           dst_width, dst_height, (uint32_t)bpp, algorithm, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
+                           out_bytes));
+    return d2h_copy_sync(ctx, out, ctx->d_out.ptr, out_bytes, ctx->stream);
 }
 
 }  // extern "C"

@@ -135,6 +135,7 @@ struct pixo_b200_ctx {
     pixo::Scratch d_trellis, h_trellis;          // JPEG trellis: status word + f32 DCT blocks; its status on the host
     pixo::Scratch d_prog, d_prog_raw, d_prog_out, h_prog;   // JPEG progressive scans: per-block state, raw strings,
                                                             // stuffed segments; bit counts / lengths on the host
+    pixo::Scratch d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
     pixo::Scratch h_in, h_out, h_misc, h_red, h_quant;
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
@@ -201,6 +202,10 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
                         uint32_t width, uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
                         uint32_t max_colors, const uint8_t *palettes, const uint32_t *palette_lens,
                         pixo_b200_png_reduced *info, uint8_t *d_out, size_t out_stride, uint32_t *d_adler);
+// pixo_b200_resize_dev after validation (resize.cu): n frames of bpp bytes per pixel, algorithm 0 Nearest,
+// 1 Bilinear, 2 Lanczos3
+int launch_resize(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, uint32_t n, uint32_t sw, uint32_t sh,
+                  uint32_t dw, uint32_t dh, uint32_t bpp, uint32_t algorithm, uint8_t *d_dst, size_t dst_stride);
 
 struct FrameGeometry;
 struct HuffTables;

@@ -110,4 +110,21 @@ yb[7, 63] = -3
 d_yb = torch.from_numpy(yb).to(dev)
 jpeg.progressive_scans_dev(d_yb, None, None, 8 * 400, 8 * 100, ColorType.Gray, Subsampling.S444, ctx=ctx)
 ctx.sync()
+# resize: every kernel at every pixel size, the wide and byte nearest copies, and Lanczos3 in one band and,
+# for a tall frame whose one destination row needs 280 MB of intermediate, in column chunks
+from pixo_b200 import resize as rs  # noqa: E402
+for ct in range(4):
+    for alg in range(3):
+        for (sw, sh, dw, dh) in ((37, 29, 100, 71), (97, 61, 37, 29), (1, 1, 3, 2), (1024, 5, 3, 2)):
+            px = rng.integers(0, 256, sw * sh * (ct + 1), dtype=np.uint8)
+            o = rs.ResizeOptions.builder(sw, sh).dst(dw, dh).color_type(ColorType(ct)).algorithm(rs.ResizeAlgorithm(alg)).build()
+            rs.resize(px, o, ctx=ctx)
+            d_px = torch.from_numpy(np.concatenate([px, px])).to(dev)
+            d_o = torch.empty(2 * dw * dh * (ct + 1) + 1, dtype=torch.uint8, device=dev)
+            torch.cuda.synchronize(dev)
+            rs.resize_dev(d_px if ct % 2 else d_px[1:], px.size, 2 if ct % 2 else 1, o, d_o[1:], dw * dh * (ct + 1),
+                          ctx=ctx)
+            ctx.sync()
+tall = rng.integers(0, 256, 16 * 70000 * 4, dtype=np.uint8)
+rs.resize(tall, rs.ResizeOptions.builder(16, 70000).dst(1000, 3).algorithm(rs.ResizeAlgorithm.Lanczos3).build(), ctx=ctx)
 print("tour done")
