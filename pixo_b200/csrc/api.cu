@@ -265,8 +265,6 @@ static int validate_jpeg(pixo_b200_ctx *ctx, uint32_t w, uint32_t h, uint32_t co
     return 0;
 }
 
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 }  // namespace pixo
 
 using namespace pixo;

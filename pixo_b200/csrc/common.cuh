@@ -12,6 +12,7 @@
 #include <string>
 #include <thread>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/pixo_b200.h"
@@ -113,6 +114,14 @@ struct ProgResult {
     std::vector<uint64_t> len;
 };
 
+// What a context has set on one kernel.  Function attributes belong to the device, and every context
+// sets the same values, so contexts sharing a device never undo each other's settings.
+struct KernelAttrs {
+    size_t smem_limit = 0;      // cudaFuncAttributeMaxDynamicSharedMemorySize as set
+    int blocks_per_sm = 0;      // occupancy query of the transform's persistent kernels, 0: not asked
+    bool carveout_set = false;  // cudaFuncAttributePreferredSharedMemoryCarveout
+};
+
 }  // namespace pixo
 
 struct pixo_b200_ctx {
@@ -143,6 +152,7 @@ struct pixo_b200_ctx {
     // How the bands coded by pixo_b200_jpeg_band_entropy_dev(_async) were cut into segments, keyed by
     // the caller's raw buffer (which holds the segments' strings, bit counts and tails until the splice).
     std::unordered_map<const void *, pixo::SegPlan> bands;
+    std::unordered_map<const void *, pixo::KernelAttrs> kernels;   // keyed by the kernel's host function
 };
 
 namespace pixo {
@@ -163,6 +173,38 @@ int ensure_pinned(pixo_b200_ctx *ctx, Scratch &s, size_t bytes);
         int rc__ = (expr);             \
         if (rc__ != 0) return rc__;    \
     } while (0)
+
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Dynamic shared memory of a launch: `bytes`, and `limit`, what the kernel's maximum is raised to.  A
+// kernel launched with varying sizes passes one fixed limit, so that no context lowers it under another.
+struct Smem {
+    size_t bytes, limit;
+    Smem(size_t b) : bytes(b), limit(b) {}
+    Smem(size_t b, size_t l) : bytes(b), limit(l) {}
+};
+
+// Raise `kernel`'s dynamic shared memory maximum to `limit` unless this context already has
+inline int allow_smem(pixo_b200_ctx *ctx, const void *kernel, size_t limit)
+{
+    size_t &set = ctx->kernels[kernel].smem_limit;
+    if (set >= limit) return 0;
+    PIXO_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+    set = limit;
+    return 0;
+}
+
+// Every kernel of the library is launched here: on the context's stream, counted (the count is
+// pixo_b200_ctx_launch_count) and checked.
+template <class... P, class... A>
+int launch(pixo_b200_ctx *ctx, void (*kernel)(P...), dim3 grid, dim3 block, Smem smem, A &&...args)
+{
+    if (smem.bytes) PIXO_TRY(allow_smem(ctx, reinterpret_cast<const void *>(kernel), smem.limit));
+    kernel<<<grid, block, smem.bytes, ctx->stream>>>(std::forward<A>(args)...);
+    ctx->launches++;
+    PIXO_CUDA(ctx, cudaGetLastError());
+    return 0;
+}
 
 // ---- launchers implemented in the .cu files ----
 // ext: write coefficient records and their extents (flags is then ignored)

@@ -823,8 +823,6 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
 
 }  // namespace
 
-static size_t a256(size_t v) { return (v + 255) / 256 * 256; }
-
 static EntropyPlan plan_entropy(uint32_t n, uint64_t nblocks, uint64_t rst_blocks)
 {
     EntropyPlan p;
@@ -835,13 +833,13 @@ static EntropyPlan plan_entropy(uint32_t n, uint64_t nblocks, uint64_t rst_block
         p.nchunks = (size_t)((n_int - 1) * cpi + (last + CB - 1) / CB);
     }
     size_t o = 0;
-    p.off_st1 = o; o += a256((size_t)n * p.nchunks * 8);
-    p.off_st2 = o; o += a256((size_t)n * p.nchunks * 8);
+    p.off_st1 = o; o += align_up((size_t)n * p.nchunks * 8, 256);
+    p.off_st2 = o; o += align_up((size_t)n * p.nchunks * 8, 256);
     p.off_ticket = o; o += 256;
-    p.off_ovf = o; o += a256((size_t)n * 4);
+    p.off_ovf = o; o += align_up((size_t)n * 4, 256);
     p.zero_bytes = o;  // everything up to here is cleared per launch
-    p.off_outlen = o; o += a256((size_t)n * 8);
-    p.off_tail = o; o += a256((size_t)n * 8);
+    p.off_outlen = o; o += align_up((size_t)n * 8, 256);
+    p.off_tail = o; o += align_up((size_t)n * 8, 256);
     p.total = o;
     return p;
 }
@@ -1255,14 +1253,14 @@ static void lay_out(SegPlan &p, uint32_t n, uint64_t bpm, size_t raw_cap)
     p.max_tiles = (uint32_t)(S * (p.raw_cap / SPL_TILE + 2));
     p.ent = plan_entropy(n * S, p.seg_mcus * bpm, 0);
     size_t o = 0;
-    p.off_ent = o; o += a256(p.ent.total);
-    p.raw_bytes = a256((size_t)n * S * p.raw_cap);
+    p.off_ent = o; o += align_up(p.ent.total, 256);
+    p.raw_bytes = align_up((size_t)n * S * p.raw_cap, 256);
     p.off_bits = p.raw_bytes;
-    p.off_tails = p.off_bits + a256((size_t)n * S * 8);
-    p.raw_total = p.off_tails + a256((size_t)n * S * 8);
-    p.off_rec = o; o += a256((size_t)n * S * sizeof(SegRec));
-    p.off_ntiles = o; o += a256((size_t)n * 4);
-    p.off_cnt = o; o += a256((size_t)n * p.max_tiles * 4);
+    p.off_tails = p.off_bits + align_up((size_t)n * S * 8, 256);
+    p.raw_total = p.off_tails + align_up((size_t)n * S * 8, 256);
+    p.off_rec = o; o += align_up((size_t)n * S * sizeof(SegRec), 256);
+    p.off_ntiles = o; o += align_up((size_t)n * 4, 256);
+    p.off_cnt = o; o += align_up((size_t)n * p.max_tiles * 4, 256);
     p.total = o;
 }
 
@@ -1277,7 +1275,7 @@ static SegPlan plan_segments(uint32_t n, uint32_t S, uint64_t total_mcus, uint64
     // that), at most what its blocks can possibly need (64 x 26 bits + DC < 216 bytes per block).  It
     // does not depend on the caller's output capacity, so an output that is too small is still measured.
     const uint64_t fair = p.seg_mcus * mcu_raw_bytes + 4096, worst = p.seg_mcus * bpm * 216 + 64;
-    lay_out(p, n, bpm, (size_t)a256(std::min(fair, worst)));
+    lay_out(p, n, bpm, (size_t)align_up(std::min(fair, worst), 256));
     return p;
 }
 
@@ -1313,10 +1311,7 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint
     PIXO_CUDA(ctx, cudaMemsetAsync(ent, 0, sp.ent.zero_bytes, st));
     const size_t want = ((size_t)P.nimages * P.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    if (check) k_huff<true, true><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
-    else k_huff<true, false><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
-    ctx->launches += 1;
-    PIXO_CUDA(ctx, cudaGetLastError());
+    PIXO_TRY(launch(ctx, check ? k_huff<true, true> : k_huff<true, false>, grid, 32 * HUFF_WARPS, 0, P, T));
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_bits, P.out_len, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_tails, P.out_tail, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -1331,7 +1326,6 @@ static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, ui
                            bool last, const uint64_t *base_dev, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
                            uint32_t *d_overflow)
 {
-    cudaStream_t st = ctx->stream;
     SegParams Q;
     Q.raw = raw_area; Q.raw_cap = sp.raw_cap;
     Q.bits = reinterpret_cast<const unsigned long long *>(raw_area + sp.off_bits);
@@ -1346,13 +1340,11 @@ static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, ui
     Q.out_len = reinterpret_cast<unsigned long long *>(d_out_len);
     Q.overflow = d_overflow;
     Q.raw_overflow = raw_overflow;
-    k_seg_prefix<<<n, SPL_THREADS, 0, st>>>(Q);
-    k_seg_count<<<dim3((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, n), SPL_THREADS, 0, st>>>(Q);
-    k_seg_scan<<<n, 1024, 0, st>>>(Q);
-    k_seg_emit<<<dim3((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, n), SPL_THREADS, 0, st>>>(Q);
-    ctx->launches += 4;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    const dim3 tiles((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, n);
+    PIXO_TRY(launch(ctx, k_seg_prefix, n, SPL_THREADS, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_count, tiles, SPL_THREADS, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_scan, n, 1024, 0, Q));
+    return launch(ctx, k_seg_emit, tiles, SPL_THREADS, 0, Q);
 }
 
 // Enqueue the entropy stage for n whole images on ctx->stream.  d_scratch: entropy_scratch_bytes.
@@ -1416,11 +1408,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     }
     const size_t want = ((size_t)n * pl.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    if (check) k_huff<false, true><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
-    else k_huff<false, false><<<grid, 32 * HUFF_WARPS, 0, st>>>(P, T);
-    ctx->launches += 1;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    return launch(ctx, check ? k_huff<false, true> : k_huff<false, false>, grid, 32 * HUFF_WARPS, 0, P, T);
 }
 
 size_t band_raw_bytes(const FrameGeometry &g)
@@ -1465,13 +1453,10 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     make_huff_dev(t, &T);
     ctx->bands[d_raw] = sp;
     PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, seg_scratch, d_raw));   // a band's arrays are the caller's (no extents)
-    k_band_totals<<<1, 32, 0, ctx->stream>>>(reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
-                                             reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
-                                             reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,
-                                             reinterpret_cast<unsigned long long *>(d_bits_tail), d_flags);
-    ctx->launches += 1;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    return launch(ctx, k_band_totals, 1, 32, 0, reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
+                  reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
+                  reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,
+                  reinterpret_cast<unsigned long long *>(d_bits_tail), d_flags);
 }
 
 // Splice the strings launch_band_entropy left in the caller's buffer d_raw into the band's scan bytes.  The

@@ -454,18 +454,17 @@ ProgLayout prog_layout(const FrameGeometry &g, uint32_t n)
     }
     L.tile_base[NSCAN] = tb;
     L.blk_base[NSCAN] = bb;
-    auto a256 = [](size_t v) { return (v + 255) / 256 * 256; };
     const size_t tiles = (size_t)n * tb, blocks = (size_t)n * bb;
     size_t o = 0;
     L.off_status = o; o += 256;
-    L.off_blen = o; o += a256(blocks * 4);
-    L.off_flag = o; o += a256(blocks);
-    L.off_tile_last = o; o += a256(tiles * 4);
-    L.off_tile_carry = o; o += a256(tiles * 4);
-    L.off_tile_bits = o; o += a256(tiles * 4);
-    L.off_tile_off = o; o += a256(tiles * 8);
-    L.off_bits = o; o += a256((size_t)n * NSCAN * 8);
-    L.off_tables = o; o += a256((size_t)n * sizeof(ProgTables));
+    L.off_blen = o; o += align_up(blocks * 4, 256);
+    L.off_flag = o; o += align_up(blocks, 256);
+    L.off_tile_last = o; o += align_up(tiles * 4, 256);
+    L.off_tile_carry = o; o += align_up(tiles * 4, 256);
+    L.off_tile_bits = o; o += align_up(tiles * 4, 256);
+    L.off_tile_off = o; o += align_up(tiles * 8, 256);
+    L.off_bits = o; o += align_up((size_t)n * NSCAN * 8, 256);
+    L.off_tables = o; o += align_up((size_t)n * sizeof(ProgTables), 256);
     L.total = o;
     return L;
 }
@@ -502,13 +501,11 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(base + L.off_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
     if (tiles) {
-        k_prog_measure<<<(unsigned)tiles, PT, 0, st>>>(P);
-        k_prog_carry<<<n * NSCAN, PT, 0, st>>>(P);
-        k_prog_count<<<(unsigned)tiles, PT, 0, st>>>(P);
+        PIXO_TRY(launch(ctx, k_prog_measure, (unsigned)tiles, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_carry, n * NSCAN, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_count, (unsigned)tiles, PT, 0, P));
     }
-    k_prog_offsets<<<n * NSCAN, PT, 0, st>>>(P);
-    ctx->launches += tiles ? 4 : 1;
-    PIXO_CUDA(ctx, cudaGetLastError());
+    PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
     const size_t nstream = (size_t)n * NSCAN;
     PIXO_TRY(ensure_pinned(ctx, ctx->h_prog, 256 + nstream * 8));
     auto *h_status = static_cast<uint32_t *>(ctx->h_prog.ptr);
@@ -538,11 +535,7 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     PIXO_CUDA(ctx, cudaMemsetAsync(outb + off_ovf, 0, nstream * 4, st));
     P.raw = reinterpret_cast<uint32_t *>(raw);
     P.raw_words = raw_cap / 4;
-    if (tiles) {
-        k_prog_emit<<<(unsigned)tiles, PT, 0, st>>>(P);
-        ctx->launches += 1;
-        PIXO_CUDA(ctx, cudaGetLastError());
-    }
+    if (tiles) PIXO_TRY(launch(ctx, k_prog_emit, (unsigned)tiles, PT, 0, P));
     auto *d_len = reinterpret_cast<uint64_t *>(outb + off_len);
     auto *d_ovf = reinterpret_cast<uint32_t *>(outb + off_ovf);
     PIXO_TRY(launch_splice(ctx, n * NSCAN, sp, outb, raw, outb + off_stage, stage_cap, d_len, d_ovf));
@@ -567,12 +560,9 @@ int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t 
     uint64_t longest = 0;
     for (uint64_t l : res.len) longest = std::max(longest, l);
     const uint32_t ctas = (uint32_t)std::min<uint64_t>(2048, std::max<uint64_t>(1, (longest + PT * 64 - 1) / (PT * 64)));
-    k_prog_pack<<<dim3(NSCAN * ctas, n), PT, 0, ctx->stream>>>(
-        ctas, res.stage, res.stage_cap, reinterpret_cast<const unsigned long long *>(res.d_len), d_out, out_cap,
-        reinterpret_cast<unsigned long long *>(d_scan_len), d_overflow);
-    ctx->launches += 1;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    return launch(ctx, k_prog_pack, dim3(NSCAN * ctas, n), PT, 0, ctas, res.stage, res.stage_cap,
+                  reinterpret_cast<const unsigned long long *>(res.d_len), d_out, out_cap,
+                  reinterpret_cast<unsigned long long *>(d_scan_len), d_overflow);
 }
 
 }  // namespace pixo

@@ -1105,7 +1105,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
 
 EncodeTiledFn tensor_map_encoder()
 {
-    static EncodeTiledFn fn = []() -> EncodeTiledFn {
+    static const EncodeTiledFn fn = []() -> EncodeTiledFn {
         void *p = nullptr;
         cudaDriverEntryPointQueryResult q;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
@@ -1137,8 +1137,8 @@ bool make_rgb_tensor_map(CUtensorMap *tm, const uint8_t *pixels, size_t pixel_st
 }
 
 // k_jpeg_420, or k_jpeg_444 when `s444`: persistent kernels with one unit per warp in flight, so the
-// grid is as many CTAs as fit on the device (the occupancy query, asked once per device, kernel and
-// output format) and no more than the units need.  Only enqueues: the caller counts the launch.
+// grid is as many CTAs as fit on the device (the occupancy query, asked once per context, kernel and
+// output format) and no more than the units need.
 int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, int out, const uint8_t *px, size_t pixel_stride,
                          uint32_t n, uint32_t w, uint32_t h, int16_t *y, size_t y_stride, int16_t *cb,
                          int16_t *cr, size_t c_stride, const CoefExtents &e, const QPairTab &qt)
@@ -1161,18 +1161,16 @@ int launch_rgb_transform(pixo_b200_ctx *ctx, bool s444, int out, const uint8_t *
     void (*const k444[4])(K1Params, QPairTab, CUtensorMap) = {k_jpeg_444<kNatural>, k_jpeg_444<kZigzag>,
                                                                k_jpeg_444<kRecords>, k_jpeg_444<kDct>};
     auto kern = s444 ? k444[out] : k420[out];
-    static int blocks_per_sm[64][2][4];  // [device][s444][out]: function attributes are per device
-    int &bps = blocks_per_sm[ctx->device & 63][s444][out];
+    int &bps = ctx->kernels[reinterpret_cast<const void *>(kern)].blocks_per_sm;
     if (!bps) {
-        PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PIXO_TRY(allow_smem(ctx, reinterpret_cast<const void *>(kern), smem));
         int nb = 0;
         PIXO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, warps * 32, smem));
         bps = nb > 0 ? nb : 1;
     }
     const uint64_t nunits = (uint64_t)P.mcus_y * P.units_x * n;
     const uint64_t grid = std::min<uint64_t>((uint64_t)ctx->sm_count * bps, (nunits + warps - 1) / warps);
-    kern<<<(unsigned)grid, warps * 32, smem, ctx->stream>>>(P, qt, tm);
-    return 0;
+    return launch(ctx, kern, (unsigned)grid, warps * 32, smem, P, qt, tm);
 }
 
 // The extents of the frames from image i0 on (none: dense arrays)
@@ -1221,13 +1219,11 @@ int transform(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, 
             void (*const kg[4])(const uint8_t *, size_t, uint32_t, uint32_t, uint32_t, uint32_t, int16_t *, size_t,
                                 uint8_t *, size_t, QPairTab) = {k_jpeg_gray<kNatural>, k_jpeg_gray<kZigzag>,
                                                                  k_jpeg_gray<kRecords>, k_jpeg_gray<kDct>};
-            kg[out]<<<grid, 64, 0, ctx->stream>>>(px, pixel_stride, w, h, bx, tiles_x, y, y_stride, e.y, e.stride, qt);
+            PIXO_TRY(launch(ctx, kg[out], grid, 64, 0, px, pixel_stride, w, h, bx, tiles_x, y, y_stride, e.y, e.stride, qt));
         } else {
             PIXO_TRY(launch_rgb_transform(ctx, subsampling == PIXO_B200_S444, out, px, pixel_stride, nb, w, h, y,
                                           y_stride, cb, cr, c_stride, e, qt));
         }
-        ctx->launches++;
-        PIXO_CUDA(ctx, cudaGetLastError());
     }
     return 0;
 }
@@ -1280,10 +1276,8 @@ int launch_jpeg_histogram(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_strid
                             uint32_t, uint32_t, unsigned long long *, int, int, int) = {
             k_jpeg_hist<kNatural>, k_jpeg_hist<kZigzag>, k_jpeg_hist<kRecords>};
         const int in = ext ? kRecords : zigzag_in ? kZigzag : kNatural;
-        kh[in]<<<grid, 256, 0, ctx->stream>>>(y, y_stride, cb, cr, c_stride, e, ny, nc, blocks_y_per_mcu, restart_interval,
-                                              hist, s0, s1, s2);
-        ctx->launches++;
-        PIXO_CUDA(ctx, cudaGetLastError());
+        PIXO_TRY(launch(ctx, kh[in], grid, 256, 0, y, y_stride, cb, cr, c_stride, e, ny, nc, blocks_y_per_mcu,
+                        restart_interval, hist, s0, s1, s2));
     }
     return 0;
 }

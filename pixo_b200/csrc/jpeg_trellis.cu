@@ -315,18 +315,9 @@ int launch_trellis(pixo_b200_ctx *ctx, const float *d_src, size_t src_stride, in
         J.r[k] = r;
     }
     auto kern = zigzag ? k_trellis<true> : k_trellis<false>;
-    const size_t smem = sizeof(TrellisShared);
-    static bool attr_set[64][2];   // function attributes are per device
-    if (!attr_set[ctx->device & 63][zigzag]) {
-        PIXO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[ctx->device & 63][zigzag] = true;
-    }
     const uint64_t grid = (total + TR_THREADS - 1) / TR_THREADS;
     if (grid > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "too many blocks for one call");
-    kern<<<(unsigned)grid, TR_THREADS, smem, ctx->stream>>>(J, d_status);
-    ctx->launches++;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    return launch(ctx, kern, (unsigned)grid, TR_THREADS, sizeof(TrellisShared), J, d_status);
 }
 
 }  // namespace pixo

@@ -990,14 +990,8 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
     const bool use_band = !sticky && strat != PIXO_B200_FILTER_BIGRAMS && band_smem <= 200 * 1024 &&
                           row_bytes < (1u << 18);
     const size_t segcap = row_bytes + 15 < (size_t)SEG_BYTES ? ((row_bytes + 15) & ~(size_t)15) : (size_t)SEG_BYTES;
-    const size_t smem = 2 * (16 + segcap) + segcap + 32 + 8192;   // + bigram "seen" bitmap
-    static bool attr_set_dev[64];  // function attributes are per device
-    bool &attr_set = attr_set_dev[ctx->device & 63];
-    if (!attr_set) {
-        PIXO_CUDA(ctx, cudaFuncSetAttribute(k_png_filter, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)(2 * (16 + SEG_BYTES) + SEG_BYTES + 32 + 8192)));
-        attr_set = true;
-    }
+    const Smem smem{2 * (16 + segcap) + segcap + 32 + 8192,   // + bigram "seen" bitmap
+                    2 * (16 + (size_t)SEG_BYTES) + SEG_BYTES + 32 + 8192};
     // misc scratch: per image {accA, accB} u64, counter u32, decided u8
     const size_t per = 2 * sizeof(unsigned long long) + sizeof(uint32_t) + 4;
     PIXO_TRY(ensure_dev(ctx, ctx->d_misc, (size_t)n_images * per + 64));
@@ -1007,13 +1001,7 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
     PIXO_CUDA(ctx, cudaMemsetAsync(ctx->d_misc.ptr, 0, (size_t)n_images * per + 64, ctx->stream));
 
     if (use_band) {
-        static bool band_attr[64];
-        if (!band_attr[ctx->device & 63]) {
-            PIXO_CUDA(ctx, cudaFuncSetAttribute(k_png_band<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            PIXO_CUDA(ctx, cudaFuncSetAttribute(k_png_band<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            PIXO_CUDA(ctx, cudaFuncSetAttribute(k_png_band<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            band_attr[ctx->device & 63] = true;
-        }
+        const auto band = oa == 4 ? k_png_band<4> : oa == 2 ? k_png_band<2> : k_png_band<0>;
         const uint32_t nbands = (height + BAND_ROWS - 1) / BAND_ROWS;
         for (uint32_t i0 = 0; i0 < n_images; i0 += 65535) {
             const uint32_t nb = n_images - i0 < 65535 ? n_images - i0 : 65535;
@@ -1028,11 +1016,7 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
             B.above = d_above;
             B.async16 = (row_bytes % 16 == 0 && in_stride % 16 == 0 &&
                          (reinterpret_cast<uintptr_t>(d_data) & 15) == 0) ? 1u : 0u;
-            if (oa == 4) k_png_band<4><<<dim3(nbands, nb), PNG_THREADS, band_smem, ctx->stream>>>(B);
-            else if (oa == 2) k_png_band<2><<<dim3(nbands, nb), PNG_THREADS, band_smem, ctx->stream>>>(B);
-            else k_png_band<0><<<dim3(nbands, nb), PNG_THREADS, band_smem, ctx->stream>>>(B);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, band, dim3(nbands, nb), PNG_THREADS, {band_smem, 200 * 1024}, B));
         }
         return 0;
     }
@@ -1056,20 +1040,14 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
         if (sticky) {
             // row 0 decides (adaptive_filter_fast), every later row reuses that filter
             P.row0 = 0; P.forced = nullptr; P.decided = decided + i0;
-            k_png_filter<<<dim3(1, nb), PNG_THREADS, smem, ctx->stream>>>(P);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_png_filter, dim3(1, nb), PNG_THREADS, smem, P));
             if (height > 1) {
                 P.row0 = 1; P.forced = decided + i0; P.decided = nullptr;
-                k_png_filter<<<dim3(height - 1, nb), PNG_THREADS, smem, ctx->stream>>>(P);
-                ctx->launches++;
-                PIXO_CUDA(ctx, cudaGetLastError());
+                PIXO_TRY(launch(ctx, k_png_filter, dim3(height - 1, nb), PNG_THREADS, smem, P));
             }
         } else {
             P.row0 = 0; P.forced = nullptr; P.decided = nullptr;
-            k_png_filter<<<dim3(height, nb), PNG_THREADS, smem, ctx->stream>>>(P);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_png_filter, dim3(height, nb), PNG_THREADS, smem, P));
         }
     }
     return 0;
@@ -1086,10 +1064,7 @@ int launch_adler32(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32
     const uint32_t cap = (uint32_t)ctx->sm_count * 8;
     if (grid > cap) grid = cap;
     if (grid == 0) grid = 1;
-    k_adler32<<<grid, 256, 0, ctx->stream>>>(d_data, len, acc, counter, d_out);
-    ctx->launches++;
-    PIXO_CUDA(ctx, cudaGetLastError());
-    return 0;
+    return launch(ctx, k_adler32, grid, 256, 0, d_data, len, acc, counter, d_out);
 }
 
 }  // namespace pixo

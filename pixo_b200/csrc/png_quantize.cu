@@ -361,8 +361,6 @@ bool remapped_none(uint32_t s)
            s == PIXO_B200_FILTER_BIGRAMS;
 }
 
-size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 }  // namespace
 
 int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
@@ -398,8 +396,8 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         PIXO_CUDA(ctx, cub::DeviceRunLengthEncode::Encode(nullptr, tmp_rle, (const unsigned long long *)nullptr,
                                                           (unsigned long long *)nullptr, (uint32_t *)nullptr,
                                                           (uint32_t *)nullptr, (int)maxk, ctx->stream));
-        const size_t off_b = al256(maxk * 8), off_u = off_b + al256(maxk * 8), off_c = off_u + al256(maxk * 8);
-        const size_t off_n = off_c + al256(maxk * 4), off_t = off_n + 256;
+        const size_t off_b = align_up(maxk * 8, 256), off_u = off_b + align_up(maxk * 8, 256), off_c = off_u + align_up(maxk * 8, 256);
+        const size_t off_n = off_c + align_up(maxk * 4, 256), off_t = off_n + 256;
         PIXO_TRY(ensure_dev(ctx, ctx->d_quant, off_t + std::max(tmp_sort, tmp_rle)));
         PIXO_TRY(ensure_pinned(ctx, ctx->h_quant, maxk * 12 + 16));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant.ptr);
@@ -416,9 +414,7 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
             S.data = d_data + (size_t)i0 * in_stride; S.in_stride = in_stride; S.n_images = nb; S.bpp = bpp;
             S.nd = nd; S.nh = nh; S.sd = sd; S.sh = sh; S.keys = ka;
             const uint32_t ctas = (uint32_t)std::min<uint64_t>(((uint64_t)nk + Q_THREADS - 1) / Q_THREADS, (uint64_t)ctx->sm_count * 16);
-            k_quant_sample<<<ctas, Q_THREADS, 0, ctx->stream>>>(S);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_quant_sample, ctas, Q_THREADS, 0, S));
             size_t tb = tmp_sort;
             PIXO_CUDA(ctx, cub::DeviceRadixSort::SortKeys(base + off_t, tb, ka, kb, nk, 0, 39, ctx->stream));
             tb = tmp_rle;
@@ -469,18 +465,18 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
 
     std::vector<uint32_t> qall;
     for (uint32_t i = 0; i < n_images; ++i) if (kind[i] != LOSSLESS) qall.push_back(i);
-    const size_t idx_stride = al256(npix);
+    const size_t idx_stride = align_up(npix, 256);
     // steps 3-5 in passes of at most QUANT_PASS quantised images: every grid.y stays within CUDA's limit
     // and the scratch (about 330 KB per image besides its indices) does not grow with the batch
     for (size_t q0 = 0; q0 < qall.size(); q0 += QUANT_PASS) {
         const std::vector<uint32_t> qids(qall.begin() + q0, qall.begin() + std::min(qall.size(), q0 + QUANT_PASS));
         const size_t nq = qids.size();
         // 3. k-means, tables, map / dither on the device
-        const size_t o_jobs = 0, jobs_bytes = al256(nq * (sizeof(KmeansJob) + sizeof(LutJob) + sizeof(MapJob) + sizeof(DitherJob)) + 1024);
-        const size_t o_pal = jobs_bytes, o_acc = o_pal + al256(nq * 256 * 4), o_col = o_acc + al256(nq * 256 * 5 * 8);
-        const size_t o_lut = o_col + al256(nq * MAX_HIST_COLORS * 8), groups = (height + 31) / 32;
-        const size_t o_edge = o_lut + al256(nq * LUT_CELLS), o_prog = o_edge + al256(nq * (groups - 1 + 1) * width * 4);
-        const size_t o_tick = o_prog + al256(nq * groups * 4), o_idx = o_tick + 256;
+        const size_t o_jobs = 0, jobs_bytes = align_up(nq * (sizeof(KmeansJob) + sizeof(LutJob) + sizeof(MapJob) + sizeof(DitherJob)) + 1024, 256);
+        const size_t o_pal = jobs_bytes, o_acc = o_pal + align_up(nq * 256 * 4, 256), o_col = o_acc + align_up(nq * 256 * 5 * 8, 256);
+        const size_t o_lut = o_col + align_up(nq * MAX_HIST_COLORS * 8, 256), groups = (height + 31) / 32;
+        const size_t o_edge = o_lut + align_up(nq * LUT_CELLS, 256), o_prog = o_edge + align_up(nq * (groups - 1 + 1) * width * 4, 256);
+        const size_t o_tick = o_prog + align_up(nq * groups * 4, 256), o_idx = o_tick + 256;
         PIXO_TRY(ensure_dev(ctx, ctx->d_quant_img, o_idx + nq * idx_stride));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant_img.ptr);
         auto *d_pal = reinterpret_cast<uint32_t *>(base + o_pal);
@@ -532,39 +528,32 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
             PIXO_CUDA(ctx, cudaMemcpyAsync(d_col, h_col.data(), h_col.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
             PIXO_CUDA(ctx, cudaMemsetAsync(d_acc, 0, nq * 256 * 5 * 8, ctx->stream));
             for (int pass = 0; pass < 2; ++pass) {
-                k_quant_kmeans<<<dim3((max_cols + Q_THREADS - 1) / Q_THREADS, (uint32_t)km.size()), Q_THREADS, 0, ctx->stream>>>(d_km);
-                k_quant_update<<<(uint32_t)km.size(), 256, 0, ctx->stream>>>(d_km);
-                ctx->launches += 2;
-                PIXO_CUDA(ctx, cudaGetLastError());
+                PIXO_TRY(launch(ctx, k_quant_kmeans, dim3((max_cols + Q_THREADS - 1) / Q_THREADS, (uint32_t)km.size()),
+                                Q_THREADS, 0, d_km));
+                PIXO_TRY(launch(ctx, k_quant_update, (uint32_t)km.size(), 256, 0, d_km));
             }
         }
-        if (!lj.empty()) {
-            k_quant_lut<<<dim3(LUT_CELLS / Q_THREADS, (uint32_t)lj.size()), Q_THREADS, 0, ctx->stream>>>(d_lj);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
-        }
+        if (!lj.empty())
+            PIXO_TRY(launch(ctx, k_quant_lut, dim3(LUT_CELLS / Q_THREADS, (uint32_t)lj.size()), Q_THREADS, 0, d_lj));
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_pal.data(), d_pal, nq * 256 * 4, cudaMemcpyDeviceToHost, ctx->stream));
         if (!mj.empty()) {
             const uint64_t want = (uint64_t)ctx->sm_count * 8 / mj.size() + 1;
             const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, (npix + Q_THREADS * MAP_PX - 1) / (Q_THREADS * MAP_PX)));
-            k_quant_map<<<dim3(ctas, (uint32_t)mj.size()), Q_THREADS, 0, ctx->stream>>>(d_mj, npix, bpp);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_quant_map, dim3(ctas, (uint32_t)mj.size()), Q_THREADS, 0, d_mj, npix, bpp));
         }
         uint32_t *d_tick = reinterpret_cast<uint32_t *>(base + o_tick);
         if (!dj.empty()) {
             PIXO_CUDA(ctx, cudaMemsetAsync(base + o_prog, 0, nq * groups * 4, ctx->stream));
             PIXO_CUDA(ctx, cudaMemsetAsync(d_tick, 0, 8, ctx->stream));
-            static bool attr_set[64];
-            if (!attr_set[ctx->device & 63]) {
+            bool &carveout_set = ctx->kernels[reinterpret_cast<const void *>(k_quant_dither)].carveout_set;
+            if (!carveout_set) {
                 PIXO_CUDA(ctx, cudaFuncSetAttribute(k_quant_dither, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-                attr_set[ctx->device & 63] = true;
+                carveout_set = true;
             }
             DitherParams D{d_dj, (uint32_t)dj.size(), width, height, bpp, (uint32_t)groups, d_tick};
             const uint64_t warps = std::min<uint64_t>((uint64_t)dj.size() * groups, (uint64_t)ctx->sm_count * 32);
-            k_quant_dither<<<(uint32_t)((warps + DITHER_WARPS - 1) / DITHER_WARPS), DITHER_WARPS * 32, 0, ctx->stream>>>(D);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_quant_dither, (uint32_t)((warps + DITHER_WARPS - 1) / DITHER_WARPS), DITHER_WARPS * 32,
+                            0, D));
         }
         uint32_t h_tick[2] = {0, 0};
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_tick, d_tick, 8, cudaMemcpyDeviceToHost, ctx->stream));

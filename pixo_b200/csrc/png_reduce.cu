@@ -358,9 +358,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
             const uint32_t nb = std::min(n_images - i0, 65535u);
             AnalyzeParams Ai = A;
             Ai.data = d_data + (size_t)i0 * in_stride; Ai.stat = d_stat + i0;
-            k_reduce_analyze<<<dim3(ctas, nb), RED_THREADS, 0, ctx->stream>>>(Ai);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_reduce_analyze, dim3(ctas, nb), RED_THREADS, 0, Ai));
         }
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_stat, d_stat, stat_bytes, cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -424,13 +422,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         }
         PIXO_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs.data(), np * sizeof(IndexJob), cudaMemcpyHostToDevice, ctx->stream));
         if (any_stats) PIXO_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, np * cnt_words * 4, ctx->stream));
-        const size_t smem = (512 + (size_t)nmax * (nmax > 0 ? nmax - 1 : 0) / 2) * 4;
-        static bool attr_set[64];
-        if (!attr_set[ctx->device & 63]) {
-            PIXO_CUDA(ctx, cudaFuncSetAttribute(k_reduce_index, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                (int)((512 + TRI_MAX) * 4)));
-            attr_set[ctx->device & 63] = true;
-        }
+        const Smem smem{(512 + (size_t)nmax * (nmax > 0 ? nmax - 1 : 0) / 2) * 4, (512 + (size_t)TRI_MAX) * 4};
         // about two waves of CTAs over the whole batch, at least 8192 pixels each
         const uint64_t want_ctas = (uint64_t)ctx->sm_count * 2;
         uint64_t per = (npix * np + want_ctas - 1) / want_ctas;
@@ -443,9 +435,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         for (size_t k0 = 0; k0 < np; k0 += 65535) {
             const uint32_t nb = (uint32_t)std::min<size_t>(np - k0, 65535);
             I.jobs = d_jobs + k0;
-            k_reduce_index<<<dim3(ctas, nb), RED_THREADS, smem, ctx->stream>>>(I);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_reduce_index, dim3(ctas, nb), RED_THREADS, smem, I));
         }
         std::vector<uint32_t> h_cnt;
         if (any_stats) {
@@ -532,9 +522,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         for (size_t k0 = 0; k0 < pack.size(); k0 += 65535) {
             const uint32_t nb = (uint32_t)std::min<size_t>(pack.size() - k0, 65535);
             K.jobs = reinterpret_cast<const PackJob *>(base) + k0;
-            k_reduce_pack<<<dim3(ctas, nb), RED_THREADS, 0, ctx->stream>>>(K);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            PIXO_TRY(launch(ctx, k_reduce_pack, dim3(ctas, nb), RED_THREADS, 0, K));
         }
     }
     // the host vectors copied asynchronously above must outlive the copies

@@ -193,20 +193,16 @@ int launch_simple(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, uin
     // pixel-wide loads when every frame's base, every row and every pixel are aligned to them
     const uintptr_t al = (uintptr_t)src | (uintptr_t)dst | (n > 1 ? (src_stride | dst_stride) : 0);
     const bool wide = (BPP == 2 || BPP == 4) && al % BPP == 0;
+    const auto kern = alg == 1 ? k_resize_bilinear<BPP>
+                      : wide   ? k_resize_nearest<BPP, (BPP == 2 || BPP == 4) ? BPP : 1>
+                               : k_resize_nearest<BPP, 1>;
+    const float xr = alg == 1 ? xb : xn, yr = alg == 1 ? yb : yn;
     for (uint32_t f0 = 0; f0 < n; f0 += 65535) {
         const uint32_t nf = std::min<uint32_t>(n - f0, 65535);
         const uint8_t *s = src + (size_t)f0 * src_stride;
         uint8_t *d = dst + (size_t)f0 * dst_stride;
-        const dim3 g = grid_for(ctx, dw, dh, nf);
-        if (alg == 1)
-            k_resize_bilinear<BPP><<<g, kThreads, 0, ctx->stream>>>(s, src_stride, sw, sh, d, dst_stride, dw, dh, xb, yb);
-        else if (wide)
-            k_resize_nearest<BPP, (BPP == 2 || BPP == 4) ? BPP : 1>
-                <<<g, kThreads, 0, ctx->stream>>>(s, src_stride, sw, sh, d, dst_stride, dw, dh, xn, yn);
-        else
-            k_resize_nearest<BPP, 1><<<g, kThreads, 0, ctx->stream>>>(s, src_stride, sw, sh, d, dst_stride, dw, dh, xn, yn);
-        ctx->launches++;
-        PIXO_CUDA(ctx, cudaGetLastError());
+        PIXO_TRY(launch(ctx, kern, grid_for(ctx, dw, dh, nf), kThreads, 0, s, src_stride, sw, sh, d, dst_stride, dw, dh,
+                        xr, yr));
     }
     return 0;
 }
@@ -257,11 +253,10 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
     resize_axis(sw, dw, true, h);
     resize_axis(sh, dh, true, v);
     // tables: h start/count, v start/count (u32), h/v offsets (u64), h/v weights (f32), each 256-aligned
-    auto al = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t o_hs = 0, o_hc = o_hs + al(4 * (size_t)dw), o_vs = o_hc + al(4 * (size_t)dw),
-                 o_vc = o_vs + al(4 * (size_t)dh), o_ho = o_vc + al(4 * (size_t)dh), o_vo = o_ho + al(8 * (size_t)dw),
-                 o_hw = o_vo + al(8 * (size_t)dh), o_vw = o_hw + al(4 * h.w.size() + 4),
-                 total = o_vw + al(4 * v.w.size() + 4);
+    const size_t o_hs = 0, o_hc = o_hs + align_up(4 * (size_t)dw, 256), o_vs = o_hc + align_up(4 * (size_t)dw, 256),
+                 o_vc = o_vs + align_up(4 * (size_t)dh, 256), o_ho = o_vc + align_up(4 * (size_t)dh, 256), o_vo = o_ho + align_up(8 * (size_t)dw, 256),
+                 o_hw = o_vo + align_up(8 * (size_t)dh, 256), o_vw = o_hw + align_up(4 * h.w.size() + 4, 256),
+                 total = o_vw + align_up(4 * v.w.size() + 4, 256);
     PIXO_TRY(ensure_dev(ctx, ctx->d_resize, total));
     uint8_t *T = reinterpret_cast<uint8_t *>(ctx->d_resize.ptr);
     const struct { size_t off; const void *p; size_t bytes; } up[] = {
@@ -289,16 +284,11 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
         const uint8_t *s = src + (size_t)f0 * src_stride;
         uint8_t *d = dst + (size_t)f0 * dst_stride;
         for (const Band &b : bands) {
-            if (b.re > b.rs) {
-                k_resize_lanczos_h<BPP><<<grid_for(ctx, b.cw, b.re - b.rs, nf), kThreads, 0, ctx->stream>>>(
-                    s, src_stride, sw, b.rs, b.re, b.x0, b.cw, hs, hc, ho, hw, tmp, tstride);
-                ctx->launches++;
-                PIXO_CUDA(ctx, cudaGetLastError());
-            }
-            k_resize_lanczos_v<BPP><<<grid_for(ctx, b.cw, b.y1 - b.y0, nf), kThreads, 0, ctx->stream>>>(
-                tmp, tstride, b.rs, b.cw, b.y0, b.y1, b.x0, vs, vc, vo, vw, d, dst_stride, dw);
-            ctx->launches++;
-            PIXO_CUDA(ctx, cudaGetLastError());
+            if (b.re > b.rs)
+                PIXO_TRY(launch(ctx, k_resize_lanczos_h<BPP>, grid_for(ctx, b.cw, b.re - b.rs, nf), kThreads, 0, s,
+                                src_stride, sw, b.rs, b.re, b.x0, b.cw, hs, hc, ho, hw, tmp, tstride));
+            PIXO_TRY(launch(ctx, k_resize_lanczos_v<BPP>, grid_for(ctx, b.cw, b.y1 - b.y0, nf), kThreads, 0, tmp,
+                            tstride, b.rs, b.cw, b.y0, b.y1, b.x0, vs, vc, vo, vw, d, dst_stride, dw));
         }
     }
     return 0;
