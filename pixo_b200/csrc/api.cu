@@ -327,7 +327,7 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw,
+    Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw, &ctx->d_hwin,
                        &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis,
                        &ctx->d_prog, &ctx->d_prog_raw, &ctx->d_prog_out, &ctx->d_resize, &ctx->d_resize_tmp};
     for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);

@@ -74,7 +74,7 @@ private:
 
 // Device scratch layout of the entropy stage for n images (all sizes in bytes, 256-aligned)
 struct EntropyPlan {
-    size_t nchunks;
+    size_t nunits;                 // k_huff work units per image
     size_t off_st1, off_st2, off_ticket, off_ovf, zero_bytes, off_outlen, off_tail, total;
 };
 
@@ -139,6 +139,7 @@ struct pixo_b200_ctx {
     std::string err;
     // reusable scratch (device + pinned host)
     pixo::Scratch d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
+    pixo::Scratch d_hwin;                        // k_huff: every warp's assembled unit, from its phase A to its phase B
     pixo::Scratch d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
     pixo::Scratch d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
     pixo::Scratch d_trellis, h_trellis;          // JPEG trellis: status word + f32 DCT blocks; its status on the host

@@ -10,26 +10,28 @@
 // One kernel, one pass over the coefficients (k_huff).  The DC predictor of a block is the
 // previous block of the same component in the coefficient array, so every block's code is
 // independent of the others; only its POSITION in the stream is not.  The kernel is persistent
-// and every warp works alone (warp-level synchronisation only): it draws a chunk of 32
-// consecutive blocks (scan order) of one image from a ticket counter, then
-//   1. each lane codes its block once into a private shared-memory slot; a 64-bit non-zero mask
-//      drives the symbol loop, so the loop runs once per non-zero coefficient and there is a single,
-//      small copy of the symbol code.  The encode paths hand over the transform's coefficient records
-//      (CoefExtents, common.cuh): the lane loads the block's extent, then only the 32-byte sectors
-//      the transform wrote, already in zig-zag order.  Caller arrays (the CHECK instantiations) are
-//      dense and in natural order: the zig-zag reorder happens in registers on the way in.  Either
-//      way the mask is computed from the words;
-//   2. the block bit lengths are scanned in the warp; the chunk total enters a decoupled
-//      look-back chain (one status word per chunk: bit count + the chunk's last 7 bits), which
-//      yields the chunk's bit offset in the image's stream and the partial byte it inherits;
+// and every warp works alone (warp-level synchronisation only): it draws a unit of 96
+// consecutive blocks (scan order, whole MCUs) of one image from a ticket counter, then
+//   1. codes them in three passes of one block per lane, each pass of one component, every block
+//      once into a private shared-memory slot; a 64-bit non-zero mask drives the symbol loop, so the
+//      loop runs once per non-zero coefficient and there is a single, small copy of the symbol code.
+//      The encode paths hand over the transform's coefficient records (CoefExtents, common.cuh):
+//      the lane loads the block's extent, then only the 32-byte sectors the transform wrote, already
+//      in zig-zag order.  Caller arrays (the CHECK instantiations) are dense and in natural order:
+//      the zig-zag reorder happens in registers on the way in.  Either way the mask is computed from
+//      the words;
+//   2. the 96 bit lengths are scanned in scan order; the unit total enters a decoupled look-back
+//      chain (one status word per unit: bit count + the unit's last 7 bits), which yields the
+//      unit's bit offset in the image's stream and the partial byte it inherits;
 //   3. the slots are funnel-shifted into a shared window aligned to the stream's 32-bit words;
-//   4. the chunk owns every byte whose last bit it wrote.  It counts its 0xFF bytes, a second
-//      look-back chain turns those counts into the number of stuffed zeros before the chunk, and
-//      the window is copied out with the 0x00s inserted, 16 bytes per store.
-// Tickets are dispensed chunk-major across the images of a batch, so their chains advance side
-// by side.  Nothing but the final scan bytes is written to global memory.  Restart intervals
+//   4. the unit owns every byte whose last bit it wrote.  It counts its 0xFF bytes, a second
+//      look-back chain turns those counts into the number of stuffed zeros before the unit, and
+//      the assembled bytes, parked meanwhile in a per-warp global buffer, are copied out with the
+//      0x00s inserted, 16 bytes per store.
+// One ticket, two look-backs and one window sweep serve 96 blocks.  Tickets are dispensed
+// unit-major across the images of a batch, so their chains advance side by side.  Restart intervals
 // (handle_restart, src/jpeg/mod.rs:1423-1445) run here too: every interval is a bit stream of its
-// own (chunks never straddle one, chain 1 restarts with it, its last chunk pads and appends the
+// own (units never straddle one, chain 1 restarts with it, its last unit pads and appends the
 // RSTn marker), while chain 2 - every byte written so far - runs across the whole image.
 #include "common.cuh"
 #include "jpeg_host.hpp"
@@ -59,14 +61,14 @@ struct EntParams {
     uint32_t bpm;                  // blocks per MCU in scan order: 6 (4:2:0), 3 (4:4:4), 1 (gray)
     uint32_t y_per_mcu;            // 4, 1, 1
     uint32_t nblocks;              // per image, scan order
-    uint32_t nchunks;              // per image
-    uint32_t rst_mcus;             // restart interval in MCUs, 0 = none (a chunk never straddles an interval)
+    uint32_t nunits;               // per image
+    uint32_t rst_mcus;             // restart interval in MCUs, 0 = none (a unit never straddles an interval)
     uint32_t rst_blocks;           // ... in blocks
-    uint32_t cpi;                  // chunks per full interval
+    uint32_t upi;                  // units per full interval
     uint32_t nimages;
-    unsigned long long *st_bits;   // [n][nchunks] look-back chain 1: stream bits
-    unsigned long long *st_ff;     // [n][nchunks] look-back chain 2: 0xFF bytes
-    uint32_t *ticket;              // chunk dispenser (launch order == dependency order)
+    unsigned long long *st_bits;   // [n][nunits] look-back chain 1: stream bits
+    unsigned long long *st_ff;     // [n][nunits] look-back chain 2: 0xFF bytes
+    uint32_t *ticket;              // unit dispenser (launch order == dependency order)
     uint8_t *out;                  // [n][out_cap]
     uint64_t out_cap;
     uint64_t *out_len;             // [n] final byte count
@@ -76,6 +78,7 @@ struct EntParams {
     uint32_t seg_per_img;
     uint32_t nblocks_last;         // blocks of an image's last segment (the others have nblocks)
     size_t seg_y_stride, seg_c_stride;   // int16 elements between the segments of an image
+    uint8_t *win;                  // !RAW: [grid * HUFF_WARPS][GWIN_B] each warp's assembled unit, from phase A to B
     const int *dc_seed_dev;        // the same three predictors in device memory (stream-ordered callers), or null
     int dc_seed[3];                // DC predictors (Y, Cb, Cr) before block 0: 0 for a whole image, the previous
                                    // band's last DCs when the arrays are one band of a frame tiled over several GPUs
@@ -84,16 +87,22 @@ struct EntParams {
                                    // bit 3: a coefficient outside the baseline range (see code_block)
 };
 
-constexpr int CB = 32;             // blocks per chunk == one warp
+constexpr int CB = 32;             // blocks coded side by side == one warp
 static_assert(CB * 4 == 128, "the slot word stride is spelled out in code_block's PTX");
+constexpr int NPASS = 3;           // passes of 32 blocks per unit
+constexpr int UB = NPASS * CB;     // blocks per unit: 16 MCUs of 4:2:0, 32 of 4:4:4, 96 gray blocks
 constexpr int HUFF_WARPS = 4;      // warps per CTA (they only share the tables)
-constexpr int HUFF_CTAS_PER_SM = 6;
+constexpr int HUFF_CTAS_PER_SM = 5;
 constexpr int SLOT_W = 16;         // words of a block's code kept in shared memory (16: 512 bits)
 constexpr int MAX_W = 54;          // worst case: 27 + 63 * 26 = 1665 bits
-constexpr int WIN_W = 256;         // stream words assembled per round (32 bytes per lane)
+constexpr int SUB_W = 256;         // window words per emitted piece (32 bytes per lane)
+constexpr int SUB_B = SUB_W * 4;
+constexpr int WIN_W = 1024;        // stream words assembled per round (the stage: a q80 noise unit, ~2.8 KB, in one)
 constexpr int WIN_B = WIN_W * 4;
-static_assert(WIN_B <= SLOT_W * CB * 4, "phase A parks the assembled window in the chunk's slot buffer");
-constexpr int SBUF_B = 2 * WIN_B + 48;    // stuffed bytes of a window + alignment slack + the head pad
+constexpr int SBUF_B = 2 * SUB_B + 48;    // stuffed bytes of a piece + alignment slack + the head pad
+constexpr int GWIN_B = 20 * SUB_B;        // a warp's assembled unit in global memory, whole pieces
+static_assert(UB * 1665 / 8 + 8 <= GWIN_B, "the longest unit (every block 1665 bits) + its head and padding bytes");
+static_assert(WIN_B % SUB_B == 0 && GWIN_B % WIN_B == 0, "rounds hold whole pieces, the parked unit whole rounds");
 constexpr uint32_t SPIN_LIMIT = 1u << 22;
 constexpr int LB_GROUPS = 4;       // look-back window: 32 * LB_GROUPS predecessors per step
 
@@ -116,8 +125,8 @@ __device__ __forceinline__ unsigned long long pack_status(unsigned long long fla
     return flag | ((unsigned long long)(tail & 0x7F) << 55) | (value & ST_VAL);
 }
 
-// Exclusive prefix over chunks [0, chunk) of one image (whole warp; decoupled look-back, 128
-// predecessors per step, four per lane).  tail_in = the 7-bit tail published by chunk-1.
+// Exclusive prefix over units [0, chunk) of one image (whole warp; decoupled look-back, 128
+// predecessors per step, four per lane).  tail_in = the 7-bit tail published by unit chunk-1.
 // Returns the prefix in the low 55 bits, tail_in in bits 55..61, bit 62 = the chain timed out.
 // (Inlined at both call sites.)
 __device__ __forceinline__ unsigned long long look_back(const unsigned long long *st, int chunk, int lane)
@@ -149,7 +158,7 @@ __device__ __forceinline__ unsigned long long look_back(const unsigned long long
             const uint32_t pm = __ballot_sync(0xffffffffu, flag == 2);
             const int stop = pm ? __ffs(pm) - 1 : 32;           // nearest inclusive prefix, if any
             if (inv & ((2u << min(stop, 31)) - 1u)) { retry = true; break; }
-            // aggregates are small (a chunk's bits / bytes): one 32-bit warp reduction
+            // aggregates are small (a unit's bits / bytes, < 2^18): one 32-bit warp reduction
             step += __reduce_add_sync(0xffffffffu, lane < stop ? (uint32_t)v[k] : 0u);
             if (pm) { step += __shfl_sync(0xffffffffu, v[k], stop) & ST_VAL; done = true; break; }
         }
@@ -320,53 +329,60 @@ __device__ __forceinline__ uint32_t warp_scan(uint32_t x, int lane, uint32_t *to
     return inc - x;
 }
 
-// Shared memory of one warp.  Two chunks are in flight (see k_huff), each with its own slots.
-// The coefficient stage is dead once a chunk's blocks are coded; the stream window and the
-// stuffed bytes reuse it.
+// Shared memory of one warp.  The coefficient stage is dead once a unit's blocks are coded; the
+// blocks' lengths and offsets (scan order), the stream window of phase A and the stuffed bytes of
+// phase B reuse it.
 struct WarpMem {
-    uint32_t slot[2][SLOT_W * CB];
+    uint32_t slot[NPASS][SLOT_W * CB];     // slot[p]: the codes of pass p, word k of lane l at k * CB + l
     union {
-        uint32_t stage[32 * CB];
-        struct {
-            uint32_t obuf[WIN_W];
-            uint8_t sbuf[SBUF_B];
-        } w;
+        uint32_t stage[32 * CB];           // one pass's coefficients, word j of lane l at j * CB + l
+        uint32_t tl[2 * UB];               // [0, UB): (length << 7) | last 7 bits, then [UB, 2 UB): bit offsets
+        uint32_t obuf[WIN_W];
+        uint8_t sbuf[SBUF_B];
     };
-    uint32_t tl[CB];
 };
 
-// What a warp remembers about a chunk between its phases (lane-private unless noted).
-struct ChunkState {
-    uint32_t chunk, img;   // uniform
-    uint32_t L, o_t;       // this lane's block: code length, bit offset inside the chunk
-    int nwt;               // words the block occupies
-    uint32_t Lc, ctail;    // uniform: chunk bits, its last 7 bits
-    int buf;               // slot / spill buffer
-    unsigned long long Pc; // uniform: bits before the chunk (after phase A)
-    uint32_t tailin;       // uniform: the 7 bits before the chunk
-    uint32_t Ftot;         // uniform: 0xFF bytes the chunk owns
-    uint32_t own;          // uniform: output bytes the chunk writes (owned + stuffed zeros + RSTn marker)
-    uint32_t marker;       // uniform: 0xD0..0xD7 when the chunk closes a restart interval, else 0
-    bool first, last, final_; // uniform: first / last chunk of its bit stream (image or interval); last of the image
-    uint32_t ffb;          // 0xFF bytes before this lane's piece of the kept window
-    bool kept;             // uniform: phase A left the assembled (single) window in the slot buffer
+// What a warp remembers about a unit between its phases (lane-private unless noted).
+struct UnitState {
+    uint32_t unit, img;    // uniform
+    uint32_t L[NPASS];     // this lane's block of pass p: code length,
+    uint32_t o_t[NPASS];   // ... bit offset inside the unit,
+    int nwt[NPASS];        // ... words it occupies
+    uint32_t Lc, ctail;    // uniform: unit bits, its last 7 bits
+    unsigned long long Pc; // uniform: bits before the unit (after phase A)
+    uint32_t tailin;       // uniform: the 7 bits before the unit
+    uint32_t own;          // uniform: output bytes the unit writes (owned + stuffed zeros + RSTn marker)
+    uint32_t marker;       // uniform: 0xD0..0xD7 when the unit closes a restart interval, else 0
+    bool first, last, final_; // uniform: first / last unit of its bit stream (image or interval); last of the image
     bool fault;
-    bool skip;             // uniform: the chunk lies past the end of a short last segment: nothing to do
+    bool skip;             // uniform: the unit lies past the end of a short last segment: nothing to do
 };
 
-// Persistent kernel; every WARP works on its own: it draws chunks of 32 blocks from the ticket
-// counter and takes each through three phases with warp-level synchronisation only,
-//   W  code the blocks into slots, publish the chunk's bit count              (chain 1)
+// Persistent kernel; every WARP works on its own: it draws units of 96 blocks (whole MCUs of one
+// image, in scan order) from the ticket counter and takes each through three phases with
+// warp-level synchronisation only,
+//   W  code the blocks into slots, publish the unit's bit count               (chain 1)
 //   A  look back for the bit offset, assemble + count 0xFF, publish the count  (chain 2)
-//   B  look back for the stuffed-byte offset, assemble again, emit
+//   B  look back for the stuffed-byte offset, emit
 // software-pipelined as  A(j) W(j+1) B(j):  a look-back runs a phase after the value it depends
 // on was published by this warp's neighbours in the chain, so it seldom has to wait for them.
+// A assembles the unit once, in windows of WIN_B bytes in shared memory, and parks the bytes in the
+// warp's piece of P.win (L2-resident: a few KB per warp), where B reads them back while W(j+1)
+// reuses the slots and the stage.
+//
+// W codes a unit in three passes of one block per lane, each pass of one component (so the
+// Huffman table is the same across the warp and the lanes' symbol loops are of similar length):
+//   4:2:0  Y of MCUs 0-7 | Y of MCUs 8-15 | Cb (lanes 0-15), Cr (lanes 16-31) of MCUs 0-15
+//   4:4:4  Y | Cb | Cr of MCUs 0-31
+//   gray   blocks 0-31 | 32-63 | 64-95
+// The blocks' bit offsets come from a scan over the 96 lengths in scan order, so the assembly
+// puts every block where the sequential coder would.
 //
 // RAW (the segments of a long image, or of a band of a frame that is tiled over several GPUs): the
 // string starts at a bit of the stream that is not known yet, so nothing that depends on
 // byte alignment can happen here.  Phase A writes the UNSTUFFED bytes of the local string
 // (bit 0 = its first bit, the last partial byte zero-filled, no 1-padding) straight from the
-// assembled windows, phase B and chain 2 do not exist, and the final chunk reports the string's
+// assembled windows, phase B and chain 2 do not exist, and the final unit reports the string's
 // bit count and its last 7 bits.  k_seg_* below splice such strings into scan bytes once their
 // bit offsets are known.
 // CHECK: see code_block; a block with a coefficient outside the baseline range sets overflow bit 3.
@@ -376,28 +392,28 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
 {
     __shared__ HuffDev T;
     __shared__ __align__(16) WarpMem wmem[HUFF_WARPS];
-    static_assert(sizeof(((WarpMem *)0)->w) <= sizeof(((WarpMem *)0)->stage), "window + stuffed bytes must fit the stage");
+    static_assert(SBUF_B <= sizeof(((WarpMem *)0)->stage), "the stuffed bytes must fit the stage");
 
     const int lane = threadIdx.x & 31;
     for (int i = threadIdx.x; i < (int)(sizeof(HuffDev) / 4); i += blockDim.x)
         reinterpret_cast<uint32_t *>(&T)[i] = reinterpret_cast<const uint32_t *>(&Tp)[i];
     __syncthreads();
     WarpMem &M = wmem[threadIdx.x >> 5];
-    uint32_t *const obuf = M.w.obuf;
-    uint8_t *const sbuf = M.w.sbuf;
+    uint32_t *const obuf = M.obuf;
+    uint8_t *const sbuf = M.sbuf;
+    uint8_t *const gwin = RAW ? nullptr : P.win + ((size_t)blockIdx.x * HUFF_WARPS + (threadIdx.x >> 5)) * GWIN_B;
     const uint32_t sa_stage = (uint32_t)__cvta_generic_to_shared(M.stage) + 4u * lane;
-    const uint32_t total_chunks = P.nchunks * P.nimages;
-    uint32_t spill[2][MAX_W - SLOT_W];  // words beyond SLOT_W (long blocks): local memory
+    const uint32_t total_units = P.nunits * P.nimages;
+    uint32_t spill[NPASS][MAX_W - SLOT_W];  // words beyond SLOT_W (long blocks): local memory
 
-    // ---- W: code the lane's block of chunk `id` into slot buffer `buf`, publish the bit count ----
-    auto phase_w = [&](uint32_t id, int buf, ChunkState &C) {
-        // chunk-major dispensing: the n images' chains advance side by side
-        C.chunk = id / P.nimages;
-        C.img = id - C.chunk * P.nimages;
-        C.buf = buf;
+    // ---- W: code the unit's blocks into the slots, publish the bit count ------------------------------
+    auto phase_w = [&](uint32_t id, UnitState &C) {
+        // unit-major dispensing: the n images' chains advance side by side
+        C.unit = id / P.nimages;
+        C.img = id - C.unit * P.nimages;
         C.fault = false;
-        // the chunk's place: with a restart interval every interval is its own bit stream
-        // (handle_restart, src/jpeg/mod.rs:1423-1445) and is cut into chunks separately
+        // the unit's place: with a restart interval every interval is its own bit stream
+        // (handle_restart, src/jpeg/mod.rs:1423-1445) and is cut into units separately
         uint32_t s0, iend, interval = 0;
         uint32_t nblk = P.nblocks;
         size_t y_off = (size_t)C.img * P.y_stride, c_off = (size_t)C.img * P.c_stride;
@@ -414,146 +430,177 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         }
         C.skip = false;
         if (P.rst_blocks) {
-            interval = C.chunk / P.cpi;
-            const uint32_t sub = C.chunk - interval * P.cpi;
-            s0 = interval * P.rst_blocks + sub * CB;
+            interval = C.unit / P.upi;
+            const uint32_t sub = C.unit - interval * P.upi;
+            s0 = interval * P.rst_blocks + sub * UB;
             iend = (uint32_t)min((unsigned long long)(interval + 1) * P.rst_blocks, (unsigned long long)nblk);
             C.first = sub == 0;
         } else {
-            s0 = C.chunk * CB;
+            s0 = C.unit * UB;
             iend = nblk;
-            C.first = C.chunk == 0;
+            C.first = C.unit == 0;
         }
-        if (s0 >= iend) { C.skip = true; return; }   // short last segment: no such chunk
-        C.last = s0 + CB >= iend;
+        if (s0 >= iend) { C.skip = true; return; }   // short last segment: no such unit
+        C.last = s0 + UB >= iend;
         C.final_ = C.last && iend == nblk;
         C.marker = (C.last && !C.final_) ? 0xD0u + (interval & 7u) : 0u;
-        const uint32_t s = s0 + lane;
-        const int nv = (int)min((uint32_t)CB, iend - s0);
-        uint32_t *const slot = M.slot[buf];
-        uint32_t L = 0, tail7 = 0;
-        int nwt = 0;
-        uint32_t M0 = 0, M1 = 0;
-        int diff = 0, tbl = 0;
-        if (s < iend) {
-            const uint32_t m = s / P.bpm;
-            const uint32_t k = s - m * P.bpm;
-            const int16_t *arr;
-            const uint8_t *earr;   // !CHECK: the array's extents (P.e is null otherwise)
-            size_t idx, eidx;
-            int seed;
-            if (k < P.y_per_mcu) { arr = P.y + y_off; earr = P.e.y; idx = (size_t)m * P.y_per_mcu + k; eidx = ey_off + idx; tbl = 0; seed = P.dc_seed[0]; }
-            else if (k == P.y_per_mcu) { arr = P.cb + c_off; earr = P.e.cb; idx = m; eidx = ec_off + idx; tbl = 1; seed = P.dc_seed[1]; }
-            else { arr = P.cr + c_off; earr = P.e.cr; idx = m; eidx = ec_off + idx; tbl = 1; seed = P.dc_seed[2]; }
-            // DC predictors restart with the interval (src/jpeg/mod.rs:1433-1443)
-            const bool dc_reset = P.rst_mcus && m % P.rst_mcus == 0 && (k == 0 || k >= P.y_per_mcu);
-            // (a later segment's first block follows the previous segment's last one in the same array)
-            if (P.dc_seed_dev && idx == 0 && !seg_prev) seed = P.dc_seed_dev[k < P.y_per_mcu ? 0 : (k == P.y_per_mcu ? 1 : 2)];
-            const int prev_dc = dc_reset ? 0 : ((idx || seg_prev) ? arr[((long long)idx - 1) * 64] : seed);
-            const uint4 *src = reinterpret_cast<const uint4 *>(arr + idx * 64);
-            int dc;
-            uint32_t w[32];  // the block in zig-zag order: word j = coefficients zz(2j), zz(2j+1)
-            if (CHECK) {
-                uint32_t n[32];  // the caller's block: natural order, two coefficients per word
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const uint4 v = __ldg(src + q);
-                    n[q * 4] = v.x; n[q * 4 + 1] = v.y; n[q * 4 + 2] = v.z; n[q * 4 + 3] = v.w;
-                }
-                dc = (int)(int16_t)(n[0] & 0xFFFF);
-                // zig-zag reorder (zigzag_reorder, src/jpeg/quantize.rs:107-113) on the way into the
-                // stage; all indices are compile-time
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int i0 = zz_nat(2 * j), i1 = zz_nat(2 * j + 1);
-                    w[j] = __byte_perm(n[i0 >> 1], n[i1 >> 1],
-                                       ((i0 & 1) ? 0x0032 : 0x0010) | ((i1 & 1) ? 0x7600 : 0x5400));
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) M.stage[j * CB + lane] = w[j];
+        // units, intervals and segments are whole MCUs: a short unit has empty lanes
+        const uint32_t nv = min((uint32_t)UB, iend - s0);
+        const uint32_t bpm = P.bpm, ypm = P.y_per_mcu, mu0 = s0 / bpm;
+        uint32_t srel[NPASS], t7[NPASS];
+#pragma unroll 1
+        for (int p = 0; p < NPASS; ++p) {
+            uint32_t mm, kk, comp;   // this lane's block: MCU inside the unit, place inside the MCU, component
+            if (ypm == 4) {
+                if (p < 2) { mm = 8 * p + (lane >> 2); kk = lane & 3; comp = 0; }
+                else { mm = lane & 15; kk = 4 + (lane >> 4); comp = 1 + (lane >> 4); }
+            } else if (bpm == 3) {
+                mm = lane; kk = p; comp = p;
             } else {
-                // the transform's record, already in zig-zag order: its written sectors (sector 0 is
-                // always there, so its load does not wait for the extent), zeros for the rest.  The
-                // symbol loop reads only the stage words of non-zero coefficients, so only the
-                // record's words are staged.
-                const int np = 2 * __ldg(earr + eidx);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const uint4 v = (q < 2 || q < np) ? __ldg(src + q) : make_uint4(0, 0, 0, 0);
-                    w[q * 4] = v.x; w[q * 4 + 1] = v.y; w[q * 4 + 2] = v.z; w[q * 4 + 3] = v.w;
+                mm = 32 * p + lane; kk = 0; comp = 0;
+            }
+            const uint32_t sr = mm * bpm + kk;   // scan position inside the unit
+            const bool valid = sr < nv;
+            uint32_t *const slot = M.slot[p];
+            uint32_t L = 0, tail7 = 0;
+            int nwt = 0;
+            if (__any_sync(0xffffffffu, valid)) {   // (a short last unit may leave a whole pass empty)
+                const uint32_t m = mu0 + mm;
+                const int16_t *arr;
+                const uint8_t *earr;   // !CHECK: the array's extents (P.e is null otherwise)
+                size_t idx, eidx;
+                int seed;
+                if (comp == 0) { arr = P.y + y_off; earr = P.e.y; idx = (size_t)m * ypm + kk; eidx = ey_off + idx; seed = P.dc_seed[0]; }
+                else if (comp == 1) { arr = P.cb + c_off; earr = P.e.cb; idx = m; eidx = ec_off + idx; seed = P.dc_seed[1]; }
+                else { arr = P.cr + c_off; earr = P.e.cr; idx = m; eidx = ec_off + idx; seed = P.dc_seed[2]; }
+                // The DC predictor is the previous block of the same component, which the lane to the
+                // left codes in this pass - except at lane 0 and at the first Cr lane of 4:2:0: those
+                // load it (or reset it: a restart interval's first MCU, src/jpeg/mod.rs:1433-1443).
+                const bool from_left = lane != 0 && !(ypm == 4 && p == 2 && lane == 16);
+                int prev_ld = 0;
+                if (valid && !from_left) {
+                    const bool dc_reset = P.rst_mcus && C.first && mm == 0;
+                    // (a later segment's first block follows the previous segment's last one in the same array)
+                    if (P.dc_seed_dev && idx == 0 && !seg_prev) seed = P.dc_seed_dev[comp];
+                    prev_ld = dc_reset ? 0 : ((idx || seg_prev) ? arr[((long long)idx - 1) * 64] : seed);
                 }
-                dc = (int)(int16_t)(w[0] & 0xFFFF);
+                int dc = 0;
+                uint32_t M0 = 0, M1 = 0;
+                if (valid) {
+                    const uint4 *src = reinterpret_cast<const uint4 *>(arr + idx * 64);
+                    uint32_t w[32];  // the block in zig-zag order: word j = coefficients zz(2j), zz(2j+1)
+                    if (CHECK) {
+                        uint32_t n[32];  // the caller's block: natural order, two coefficients per word
 #pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    if (q < 2 || q < np) {
+                        for (int q = 0; q < 8; ++q) {
+                            const uint4 v = __ldg(src + q);
+                            n[q * 4] = v.x; n[q * 4 + 1] = v.y; n[q * 4 + 2] = v.z; n[q * 4 + 3] = v.w;
+                        }
+                        dc = (int)(int16_t)(n[0] & 0xFFFF);
+                        // zig-zag reorder (zigzag_reorder, src/jpeg/quantize.rs:107-113) on the way into the
+                        // stage; all indices are compile-time
 #pragma unroll
-                        for (int t = 0; t < 4; ++t) M.stage[(q * 4 + t) * CB + lane] = w[q * 4 + t];
+                        for (int j = 0; j < 32; ++j) {
+                            const int i0 = zz_nat(2 * j), i1 = zz_nat(2 * j + 1);
+                            w[j] = __byte_perm(n[i0 >> 1], n[i1 >> 1],
+                                               ((i0 & 1) ? 0x0032 : 0x0010) | ((i1 & 1) ? 0x7600 : 0x5400));
+                        }
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) M.stage[j * CB + lane] = w[j];
+                    } else {
+                        // the transform's record, already in zig-zag order: its written sectors (sector 0 is
+                        // always there, so its load does not wait for the extent), zeros for the rest.  The
+                        // symbol loop reads only the stage words of non-zero coefficients, so only the
+                        // record's words are staged.
+                        const int np = 2 * __ldg(earr + eidx);
+#pragma unroll
+                        for (int q = 0; q < 8; ++q) {
+                            const uint4 v = (q < 2 || q < np) ? __ldg(src + q) : make_uint4(0, 0, 0, 0);
+                            w[q * 4] = v.x; w[q * 4 + 1] = v.y; w[q * 4 + 2] = v.z; w[q * 4 + 3] = v.w;
+                        }
+                        dc = (int)(int16_t)(w[0] & 0xFFFF);
+#pragma unroll
+                        for (int q = 0; q < 8; ++q) {
+                            if (q < 2 || q < np) {
+#pragma unroll
+                                for (int t = 0; t < 4; ++t) M.stage[(q * 4 + t) * CB + lane] = w[q * 4 + t];
+                            }
+                        }
+                    }
+                    asm volatile("" ::: "memory");  // the stage is read back through ld.shared below
+                    {   // bit i = zig-zag coefficient i != 0
+                        uint32_t e0 = 0, e1 = 0;
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            e0 += __vminu2(w[j], 0x00010001u) * (1u << j);       // disjoint bits: + is |
+                            e1 += __vminu2(w[16 + j], 0x00010001u) * (1u << j);
+                        }
+                        M0 = interleave16(e0); M1 = interleave16(e1);
                     }
                 }
-            }
-            asm volatile("" ::: "memory");  // the stage is read back through ld.shared below
-            {   // bit i = zig-zag coefficient i != 0
-                uint32_t e0 = 0, e1 = 0;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    e0 += __vminu2(w[j], 0x00010001u) * (1u << j);       // disjoint bits: + is |
-                    e1 += __vminu2(w[16 + j], 0x00010001u) * (1u << j);
+                const int left = __shfl_up_sync(0xffffffffu, dc, 1);
+                const int diff = (int)(int16_t)(dc - (from_left ? left : prev_ld));
+                if (valid) {
+                    const int tbl = comp ? 1 : 0;   // the same in every lane of the pass
+                    const uint32_t sa_ac = (uint32_t)__cvta_generic_to_shared(&T.ac[tbl][0]);
+                    const uint32_t sa_slot = (uint32_t)__cvta_generic_to_shared(slot) + 4u * lane;
+                    uint32_t acc;
+                    bool bad;
+                    L = code_block<false, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
+                    if (L > SLOT_W * 32u)  // long block: run again, keeping the words past the slot in local memory
+                        L = code_block<true, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
+                    if (CHECK && bad) atomicOr(&P.overflow[C.img], 8u);
+                    asm volatile("" ::: "memory");  // slot words were written through st.shared
+                    const int nw = (int)(L >> 5), filled = (int)(L & 31u);
+                    nwt = nw;
+                    if (filled) {
+                        if (nw < SLOT_W) slot[nw * CB + lane] = acc; else spill[p][nw - SLOT_W] = acc;
+                        nwt = nw + 1;
+                    }
+                    const uint32_t lastw = nw == 0 ? 0u : (nw - 1 < SLOT_W ? slot[(nw - 1) * CB + lane] : spill[p][nw - 1 - SLOT_W]);
+                    tail7 = __funnelshift_rc(acc, lastw, 32 - filled) & 0x7Fu;
                 }
-                M0 = interleave16(e0); M1 = interleave16(e1);
             }
-            diff = (int)(int16_t)(dc - prev_dc);
+            if (p == 0) { C.L[0] = L; C.nwt[0] = nwt; t7[0] = tail7; srel[0] = sr; }
+            else if (p == 1) { C.L[1] = L; C.nwt[1] = nwt; t7[1] = tail7; srel[1] = sr; }
+            else { C.L[2] = L; C.nwt[2] = nwt; t7[2] = tail7; srel[2] = sr; }
         }
-        if (s < iend) {
-            const uint32_t sa_ac = (uint32_t)__cvta_generic_to_shared(&T.ac[tbl][0]);
-            const uint32_t sa_slot = (uint32_t)__cvta_generic_to_shared(slot) + 4u * lane;
-            uint32_t acc;
-            bool bad;
-            L = code_block<false, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc, &bad);
-            if (L > SLOT_W * 32u)  // long block: run again, keeping the words past the slot in local memory
-                L = code_block<true, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[buf], &acc, &bad);
-            if (CHECK && bad) atomicOr(&P.overflow[C.img], 8u);
-            asm volatile("" ::: "memory");  // slot words were written through st.shared
-            const int nw = (int)(L >> 5), filled = (int)(L & 31u);
-            nwt = nw;
-            if (filled) {
-                if (nw < SLOT_W) slot[nw * CB + lane] = acc; else spill[buf][nw - SLOT_W] = acc;
-                nwt = nw + 1;
-            }
-            const uint32_t lastw = nw == 0 ? 0u : (nw - 1 < SLOT_W ? slot[(nw - 1) * CB + lane] : spill[buf][nw - 1 - SLOT_W]);
-            tail7 = __funnelshift_rc(acc, lastw, 32 - filled) & 0x7Fu;
-        }
-        M.tl[lane] = (L << 7) | tail7;
-        __syncwarp();  // every lane is done with the stage; tl[] visible
-        C.L = L;
-        C.nwt = nwt;
-        C.o_t = warp_scan(L, lane, &C.Lc);
+        __syncwarp();  // every lane is done with the stage
+        // the bit offsets: an exclusive scan over the 96 lengths in scan order, positions 3l..3l+2 in lane l
+        uint32_t *const tl = M.tl, *const off = M.tl + UB;
+#pragma unroll
+        for (int p = 0; p < NPASS; ++p) tl[srel[p]] = (C.L[p] << 7) | t7[p];
+        __syncwarp();
+        const uint32_t l0 = tl[3 * lane] >> 7, l1 = tl[3 * lane + 1] >> 7, l2 = tl[3 * lane + 2] >> 7;
+        const uint32_t ex = warp_scan(l0 + l1 + l2, lane, &C.Lc);
+        off[3 * lane] = ex; off[3 * lane + 1] = ex + l0; off[3 * lane + 2] = ex + l0 + l1;
         uint32_t ctail = 0;
-        if (lane == 0) {  // the chunk's last 7 bits (a block has >= 2 bits: at most 4 steps)
+        if (lane == 0) {  // the unit's last 7 bits (a block has >= 2 bits: at most 4 steps)
             int got = 0;
-            for (int k = nv - 1; k >= 0 && got < 7; --k) {
-                const uint32_t x = M.tl[k];
+            for (int k = (int)nv - 1; k >= 0 && got < 7; --k) {
+                const uint32_t x = tl[k];
                 const int take = min((int)(x >> 7), 7 - got);
                 ctail |= (x & ((1u << take) - 1u)) << got;
                 got += take;
             }
-            st_status(P.st_bits + (size_t)C.img * P.nchunks + C.chunk,
+            st_status(P.st_bits + (size_t)C.img * P.nunits + C.unit,
                       pack_status(C.first ? ST_PFX : ST_AGG, ctail, C.Lc));
         }
+        __syncwarp();
+#pragma unroll
+        for (int p = 0; p < NPASS; ++p) C.o_t[p] = off[srel[p]];
         C.ctail = __shfl_sync(0xffffffffu, ctail, 0);
         C.Pc = 0;
         C.tailin = 0;
-        C.Ftot = 0;
         C.own = 0;
-        C.ffb = 0;
-        C.kept = false;
         __syncwarp();
     };
 
-    // ---- stuffed bytes of one window (this lane's 32 bytes in wv) -> sbuf -> global ----------------
-    // a, b: the chunk's owned byte range inside the window; ffb / Fr: 0xFF bytes before this
-    // lane's piece / in the whole window; G: output index of the window's first owned byte.
-    // mk: RSTn marker byte to append after the window's bytes (0 = none).
-    auto emit_window = [&](const ChunkState &C, const uint32_t (&wv)[8], uint32_t ffb, uint32_t Fr, int a, int b,
+    // ---- stuffed bytes of one piece (this lane's 32 bytes in wv) -> sbuf -> global ----------------
+    // a, b: the unit's owned byte range inside the piece; ffb / Fr: 0xFF bytes before this
+    // lane's 32 bytes / in the whole piece; G: output index of the piece's first owned byte.
+    // mk: RSTn marker byte to append after the piece's bytes (0 = none).
+    auto emit_window = [&](const UnitState &C, const uint32_t (&wv)[8], uint32_t ffb, uint32_t Fr, int a, int b,
                            unsigned long long G, uint32_t mk) {
         uint8_t *outp = P.out + (size_t)C.img * P.out_cap;
         const uint32_t nr0 = (uint32_t)max(b - a, 0) + Fr;
@@ -561,7 +608,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         const uint32_t shb = (uint32_t)((reinterpret_cast<uintptr_t>(outp) + G) & 15u);
         // Every lane with owned bytes emits its whole 32-byte piece (bytes outside the owned
         // range land outside the part of sbuf that is copied out); sbuf index 16 + shb is
-        // the chunk's first owned byte of this window.
+        // the unit's first owned byte of this piece.
         if (32 * lane < b) {
             uint32_t dst = 16u + shb + (uint32_t)(32 * lane) - (uint32_t)a + ffb;
             // A lane without a 0xFF among its 32 bytes (all of them on smooth content, ~7 of 8 on
@@ -627,33 +674,34 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         } else if (lane == 0) {
             atomicOr(&P.overflow[C.img], 1u);
         }
-        __syncwarp();  // sbuf is rewritten by the next window, or by the next chunk's stage
+        __syncwarp();  // sbuf is rewritten by the next piece, or by the next unit's stage
     };
 
-    // ---- assemble the chunk's stream window by window; count its 0xFF bytes (EMIT: and write) ----
-    // gbase: output index of the chunk's first owned byte (EMIT only).  Returns the 0xFF count.
-    auto sweep = [&](ChunkState &C, bool emit, unsigned long long gbase) -> uint32_t {
-        const uint32_t *const slot = M.slot[C.buf];
-        const uint32_t *const spl = spill[C.buf];
-        const bool last_chunk = C.last;
-        const uint32_t q0 = (uint32_t)C.Pc & 31u;         // bit offset of the chunk inside window word 0
-        const uint32_t endbit = q0 + C.Lc;                // window bit index one past the chunk
-        const uint32_t padc = (last_chunk && !RAW) ? ((8u - (endbit & 7u)) & 7u) : 0u;   // 1-padding (bits.rs:261-272)
-        const uint32_t ob0 = q0 >> 3;                     // owned window bytes [ob0, ob1)
-        const uint32_t ob1 = RAW ? ((last_chunk ? endbit + 7u : endbit) >> 3) : (endbit >> 3) + (padc ? 1u : 0u);
-        const int nrounds = max(1, (int)((ob1 + WIN_B - 1) / WIN_B));
-        // per-lane constants of the funnel-shifted copy
-        const uint32_t D = q0 + C.o_t;
-        const int d0 = (int)(D >> 5), sh = (int)(D & 31u);
-        const int nd = C.L ? (int)((sh + C.L + 31u) >> 5) : 0;   // destination words
-        const int nwt = C.nwt;
+    // ---- A: the unit's stream, window by window: assemble, then per 1 KB piece count its 0xFF bytes
+    // and park the piece in gwin (RAW: write its unstuffed bytes).  Returns the 0xFF count.
+    auto sweep = [&](UnitState &C) -> uint32_t {
+        const uint32_t q0 = (uint32_t)C.Pc & 31u;         // bit offset of the unit inside window word 0
+        const uint32_t endbit = q0 + C.Lc;                // window bit index one past the unit
+        const uint32_t padc = (C.last && !RAW) ? ((8u - (endbit & 7u)) & 7u) : 0u;   // 1-padding (bits.rs:261-272)
+        const int ob0 = (int)(q0 >> 3);                   // owned window bytes [ob0, ob1)
+        const int ob1 = (int)(RAW ? ((C.last ? endbit + 7u : endbit) >> 3) : (endbit >> 3) + (padc ? 1u : 0u));
+        const int nrounds = max(1, (ob1 + WIN_B - 1) / WIN_B);
+        const int wtop = (int)((endbit + padc + 31u) >> 5);   // window words written, over all rounds
         uint32_t Fsum = 0;
 #pragma unroll 1
         for (int r = 0; r < nrounds; ++r) {
-            for (int i = lane; i < WIN_W / 4; i += 32) reinterpret_cast<uint4 *>(obuf)[i] = make_uint4(0, 0, 0, 0);
+            const int wlo = r * WIN_W, wb0 = r * WIN_B;
+            const int nsub = max(1, (min(wtop - wlo, WIN_W) + SUB_W - 1) / SUB_W);   // pieces this round holds
+            for (int i = lane; i < nsub * SUB_W / 4; i += 32) reinterpret_cast<uint4 *>(obuf)[i] = make_uint4(0, 0, 0, 0);
             __syncwarp();
-            {
-                const int wlo = r * WIN_W;
+#pragma unroll
+            for (int p = 0; p < NPASS; ++p) {   // the lane's three blocks, each funnel-shifted to its place
+                const uint32_t *const slot = M.slot[p];
+                const uint32_t *const spl = spill[p];
+                const uint32_t D = q0 + C.o_t[p];
+                const int d0 = (int)(D >> 5), sh = (int)(D & 31u);
+                const int nd = C.L[p] ? (int)((sh + C.L[p] + 31u) >> 5) : 0;   // destination words
+                const int nwt = C.nwt[p];
                 const int kb = max(0, wlo - d0), ke = min(nd, wlo + WIN_W - d0);
                 uint32_t prev = 0;
                 if (nwt <= SLOT_W) {  // the usual case: every word is in the slot
@@ -676,91 +724,104 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                         prev = cur;
                     }
                 }
-                if (lane == 0) {
-                    const uint32_t q = q0 & 7u;  // inherited bits of the straddling first byte
-                    if (r == 0 && q) atomicOr(&obuf[0], (C.tailin & ((1u << q) - 1u)) << (32u - q0));
-                    const int pw = (int)(endbit >> 5) - wlo;
-                    if (padc && pw >= 0 && pw < WIN_W)
-                        atomicOr(&obuf[pw], ((1u << padc) - 1u) << (32u - (endbit & 31u) - padc));
-                }
+            }
+            if (lane == 0) {
+                const uint32_t q = q0 & 7u;  // inherited bits of the straddling first byte
+                if (r == 0 && q) atomicOr(&obuf[0], (C.tailin & ((1u << q) - 1u)) << (32u - q0));
+                const int pw = (int)(endbit >> 5) - wlo;
+                if (padc && pw >= 0 && pw < WIN_W)
+                    atomicOr(&obuf[pw], ((1u << padc) - 1u) << (32u - (endbit & 31u) - padc));
             }
             __syncwarp();
-            // Count the 0xFF bytes in this lane's 32 window bytes.  No bounds: a window byte the
-            // chunk does not own is either untouched (0) or the unfinished last byte, whose low
-            // bits are still 0 - never 0xFF.
-            const int wb0 = r * WIN_B;
-            const int a = max((int)ob0 - wb0, 0), b = min((int)ob1 - wb0, WIN_B);
-            uint32_t wv[8];
-            {
-                const uint4 x = reinterpret_cast<const uint4 *>(obuf)[2 * lane];
-                const uint4 y = reinterpret_cast<const uint4 *>(obuf)[2 * lane + 1];
-                wv[0] = x.x; wv[1] = x.y; wv[2] = x.z; wv[3] = x.w; wv[4] = y.x; wv[5] = y.y; wv[6] = y.z; wv[7] = y.w;
-            }
-            if (RAW) {
-                // window byte i is byte (Pc >> 5) * 4 + wb0 + i of the band's raw string
-                uint8_t *outp = P.out + (size_t)C.img * P.out_cap;
-                const unsigned long long wbase = (C.Pc >> 5) * 4ull + (unsigned long long)wb0;
-                if (wbase + (unsigned long long)max(b, 0) <= P.out_cap) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int i0 = 32 * lane + 4 * j;
-                        if (i0 >= a && i0 + 4 <= b) {
-                            *reinterpret_cast<uint32_t *>(outp + wbase + i0) = __byte_perm(wv[j], 0, 0x0123);
-                        } else if (i0 + 4 > a && i0 < b) {
-#pragma unroll
-                            for (int t = 0; t < 4; ++t)
-                                if (i0 + t >= a && i0 + t < b) outp[wbase + i0 + t] = (uint8_t)(wv[j] >> (24 - 8 * t));
-                        }
-                    }
-                } else if (lane == 0) {
-                    atomicOr(&P.overflow[C.img], 1u);
+#pragma unroll 1
+            for (int s = 0; s < nsub; ++s) {
+                // Count the 0xFF bytes in this lane's 32 bytes.  No bounds: a window byte the unit
+                // does not own is either untouched (0) or the unfinished last byte, whose low bits
+                // are still 0 - never 0xFF.
+                const int pb0 = wb0 + s * SUB_B;             // unit byte index of the piece's byte 0
+                uint32_t wv[8];
+                {
+                    const uint4 x = reinterpret_cast<const uint4 *>(obuf + s * SUB_W)[2 * lane];
+                    const uint4 y = reinterpret_cast<const uint4 *>(obuf + s * SUB_W)[2 * lane + 1];
+                    wv[0] = x.x; wv[1] = x.y; wv[2] = x.z; wv[3] = x.w; wv[4] = y.x; wv[5] = y.y; wv[6] = y.z; wv[7] = y.w;
                 }
-                __syncwarp();
-                continue;
+                if (RAW) {
+                    // piece byte i is byte (Pc >> 5) * 4 + pb0 + i of the band's raw string
+                    const int a = max(ob0 - pb0, 0), b = min(ob1 - pb0, SUB_B);
+                    uint8_t *outp = P.out + (size_t)C.img * P.out_cap;
+                    const unsigned long long wbase = (C.Pc >> 5) * 4ull + (unsigned long long)pb0;
+                    if (wbase + (unsigned long long)max(b, 0) <= P.out_cap) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int i0 = 32 * lane + 4 * j;
+                            if (i0 >= a && i0 + 4 <= b) {
+                                *reinterpret_cast<uint32_t *>(outp + wbase + i0) = __byte_perm(wv[j], 0, 0x0123);
+                            } else if (i0 + 4 > a && i0 < b) {
+#pragma unroll
+                                for (int t = 0; t < 4; ++t)
+                                    if (i0 + t >= a && i0 + t < b) outp[wbase + i0 + t] = (uint8_t)(wv[j] >> (24 - 8 * t));
+                            }
+                        }
+                    } else if (lane == 0) {
+                        atomicOr(&P.overflow[C.img], 1u);
+                    }
+                    continue;
+                }
+                uint32_t cnt = 0;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) cnt += __popc(ff_bytes(wv[j]));
+                Fsum += __reduce_add_sync(0xffffffffu, cnt);
+                uint4 *g = reinterpret_cast<uint4 *>(gwin + pb0) + 2 * lane;   // read back by this lane in B
+                g[0] = make_uint4(wv[0], wv[1], wv[2], wv[3]);
+                g[1] = make_uint4(wv[4], wv[5], wv[6], wv[7]);
             }
+            __syncwarp();  // obuf is rewritten by the next round, or by the next unit's stage
+        }
+        C.own = (uint32_t)(ob1 - ob0) + Fsum + (C.marker ? 2u : 0u);
+        return Fsum;
+    };
+
+    // ---- B: the parked pieces, stuffed, to the output from byte gbase on ---------------------------------
+    auto emit = [&](UnitState &C, unsigned long long gbase) {
+        const uint32_t q0 = (uint32_t)C.Pc & 31u, endbit = q0 + C.Lc;
+        const uint32_t padc = C.last ? ((8u - (endbit & 7u)) & 7u) : 0u;
+        const int ob0 = (int)(q0 >> 3), ob1 = (int)((endbit >> 3) + (padc ? 1u : 0u));
+        const int npieces = max(1, (ob1 + SUB_B - 1) / SUB_B);
+        unsigned long long G = gbase;
+#pragma unroll 1
+        for (int s = 0; s < npieces; ++s) {
+            const int pb0 = s * SUB_B;
+            const uint4 *g = reinterpret_cast<const uint4 *>(gwin + pb0) + 2 * lane;
+            const uint4 x = g[0], y = g[1];
+            const uint32_t wv[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
             uint32_t cnt = 0;
 #pragma unroll
             for (int j = 0; j < 8; ++j) cnt += __popc(ff_bytes(wv[j]));
             uint32_t Fr;
             const uint32_t ffb = warp_scan(cnt, lane, &Fr);
-            if (!emit && nrounds == 1) {
-                // the usual case: keep the assembled window (in the chunk's slot buffer, which is
-                // not needed any more) so that phase B emits it without assembling again
-                uint4 *keep = reinterpret_cast<uint4 *>(M.slot[C.buf]);
-                keep[2 * lane] = make_uint4(wv[0], wv[1], wv[2], wv[3]);
-                keep[2 * lane + 1] = make_uint4(wv[4], wv[5], wv[6], wv[7]);
-                C.ffb = ffb;
-                C.kept = true;
-            }
-            if (emit) {
-                emit_window(C, wv, ffb, Fr, a, b, gbase + (r == 0 ? 0u : (uint32_t)(wb0 - (int)ob0)) + Fsum,
-                            r == nrounds - 1 ? C.marker : 0u);
-            }
-            Fsum += Fr;
-            __syncwarp();  // obuf / sbuf are rewritten by the next round, or by the next chunk's stage
+            const int a = max(ob0 - pb0, 0), b = min(ob1 - pb0, SUB_B);
+            emit_window(C, wv, ffb, Fr, a, b, G, s == npieces - 1 ? C.marker : 0u);
+            G += (unsigned long long)(max(b - a, 0) + (int)Fr);
         }
-        if (emit && lane == 0 && C.final_) {
-            const unsigned long long total = gbase + (ob1 - ob0) + Fsum;
-            P.out_len[C.img] = total;
-            if (total > P.out_cap) atomicOr(&P.overflow[C.img], 1u);
+        if (lane == 0 && C.final_) {
+            P.out_len[C.img] = G;
+            if (G > P.out_cap) atomicOr(&P.overflow[C.img], 1u);
         }
-        if (!emit) C.own = (ob1 - ob0) + Fsum + (C.marker ? 2u : 0u);
-        return Fsum;
     };
 
-    // ---- A: bit offset from chain 1, then the chunk's 0xFF count into chain 2 ------------------------
-    auto phase_a = [&](ChunkState &C) {
+    // ---- A: bit offset from chain 1, then the unit's 0xFF count into chain 2 ------------------------
+    auto phase_a = [&](UnitState &C) {
         if (C.skip) return;
-        unsigned long long *st1 = P.st_bits + (size_t)C.img * P.nchunks;
-        unsigned long long *st2 = P.st_ff + (size_t)C.img * P.nchunks;
+        unsigned long long *st1 = P.st_bits + (size_t)C.img * P.nunits;
+        unsigned long long *st2 = P.st_ff + (size_t)C.img * P.nunits;
         if (!C.first) {
-            const unsigned long long lb = look_back(st1, (int)C.chunk, lane);
+            const unsigned long long lb = look_back(st1, (int)C.unit, lane);
             C.Pc = lb & ST_VAL;
             C.tailin = (uint32_t)(lb >> 55) & 0x7Fu;
             C.fault |= (lb >> 62) != 0;
-            if (lane == 0) st_status(st1 + C.chunk, pack_status(ST_PFX, C.ctail, C.Pc + C.Lc));
+            if (lane == 0) st_status(st1 + C.unit, pack_status(ST_PFX, C.ctail, C.Pc + C.Lc));
         }
-        C.Ftot = sweep(C, false, 0);
+        sweep(C);
         if (RAW) {
             if (lane == 0 && C.final_) {
                 P.out_len[C.img] = C.Pc + C.Lc;       // BITS
@@ -770,54 +831,36 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], 2u);
             return;
         }
-        if (lane == 0) st_status(st2 + C.chunk, pack_status(C.chunk == 0 ? ST_PFX : ST_AGG, 0, C.own));
+        if (lane == 0) st_status(st2 + C.unit, pack_status(C.unit == 0 ? ST_PFX : ST_AGG, 0, C.own));
     };
     // ---- B: stuffed-byte offset from chain 2, then the bytes ------------------------------------------
-    auto phase_b = [&](ChunkState &C) {
+    auto phase_b = [&](UnitState &C) {
         if (RAW || C.skip) return;
-        unsigned long long *st2 = P.st_ff + (size_t)C.img * P.nchunks;
+        unsigned long long *st2 = P.st_ff + (size_t)C.img * P.nunits;
         unsigned long long ffx = 0;
-        if (C.chunk) {
-            const unsigned long long lb = look_back(st2, (int)C.chunk, lane);
+        if (C.unit) {
+            const unsigned long long lb = look_back(st2, (int)C.unit, lane);
             ffx = lb & ST_VAL;
             C.fault |= (lb >> 62) != 0;
-            if (lane == 0) st_status(st2 + C.chunk, pack_status(ST_PFX, 0, ffx + C.own));
+            if (lane == 0) st_status(st2 + C.unit, pack_status(ST_PFX, 0, ffx + C.own));
         }
-        const unsigned long long gbase = ffx;  // chain 2 counts every byte written before this chunk
-        if (C.kept) {
-            const uint32_t q0 = (uint32_t)C.Pc & 31u, endbit = q0 + C.Lc;
-            const uint32_t padc = C.last ? ((8u - (endbit & 7u)) & 7u) : 0u;
-            const uint32_t ob0 = q0 >> 3, ob1 = (endbit >> 3) + (padc ? 1u : 0u);
-            const uint4 *keep = reinterpret_cast<const uint4 *>(M.slot[C.buf]);
-            const uint4 x = keep[2 * lane], y = keep[2 * lane + 1];
-            const uint32_t wv[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
-            emit_window(C, wv, C.ffb, C.Ftot, (int)ob0, (int)ob1, gbase, C.marker);
-            if (lane == 0 && C.final_) {
-                const unsigned long long total = gbase + (ob1 - ob0) + C.Ftot;
-                P.out_len[C.img] = total;
-                if (total > P.out_cap) atomicOr(&P.overflow[C.img], 1u);
-            }
-        } else {
-            sweep(C, true, gbase);
-        }
+        emit(C, ffx);   // chain 2 counts every byte written before this unit
         if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], 2u);
     };
 
-    ChunkState cur, pend;
+    UnitState cur, pend;
     bool have_pend = false;
-    int buf = 0;
     for (;;) {
         uint32_t id = 0;
         if (lane == 0) id = atomicAdd(P.ticket, 1u);
         id = __shfl_sync(0xffffffffu, id, 0);
-        const bool have = id < total_chunks;
+        const bool have = id < total_units;
         if (have_pend) phase_a(pend);
-        if (have) phase_w(id, buf, cur);
+        if (have) phase_w(id, cur);
         if (have_pend) phase_b(pend);
         if (!have) break;
         pend = cur;
         have_pend = true;
-        buf ^= 1;
     }
 }
 
@@ -826,15 +869,15 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
 static EntropyPlan plan_entropy(uint32_t n, uint64_t nblocks, uint64_t rst_blocks)
 {
     EntropyPlan p;
-    p.nchunks = (size_t)((nblocks + CB - 1) / CB);
-    if (rst_blocks && rst_blocks < nblocks) {  // every interval is chunked on its own
-        const uint64_t n_int = (nblocks + rst_blocks - 1) / rst_blocks, cpi = (rst_blocks + CB - 1) / CB;
+    p.nunits = (size_t)((nblocks + UB - 1) / UB);
+    if (rst_blocks && rst_blocks < nblocks) {  // every interval is cut into units on its own
+        const uint64_t n_int = (nblocks + rst_blocks - 1) / rst_blocks, upi = (rst_blocks + UB - 1) / UB;
         const uint64_t last = nblocks - (n_int - 1) * rst_blocks;
-        p.nchunks = (size_t)((n_int - 1) * cpi + (last + CB - 1) / CB);
+        p.nunits = (size_t)((n_int - 1) * upi + (last + UB - 1) / UB);
     }
     size_t o = 0;
-    p.off_st1 = o; o += align_up((size_t)n * p.nchunks * 8, 256);
-    p.off_st2 = o; o += align_up((size_t)n * p.nchunks * 8, 256);
+    p.off_st1 = o; o += align_up((size_t)n * p.nunits * 8, 256);
+    p.off_st2 = o; o += align_up((size_t)n * p.nunits * 8, 256);
     p.off_ticket = o; o += 256;
     p.off_ovf = o; o += align_up((size_t)n * 4, 256);
     p.zero_bytes = o;  // everything up to here is cleared per launch
@@ -1235,7 +1278,7 @@ static uint32_t segments_for(uint32_t n, uint64_t total_mcus, uint64_t bpm)
     // chunks) the extra launches cost more than the shorter chains save (one frame: unsegmented
     // 0.108-0.110 ms, 4-256 segments 0.124-0.130 ms; tools/segment_sweep.py, profiles/h100_segment_sweep.json); a 16 384^2 frame (196 608 chunks on ONE chain) is
     // where the look-back distance hurts.  So: few images, each long.
-    const uint64_t chunks = total_mcus * bpm / CB;
+    const uint64_t chunks = total_mcus * bpm / 32;   // (the thresholds below count 32-block chunks)
     if (n > 8 || chunks < 16384) return 1;
     // 16 384^2 frame on the same H100: unsegmented 2.53-2.67 ms, 16 segments 2.11, 32: 1.90, 64: 1.73,
     // 128: 1.62, 256: 1.53-1.59 (more chains in flight keep the nearest inclusive prefix inside one
@@ -1296,10 +1339,10 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint
     P.seg_per_img = sp.S;
     P.nblocks = (uint32_t)(sp.seg_mcus * bpm);
     P.nblocks_last = (uint32_t)(sp.last_mcus * bpm);
-    P.nchunks = (uint32_t)sp.ent.nchunks;
+    P.nunits = (uint32_t)sp.ent.nunits;
     P.seg_y_stride = (size_t)sp.seg_mcus * g.y_per_mcu * 64;
     P.seg_c_stride = (size_t)sp.seg_mcus * 64;
-    P.rst_blocks = P.rst_mcus = P.cpi = 0;
+    P.rst_blocks = P.rst_mcus = P.upi = 0;
     P.st_bits = reinterpret_cast<unsigned long long *>(ent + sp.ent.off_st1);
     P.st_ff = reinterpret_cast<unsigned long long *>(ent + sp.ent.off_st2);
     P.ticket = reinterpret_cast<uint32_t *>(ent + sp.ent.off_ticket);
@@ -1309,7 +1352,7 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint
     P.out = raw_area;
     P.out_cap = sp.raw_cap;
     PIXO_CUDA(ctx, cudaMemsetAsync(ent, 0, sp.ent.zero_bytes, st));
-    const size_t want = ((size_t)P.nimages * P.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
+    const size_t want = ((size_t)P.nimages * P.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
     PIXO_TRY(launch(ctx, check ? k_huff<true, true> : k_huff<true, false>, grid, 32 * HUFF_WARPS, 0, P, T));
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_bits, P.out_len, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
@@ -1364,7 +1407,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     uint64_t rst_blocks = (uint64_t)restart_interval * bpm_;
     if (rst_blocks >= nblocks) rst_blocks = 0;  // a single interval: no marker is ever written
     const EntropyPlan pl = plan_entropy(n, nblocks, rst_blocks);
-    if (nblocks > 0xFFFFFFFFull || (uint64_t)n * pl.nchunks > 0x7FFFFFFFull)
+    if (nblocks > 0xFFFFFFFFull || (uint64_t)n * pl.nunits > 0x7FFFFFFFull)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "entropy stage: too many blocks per call");
     EntParams P;
     P.y = d_y; P.cb = d_cb; P.cr = d_cr; P.y_stride = y_stride; P.c_stride = c_stride;
@@ -1372,10 +1415,10 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     P.bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     P.y_per_mcu = g.y_per_mcu;
     P.nblocks = (uint32_t)nblocks;
-    P.nchunks = (uint32_t)pl.nchunks;
+    P.nunits = (uint32_t)pl.nunits;
     P.rst_blocks = (uint32_t)rst_blocks;
     P.rst_mcus = rst_blocks ? restart_interval : 0u;
-    P.cpi = rst_blocks ? (uint32_t)((rst_blocks + CB - 1) / CB) : 0u;
+    P.upi = rst_blocks ? (uint32_t)((rst_blocks + UB - 1) / UB) : 0u;
     P.nimages = n;
     P.st_bits = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_st1);
     P.st_ff = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_st2);
@@ -1386,6 +1429,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     P.out_tail = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_tail);
     P.dc_seed[0] = P.dc_seed[1] = P.dc_seed[2] = 0;
     P.dc_seed_dev = nullptr;
+    P.win = nullptr;   // set below; k_huff<RAW> has no phase B
     *d_out_len = P.out_len;
     *d_overflow = P.overflow;
 
@@ -1406,8 +1450,10 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                                reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), 0, 0, true,
                                nullptr, d_out, out_cap, P.out_len, P.overflow);
     }
-    const size_t want = ((size_t)n * pl.nchunks + HUFF_WARPS - 1) / HUFF_WARPS;
+    const size_t want = ((size_t)n * pl.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
+    PIXO_TRY(ensure_dev(ctx, ctx->d_hwin, (size_t)grid * HUFF_WARPS * GWIN_B));
+    P.win = reinterpret_cast<uint8_t *>(ctx->d_hwin.ptr);
     return launch(ctx, check ? k_huff<false, true> : k_huff<false, false>, grid, 32 * HUFF_WARPS, 0, P, T);
 }
 

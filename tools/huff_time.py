@@ -14,7 +14,7 @@ g = synthetic.gradient_rgb(W, H).reshape(H, W * 3)
 _, _, lq, cq = jpeg.quant_tables(80)
 ny, nc = jpeg.block_counts(W, H, 2, 1)
 res = []
-for n, kind in [(1, "noise"), (1, "grad"), (8, "mix"), (32, "mix")]:
+for n, kind in [(1, "noise"), (1, "grad"), (8, "mix"), (32, "mix"), (32, "grad"), (32, "noise")]:
     fr = np.stack([np.roll(g, k, axis=0).reshape(-1) if (kind == "grad" or (kind == "mix" and k % 2 == 0))
                    else synthetic.noise(W, H, 3, 42 + k).reshape(-1) for k in range(n)])
     px = torch.from_numpy(fr).cuda()
