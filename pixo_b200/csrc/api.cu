@@ -36,35 +36,26 @@ int cuda_fail(pixo_b200_ctx *ctx, cudaError_t e, const char *what)
     return set_error(ctx, code, "CUDA error %d (%s) in %s", (int)e, cudaGetErrorString(e), what);
 }
 
-int ensure_dev(pixo_b200_ctx *ctx, Scratch &s, size_t bytes)
+template <bool Pinned>
+int Buffer<Pinned>::ensure(pixo_b200_ctx *ctx, size_t bytes)
 {
-    if (s.cap >= bytes) return 0;
-    if (s.ptr) {
+    if (cap >= bytes) return 0;
+    if (ptr) {
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        PIXO_CUDA(ctx, cudaFree(s.ptr));
-        s.ptr = nullptr;
-        s.cap = 0;
+        if constexpr (Pinned) PIXO_CUDA(ctx, cudaFreeHost(ptr));
+        else PIXO_CUDA(ctx, cudaFree(ptr));
+        ptr = nullptr;
+        cap = 0;
     }
     const size_t want = bytes + bytes / 8 + 256;
-    PIXO_CUDA(ctx, cudaMalloc(&s.ptr, want));
-    s.cap = want;
+    if constexpr (Pinned) PIXO_CUDA(ctx, cudaMallocHost(&ptr, want));
+    else PIXO_CUDA(ctx, cudaMalloc(&ptr, want));
+    cap = want;
     return 0;
 }
 
-int ensure_pinned(pixo_b200_ctx *ctx, Scratch &s, size_t bytes)
-{
-    if (s.cap >= bytes) return 0;
-    if (s.ptr) {
-        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        PIXO_CUDA(ctx, cudaFreeHost(s.ptr));
-        s.ptr = nullptr;
-        s.cap = 0;
-    }
-    const size_t want = bytes + bytes / 8 + 256;
-    PIXO_CUDA(ctx, cudaMallocHost(&s.ptr, want));
-    s.cap = want;
-    return 0;
-}
+template struct Buffer<false>;
+template struct Buffer<true>;
 
 HostPool::HostPool(int nthreads)
 {
@@ -129,9 +120,9 @@ static HostPool *host_pool(pixo_b200_ctx *ctx)
     if (!ctx->pool) {
         int n = ctx->host_threads - 1;
         n = n < 1 ? 1 : (n > 5 ? 5 : n);   // five helpers + the caller saturate a socket's copy bandwidth
-        ctx->pool = new HostPool(n);
+        ctx->pool = std::make_unique<HostPool>(n);
     }
-    return ctx->pool;
+    return ctx->pool.get();
 }
 
 // Copy into a pinned staging slot with NON-TEMPORAL stores.  An ordinary memcpy of a 1 MB piece
@@ -187,7 +178,7 @@ static int h2d_copy(pixo_b200_ctx *ctx, void *dst, const void *src, size_t bytes
         PIXO_CUDA(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
         return 0;
     }
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_in, SLOT * NSLOT));
+    PIXO_TRY(ctx->h_in.ensure(ctx, SLOT * NSLOT));
     while (ctx->stage_events.size() < (size_t)NSLOT) {
         cudaEvent_t ev;
         PIXO_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -239,7 +230,7 @@ static int d2h_copy_sync(pixo_b200_ctx *ctx, void *dst, const void *src, size_t 
         PIXO_CUDA(ctx, cudaStreamSynchronize(st));
         return 0;
     }
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_out, bytes));
+    PIXO_TRY(ctx->h_out.ensure(ctx, bytes));
     PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_out.ptr, src, bytes, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaStreamSynchronize(st));
     const int n = (int)((bytes + PIECE - 1) / PIECE);
@@ -249,6 +240,22 @@ static int d2h_copy_sync(pixo_b200_ctx *ctx, void *dst, const void *src, size_t 
     });
     return 0;
 }
+
+// Synchronises every stream of the context when an entry point leaves early, so that no queued
+// copy still reads the caller's pixels or writes the caller's output after the error return.
+struct DrainOnError {
+    pixo_b200_ctx *ctx;
+    bool armed = true;
+    explicit DrainOnError(pixo_b200_ctx *c) : ctx(c) {}
+    ~DrainOnError()
+    {
+        if (!armed) return;
+        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->copy_stream);
+        cudaStreamSynchronize(ctx->d2h_stream);
+        cudaGetLastError();
+    }
+};
 
 static int validate_jpeg(pixo_b200_ctx *ctx, uint32_t w, uint32_t h, uint32_t color_type,
                          uint32_t subsampling)
@@ -268,6 +275,15 @@ static int validate_jpeg(pixo_b200_ctx *ctx, uint32_t w, uint32_t h, uint32_t co
 }  // namespace pixo
 
 using namespace pixo;
+
+pixo_b200_ctx::~pixo_b200_ctx()
+{
+    for (cudaEvent_t ev : events) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : stage_events) cudaEventDestroy(ev);
+    if (own_stream) cudaStreamDestroy(own_stream);
+    if (copy_stream) cudaStreamDestroy(copy_stream);
+    if (d2h_stream) cudaStreamDestroy(d2h_stream);
+}
 
 extern "C" {
 
@@ -294,31 +310,20 @@ int pixo_b200_ctx_create(int device, pixo_b200_ctx **out)
     }
     if (device < 0 || device >= n)
         return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "device %d out of range (0..%d)", device, n - 1);
-    pixo_b200_ctx *ctx = new pixo_b200_ctx();
+    auto ctx = std::make_unique<pixo_b200_ctx>();
     ctx->device = device;
-    if ((e = cudaSetDevice(device)) != cudaSuccess) {
-        const int rc = cuda_fail(nullptr, e, "cudaSetDevice");
-        delete ctx;
-        return rc;
-    }
+    if ((e = cudaSetDevice(device)) != cudaSuccess) return cuda_fail(nullptr, e, "cudaSetDevice");
     cudaDeviceProp prop;
-    if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) {
-        const int rc = cuda_fail(nullptr, e, "cudaGetDeviceProperties");
-        delete ctx;
-        return rc;
-    }
+    if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return cuda_fail(nullptr, e, "cudaGetDeviceProperties");
     ctx->sm_count = prop.multiProcessorCount;
     if ((e = cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||
-        (e = cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking)) != cudaSuccess) {
-        const int rc = cuda_fail(nullptr, e, "cudaStreamCreate");
-        delete ctx;
-        return rc;
-    }
+        (e = cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking)) != cudaSuccess)
+        return cuda_fail(nullptr, e, "cudaStreamCreate");
     ctx->stream = ctx->own_stream;
     unsigned hc = std::thread::hardware_concurrency();
     ctx->host_threads = hc ? (int)hc : 1;
-    *out = ctx;
+    *out = ctx.release();
     return 0;
 }
 
@@ -327,18 +332,6 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    Scratch *dev[] = {&ctx->d_in, &ctx->d_y, &ctx->d_cb, &ctx->d_cr, &ctx->d_misc, &ctx->d_out, &ctx->d_ent, &ctx->d_coef, &ctx->d_retry, &ctx->d_raw, &ctx->d_hwin,
-                       &ctx->d_red, &ctx->d_red_idx, &ctx->d_red_img, &ctx->d_quant, &ctx->d_quant_img, &ctx->d_trellis,
-                       &ctx->d_prog, &ctx->d_prog_raw, &ctx->d_prog_out, &ctx->d_resize, &ctx->d_resize_tmp};
-    for (Scratch *s : dev) if (s->ptr) cudaFree(s->ptr);
-    Scratch *host[] = {&ctx->h_in, &ctx->h_out, &ctx->h_misc, &ctx->h_red, &ctx->h_quant, &ctx->h_trellis, &ctx->h_prog};
-    for (Scratch *s : host) if (s->ptr) cudaFreeHost(s->ptr);
-    for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : ctx->stage_events) cudaEventDestroy(ev);
-    if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    if (ctx->d2h_stream) cudaStreamDestroy(ctx->d2h_stream);
-    delete ctx->pool;
     delete ctx;
 }
 
@@ -445,6 +438,23 @@ static void tables_from(const uint64_t *hist, bool has_chroma, HuffTables &t)
     if (!(hist && huff_from_histogram(hist, has_chroma, t))) huff_standard(t);
 }
 
+// The Huffman tables of `cnt` frames.  optimize: each frame's from its statistics (K3) in d_hist, read
+// back to h_hist (in the pinned h_misc) once the stream has drained; otherwise one set of standard tables.
+static int build_tables(pixo_b200_ctx *ctx, bool optimize, const uint64_t *d_hist, uint64_t *h_hist, uint32_t cnt,
+                        bool has_chroma, std::vector<HuffTables> &tb)
+{
+    tb.resize(optimize ? cnt : 1);
+    if (!optimize) {
+        tables_from(nullptr, has_chroma, tb[0]);
+        return 0;
+    }
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                                   ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, has_chroma, tb[k]);
+    return 0;
+}
+
 // need: bytes of headers, scan and EOI marker
 static int check_room(pixo_b200_ctx *ctx, size_t out_cap, size_t need)
 {
@@ -519,7 +529,7 @@ int pixo_b200_jpeg_block_counts(uint32_t width, uint32_t height, uint32_t color_
 // Bit 0 of the trellis status word, read back after the context's stream has drained
 static int trellis_status(pixo_b200_ctx *ctx, const uint32_t *d_status)
 {
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_trellis, sizeof(uint32_t)));
+    PIXO_TRY(ctx->h_trellis.ensure(ctx, sizeof(uint32_t)));
     PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_trellis.ptr, d_status, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (*static_cast<const uint32_t *>(ctx->h_trellis.ptr))
@@ -553,7 +563,7 @@ static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, siz
                               ? g.mcus_y
                               : (uint32_t)std::max<size_t>(1, std::min<size_t>(g.mcus_y, kTrellisScratch / row_bytes));
     const size_t piece_bytes = band < g.mcus_y ? row_bytes * band : frame_bytes * group;
-    PIXO_TRY(ensure_dev(ctx, ctx->d_trellis, 256 + piece_bytes));
+    PIXO_TRY(ctx->d_trellis.ensure(ctx, 256 + piece_bytes));
     auto *status = static_cast<uint32_t *>(ctx->d_trellis.ptr);
     float *fy = reinterpret_cast<float *>(static_cast<uint8_t *>(ctx->d_trellis.ptr) + 256);
     PIXO_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(uint32_t), ctx->stream));
@@ -624,7 +634,8 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
     return 0;
 }
 
-// upload, transform (+ histogram), download the coefficients
+// Like every host-buffer entry point: the input staged in the context's scratch, the `_dev` twin on it as
+// a batch of one, the results copied out
 int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t width,
                                 uint32_t height, uint32_t color_type, uint32_t subsampling,
                                 const float lum_q[64], const float chr_q[64], int16_t *y,
@@ -640,40 +651,31 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     const size_t in_bytes = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t yb = g.ny * 64 * sizeof(int16_t), cbb = g.nc * 64 * sizeof(int16_t);
+    const size_t hist_bytes = kHistWords * sizeof(uint64_t);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_y, yb));
+    PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
+    PIXO_TRY(ctx->d_y.ensure(ctx, yb));
     if (cbb) {
-        PIXO_TRY(ensure_dev(ctx, ctx->d_cb, cbb));
-        PIXO_TRY(ensure_dev(ctx, ctx->d_cr, cbb));
+        PIXO_TRY(ctx->d_cb.ensure(ctx, cbb));
+        PIXO_TRY(ctx->d_cr.ensure(ctx, cbb));
     }
+    if (hist) PIXO_TRY(ctx->d_out.ensure(ctx, hist_bytes));
+    auto *dy = static_cast<int16_t *>(ctx->d_y.ptr);
+    auto *dcb = cbb ? static_cast<int16_t *>(ctx->d_cb.ptr) : nullptr;
+    auto *dcr = cbb ? static_cast<int16_t *>(ctx->d_cr.ptr) : nullptr;
+    auto *d_hist = hist ? static_cast<uint64_t *>(ctx->d_out.ptr) : nullptr;
+    DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, pixels, in_bytes, ctx->stream));
-    auto *dy = reinterpret_cast<int16_t *>(ctx->d_y.ptr);
-    auto *dcb = reinterpret_cast<int16_t *>(ctx->d_cb.ptr);
-    auto *dcr = reinterpret_cast<int16_t *>(ctx->d_cr.ptr);
-    if (flags & PIXO_B200_COEF_TRELLIS)
-        PIXO_TRY(trellis_coefficients(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
-                                      height, color_type, subsampling, lum_q, chr_q, dy, g.ny * 64,
-                                      cbb ? dcb : nullptr, cbb ? dcr : nullptr, g.nc * 64,
-                                      (flags & PIXO_B200_COEF_ZIGZAG) != 0));
-    else
-        PIXO_TRY(launch_jpeg_transform(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
-                                       width, height, color_type, subsampling, lum_q, chr_q,
-                                       dy, g.ny * 64, dcb, dcr, g.nc * 64, flags));
-    if (hist) {
-        PIXO_TRY(ensure_dev(ctx, ctx->d_out, kHistWords * sizeof(uint64_t)));
-        PIXO_TRY(launch_jpeg_histogram(ctx, dy, g.ny * 64, dcb, dcr, g.nc * 64, 1, g.ny, g.nc,
-                                       g.y_per_mcu, 0, (flags & PIXO_B200_COEF_ZIGZAG) != 0, nullptr,
-                                       reinterpret_cast<uint64_t *>(ctx->d_out.ptr)));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(hist, ctx->d_out.ptr, kHistWords * sizeof(uint64_t),
-                                       cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    PIXO_CUDA(ctx, cudaMemcpyAsync(y, dy, yb, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_TRY(pixo_b200_jpeg_coefficients_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
+                                             height, color_type, subsampling, lum_q, chr_q, dy, g.ny * 64, dcb, dcr,
+                                             g.nc * 64, flags, d_hist));
+    PIXO_TRY(d2h_copy_sync(ctx, y, dy, yb, ctx->stream));
     if (cbb) {
-        PIXO_CUDA(ctx, cudaMemcpyAsync(cb, dcb, cbb, cudaMemcpyDeviceToHost, ctx->stream));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(cr, dcr, cbb, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_TRY(d2h_copy_sync(ctx, cb, dcb, cbb, ctx->stream));
+        PIXO_TRY(d2h_copy_sync(ctx, cr, dcr, cbb, ctx->stream));
     }
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (hist) PIXO_TRY(d2h_copy_sync(ctx, hist, d_hist, hist_bytes, ctx->stream));
+    drain.armed = false;
     return 0;
 }
 
@@ -690,7 +692,7 @@ int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, 
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "block buffers must be 16-byte aligned");
     if (n_blocks == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_trellis, 256));
+    PIXO_TRY(ctx->d_trellis.ensure(ctx, 256));
     auto *status = static_cast<uint32_t *>(ctx->d_trellis.ptr);
     PIXO_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(uint32_t), ctx->stream));
     PIXO_TRY(launch_trellis(ctx, d_dct, 0, d_out, 0, n_blocks, 1, q, lambda, (flags & PIXO_B200_COEF_ZIGZAG) != 0,
@@ -711,22 +713,6 @@ static int validate_encode(pixo_b200_ctx *ctx, size_t pixels_len, uint32_t width
                          "Invalid data length: expected %zu bytes, got %zu", expected, pixels_len);
     return 0;
 }
-
-// Synchronises every stream of the context when an entry point leaves early, so that no queued
-// copy still reads the caller's pixels or writes the caller's output after the error return.
-struct DrainOnError {
-    pixo_b200_ctx *ctx;
-    bool armed = true;
-    explicit DrainOnError(pixo_b200_ctx *c) : ctx(c) {}
-    ~DrainOnError()
-    {
-        if (!armed) return;
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->copy_stream);
-        cudaStreamSynchronize(ctx->d2h_stream);
-        cudaGetLastError();
-    }
-};
 
 // Device scan capacity per frame: a JPEG that needs more than half its raw size (noise at very
 // high quality) is coded a second time with the exact size the kernel reported.
@@ -757,7 +743,7 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
     const size_t ent = entropy_scratch_bytes(1, g, restart_interval);
     for (int pass = 0;; ++pass) {
         const size_t scan_bytes = align_up(cap, 256);
-        PIXO_TRY(ensure_dev(ctx, ctx->d_retry, scan_bytes + ent + 256));
+        PIXO_TRY(ctx->d_retry.ensure(ctx, scan_bytes + ent + 256));
         auto *buf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
         uint64_t *d_len = nullptr;
         uint32_t *d_ovf = nullptr;
@@ -772,9 +758,9 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
             *len = (size_t)n;
             return 0;
         }
-        if (ovf & 8u) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
-        if ((ovf & 2u) || pass == 2) return kGaveUp;
-        if (ovf & 4u) {
+        if (ovf & kOvfRange) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
+        if ((ovf & kOvfFault) || pass == 2) return kGaveUp;
+        if (ovf & kOvfSegment) {
             segments = false;
             continue;
         }
@@ -831,13 +817,13 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     const uint32_t ngroups = (n_images + G - 1) / G;
 
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, 2 * (size_t)G * in_stride));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, 2 * (size_t)G * L.each));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_ent, ent_bytes(G)));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_out, 2 * (size_t)G * scan_cap));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_misc, (size_t)G * kHistWords * sizeof(uint64_t) + 256));
+    PIXO_TRY(ctx->d_in.ensure(ctx, 2 * (size_t)G * in_stride));
+    PIXO_TRY(ctx->d_coef.ensure(ctx, 2 * (size_t)G * L.each));
+    PIXO_TRY(ctx->d_ent.ensure(ctx, ent_bytes(G)));
+    PIXO_TRY(ctx->d_out.ensure(ctx, 2 * (size_t)G * scan_cap));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, (size_t)G * kHistWords * sizeof(uint64_t) + 256));
     const size_t meta_slot = align_up((size_t)G * 12, 256);
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, 2 * meta_slot + (size_t)G * kHistWords * sizeof(uint64_t) + 256));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, 2 * meta_slot + (size_t)G * kHistWords * sizeof(uint64_t) + 256));
     while (ctx->events.size() < 8) {
         cudaEvent_t ev;
         PIXO_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -850,6 +836,7 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto *d_in = reinterpret_cast<uint8_t *>(ctx->d_in.ptr);
     auto *d_scan = reinterpret_cast<uint8_t *>(ctx->d_out.ptr);
     auto *h_meta = reinterpret_cast<uint8_t *>(ctx->h_misc.ptr);
+    auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
     auto *h_hist = reinterpret_cast<uint64_t *>(h_meta + 2 * meta_slot);
     auto h_len_of = [&](int slot) { return reinterpret_cast<uint64_t *>(h_meta + (size_t)slot * meta_slot); };
     auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
@@ -881,19 +868,11 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         if (optimize || !trellis)
             PIXO_TRY(launch_jpeg_transform(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
                                            chr, L.y(c), cs, cb, cr, cs, 0));
-        std::vector<HuffTables> &tb = tables[slot];
-        tb.resize(optimize ? cnt : 1);
-        if (optimize) {
-            auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
+        if (optimize)
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
                                            false, nullptr, d_hist));
-            PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t),
-                                           cudaMemcpyDeviceToHost, ctx->stream));
-            PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, g.has_chroma, tb[k]);
-        } else {
-            tables_from(nullptr, g.has_chroma, tb[0]);
-        }
+        std::vector<HuffTables> &tb = tables[slot];
+        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
         if (trellis)
             PIXO_TRY(trellis_coefficients(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
                                           chr, L.y(c), cs, cb, cr, cs, false));
@@ -941,19 +920,11 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
                                        g.height, g.color_type, g.subsampling, lum, chr, L.y(c), cs,
                                        g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr, cs, 0, &ec));
         PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
-        std::vector<HuffTables> &tb = tables[slot];
-        tb.resize(optimize ? cnt : 1);
-        if (optimize) {
-            auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
+        if (optimize)
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g.ny, g.nc, g.y_per_mcu,
                                            restart_interval, false, &ec, d_hist));
-            PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t),
-                                           cudaMemcpyDeviceToHost, ctx->stream));
-            PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the table build needs the statistics
-            for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, g.has_chroma, tb[k]);
-        } else {
-            tables_from(nullptr, g.has_chroma, tb[0]);
-        }
+        std::vector<HuffTables> &tb = tables[slot];
+        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
         if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_out[slot], 0));  // slot's previous D2H drained
         uint64_t *d_len = nullptr;
@@ -1021,9 +992,9 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             // enough room.  Bit 1 (a faulted chain) goes to the host coder.
             int rc = kGaveUp;
             size_t body = 0;
-            if (!(h_ovf[k] & 2u) && ctx->gpu_retry) {
-                const size_t need = (h_ovf[k] & 4u) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
-                if (!(h_ovf[k] & 4u)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
+            if (!(h_ovf[k] & kOvfFault) && ctx->gpu_retry) {
+                const size_t need = (h_ovf[k] & kOvfSegment) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
+                if (!(h_ovf[k] & kOvfSegment)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
                 const CoefExtents ef = L.extents(f);
                 rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), &ef, g, t, restart_interval, false, align_up(need + 64, 256),
                                  hdr[k], out_cap_each, &body);
@@ -1037,7 +1008,7 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             }
             // last resort: the host entropy coder on the GPU's coefficient records, made dense
             ctx->host_fallbacks += 1;
-            PIXO_TRY(ensure_pinned(ctx, ctx->h_out, L.each));
+            PIXO_TRY(ctx->h_out.ensure(ctx, L.each));
             auto *hc = reinterpret_cast<uint8_t *>(ctx->h_out.ptr);
             PIXO_CUDA(ctx, cudaMemcpyAsync(hc, f, L.each, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1135,6 +1106,17 @@ int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *p
                          optimize_huffman != 0, out, out_cap_each, out_lens, true, trellis_quant != 0);
 }
 
+// Caller coefficient arrays on the device: the statistics, Huffman and progressive kernels load each
+// block as 16-byte vectors, so an array that is not 16-byte aligned is refused before anything is launched.
+static int check_coef_alignment(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                                bool has_chroma)
+{
+    auto mis = [](const int16_t *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
+    if (mis(d_y) || (has_chroma && (mis(d_cb) || mis(d_cr))))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient arrays must be 16-byte aligned");
+    return 0;
+}
+
 int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                                          const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
                                          uint32_t n_frames, uint32_t width, uint32_t height, uint32_t color_type,
@@ -1147,9 +1129,7 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
     if (!d_y || !d_out || !d_scan_len || !d_overflow || (chroma && (!d_cb || !d_cr)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    auto mis = [](const int16_t *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
-    if (mis(d_y) || (chroma && (mis(d_cb) || mis(d_cr))))
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient arrays must be 16-byte aligned");
+    PIXO_TRY(check_coef_alignment(ctx, d_y, d_cb, d_cr, chroma));
     if ((y_stride & 7) || (chroma && (c_stride & 7)))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient strides must be multiples of 8 elements");
     if (n_frames > 1 && (y_stride < g.ny * 64 || (chroma && c_stride < g.nc * 64)))
@@ -1218,8 +1198,8 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     quant_tables((int)quality, nullptr, nullptr, lum, chr);
     const CoefLayout L(g);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_coef, (size_t)n_images * L.each));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_ent, entropy_scratch_bytes(n_images, g, 0)));
+    PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)n_images * L.each));
+    PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(n_images, g, 0)));
     void *c = ctx->d_coef.ptr;
     const CoefExtents ec = L.extents(c);
     PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
@@ -1247,17 +1227,6 @@ static int check_range(pixo_b200_ctx *ctx, const int16_t *y, const int16_t *cb, 
         (g.has_chroma && (!coefficients_in_range(cb, g.nc, restart_interval, 1, seed ? seed[1] : 0) ||
                           !coefficients_in_range(cr, g.nc, restart_interval, 1, seed ? seed[2] : 0))))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
-    return 0;
-}
-
-// Caller coefficient arrays on the device: the statistics and Huffman kernels load each block as
-// 16-byte vectors, so an array that is not 16-byte aligned is refused before anything is launched.
-static int check_coef_alignment(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
-                                bool has_chroma)
-{
-    auto mis = [](const int16_t *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
-    if (mis(d_y) || (has_chroma && (mis(d_cb) || mis(d_cr))))
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient arrays must be 16-byte aligned");
     return 0;
 }
 
@@ -1306,19 +1275,16 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    uint64_t *h_hist = nullptr;
     if (optimize_huffman) {
-        PIXO_TRY(ensure_dev(ctx, ctx->d_misc, kHistWords * sizeof(uint64_t) + 256));
-        PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, kHistWords * sizeof(uint64_t) + 256));
-        auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-        h_hist = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
+        PIXO_TRY(ctx->d_misc.ensure(ctx, kHistWords * sizeof(uint64_t) + 256));
+        PIXO_TRY(ctx->h_misc.ensure(ctx, kHistWords * sizeof(uint64_t) + 256));
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                       false, nullptr, d_hist));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, kHistWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+                                       false, nullptr, static_cast<uint64_t *>(ctx->d_misc.ptr)));
     }
-    HuffTables t;
-    tables_from(h_hist, g.has_chroma, t);
+    std::vector<HuffTables> tb;
+    PIXO_TRY(build_tables(ctx, optimize_huffman != 0, static_cast<uint64_t *>(ctx->d_misc.ptr),
+                          static_cast<uint64_t *>(ctx->h_misc.ptr), 1, g.has_chroma, tb));
+    const HuffTables &t = tb[0];
     const size_t hdr = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
     // The device scan buffer follows the size a JPEG of this geometry normally has, not the caller's
     // worst-case capacity (tens of GB for a gigapixel frame); a scan that needs more is coded again
@@ -1385,8 +1351,8 @@ int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, cons
     tables_from(hist, g.has_chroma, t);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     // the stream-ordered flow into a small device scratch: {bits, tail}, then the flags k_band_totals ORs into
-    PIXO_TRY(ensure_dev(ctx, ctx->d_misc, 256));
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, 256));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, 256));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, 256));
     auto *d = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
     auto *h = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
     uint32_t ovf = 0;
@@ -1398,12 +1364,12 @@ int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, cons
         PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, 20, cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         ovf = *reinterpret_cast<uint32_t *>(h + 2);
-        if (!(segments && ovf == 1u && ctx->bands[d_raw].S > 1)) break;
+        if (!(segments && ovf == kOvfNoFit && ctx->bands[d_raw].S > 1)) break;
     }
     *nbits = h[0];
     *tail7 = (uint32_t)h[1];
-    if (ovf & 8) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
-    if (ovf & 2) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish (flags %u)", ovf);
+    if (ovf & kOvfRange) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
+    if (ovf & kOvfFault) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish (flags %u)", ovf);
     if (ovf) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %zu too small (need %llu)", raw_cap,
                               (unsigned long long)((h[0] + 7) / 8));
     return 0;
@@ -1421,8 +1387,8 @@ int pixo_b200_jpeg_band_splice_dev(pixo_b200_ctx *ctx, const uint8_t *d_raw, uin
     }
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     // the stream-ordered flow into a small device scratch: the length, then the flags (OR-ed into)
-    PIXO_TRY(ensure_dev(ctx, ctx->d_misc, 256));
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_misc, 256));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, 256));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, 256));
     auto *d = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
     PIXO_CUDA(ctx, cudaMemsetAsync(d, 0, 16, ctx->stream));
     PIXO_TRY(launch_band_splice(ctx, d_raw, start_bit, tail_in, is_last_band != 0, nullptr, d_out, out_cap, d,
@@ -1530,13 +1496,33 @@ int pixo_b200_jpeg_write_headers(uint32_t width, uint32_t height, uint32_t color
 
 // ---- PNG ----------------------------------------------------------------------------------
 
-static int validate_png(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, size_t row_bytes,
-                        uint32_t bpp, uint32_t strategy)
+// Frames of a batch (n > 1) must not overlap: each frame's input is read whole while other frames'
+// threads write their outputs.  out_name: the caller's name of the output stride.
+static int check_batch_strides(pixo_b200_ctx *ctx, uint32_t n, size_t in_stride, size_t in_bytes,
+                               const char *out_name, size_t out_stride, size_t out_bytes)
 {
-    if (width == 0 || height == 0 || row_bytes == 0)
+    if (n > 1 && in_stride < in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, in_stride);
+    if (n > 1 && out_stride < out_bytes)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "%s %zu below %zu", out_name, out_stride, out_bytes);
+    return 0;
+}
+
+// encode_into's dimension checks (src/png/mod.rs:442-467); empty_rows: rows of 0 bytes
+static int check_png_dimensions(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, bool empty_rows = false)
+{
+    if (width == 0 || height == 0 || empty_rows)
         return set_error(ctx, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", width, height);
     if (width > (1u << 24) || height > (1u << 24))  // src/png/mod.rs:21
         return set_error(ctx, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Image dimensions %ux%u exceed maximum %u", width, height, 1u << 24);
+    return 0;
+}
+
+static int validate_png(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, size_t row_bytes,
+                        uint32_t bpp, uint32_t strategy)
+{
+    PIXO_TRY(check_png_dimensions(ctx, width, height, row_bytes == 0));
     if (bpp < 1 || bpp > 4)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "bytes_per_pixel %u not in 1..4", bpp);
     if ((strategy & ~PIXO_B200_PNG_OPTIMIZE_ALPHA) > PIXO_B200_FILTER_BIGRAMS)
@@ -1552,13 +1538,8 @@ int pixo_b200_png_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t i
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     PIXO_TRY(validate_png(ctx, width, height, row_bytes, bytes_per_pixel, strategy));
     if (!d_data || !d_out) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    // frames of a batch must not overlap: every image's rows are read whole, and its CTAs write
-    // its filtered stream while other images' CTAs write theirs
-    const size_t raw = row_bytes * height, need = (row_bytes + 1) * (size_t)height;
-    if (n_images > 1 && in_stride < raw)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
-    if (n_images > 1 && out_stride < need)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
+    PIXO_TRY(check_batch_strides(ctx, n_images, in_stride, row_bytes * height, "out_stride", out_stride,
+                                 (row_bytes + 1) * (size_t)height));
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return launch_png_filter_rows(ctx, d_data, in_stride, n_images, width, height, row_bytes,
@@ -1574,19 +1555,18 @@ int pixo_b200_png_filter(pixo_b200_ctx *ctx, const uint8_t *data, uint32_t width
     if (!data || !out) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
     const size_t in_bytes = row_bytes * height, out_bytes = (row_bytes + 1) * (size_t)height;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes + 16));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
+    PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
+    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
+    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
+    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
+    uint32_t *d_adler = adler32_out ? static_cast<uint32_t *>(ctx->d_y.ptr) : nullptr;
+    DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
-    uint32_t *d_adler = adler32_out ? reinterpret_cast<uint32_t *>(ctx->d_y.ptr) : nullptr;
-    PIXO_TRY(launch_png_filter_rows(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1,
-                                    width, height, row_bytes, bytes_per_pixel, strategy,
-                                    reinterpret_cast<uint8_t *>(ctx->d_out.ptr), out_bytes, d_adler, nullptr,
-                                    height));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    if (adler32_out)
-        PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    PIXO_TRY(pixo_b200_png_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
+                                      row_bytes, bytes_per_pixel, strategy, d_out, out_bytes, d_adler));
+    PIXO_TRY(d2h_copy_sync(ctx, out, d_out, out_bytes, ctx->stream));
+    if (adler32_out) PIXO_TRY(d2h_copy_sync(ctx, adler32_out, d_adler, 4, ctx->stream));
+    drain.armed = false;
     return 0;
 }
 
@@ -1610,10 +1590,7 @@ int pixo_b200_png_filter_rows_dev(pixo_b200_ctx *ctx, const uint8_t *d_rows, con
 static int validate_png_reduce(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, uint32_t color_type,
                                uint32_t strategy_and_flags)
 {
-    if (width == 0 || height == 0)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", width, height);
-    if (width > (1u << 24) || height > (1u << 24))  // src/png/mod.rs:21
-        return set_error(ctx, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Image dimensions %ux%u exceed maximum %u", width, height, 1u << 24);
+    PIXO_TRY(check_png_dimensions(ctx, width, height));
     if (color_type > PIXO_B200_RGBA)
         return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED_COLOR, "Unsupported color type: %u", color_type);
     const uint32_t known = 0xFFu | PIXO_B200_PNG_OPTIMIZE_ALPHA | PIXO_B200_PNG_REDUCE_COLOR_TYPE | PIXO_B200_PNG_REDUCE_PALETTE;
@@ -1630,12 +1607,8 @@ int pixo_b200_png_reduce_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, s
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     PIXO_TRY(validate_png_reduce(ctx, width, height, color_type, strategy_and_flags));
     if (!d_data || !d_out || !info) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    const size_t raw = (size_t)width * height * (color_type + 1);
-    if (n_images > 1 && in_stride < raw)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
-    const size_t need = (size_t)height * ((size_t)width * (color_type + 1) + 1);
-    if (n_images > 1 && out_stride < need)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
+    PIXO_TRY(check_batch_strides(ctx, n_images, in_stride, (size_t)width * height * (color_type + 1), "out_stride",
+                                 out_stride, (size_t)height * ((size_t)width * (color_type + 1) + 1)));
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return png_reduce_filter(ctx, d_data, in_stride, n_images, width, height, color_type, strategy_and_flags, info,
@@ -1656,24 +1629,21 @@ int pixo_b200_png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t 
                          in_bytes, data_len);
     const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes + 16));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
+    PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
+    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
+    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
+    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
+    auto *d_adler = static_cast<uint32_t *>(ctx->d_y.ptr);
+    DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
-    uint32_t *d_adler = reinterpret_cast<uint32_t *>(ctx->d_y.ptr);
-    PIXO_TRY(png_reduce_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
-                               color_type, strategy_and_flags, info, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
-                               out_bytes, d_adler));
+    PIXO_TRY(pixo_b200_png_reduce_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
+                                             height, color_type, strategy_and_flags, info, d_out, out_bytes, d_adler));
     const size_t got = (size_t)height * (info->row_bytes + 1);
     *out_len = got;
-    if (got > out_cap) {
-        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
-    }
-    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, got, cudaMemcpyDeviceToHost, ctx->stream));
-    if (adler32_out)
-        PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (got > out_cap) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
+    PIXO_TRY(d2h_copy_sync(ctx, out, d_out, got, ctx->stream));
+    if (adler32_out) PIXO_TRY(d2h_copy_sync(ctx, adler32_out, d_adler, 4, ctx->stream));
+    drain.armed = false;
     return 0;
 }
 
@@ -1703,12 +1673,8 @@ int pixo_b200_png_quantize_filter_dev(pixo_b200_ctx *ctx, const uint8_t *d_data,
     for (uint32_t i = 0; palettes && i < n_images; ++i)
         if (palette_lens[i] > 256)
             return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "palette_lens[%u] = %u not in 0..256", i, palette_lens[i]);
-    const size_t raw = (size_t)width * height * (color_type + 1);
-    if (n_images > 1 && in_stride < raw)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, in_stride);
-    const size_t need = (size_t)height * ((size_t)width * (color_type + 1) + 1);
-    if (n_images > 1 && out_stride < need)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "out_stride %zu below %zu", out_stride, need);
+    PIXO_TRY(check_batch_strides(ctx, n_images, in_stride, (size_t)width * height * (color_type + 1), "out_stride",
+                                 out_stride, (size_t)height * ((size_t)width * (color_type + 1) + 1)));
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return png_quantize_filter(ctx, d_data, in_stride, n_images, width, height, color_type, strategy_and_flags,
@@ -1734,25 +1700,23 @@ int pixo_b200_png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_
     if (palette) memcpy(pal256, palette, (size_t)palette_len * 4);
     const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes + 16));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
+    PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
+    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
+    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
+    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
+    auto *d_adler = static_cast<uint32_t *>(ctx->d_y.ptr);
+    DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
-    uint32_t *d_adler = reinterpret_cast<uint32_t *>(ctx->d_y.ptr);
-    PIXO_TRY(png_quantize_filter(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
-                                 color_type, strategy_and_flags, max_colors, palette ? pal256 : nullptr,
-                                 palette ? &palette_len : nullptr, info, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
-                                 out_bytes, d_adler));
+    PIXO_TRY(pixo_b200_png_quantize_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
+                                               height, color_type, strategy_and_flags, max_colors,
+                                               palette ? pal256 : nullptr, palette ? &palette_len : nullptr, info,
+                                               d_out, out_bytes, d_adler));
     const size_t got = (size_t)height * (info->row_bytes + 1);
     *out_len = got;
-    if (got > out_cap) {
-        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
-    }
-    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.ptr, got, cudaMemcpyDeviceToHost, ctx->stream));
-    if (adler32_out)
-        PIXO_CUDA(ctx, cudaMemcpyAsync(adler32_out, d_adler, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (got > out_cap) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, got);
+    PIXO_TRY(d2h_copy_sync(ctx, out, d_out, got, ctx->stream));
+    if (adler32_out) PIXO_TRY(d2h_copy_sync(ctx, adler32_out, d_adler, 4, ctx->stream));
+    drain.armed = false;
     return 0;
 }
 
@@ -1778,14 +1742,14 @@ int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint3
     if (!ctx || !out || (!data && len))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, len + 16));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_y, 64));
-    if (len)
-        PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, len, ctx->stream));
-    PIXO_TRY(launch_adler32(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), len,
-                            reinterpret_cast<uint32_t *>(ctx->d_y.ptr)));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_y.ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    PIXO_TRY(ctx->d_in.ensure(ctx, len + 16));
+    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
+    auto *d_sum = static_cast<uint32_t *>(ctx->d_y.ptr);
+    DrainOnError drain(ctx);
+    if (len) PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, len, ctx->stream));
+    PIXO_TRY(pixo_b200_adler32_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), len, d_sum));
+    PIXO_TRY(d2h_copy_sync(ctx, out, d_sum, 4, ctx->stream));
+    drain.armed = false;
     return 0;
 }
 
@@ -1841,12 +1805,9 @@ int pixo_b200_resize_dev(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_st
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     PIXO_TRY(validate_resize(ctx, src_width, src_height, dst_width, dst_height, color_type, algorithm));
     if (!d_src || !d_dst) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    // frames of a batch must not overlap: a frame's threads write its output while others read theirs
-    const size_t bpp = color_type + 1, raw = (size_t)src_width * src_height * bpp, need = (size_t)dst_width * dst_height * bpp;
-    if (n_images > 1 && src_stride < raw)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu", raw, src_stride);
-    if (n_images > 1 && dst_stride < need)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "dst_stride %zu below %zu", dst_stride, need);
+    const size_t bpp = color_type + 1;
+    PIXO_TRY(check_batch_strides(ctx, n_images, src_stride, (size_t)src_width * src_height * bpp, "dst_stride",
+                                 dst_stride, (size_t)dst_width * dst_height * bpp));
     if (n_images == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     return launch_resize(ctx, d_src, src_stride, n_images, src_width, src_height, dst_width, dst_height,
@@ -1869,13 +1830,16 @@ int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, u
     if (out_cap < out_bytes)
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, out_bytes);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_in, in_bytes));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_out, out_bytes));
+    PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
+    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes));
+    DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
-    PIXO_TRY(launch_resize(ctx, reinterpret_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, src_width, src_height,
-                           dst_width, dst_height, (uint32_t)bpp, algorithm, reinterpret_cast<uint8_t *>(ctx->d_out.ptr),
-                           out_bytes));
-    return d2h_copy_sync(ctx, out, ctx->d_out.ptr, out_bytes, ctx->stream);
+    PIXO_TRY(pixo_b200_resize_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, src_width, src_height,
+                                  dst_width, dst_height, color_type, algorithm, static_cast<uint8_t *>(ctx->d_out.ptr),
+                                  out_bytes));
+    PIXO_TRY(d2h_copy_sync(ctx, out, ctx->d_out.ptr, out_bytes, ctx->stream));
+    drain.armed = false;
+    return 0;
 }
 
 }  // extern "C"

@@ -8,6 +8,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -44,10 +45,33 @@ struct CoefExtents {
     size_t stride;
 };
 
-struct Scratch {
+// Bits of the entropy stage's per-frame (or per-band) overflow word; their values are public
+// (include/pixo_b200.h)
+constexpr uint32_t kOvfNoFit = 1u;     // the scan did not fit its capacity; its length is the size it needs
+constexpr uint32_t kOvfFault = 2u;     // a look-back chain timed out
+constexpr uint32_t kOvfSegment = 4u;   // a segment's raw string outgrew its share
+constexpr uint32_t kOvfRange = 8u;     // a coefficient outside the baseline range
+
+// Reusable scratch of a context: device memory (Buffer<false>, DevBuf) or page-locked host memory
+// (Buffer<true>, PinnedBuf), two types so that one cannot be passed where the other is meant.  Freed
+// with the context.
+template <bool Pinned>
+struct Buffer {
     void *ptr = nullptr;
     size_t cap = 0;
+    Buffer() = default;
+    Buffer(const Buffer &) = delete;
+    Buffer &operator=(const Buffer &) = delete;
+    ~Buffer()
+    {
+        if (ptr) Pinned ? cudaFreeHost(ptr) : cudaFree(ptr);
+    }
+    // at least `bytes`: a smaller buffer is freed, once the context's stream has drained, and
+    // allocated again with room to grow
+    int ensure(pixo_b200_ctx *ctx, size_t bytes);
 };
+using DevBuf = Buffer<false>;
+using PinnedBuf = Buffer<true>;
 
 // A few persistent host threads per context for the one host-side job that is worth spreading:
 // copying a caller's ordinary (pageable) memory into / out of the pinned staging ring while the DMA
@@ -58,7 +82,6 @@ public:
     ~HostPool();
     // fn(job) for job in [0, njobs), on the pool's threads and the caller; returns when all are done
     void run(int njobs, const std::function<void(int)> &fn);
-    int size() const { return (int)threads_.size(); }
 
 private:
     void worker();
@@ -137,31 +160,33 @@ struct pixo_b200_ctx {
     size_t scan_cap_override = 0;  // device scan bytes per frame; 0 = the built-in heuristic
     bool gpu_retry = true;         // re-run k_huff with the exact size when the heuristic was too small
     std::string err;
-    // reusable scratch (device + pinned host)
-    pixo::Scratch d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
-    pixo::Scratch d_hwin;                        // k_huff: every warp's assembled unit, from its phase A to its phase B
-    pixo::Scratch d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
-    pixo::Scratch d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
-    pixo::Scratch d_trellis, h_trellis;          // JPEG trellis: status word + f32 DCT blocks; its status on the host
-    pixo::Scratch d_prog, d_prog_raw, d_prog_out, h_prog;   // JPEG progressive scans: per-block state, raw strings,
-                                                            // stuffed segments; bit counts / lengths on the host
-    pixo::Scratch d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
-    pixo::Scratch h_in, h_out, h_misc, h_red, h_quant;
+    // reusable scratch
+    pixo::DevBuf d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
+    pixo::DevBuf d_hwin;                        // k_huff: every warp's assembled unit, from its phase A to its phase B
+    pixo::DevBuf d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
+    pixo::DevBuf d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
+    pixo::DevBuf d_trellis;                     // JPEG trellis: status word + f32 DCT blocks
+    pixo::DevBuf d_prog, d_prog_raw, d_prog_out;   // JPEG progressive scans: per-block state, raw strings,
+                                                   // stuffed segments
+    pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
+    pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
+    pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
-    pixo::HostPool *pool = nullptr;         // see HostPool
+    std::unique_ptr<pixo::HostPool> pool;   // see HostPool
     // How the bands coded by pixo_b200_jpeg_band_entropy_dev(_async) were cut into segments, keyed by
     // the caller's raw buffer (which holds the segments' strings, bit counts and tails until the splice).
     std::unordered_map<const void *, pixo::SegPlan> bands;
     std::unordered_map<const void *, pixo::KernelAttrs> kernels;   // keyed by the kernel's host function
+
+    pixo_b200_ctx() = default;
+    ~pixo_b200_ctx();   // destroys the streams and events; the scratch frees itself
 };
 
 namespace pixo {
 
 int set_error(pixo_b200_ctx *ctx, int code, const char *fmt, ...);
 int cuda_fail(pixo_b200_ctx *ctx, cudaError_t e, const char *what);
-int ensure_dev(pixo_b200_ctx *ctx, Scratch &s, size_t bytes);
-int ensure_pinned(pixo_b200_ctx *ctx, Scratch &s, size_t bytes);
 
 #define PIXO_CUDA(ctx, call)                                            \
     do {                                                                \

@@ -549,7 +549,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                     L = code_block<false, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
                     if (L > SLOT_W * 32u)  // long block: run again, keeping the words past the slot in local memory
                         L = code_block<true, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
-                    if (CHECK && bad) atomicOr(&P.overflow[C.img], 8u);
+                    if (CHECK && bad) atomicOr(&P.overflow[C.img], kOvfRange);
                     asm volatile("" ::: "memory");  // slot words were written through st.shared
                     const int nw = (int)(L >> 5), filled = (int)(L & 31u);
                     nwt = nw;
@@ -672,7 +672,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             const bool in_tail = lane >= 16 && full_hi >= full_lo && hb < end;
             if (in_head || in_tail) gdst[hb] = sb[hb];
         } else if (lane == 0) {
-            atomicOr(&P.overflow[C.img], 1u);
+            atomicOr(&P.overflow[C.img], kOvfNoFit);
         }
         __syncwarp();  // sbuf is rewritten by the next piece, or by the next unit's stage
     };
@@ -763,7 +763,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                             }
                         }
                     } else if (lane == 0) {
-                        atomicOr(&P.overflow[C.img], 1u);
+                        atomicOr(&P.overflow[C.img], kOvfNoFit);
                     }
                     continue;
                 }
@@ -805,7 +805,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         }
         if (lane == 0 && C.final_) {
             P.out_len[C.img] = G;
-            if (G > P.out_cap) atomicOr(&P.overflow[C.img], 1u);
+            if (G > P.out_cap) atomicOr(&P.overflow[C.img], kOvfNoFit);
         }
     };
 
@@ -826,9 +826,9 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             if (lane == 0 && C.final_) {
                 P.out_len[C.img] = C.Pc + C.Lc;       // BITS
                 P.out_tail[C.img] = C.ctail;
-                if (((C.Pc + C.Lc + 7) >> 3) > P.out_cap) atomicOr(&P.overflow[C.img], 1u);
+                if (((C.Pc + C.Lc + 7) >> 3) > P.out_cap) atomicOr(&P.overflow[C.img], kOvfNoFit);
             }
-            if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], 2u);
+            if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], kOvfFault);
             return;
         }
         if (lane == 0) st_status(st2 + C.unit, pack_status(C.unit == 0 ? ST_PFX : ST_AGG, 0, C.own));
@@ -845,7 +845,7 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             if (lane == 0) st_status(st2 + C.unit, pack_status(ST_PFX, 0, ffx + C.own));
         }
         emit(C, ffx);   // chain 2 counts every byte written before this unit
-        if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], 2u);
+        if (lane == 0 && C.fault) atomicOr(&P.overflow[C.img], kOvfFault);
     };
 
     UnitState cur, pend;
@@ -1084,7 +1084,7 @@ __global__ void __launch_bounds__(SPL_THREADS) k_seg_prefix(const __grid_constan
         P.ntiles[i] = total_tiles;
         // a raw segment that did not fit (or a faulted chain): the caller codes the image again unsegmented;
         // a coefficient outside the baseline range (bit 3) is passed on, the caller does not retry it
-        if (bad || total_tiles > P.max_tiles) { P.overflow[i] = 4u | (bad & 10u); P.ntiles[i] = 0; P.out_len[i] = 0; }
+        if (bad || total_tiles > P.max_tiles) { P.overflow[i] = kOvfSegment | (bad & (kOvfFault | kOvfRange)); P.ntiles[i] = 0; P.out_len[i] = 0; }
         else if (total_tiles == 0) P.out_len[i] = 0;
     }
 }
@@ -1242,7 +1242,7 @@ __global__ void __launch_bounds__(SPL_THREADS) k_seg_emit(const __grid_constant_
         const unsigned long long tile_n = min((unsigned long long)SPL_TILE, r.nbytes - tile_first);
         const uint32_t nout = (uint32_t)tile_n + total;
         if (g0 + nout <= P.out_cap) copy_out16(outp, g0, sb, shb, nout, tid);
-        else if (tid == 0) atomicOr(&P.overflow[i], 1u);
+        else if (tid == 0) atomicOr(&P.overflow[i], kOvfNoFit);
         if (tid == 0 && t == nt - 1) P.out_len[i] = g0 + nout;   // the size needed, also when it did not fit
         __syncthreads();   // the stage and wsum are rewritten by the next tile
     }
@@ -1442,7 +1442,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     const uint32_t S = (rst_blocks == 0 && allow_segments) ? segments_for(n, g.total_mcus(), bpm_) : 1;
     const SegPlan sp = plan_segments(n, S, g.total_mcus(), bpm_, mcu_raw_bytes(g));
     if (sp.S > 1) {
-        PIXO_TRY(ensure_dev(ctx, ctx->d_raw, sp.total + sp.raw_total));
+        PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total + sp.raw_total));
         auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
         uint8_t *raw_area = seg_scratch + sp.total;
         PIXO_TRY(code_segments(ctx, P, T, n, g, sp, seg_scratch, raw_area));
@@ -1452,7 +1452,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     }
     const size_t want = ((size_t)n * pl.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    PIXO_TRY(ensure_dev(ctx, ctx->d_hwin, (size_t)grid * HUFF_WARPS * GWIN_B));
+    PIXO_TRY(ctx->d_hwin.ensure(ctx, (size_t)grid * HUFF_WARPS * GWIN_B));
     P.win = reinterpret_cast<uint8_t *>(ctx->d_hwin.ptr);
     return launch(ctx, check ? k_huff<false, true> : k_huff<false, false>, grid, 32 * HUFF_WARPS, 0, P, T);
 }
@@ -1487,7 +1487,7 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
                              (unsigned long long)raw_cap, sp.raw_total);
         lay_out(sp, 1, bpm, (size_t)(raw_cap - trailer) / 256 * 256);
     }
-    PIXO_TRY(ensure_dev(ctx, ctx->d_raw, sp.total));
+    PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total));
     auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
     EntParams P;
     memset(&P, 0, sizeof P);
@@ -1516,7 +1516,7 @@ int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_b
     if (it == ctx->bands.end())
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "this raw buffer was not coded by pixo_b200_jpeg_band_entropy_dev");
     const SegPlan sp = it->second;
-    PIXO_TRY(ensure_dev(ctx, ctx->d_raw, sp.total));
+    PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total));
     return splice_segments(ctx, 1, sp, reinterpret_cast<uint8_t *>(ctx->d_raw.ptr), d_raw, nullptr, base_bit, base_tail,
                            last, d_base, d_out, out_cap, d_out_len, d_flags);
 }

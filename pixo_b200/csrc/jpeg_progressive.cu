@@ -477,7 +477,7 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
 {
     cudaStream_t st = ctx->stream;
     const ProgLayout L = prog_layout(g, n);
-    PIXO_TRY(ensure_dev(ctx, ctx->d_prog, L.total));
+    PIXO_TRY(ctx->d_prog.ensure(ctx, L.total));
     auto *base = static_cast<uint8_t *>(ctx->d_prog.ptr);
     ProgParams P;
     memset(&P, 0, sizeof P);
@@ -507,7 +507,7 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     }
     PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
     const size_t nstream = (size_t)n * NSCAN;
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_prog, 256 + nstream * 8));
+    PIXO_TRY(ctx->h_prog.ensure(ctx, 256 + nstream * 8));
     auto *h_status = static_cast<uint32_t *>(ctx->h_prog.ptr);
     auto *h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
@@ -526,8 +526,8 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     const size_t stage_cap = (2 * raw_cap + 256) / 256 * 256;   // every byte 0xFF still fits
     const size_t off_len = sp.total, off_ovf = off_len + (nstream * 8 + 255) / 256 * 256;
     const size_t off_stage = off_ovf + (nstream * 4 + 255) / 256 * 256;
-    PIXO_TRY(ensure_dev(ctx, ctx->d_prog_raw, sp.raw_total));
-    PIXO_TRY(ensure_dev(ctx, ctx->d_prog_out, off_stage + nstream * stage_cap));
+    PIXO_TRY(ctx->d_prog_raw.ensure(ctx, sp.raw_total));
+    PIXO_TRY(ctx->d_prog_out.ensure(ctx, off_stage + nstream * stage_cap));
     auto *raw = static_cast<uint8_t *>(ctx->d_prog_raw.ptr);
     auto *outb = static_cast<uint8_t *>(ctx->d_prog_out.ptr);
     PIXO_CUDA(ctx, cudaMemsetAsync(raw, 0, sp.raw_total, st));
@@ -539,7 +539,7 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     auto *d_len = reinterpret_cast<uint64_t *>(outb + off_len);
     auto *d_ovf = reinterpret_cast<uint32_t *>(outb + off_ovf);
     PIXO_TRY(launch_splice(ctx, n * NSCAN, sp, outb, raw, outb + off_stage, stage_cap, d_len, d_ovf));
-    PIXO_TRY(ensure_pinned(ctx, ctx->h_prog, 256 + nstream * 12));
+    PIXO_TRY(ctx->h_prog.ensure(ctx, 256 + nstream * 12));
     h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
     auto *h_ovf = reinterpret_cast<uint32_t *>(h_bits + nstream);
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, d_len, nstream * 8, cudaMemcpyDeviceToHost, st));

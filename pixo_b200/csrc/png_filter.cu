@@ -994,7 +994,7 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
                     2 * (16 + (size_t)SEG_BYTES) + SEG_BYTES + 32 + 8192};
     // misc scratch: per image {accA, accB} u64, counter u32, decided u8
     const size_t per = 2 * sizeof(unsigned long long) + sizeof(uint32_t) + 4;
-    PIXO_TRY(ensure_dev(ctx, ctx->d_misc, (size_t)n_images * per + 64));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, (size_t)n_images * per + 64));
     auto *acc = reinterpret_cast<unsigned long long *>(ctx->d_misc.ptr);
     auto *counter = reinterpret_cast<uint32_t *>(acc + 2 * (size_t)n_images);
     auto *decided = reinterpret_cast<uint8_t *>(counter + n_images);
@@ -1055,7 +1055,7 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
 
 int launch_adler32(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32_t *d_out)
 {
-    PIXO_TRY(ensure_dev(ctx, ctx->d_misc, 64));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, 64));
     auto *acc = reinterpret_cast<unsigned long long *>(ctx->d_misc.ptr);
     auto *counter = reinterpret_cast<uint32_t *>(acc + 2);
     PIXO_CUDA(ctx, cudaMemsetAsync(ctx->d_misc.ptr, 0, 64, ctx->stream));

@@ -398,8 +398,8 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
                                                           (uint32_t *)nullptr, (int)maxk, ctx->stream));
         const size_t off_b = align_up(maxk * 8, 256), off_u = off_b + align_up(maxk * 8, 256), off_c = off_u + align_up(maxk * 8, 256);
         const size_t off_n = off_c + align_up(maxk * 4, 256), off_t = off_n + 256;
-        PIXO_TRY(ensure_dev(ctx, ctx->d_quant, off_t + std::max(tmp_sort, tmp_rle)));
-        PIXO_TRY(ensure_pinned(ctx, ctx->h_quant, maxk * 12 + 16));
+        PIXO_TRY(ctx->d_quant.ensure(ctx, off_t + std::max(tmp_sort, tmp_rle)));
+        PIXO_TRY(ctx->h_quant.ensure(ctx, maxk * 12 + 16));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant.ptr);
         auto *ka = reinterpret_cast<unsigned long long *>(base), *kb = reinterpret_cast<unsigned long long *>(base + off_b);
         auto *uq = reinterpret_cast<unsigned long long *>(base + off_u);
@@ -477,7 +477,7 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         const size_t o_lut = o_col + align_up(nq * MAX_HIST_COLORS * 8, 256), groups = (height + 31) / 32;
         const size_t o_edge = o_lut + align_up(nq * LUT_CELLS, 256), o_prog = o_edge + align_up(nq * (groups - 1 + 1) * width * 4, 256);
         const size_t o_tick = o_prog + align_up(nq * groups * 4, 256), o_idx = o_tick + 256;
-        PIXO_TRY(ensure_dev(ctx, ctx->d_quant_img, o_idx + nq * idx_stride));
+        PIXO_TRY(ctx->d_quant_img.ensure(ctx, o_idx + nq * idx_stride));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant_img.ptr);
         auto *d_pal = reinterpret_cast<uint32_t *>(base + o_pal);
         auto *d_acc = reinterpret_cast<unsigned long long *>(base + o_acc);

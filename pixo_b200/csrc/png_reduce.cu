@@ -345,8 +345,8 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
     if (want_pal || want_ct) {
         // 1. analysis of the whole batch
         const size_t stat_bytes = (size_t)n_images * sizeof(ReduceStat);
-        PIXO_TRY(ensure_dev(ctx, ctx->d_red, stat_bytes));
-        PIXO_TRY(ensure_pinned(ctx, ctx->h_red, stat_bytes));
+        PIXO_TRY(ctx->d_red.ensure(ctx, stat_bytes));
+        PIXO_TRY(ctx->h_red.ensure(ctx, stat_bytes));
         auto *d_stat = reinterpret_cast<ReduceStat *>(ctx->d_red.ptr);
         auto *h_stat = reinterpret_cast<ReduceStat *>(ctx->h_red.ptr);
         PIXO_CUDA(ctx, cudaMemsetAsync(d_stat, 0, stat_bytes, ctx->stream));
@@ -400,7 +400,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         const size_t np = pal_ids.size();
         const size_t jobs_off = (np * npix + 255) & ~(size_t)255;
         const size_t cnt_off = jobs_off + ((np * sizeof(IndexJob) + 255) & ~(size_t)255);
-        PIXO_TRY(ensure_dev(ctx, ctx->d_red_idx, cnt_off + np * cnt_words * 4));
+        PIXO_TRY(ctx->d_red_idx.ensure(ctx, cnt_off + np * cnt_words * 4));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_red_idx.ptr);
         auto *d_jobs = reinterpret_cast<IndexJob *>(base + jobs_off);
         auto *d_cnt = reinterpret_cast<uint32_t *>(base + cnt_off);
@@ -506,7 +506,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
     if (!pack.empty()) {
         const size_t jobs_bytes = pack.size() * sizeof(PackJob);
         const size_t img_off = (jobs_bytes + 255) & ~(size_t)255;
-        PIXO_TRY(ensure_dev(ctx, ctx->d_red_img, img_off + (size_t)n_images * red_stride));
+        PIXO_TRY(ctx->d_red_img.ensure(ctx, img_off + (size_t)n_images * red_stride));
         auto *base = reinterpret_cast<uint8_t *>(ctx->d_red_img.ptr);
         d_red_img = base + img_off;
         for (size_t k = 0; k < pack.size(); ++k) pack[k].dst = d_red_img + (size_t)pack_img[k] * red_stride;

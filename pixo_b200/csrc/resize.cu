@@ -257,7 +257,7 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
                  o_vc = o_vs + align_up(4 * (size_t)dh, 256), o_ho = o_vc + align_up(4 * (size_t)dh, 256), o_vo = o_ho + align_up(8 * (size_t)dw, 256),
                  o_hw = o_vo + align_up(8 * (size_t)dh, 256), o_vw = o_hw + align_up(4 * h.w.size() + 4, 256),
                  total = o_vw + align_up(4 * v.w.size() + 4, 256);
-    PIXO_TRY(ensure_dev(ctx, ctx->d_resize, total));
+    PIXO_TRY(ctx->d_resize.ensure(ctx, total));
     uint8_t *T = reinterpret_cast<uint8_t *>(ctx->d_resize.ptr);
     const struct { size_t off; const void *p; size_t bytes; } up[] = {
         {o_hs, h.start.data(), 4 * (size_t)dw}, {o_hc, h.count.data(), 4 * (size_t)dw},
@@ -277,7 +277,7 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
     // frames per pass: as many whole intermediates as the cap holds (only when one band covers the frame)
     const uint32_t per_pass = bands.size() == 1 ? (uint32_t)std::min<size_t>({n, 65535, std::max<size_t>(1, kResizeScratch / most)}) : 1;
     const size_t tstride = (most + 255) / 256 * 256;
-    PIXO_TRY(ensure_dev(ctx, ctx->d_resize_tmp, tstride * per_pass));
+    PIXO_TRY(ctx->d_resize_tmp.ensure(ctx, tstride * per_pass));
     uint8_t *tmp = reinterpret_cast<uint8_t *>(ctx->d_resize_tmp.ptr);
     for (uint32_t f0 = 0; f0 < n; f0 += per_pass) {
         const uint32_t nf = std::min(per_pass, n - f0);
