@@ -10,8 +10,24 @@
  *
  * Conventions
  *  - plain pointers and sizes only; the caller owns every buffer; the library never retains
- *    or frees caller memory.  `_dev` variants take device pointers and are asynchronous on the
- *    context's stream; the others take host pointers and return after the result is in `out`.
+ *    or frees caller memory.  `_dev` variants take device pointers and run in order on the
+ *    context's stream: after the work queued on it before the call, before the work queued after.
+ *    These return with their work still queued (a call that grows the context's scratch first
+ *    waits for the stream once, to free the smaller buffer):
+ *      jpeg_coefficients_dev (without PIXO_B200_COEF_TRELLIS), jpeg_encode_dev, png_filter_dev,
+ *      png_filter_rows_dev, adler32_dev, resize_dev, jpeg_band_histogram_dev,
+ *      jpeg_band_entropy_dev_async, jpeg_band_splice_dev_async.
+ *    (resize_dev with Lanczos3 stages its weight tables in one of the context's two pinned buffers,
+ *    in turn, and first waits until the copy out of that buffer, two Lanczos3 calls back, has run.)
+ *    These wait for the work queued before them, and for part of their own, before they return,
+ *    because a result they read back decides what they do next or is a host output (the last
+ *    kernels or copies of progressive_scans_dev, reduce_filter_dev and quantize_filter_dev are
+ *    still queued when they return):
+ *      jpeg_coefficients_dev with PIXO_B200_COEF_TRELLIS, jpeg_trellis_quantize_dev,
+ *      jpeg_progressive_scans_dev, jpeg_entropy_encode_dev, jpeg_band_last_dc,
+ *      jpeg_band_entropy_dev, jpeg_band_splice_dev, png_reduce_filter_dev,
+ *      png_quantize_filter_dev.
+ *    The others take host pointers and return after the result is in `out`.
  *  - every function returns a pixo_b200_status (0 = ok).  pixo_b200_last_error(ctx) gives the
  *    message a Rust shim would wrap in Error::CompressionError(String) (src/error.rs:41).
  *    Validation errors mirror the reference's own checks (src/jpeg/mod.rs:333-373,
@@ -76,7 +92,12 @@ void pixo_b200_ctx_destroy(pixo_b200_ctx *ctx);
 /* last error message of this context (thread's last error when ctx == NULL); never NULL */
 const char *pixo_b200_last_error(const pixo_b200_ctx *ctx);
 /* adopt an external CUDA stream (cudaStream_t) for all work of this context; NULL restores
- * the context's own stream */
+ * the context's own stream.  Work queued before the switch is ordered before work queued after it:
+ * the new stream waits, on the device, for the old one's work so far (the host does not wait), so
+ * the context's scratch, pixo_b200_ctx_sync, pixo_b200_download and pixo_b200_ctx_destroy stay
+ * correct across the switch.  Switching to the current stream does nothing.  An adopted stream must
+ * stay valid until the context has switched away from it (the switch records an event on it) or has
+ * been destroyed (pixo_b200_ctx_sync and pixo_b200_ctx_destroy synchronise it). */
 int pixo_b200_ctx_set_stream(pixo_b200_ctx *ctx, void *cuda_stream);
 void *pixo_b200_ctx_stream(pixo_b200_ctx *ctx);
 int pixo_b200_ctx_sync(pixo_b200_ctx *ctx);
@@ -498,7 +519,7 @@ int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, u
  * alignment and any n_images.  Frames must not overlap: with n_images > 1, src_stride below a source
  * frame returns PIXO_B200_ERR_INVALID_DATA_LENGTH and dst_stride below a destination frame
  * PIXO_B200_ERR_OUTPUT_TOO_SMALL.  Nothing is launched unless the call is valid.  Lanczos3's weight tables
- * are uploaded before the call returns; its intermediate stays within 256 MiB of device scratch (larger
+ * are computed on the host and uploaded on the stream from the context's pinned buffers; its intermediate stays within 256 MiB of device scratch (larger
  * frames go in bands of destination rows).  The output is packed pixels, what
  * pixo_b200_jpeg_encode_dev and pixo_b200_png_filter_dev read. */
 int pixo_b200_resize_dev(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, uint32_t n_images,

@@ -280,6 +280,9 @@ pixo_b200_ctx::~pixo_b200_ctx()
 {
     for (cudaEvent_t ev : events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : stage_events) cudaEventDestroy(ev);
+    if (switch_event) cudaEventDestroy(switch_event);
+    for (cudaEvent_t ev : resize_events)
+        if (ev) cudaEventDestroy(ev);
     if (own_stream) cudaStreamDestroy(own_stream);
     if (copy_stream) cudaStreamDestroy(copy_stream);
     if (d2h_stream) cudaStreamDestroy(d2h_stream);
@@ -320,6 +323,10 @@ int pixo_b200_ctx_create(int device, pixo_b200_ctx **out)
         (e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking)) != cudaSuccess)
         return cuda_fail(nullptr, e, "cudaStreamCreate");
+    if ((e = cudaEventCreateWithFlags(&ctx->switch_event, cudaEventDisableTiming)) != cudaSuccess ||
+        (e = cudaEventCreateWithFlags(&ctx->resize_events[0], cudaEventDisableTiming)) != cudaSuccess ||
+        (e = cudaEventCreateWithFlags(&ctx->resize_events[1], cudaEventDisableTiming)) != cudaSuccess)
+        return cuda_fail(nullptr, e, "cudaEventCreate");
     ctx->stream = ctx->own_stream;
     unsigned hc = std::thread::hardware_concurrency();
     ctx->host_threads = hc ? (int)hc : 1;
@@ -343,7 +350,15 @@ const char *pixo_b200_last_error(const pixo_b200_ctx *ctx)
 int pixo_b200_ctx_set_stream(pixo_b200_ctx *ctx, void *cuda_stream)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    ctx->stream = cuda_stream ? reinterpret_cast<cudaStream_t>(cuda_stream) : ctx->own_stream;
+    cudaStream_t next = cuda_stream ? reinterpret_cast<cudaStream_t>(cuda_stream) : ctx->own_stream;
+    if (next == ctx->stream) return 0;
+    // Work queued on the old stream still uses the context's scratch, and ctx_sync, ctx_destroy and the
+    // scratch's grow-and-free only wait on the current stream: the new stream waits for the old one's
+    // work, on the device, so everything queued before the switch is ordered before everything after it.
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_CUDA(ctx, cudaEventRecord(ctx->switch_event, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamWaitEvent(next, ctx->switch_event, 0));
+    ctx->stream = next;
     return 0;
 }
 

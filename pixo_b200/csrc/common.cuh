@@ -171,8 +171,12 @@ struct pixo_b200_ctx {
     pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
+    pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn
     std::vector<cudaEvent_t> events;
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
+    cudaEvent_t switch_event = nullptr;     // pixo_b200_ctx_set_stream: the new stream waits for the old one
+    cudaEvent_t resize_events[2] = {};      // the last copy out of h_resize[i] has run
+    uint64_t resize_uploads = 0;            // Lanczos3 table uploads so far (h_resize[resize_uploads % 2] is next)
     std::unique_ptr<pixo::HostPool> pool;   // see HostPool
     // How the bands coded by pixo_b200_jpeg_band_entropy_dev(_async) were cut into segments, keyed by
     // the caller's raw buffer (which holds the segments' strings, bit counts and tails until the splice).

@@ -9,6 +9,8 @@
 // kResizeScratch bytes: frames that fit go through together, a larger frame is done in bands of
 // destination rows (and, where one row's taps alone exceed the cap, in column chunks).  The weight tables
 // come from the host (resize_host.cpp): pixo's sinf is not CUDA's.
+#include <string.h>
+
 #include <algorithm>
 
 #include "common.cuh"
@@ -264,8 +266,18 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
         {o_vs, v.start.data(), 4 * (size_t)dh}, {o_vc, v.count.data(), 4 * (size_t)dh},
         {o_ho, h.offset.data(), 8 * (size_t)dw}, {o_vo, v.offset.data(), 8 * (size_t)dh},
         {o_hw, h.w.data(), 4 * h.w.size()},      {o_vw, v.w.data(), 4 * v.w.size()}};
+    // One copy from one of the context's two pinned buffers, in turn.  A copy from the pageable vectors
+    // lets the driver wait for the stream before the call returns (it does for some MB of tables); a
+    // pinned one is only queued.  A buffer is rewritten once the copy out of it, two uploads back, has run.
+    const int slot = (int)(ctx->resize_uploads % 2);
+    PIXO_CUDA(ctx, cudaEventSynchronize(ctx->resize_events[slot]));
+    PIXO_TRY(ctx->h_resize[slot].ensure(ctx, total));
+    uint8_t *H = reinterpret_cast<uint8_t *>(ctx->h_resize[slot].ptr);
     for (const auto &u : up)
-        if (u.bytes) PIXO_CUDA(ctx, cudaMemcpyAsync(T + u.off, u.p, u.bytes, cudaMemcpyHostToDevice, ctx->stream));
+        if (u.bytes) memcpy(H + u.off, u.p, u.bytes);
+    PIXO_CUDA(ctx, cudaMemcpyAsync(T, H, total, cudaMemcpyHostToDevice, ctx->stream));
+    PIXO_CUDA(ctx, cudaEventRecord(ctx->resize_events[slot], ctx->stream));
+    ctx->resize_uploads++;
     const uint32_t *hs = reinterpret_cast<const uint32_t *>(T + o_hs), *hc = reinterpret_cast<const uint32_t *>(T + o_hc);
     const uint32_t *vs = reinterpret_cast<const uint32_t *>(T + o_vs), *vc = reinterpret_cast<const uint32_t *>(T + o_vc);
     const uint64_t *ho = reinterpret_cast<const uint64_t *>(T + o_ho), *vo = reinterpret_cast<const uint64_t *>(T + o_vo);
