@@ -85,6 +85,8 @@ void HostPool::worker()
             seen = generation_;
             fn = fn_;
             n = njobs_;
+            // woke after that run() had returned: claiming from next_ now would take a job of the next run()
+            if (!fn) continue;
             ++active_;
         }
         for (int j; (j = next_.fetch_add(1)) < n;) (*fn)(j);
@@ -278,10 +280,9 @@ using namespace pixo;
 
 pixo_b200_ctx::~pixo_b200_ctx()
 {
-    for (cudaEvent_t ev : events) cudaEventDestroy(ev);
     for (cudaEvent_t ev : stage_events) cudaEventDestroy(ev);
-    if (switch_event) cudaEventDestroy(switch_event);
-    for (cudaEvent_t ev : resize_events)
+    for (cudaEvent_t ev : {switch_event, resize_events[0], resize_events[1], ev_in[0], ev_in[1], ev_used[0], ev_used[1],
+                           ev_out[0], ev_out[1], ev_len[0], ev_len[1]})
         if (ev) cudaEventDestroy(ev);
     if (own_stream) cudaStreamDestroy(own_stream);
     if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -323,10 +324,11 @@ int pixo_b200_ctx_create(int device, pixo_b200_ctx **out)
         (e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking)) != cudaSuccess)
         return cuda_fail(nullptr, e, "cudaStreamCreate");
-    if ((e = cudaEventCreateWithFlags(&ctx->switch_event, cudaEventDisableTiming)) != cudaSuccess ||
-        (e = cudaEventCreateWithFlags(&ctx->resize_events[0], cudaEventDisableTiming)) != cudaSuccess ||
-        (e = cudaEventCreateWithFlags(&ctx->resize_events[1], cudaEventDisableTiming)) != cudaSuccess)
-        return cuda_fail(nullptr, e, "cudaEventCreate");
+    for (cudaEvent_t *ev : {&ctx->switch_event, &ctx->resize_events[0], &ctx->resize_events[1], &ctx->ev_in[0],
+                            &ctx->ev_in[1], &ctx->ev_used[0], &ctx->ev_used[1], &ctx->ev_out[0], &ctx->ev_out[1],
+                            &ctx->ev_len[0], &ctx->ev_len[1]})
+        if ((e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming)) != cudaSuccess)
+            return cuda_fail(nullptr, e, "cudaEventCreate");
     ctx->stream = ctx->own_stream;
     unsigned hc = std::thread::hardware_concurrency();
     ctx->host_threads = hc ? (int)hc : 1;
@@ -715,20 +717,6 @@ int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, 
     return trellis_status(ctx, status);
 }
 
-static int validate_encode(pixo_b200_ctx *ctx, size_t pixels_len, uint32_t width, uint32_t height,
-                           uint32_t color_type, uint32_t quality, uint32_t subsampling,
-                           uint32_t restart_interval)
-{
-    PIXO_TRY(validate_options(ctx, quality, restart_interval));
-    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
-    const size_t bpp = color_type == PIXO_B200_GRAY ? 1 : 3;
-    const size_t expected = (size_t)width * height * bpp;
-    if (pixels_len != expected)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH,
-                         "Invalid data length: expected %zu bytes, got %zu", expected, pixels_len);
-    return 0;
-}
-
 // Device scan capacity per frame: a JPEG that needs more than half its raw size (noise at very
 // high quality) is coded a second time with the exact size the kernel reported.
 static uint64_t default_scan_cap(const pixo_b200_ctx *ctx, size_t raw_bytes)
@@ -748,7 +736,7 @@ static const char kOutOfRange[] = "coefficient out of the baseline range (|AC| <
 // the size it needs) runs again with room for that size, unless headers, scan and EOI would no
 // longer fit out_cap.  Three passes at most.  Returns 0 with the scan at the start of d_retry and
 // its length in *len, kGaveUp, or an error.  It touches no other scratch of the context but
-// d_raw (segmented passes), so encode_frames can use it while the next group's work is queued.
+// d_raw (segmented passes), so the baseline group loop can use it while the next group's work is queued.
 // ext: the transform's coefficient records (always in range); null: the caller's arrays, checked
 // (launch_jpeg_entropy).
 static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
@@ -784,71 +772,117 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
     }
 }
 
-// Encode n frames of identical geometry and options.  GPU: colour/DCT/quantise (K1/K2), symbol
-// statistics when optimize_huffman (K3), Huffman bit packing + 0xFF stuffing + restart markers
-// (k_huff); host: headers, optimised-table construction, EOI.  Frames are processed in groups of
-// up to 16 (about 96 MB of input) on three streams: the H2D copy of group g+1 (copy stream) and the D2H copy of group
-// g-1's scan bytes (d2h stream) run under the kernels of group g, and the host never drains the
-// compute stream between groups - it only waits for the event behind a group's 12-byte-per-frame
-// length readback before it queues that group's D2H.  Only finished scan bytes come back over
-// PCIe.  A frame whose scan outgrows the device buffer is coded again on the GPU with the exact
-// size; the host entropy coder (same GPU coefficient arrays) is the last resort for a faulted
-// device stage and is counted in ctx->host_fallbacks.
-// progressive (encode_progressive, src/jpeg/mod.rs:872-927): the transform writes dense natural-order
-// arrays instead of records (K3 reads them for the optimised tables, which pixo builds from the
-// plain-rounded coefficients, restart interval included); with trellis the arrays are then overwritten by
-// COEF_TRELLIS (the plain transform is skipped when no table needs it); the progressive stage codes the 7
-// scans, and the host writes SOF2, the SOS of each scan and copies the segments in between.  A group is
-// finished before the next one is computed (the stage's buffers are the context's).
-static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_each, uint32_t n_images,
-                         const FrameGeometry &g, uint32_t quality, uint32_t restart_interval,
-                         bool optimize, uint8_t *out, size_t out_cap_each, size_t *out_lens,
-                         bool progressive = false, bool trellis = false)
+// The transform of cnt frames, pixel_stride bytes apart, into coefficient records at c (layout L)
+static int transform_records(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t cnt,
+                             const FrameGeometry &g, const float *lum, const float *chr, const CoefLayout &L, uint8_t *c)
 {
-    if (out_cap_each < 1024 + 2)  // before any GPU work is queued
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap_each);
+    const CoefExtents ec = L.extents(c);
+    return launch_jpeg_transform(ctx, d_pixels, pixel_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
+                                 chr, L.y(c), L.stride(), g.has_chroma ? L.cb(c) : nullptr,
+                                 g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0, &ec);
+}
+
+// k_huff, segments allowed, over the coefficient records of cnt frames at c: one pass with tables tb[0], or with a
+// table per frame one pass per frame, each in its own scratch.  Frame k's scan goes to scan + k * scan_cap, its
+// length and overflow flags to len[k] and ovf[k] (host or device memory, as `kind` says).
+static int code_records(pixo_b200_ctx *ctx, const CoefLayout &L, uint8_t *c, uint32_t cnt, const FrameGeometry &g,
+                        const HuffTables *tb, bool per_frame, uint32_t restart_interval, uint8_t *ent, uint8_t *scan,
+                        uint64_t scan_cap, uint64_t *len, uint32_t *ovf, cudaMemcpyKind kind)
+{
+    const size_t cs = L.stride(), ent_one = per_frame ? entropy_scratch_bytes(1, g, restart_interval) : 0;
+    const uint32_t passes = per_frame ? cnt : 1, each = per_frame ? 1 : cnt;   // frames per pass
+    for (uint32_t k = 0; k < passes; ++k) {
+        uint8_t *f = c + (size_t)k * L.each;
+        const CoefExtents ef = L.extents(f);
+        uint64_t *d_len = nullptr;
+        uint32_t *d_ovf = nullptr;
+        PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, each, g, tb[k], restart_interval, true, &ef,
+                                     ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len, &d_ovf));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(len + k, d_len, (size_t)each * 8, kind, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(ovf + k, d_ovf, (size_t)each * 4, kind, ctx->stream));
+    }
+    return 0;
+}
+
+// k_huff scratch of a baseline group of k frames: with per-frame tables (optimize) each frame has its own
+static size_t group_ent_bytes(uint32_t k, const FrameGeometry &g, uint32_t restart_interval, bool optimize)
+{
+    return optimize ? (size_t)k * entropy_scratch_bytes(1, g, restart_interval)
+                    : entropy_scratch_bytes(k, g, restart_interval);
+}
+
+// What the two group loops of the host encode share: n frames, G per group, each group's pixels uploaded on the
+// copy stream into one of two input slots of d_in, in turn, while the context's stream works on the group before.
+struct EncodeGroups {
+    pixo_b200_ctx *ctx;
+    const uint8_t *pixels;
+    size_t len_each, in_stride;
+    uint32_t n, G;
+
+    uint32_t count() const { return (n + G - 1) / G; }
+    uint32_t size(uint32_t gi) const { return std::min(G, n - gi * G); }
+    uint8_t *input(uint32_t gi) const { return static_cast<uint8_t *>(ctx->d_in.ptr) + (gi & 1) * G * in_stride; }
+    // Group gi's frames into its input slot.  Group 0 first makes both copy streams wait for whatever the caller
+    // already queued on the context's stream (ev_out[0] is free until group 0's scan bytes are copied back);
+    // group gi >= 2 waits until the transform of group gi - 2 has read the slot.
+    int upload(uint32_t gi) const
+    {
+        const int slot = (int)(gi & 1);
+        if (gi == 0) {
+            PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_out[0], ctx->stream));
+            PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_out[0], 0));
+            PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->d2h_stream, ctx->ev_out[0], 0));
+        }
+        if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[slot], 0));
+        for (uint32_t k = 0; k < size(gi); ++k)
+            PIXO_TRY(h2d_copy(ctx, input(gi) + k * in_stride, pixels + ((size_t)gi * G + k) * len_each, len_each,
+                              ctx->copy_stream));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_in[slot], ctx->copy_stream));
+        return 0;
+    }
+};
+
+// The groups of a host encode call: about 96 MB of input (4 frames at 4K, 15 at 1080p), at most 16, at
+// least two groups per call: long enough for full-rate DMA and to amortise the launches, short enough that what
+// no upload can hide - the last group's kernels and the read-back of its scan bytes - stays small.  Fewer while
+// the baseline loop's scratch for two groups would pass 4 GiB; the progressive loop groups its frames the same way.
+static EncodeGroups make_groups(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t n, size_t len_each,
+                                const FrameGeometry &g, uint32_t restart_interval, bool optimize)
+{
+    const size_t in_stride = align_up(len_each, 256), coef_each = CoefLayout(g).each;
+    const uint64_t scan_cap = default_scan_cap(ctx, len_each);
+    uint32_t G = (uint32_t)std::min<size_t>(16, std::max<size_t>(1, (((size_t)96 << 20) + len_each / 2) / len_each));
+    G = std::min(G, std::max(1u, (n + 1) / 2));
+    auto group_bytes = [&](uint32_t k) {
+        return 2 * (size_t)k * (in_stride + coef_each + scan_cap) + group_ent_bytes(k, g, restart_interval, optimize);
+    };
+    while (G > 1 && group_bytes(G) > ((size_t)4 << 30)) --G;
+    return EncodeGroups{ctx, pixels, len_each, in_stride, n, G};
+}
+
+// Baseline frames.  GPU: colour/DCT/quantise into coefficient records (K1/K2), symbol statistics when optimize
+// (K3), k_huff; host: headers, optimised tables, EOI.  The H2D copy of group g+1 and the D2H copy of group g-1's
+// scan bytes (d2h stream) run under the kernels of group g: the host never drains the compute stream between
+// groups, it waits only for the event behind a group's lengths before it queues that group's D2H of finished
+// scan bytes.  A scan that does not fit is coded again on the GPU with the exact size; the host entropy coder is
+// the last resort for a faulted device stage, counted in ctx->host_fallbacks.
+static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, const FrameGeometry &g,
+                                  uint32_t quality, uint32_t restart_interval, bool optimize, uint8_t *out,
+                                  size_t out_cap_each, size_t *out_lens)
+{
     float lum[64], chr[64];
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, lum, chr);
     const CoefLayout L(g);
     const size_t cs = L.stride();
-    const size_t in_stride = align_up(len_each, 256);
-    const uint64_t scan_cap = default_scan_cap(ctx, len_each);
-    const size_t ent_one = entropy_scratch_bytes(1, g, restart_interval);
-
-    // Groups of about 96 MB of input (4 frames at 4K, 15 at 1080p), at least two per call: long enough for
-    // full-rate DMA and to amortise the launches, short enough that what no upload can hide - the last
-    // group's kernels and the read-back of its scan bytes - stays small.
-    uint32_t G = (uint32_t)std::min<size_t>(16, std::max<size_t>(1, (((size_t)96 << 20) + len_each / 2) / len_each));
-    G = std::min(G, std::max(1u, (n_images + 1) / 2));
-    const size_t budget = (size_t)4 << 30;
-    auto ent_bytes = [&](uint32_t k) {  // per-image tables run one k_huff pass per image, each with its own scratch
-        return optimize ? (size_t)k * ent_one : entropy_scratch_bytes(k, g, restart_interval);
-    };
-    auto group_bytes = [&](uint32_t k) {
-        return 2 * (size_t)k * in_stride + 2 * (size_t)k * L.each + ent_bytes(k) + 2 * (size_t)k * scan_cap;
-    };
-    while (G > 1 && group_bytes(G) > budget) --G;
-    const uint32_t ngroups = (n_images + G - 1) / G;
-
-    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ctx->d_in.ensure(ctx, 2 * (size_t)G * in_stride));
+    const uint32_t G = grp.G;
+    const uint64_t scan_cap = default_scan_cap(ctx, grp.len_each);
     PIXO_TRY(ctx->d_coef.ensure(ctx, 2 * (size_t)G * L.each));
-    PIXO_TRY(ctx->d_ent.ensure(ctx, ent_bytes(G)));
+    PIXO_TRY(ctx->d_ent.ensure(ctx, group_ent_bytes(G, g, restart_interval, optimize)));
     PIXO_TRY(ctx->d_out.ensure(ctx, 2 * (size_t)G * scan_cap));
     PIXO_TRY(ctx->d_misc.ensure(ctx, (size_t)G * kHistWords * sizeof(uint64_t) + 256));
     const size_t meta_slot = align_up((size_t)G * 12, 256);
     PIXO_TRY(ctx->h_misc.ensure(ctx, 2 * meta_slot + (size_t)G * kHistWords * sizeof(uint64_t) + 256));
-    while (ctx->events.size() < 8) {
-        cudaEvent_t ev;
-        PIXO_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        ctx->events.push_back(ev);
-    }
-    cudaEvent_t *ev_in = &ctx->events[0];    // [2] input slot filled
-    cudaEvent_t *ev_used = &ctx->events[2];  // [2] input slot consumed by the transform kernel
-    cudaEvent_t *ev_out = &ctx->events[4];   // [2] scan bytes of the slot copied back
-    cudaEvent_t *ev_len = &ctx->events[6];   // [2] the slot's lengths / overflow flags are on the host
-    auto *d_in = reinterpret_cast<uint8_t *>(ctx->d_in.ptr);
     auto *d_scan = reinterpret_cast<uint8_t *>(ctx->d_out.ptr);
     auto *h_meta = reinterpret_cast<uint8_t *>(ctx->h_misc.ptr);
     auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
@@ -857,126 +891,40 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
     auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
     auto coef_of = [&](int slot) { return reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * L.each; };
     std::vector<HuffTables> tables[2];
-    ProgResult prog;
     const bool out_locked = is_page_locked(out);
-    DrainOnError drain(ctx);
-
-    auto upload = [&](uint32_t gi) -> int {
-        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
-        const int slot = (int)(gi & 1);
-        if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ev_used[slot], 0));
-        for (uint32_t k = 0; k < cnt; ++k)
-            PIXO_TRY(h2d_copy(ctx, d_in + ((size_t)slot * G + k) * in_stride,
-                              pixels + (size_t)(first + k) * len_each, len_each, ctx->copy_stream));
-        PIXO_CUDA(ctx, cudaEventRecord(ev_in[slot], ctx->copy_stream));
-        return 0;
-    };
-
-    // progressive: coefficients, tables and the 7 segments of every frame of group gi (waits for the device)
-    auto compute_progressive = [&](uint32_t gi) -> int {
-        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
-        const int slot = (int)(gi & 1);
-        uint8_t *c = coef_of(slot);
-        const uint8_t *px = d_in + (size_t)slot * G * in_stride;
-        int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
-        PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_in[slot], 0));
-        if (optimize || !trellis)
-            PIXO_TRY(launch_jpeg_transform(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
-                                           chr, L.y(c), cs, cb, cr, cs, 0));
-        if (optimize)
-            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                           false, nullptr, d_hist));
-        std::vector<HuffTables> &tb = tables[slot];
-        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
-        if (trellis)
-            PIXO_TRY(trellis_coefficients(ctx, px, in_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
-                                          chr, L.y(c), cs, cb, cr, cs, false));
-        PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
-        std::vector<ProgTables> pt(tb.size());
-        for (size_t k = 0; k < tb.size(); ++k) {
-            const uint8_t *vals[4] = {tb[k].vals[0], tb[k].vals[1], tb[k].vals[2], tb[k].vals[3]};
-            prog_tables(tb[k].bits, vals, &pt[k]);
-        }
-        return launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, pt.data(), optimize, false, &prog);
-    };
-
-    // progressive: SOF2 headers, then per scan its SOS and its segment (from the device), EOI
-    auto finish_progressive = [&](uint32_t gi) -> int {
-        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
-        const std::vector<HuffTables> &tb = tables[(int)(gi & 1)];
-        for (uint32_t k = 0; k < cnt; ++k) {
-            const uint32_t img = first + k;
-            uint8_t *o = out + (size_t)img * out_cap_each;
-            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
-            size_t need = pos + 2;
-            for (int s = 0; s < 7; ++s) need += 10 + (size_t)prog.len[(size_t)k * 7 + s];
-            PIXO_TRY(check_room(ctx, out_cap_each, need));
-            for (int s = 0; s < 7; ++s) {
-                pos += write_sos_progressive(o + pos, s);
-                const size_t n = (size_t)prog.len[(size_t)k * 7 + s];
-                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, prog.stage + ((size_t)k * 7 + s) * prog.stage_cap, n, ctx->stream));
-                pos += n;
-            }
-            o[pos] = 0xFF;
-            o[pos + 1] = 0xD9;
-            out_lens[img] = pos + 2;
-        }
-        return 0;
-    };
 
     // queue the kernels of group gi and the readback of its lengths
     auto compute = [&](uint32_t gi) -> int {
-        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
+        const uint32_t cnt = grp.size(gi);
         const int slot = (int)(gi & 1);
         uint8_t *c = coef_of(slot);
         const CoefExtents ec = L.extents(c);
-        PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_in[slot], 0));
-        PIXO_TRY(launch_jpeg_transform(ctx, d_in + (size_t)slot * G * in_stride, in_stride, cnt, g.width,
-                                       g.height, g.color_type, g.subsampling, lum, chr, L.y(c), cs,
-                                       g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr, cs, 0, &ec));
-        PIXO_CUDA(ctx, cudaEventRecord(ev_used[slot], ctx->stream));
+        PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[slot], 0));
+        PIXO_TRY(transform_records(ctx, grp.input(gi), grp.in_stride, cnt, g, lum, chr, L, c));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[slot], ctx->stream));
         if (optimize)
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g.ny, g.nc, g.y_per_mcu,
                                            restart_interval, false, &ec, d_hist));
         std::vector<HuffTables> &tb = tables[slot];
         PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
-        uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
-        if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_out[slot], 0));  // slot's previous D2H drained
-        uint64_t *d_len = nullptr;
-        uint32_t *d_ovf = nullptr;
-        auto *ent = reinterpret_cast<uint8_t *>(ctx->d_ent.ptr);
-        uint64_t *h_len = h_len_of(slot);
-        uint32_t *h_ovf = h_ovf_of(slot);
-        if (!optimize) {
-            PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g, tb[0], restart_interval, true,
-                                         &ec, ent, scan, scan_cap, &d_len, &d_ovf));
-            PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, d_len, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        } else {
-            for (uint32_t k = 0; k < cnt; ++k) {  // per-image tables: one pass per image, each in its own scratch
-                uint8_t *f = c + (size_t)k * L.each;
-                const CoefExtents ef = L.extents(f);
-                PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, 1, g, tb[k], restart_interval, true,
-                                             &ef, ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len,
-                                             &d_ovf));
-                PIXO_CUDA(ctx, cudaMemcpyAsync(h_len + k, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
-                PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf + k, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
-            }
-        }
-        PIXO_CUDA(ctx, cudaEventRecord(ev_len[slot], ctx->stream));
+        if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out[slot], 0));  // slot's previous D2H drained
+        PIXO_TRY(code_records(ctx, L, c, cnt, g, tb.data(), optimize, restart_interval,
+                              reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan + (size_t)slot * G * scan_cap, scan_cap,
+                              h_len_of(slot), h_ovf_of(slot), cudaMemcpyDeviceToHost));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_len[slot], ctx->stream));
         return 0;
     };
 
     // headers on the host, scan bytes straight from the device (d2h stream), EOI
     auto finish = [&](uint32_t gi) -> int {
-        const uint32_t first = gi * G, cnt = std::min(G, n_images - first);
+        const uint32_t first = gi * G, cnt = grp.size(gi);
         const int slot = (int)(gi & 1);
         uint8_t *c = coef_of(slot);
         const std::vector<HuffTables> &tb = tables[slot];
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
         const uint64_t *h_len = h_len_of(slot);
         const uint32_t *h_ovf = h_ovf_of(slot);
-        PIXO_CUDA(ctx, cudaEventSynchronize(ev_len[slot]));
+        PIXO_CUDA(ctx, cudaEventSynchronize(ctx->ev_len[slot]));
         std::vector<size_t> hdr(cnt);
         bool redo = false;
         for (uint32_t k = 0; k < cnt; ++k) {
@@ -992,7 +940,7 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
             else   // ordinary caller memory: through the pinned ring, copied out by the host pool
                 PIXO_TRY(d2h_copy_sync(ctx, o + hdr[k], scan + (size_t)k * scan_cap, body, ctx->d2h_stream));
         }
-        PIXO_CUDA(ctx, cudaEventRecord(ev_out[slot], ctx->d2h_stream));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_out[slot], ctx->d2h_stream));
         if (!redo) return 0;
         // Frames the first pass did not finish.  Their coefficients are still in this slot of
         // d_coef (the next group's transform writes the other one).
@@ -1035,22 +983,117 @@ static int encode_frames(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_e
         return 0;
     };
 
-    // the copy streams start after whatever the caller already queued on the main stream
-    PIXO_CUDA(ctx, cudaEventRecord(ev_out[0], ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ev_out[0], 0));
-    PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->d2h_stream, ev_out[0], 0));
-    PIXO_TRY(upload(0));
-    for (uint32_t gi = 0; gi < ngroups; ++gi) {
-        if (gi + 1 < ngroups) PIXO_TRY(upload(gi + 1));
-        if (progressive) {
-            PIXO_TRY(compute_progressive(gi));
-            PIXO_TRY(finish_progressive(gi));
-            continue;
-        }
+    PIXO_TRY(grp.upload(0));
+    for (uint32_t gi = 0; gi < grp.count(); ++gi) {
+        if (gi + 1 < grp.count()) PIXO_TRY(grp.upload(gi + 1));
         PIXO_TRY(compute(gi));
         if (gi > 0) PIXO_TRY(finish(gi - 1));
     }
-    if (!progressive) PIXO_TRY(finish(ngroups - 1));
+    return finish(grp.count() - 1);
+}
+
+// Progressive frames (encode_progressive, src/jpeg/mod.rs:872-927): the transform writes dense natural-order
+// arrays (K3 reads them for the optimised tables, which pixo builds from the plain-rounded coefficients,
+// restart interval included), COEF_TRELLIS then overwrites them with trellis, the progressive stage codes the 7
+// scans, and the host writes SOF2 and each scan's SOS and segment.  The stage's buffers are the context's, so
+// a group is finished before the next is computed: one coefficient slot and one set of tables serve them all.
+static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, const FrameGeometry &g,
+                                     uint32_t quality, uint32_t restart_interval, bool optimize, bool trellis,
+                                     uint8_t *out, size_t out_cap_each, size_t *out_lens)
+{
+    float lum[64], chr[64];
+    uint8_t lum_zz[64], chr_zz[64];
+    quant_tables((int)quality, lum_zz, chr_zz, lum, chr);
+    const CoefLayout L(g);
+    const size_t cs = L.stride(), hist_bytes = (size_t)grp.G * kHistWords * sizeof(uint64_t) + 256;
+    PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)grp.G * L.each));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, hist_bytes));
+    auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
+    int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
+    auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
+    auto *h_hist = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
+    std::vector<HuffTables> tb;
+    ProgResult prog;
+    PIXO_TRY(grp.upload(0));
+    for (uint32_t gi = 0; gi < grp.count(); ++gi) {
+        if (gi + 1 < grp.count()) PIXO_TRY(grp.upload(gi + 1));
+        // coefficients, tables and the 7 segments of every frame of the group (waits for the device)
+        const uint32_t cnt = grp.size(gi);
+        const uint8_t *px = grp.input(gi);
+        PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi & 1], 0));
+        if (optimize || !trellis)
+            PIXO_TRY(launch_jpeg_transform(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
+                                           lum, chr, L.y(c), cs, cb, cr, cs, 0));
+        if (optimize)
+            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
+                                           false, nullptr, d_hist));
+        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
+        if (trellis)
+            PIXO_TRY(trellis_coefficients(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
+                                          lum, chr, L.y(c), cs, cb, cr, cs, false));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[gi & 1], ctx->stream));
+        std::vector<ProgTables> pt(tb.size());
+        for (size_t k = 0; k < tb.size(); ++k) {
+            const uint8_t *vals[4] = {tb[k].vals[0], tb[k].vals[1], tb[k].vals[2], tb[k].vals[3]};
+            prog_tables(tb[k].bits, vals, &pt[k]);
+        }
+        PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, pt.data(), optimize, false, &prog));
+        // SOF2 headers, then per scan its SOS and its segment (from the device), EOI
+        for (uint32_t k = 0; k < cnt; ++k) {
+            const uint32_t img = gi * grp.G + k;
+            uint8_t *o = out + (size_t)img * out_cap_each;
+            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
+            size_t need = pos + 2;
+            for (int s = 0; s < 7; ++s) need += 10 + (size_t)prog.len[(size_t)k * 7 + s];
+            PIXO_TRY(check_room(ctx, out_cap_each, need));
+            for (int s = 0; s < 7; ++s) {
+                pos += write_sos_progressive(o + pos, s);
+                const size_t n = (size_t)prog.len[(size_t)k * 7 + s];
+                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, prog.stage + ((size_t)k * 7 + s) * prog.stage_cap, n, ctx->stream));
+                pos += n;
+            }
+            o[pos] = 0xFF;
+            o[pos + 1] = 0xD9;
+            out_lens[img] = pos + 2;
+        }
+    }
+    return 0;
+}
+
+// The scans a host encode call writes; Refused: pixo_b200_jpeg_encode with progressive = 1
+enum class Scans { Baseline, Progressive, Refused };
+
+// The four host encode entry points: their checks, in this order, then the frames in groups through the
+// baseline or the progressive loop, which leave work queued; an error return drains every stream first.
+static int encode_host(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_each, uint32_t n_images, uint32_t width,
+                       uint32_t height, uint32_t color_type, uint32_t quality, uint32_t subsampling,
+                       uint32_t restart_interval, bool optimize, Scans scans, bool trellis, uint8_t *out,
+                       size_t out_cap_each, size_t *out_lens)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
+    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
+    const size_t expected = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
+    if (len_each != expected)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         expected, len_each);
+    if (!pixels || !out || !out_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (scans == Scans::Refused)
+        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED,
+                         "progressive JPEGs are encoded by pixo_b200_jpeg_encode_progressive");
+    if (n_images == 0) return 0;
+    if (out_cap_each < 1024 + 2)  // before any GPU work is queued
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap_each);
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    const EncodeGroups grp = make_groups(ctx, pixels, n_images, len_each, g, restart_interval, optimize);
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ctx->d_in.ensure(ctx, 2 * (size_t)grp.G * grp.in_stride));
+    DrainOnError drain(ctx);
+    PIXO_TRY(scans == Scans::Progressive
+                 ? encode_progressive_groups(ctx, grp, g, quality, restart_interval, optimize, trellis, out, out_cap_each,
+                                             out_lens)
+                 : encode_baseline_groups(ctx, grp, g, quality, restart_interval, optimize, out, out_cap_each, out_lens));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     drain.armed = false;
@@ -1063,16 +1106,9 @@ int pixo_b200_jpeg_encode(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixe
                           uint32_t optimize_huffman, uint32_t progressive, uint32_t trellis_quant,
                           uint8_t *out, size_t out_cap, size_t *out_len)
 {
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len, width, height, color_type, quality, subsampling, restart_interval));
-    if (!pixels || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    if (progressive)
-        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED,
-                         "progressive JPEGs are encoded by pixo_b200_jpeg_encode_progressive");
     (void)trellis_quant;  // baseline encode_scan ignores use_trellis (src/jpeg/mod.rs:1408-1563)
-    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    return encode_frames(ctx, pixels, pixels_len, 1, g, quality, restart_interval, optimize_huffman != 0, out,
-                         out_cap, out_len);
+    return encode_host(ctx, pixels, pixels_len, 1, width, height, color_type, quality, subsampling, restart_interval,
+                       optimize_huffman, progressive ? Scans::Refused : Scans::Baseline, false, out, out_cap, out_len);
 }
 
 int pixo_b200_jpeg_encode_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len_each,
@@ -1081,14 +1117,8 @@ int pixo_b200_jpeg_encode_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_
                                 uint32_t restart_interval, uint32_t optimize_huffman,
                                 uint8_t *out, size_t out_cap_each, size_t *out_lens)
 {
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len_each, width, height, color_type, quality, subsampling,
-                             restart_interval));
-    if (!pixels || !out || !out_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    if (n_images == 0) return 0;
-    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    return encode_frames(ctx, pixels, pixels_len_each, n_images, g, quality, restart_interval,
-                         optimize_huffman != 0, out, out_cap_each, out_lens);
+    return encode_host(ctx, pixels, pixels_len_each, n_images, width, height, color_type, quality, subsampling,
+                       restart_interval, optimize_huffman, Scans::Baseline, false, out, out_cap_each, out_lens);
 }
 
 int pixo_b200_jpeg_encode_progressive(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len,
@@ -1096,12 +1126,8 @@ int pixo_b200_jpeg_encode_progressive(pixo_b200_ctx *ctx, const uint8_t *pixels,
                                       uint32_t subsampling, uint32_t restart_interval, uint32_t optimize_huffman,
                                       uint32_t trellis_quant, uint8_t *out, size_t out_cap, size_t *out_len)
 {
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len, width, height, color_type, quality, subsampling, restart_interval));
-    if (!pixels || !out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    return encode_frames(ctx, pixels, pixels_len, 1, g, quality, restart_interval, optimize_huffman != 0, out,
-                         out_cap, out_len, true, trellis_quant != 0);
+    return encode_host(ctx, pixels, pixels_len, 1, width, height, color_type, quality, subsampling, restart_interval,
+                       optimize_huffman, Scans::Progressive, trellis_quant, out, out_cap, out_len);
 }
 
 int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t pixels_len_each,
@@ -1111,14 +1137,9 @@ int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *p
                                             uint32_t trellis_quant, uint8_t *out, size_t out_cap_each,
                                             size_t *out_lens)
 {
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_encode(ctx, pixels_len_each, width, height, color_type, quality, subsampling,
-                             restart_interval));
-    if (!pixels || !out || !out_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    if (n_images == 0) return 0;
-    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    return encode_frames(ctx, pixels, pixels_len_each, n_images, g, quality, restart_interval,
-                         optimize_huffman != 0, out, out_cap_each, out_lens, true, trellis_quant != 0);
+    return encode_host(ctx, pixels, pixels_len_each, n_images, width, height, color_type, quality, subsampling,
+                       restart_interval, optimize_huffman, Scans::Progressive, trellis_quant, out, out_cap_each,
+                       out_lens);
 }
 
 // Caller coefficient arrays on the device: the statistics, Huffman and progressive kernels load each
@@ -1215,21 +1236,12 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)n_images * L.each));
     PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(n_images, g, 0)));
-    void *c = ctx->d_coef.ptr;
-    const CoefExtents ec = L.extents(c);
-    PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
-                                   lum, chr, L.y(c), L.stride(), g.has_chroma ? L.cb(c) : nullptr,
-                                   g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0, &ec));
+    auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
+    PIXO_TRY(transform_records(ctx, d_pixels, pixel_stride, n_images, g, lum, chr, L, c));
     HuffTables t;
     huff_standard(t);
-    uint64_t *len_src = nullptr;
-    uint32_t *ovf_src = nullptr;
-    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), L.stride(), L.cb(c), L.cr(c), L.stride(), n_images, g, t, 0, true, &ec,
-                                 reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan, scan_cap_each,
-                                 &len_src, &ovf_src));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(d_scan_len, len_src, (size_t)n_images * 8, cudaMemcpyDeviceToDevice, ctx->stream));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(d_overflow, ovf_src, (size_t)n_images * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-    return 0;
+    return code_records(ctx, L, c, n_images, g, &t, false, 0, reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan,
+                        scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice);
 }
 
 // Host coefficient arrays: baseline Huffman tables code DC differences of category <= 11 and AC values

@@ -156,7 +156,7 @@ struct pixo_b200_ctx {
     int sm_count = 0;
     int host_threads = 0;
     uint64_t launches = 0;
-    uint64_t host_fallbacks = 0;   // frames finished by the host entropy coder (see encode_frames)
+    uint64_t host_fallbacks = 0;   // frames finished by the host entropy coder (see encode_baseline_groups)
     size_t scan_cap_override = 0;  // device scan bytes per frame; 0 = the built-in heuristic
     bool gpu_retry = true;         // re-run k_huff with the exact size when the heuristic was too small
     std::string err;
@@ -172,7 +172,8 @@ struct pixo_b200_ctx {
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn
-    std::vector<cudaEvent_t> events;
+    // host encode, per input slot: pixels uploaded, read by the transform, scan bytes copied back, lengths on host
+    cudaEvent_t ev_in[2] = {}, ev_used[2] = {}, ev_out[2] = {}, ev_len[2] = {};
     std::vector<cudaEvent_t> stage_events;  // one per pinned staging slot of h2d_copy
     cudaEvent_t switch_event = nullptr;     // pixo_b200_ctx_set_stream: the new stream waits for the old one
     cudaEvent_t resize_events[2] = {};      // the last copy out of h_resize[i] has run

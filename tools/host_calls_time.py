@@ -1,6 +1,7 @@
-"""Times the six host-buffer entry points on one 4K frame in ordinary (pageable) numpy buffers, as a pixo
-caller hands them over: each call stages the frame to the device, runs its kernels and copies the results
-back, so a call's wall time is what the caller waits for.
+"""Times the host-buffer entry points on 4K frames in ordinary (pageable) numpy buffers, as a pixo caller hands
+them over: each call stages its frames to the device, runs its kernels and copies the results back, so a call's
+wall time is what the caller waits for.  One frame per call, except the JPEG batch calls: 8 baseline frames
+(two groups of 4) and 4 progressive frames (two groups of 2).
 
     python tools/host_calls_time.py [--reps N]                      (the library PIXO_B200_SO selects)
     python tools/host_calls_time.py --ab A.so B.so [--rounds R] [--out out.json]
@@ -8,7 +9,7 @@ back, so a call's wall time is what the caller waits for.
 --ab runs the two libraries in alternating fresh processes, R rounds each, and reports per call the median
 of each round (milliseconds), the median over the rounds, B / A, and whether both computed the same bytes.
 The card's name, power limit and maximum SM clock are read in the same run.  profiles/h100_host_calls.json
-holds such a comparison.
+and profiles/h100_host_encode_calls.json hold such comparisons.
 """
 import argparse
 import json
@@ -53,6 +54,9 @@ def calls(ctx):
     from pixo_b200.jpeg import Subsampling
     from pixo_b200.png import FilterStrategy, PngOptions, QuantizationMode
     rgb, rgba, indexed = frame(3, 1), frame(4, 2), few_colours(4000, 3)
+    batch = np.stack([rgb] + [frame(3, 10 + k) for k in range(7)])
+    q80 = jpeg.JpegOptions(W, H, ColorType.Rgb, 80, Subsampling.S420)
+    pmax = jpeg.JpegOptions.max(W, H, 80)
     quant = PngOptions(W, H, ColorType.Rgba, FilterStrategy.Adaptive, True, True, True, QuantizationMode.Force, 256, True)
     lanczos = rs.ResizeOptions.builder(W, H).dst(1920, 1080).color_type(ColorType.Rgba).algorithm(
         rs.ResizeAlgorithm.Lanczos3).build()
@@ -68,6 +72,11 @@ def calls(ctx):
         "png_quantize_filter_256_dither": lambda: png.quantize_and_filter(indexed, quant, ctx=ctx)[1].tobytes(),
         "adler32": lambda: png.adler32(rgba, ctx=ctx).to_bytes(4, "little"),
         "resize_lanczos3_to_1080p": lambda: rs.resize(rgba, lanczos, ctx=ctx).tobytes(),
+        "jpeg_encode_420_q80": lambda: jpeg.encode(rgb, q80, ctx=ctx),
+        "jpeg_encode_batch_8x_420_q80": lambda: b"".join(jpeg.encode_batch(batch, q80, ctx=ctx)),
+        "jpeg_encode_progressive_max_q80": lambda: jpeg.encode_progressive(rgb, pmax, ctx=ctx),
+        "jpeg_encode_progressive_batch_4x_max_q80": lambda: b"".join(
+            jpeg.encode_progressive_batch(batch[:4], pmax, ctx=ctx)),
     }
 
 
@@ -113,7 +122,7 @@ def main():
         for key, so in zip("AB", args.ab):
             runs[key].append(run_child(so, args.reps))
     rec = {"card (name, power limit, max SM clock)": gpu_info(), "A": args.ab[0], "B": args.ab[1],
-           "note": f"ms per call on one {W}x{H} frame in pageable numpy memory: median of {args.reps} calls after "
+           "note": f"ms per call on {W}x{H} frames in pageable numpy memory: median of {args.reps} calls after "
                    f"two warm-up calls, per round; {args.rounds} rounds per library, alternating A and B",
            "calls": {}}
     for name in runs["A"][0]:
