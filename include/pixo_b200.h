@@ -14,7 +14,7 @@
  *    context's stream: after the work queued on it before the call, before the work queued after.
  *    These return with their work still queued (a call that grows the context's scratch first
  *    waits for the stream once, to free the smaller buffer):
- *      jpeg_coefficients_dev (without PIXO_B200_COEF_TRELLIS), jpeg_encode_dev, png_filter_dev,
+ *      jpeg_coefficients_dev (without PIXO_B200_COEF_TRELLIS), jpeg_encode_dev, jpeg_encode_dev_opts, png_filter_dev,
  *      png_filter_rows_dev, adler32_dev, resize_dev, jpeg_band_histogram_dev,
  *      jpeg_band_entropy_dev_async, jpeg_band_splice_dev_async.
  *    (resize_dev with Lanczos3 stages its weight tables in one of the context's two pinned buffers,
@@ -249,13 +249,30 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
  * count in d_scan_len[i] (the size needed, also when it did not fit); d_overflow[i] != 0 when the
  * frame was not finished: bit 0 scan_cap_each was too small, bit 1 a device fault (spin limit), bit 2 a
  * segment of a frame that is coded in segments (few large frames) outgrew its internal buffer - does
- * not happen for JPEGs smaller than their raw pixels; pixo_b200_jpeg_encode* handle all three.  Baseline, standard Huffman tables, no restart interval.
+ * not happen for JPEGs smaller than their raw pixels; pixo_b200_jpeg_encode* handle all three.  Baseline, standard Huffman tables, no restart interval:
+ * the same as pixo_b200_jpeg_encode_dev_opts(.., 0, 0, .., NULL), which also takes a restart interval and
+ * optimised tables (pixo's balanced preset).
  * Headers/EOI are the caller's (pixo_b200_jpeg_encode* add them). */
 int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
                               uint32_t n_images, uint32_t width, uint32_t height,
                               uint32_t color_type, uint32_t quality, uint32_t subsampling,
                               uint8_t *d_scan, size_t scan_cap_each, uint64_t *d_scan_len,
                               uint32_t *d_overflow);
+
+/* pixo_b200_jpeg_encode_dev with pixo's remaining baseline options: restart_interval (0 = None; RSTn
+ * markers in the scan, src/jpeg/mod.rs:1423-1445) and optimize_huffman (every frame gets the tables
+ * build_optimized_huffman_tables(..).unwrap_or_default() gives its own statistics, src/jpeg/mod.rs:379-392,
+ * built on the GPU).  Same arguments, checks and overflow bits as pixo_b200_jpeg_encode_dev, and queued on the
+ * context's stream like it: the statistics, the tables and the scans never wait for the host.
+ * d_dht (device, may be NULL): n_images x 1088 bytes, frame i's tables at d_dht + i*1088 as 4 x (16 counts +
+ * 256 values, unused values 0) in the order dc_lum, dc_chrom, ac_lum, ac_chrom - the layout
+ * pixo_b200_jpeg_progressive_scans_dev takes - standard ones unless optimize_huffman.  A file is
+ * pixo_b200_jpeg_write_headers_dht(frame i's tables), the scan bytes, then EOI (0xFF 0xD9). */
+int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                                   uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                   uint32_t quality, uint32_t subsampling, uint32_t restart_interval,
+                                   uint32_t optimize_huffman, uint8_t *d_scan, size_t scan_cap_each,
+                                   uint64_t *d_scan_len, uint32_t *d_overflow, uint8_t *d_dht);
 
 /* Entropy-code caller-provided coefficient arrays (host) into a baseline JPEG: the host half of
  * pixo_b200_jpeg_encode on its own (src/jpeg/mod.rs:395-447,1408-1563 consuming arrays shaped
@@ -365,6 +382,14 @@ int pixo_b200_jpeg_band_splice(const uint8_t *raw, uint64_t nbits, uint64_t star
 int pixo_b200_jpeg_write_headers(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
                                  uint32_t subsampling, uint32_t restart_interval, const uint64_t *hist,
                                  uint8_t *out, size_t out_cap, size_t *out_len);
+/* The same headers with the Huffman tables given as DHT data (host, 1088 bytes, the layout
+ * pixo_b200_jpeg_encode_dev_opts writes to d_dht): a file's headers for exactly the tables its scan was
+ * coded with.  Tables built from hist give the bytes pixo_b200_jpeg_write_headers(.., hist, ..) gives.
+ * PIXO_B200_ERR_INVALID_ARGUMENT for a table of more than 256 values or with a code that does not fit its
+ * length; out_cap >= 1024, and >= the headers' length (at most 281 bytes + the tables' values).  Host-only. */
+int pixo_b200_jpeg_write_headers_dht(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                     uint32_t subsampling, uint32_t restart_interval, const uint8_t *dht,
+                                     uint8_t *out, size_t out_cap, size_t *out_len);
 
 /* ---- PNG -------------------------------------------------------------------------------- */
 

@@ -785,9 +785,11 @@ static int transform_records(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t
 // k_huff, segments allowed, over the coefficient records of cnt frames at c: one pass with tables tb[0], or with a
 // table per frame one pass per frame, each in its own scratch.  Frame k's scan goes to scan + k * scan_cap, its
 // length and overflow flags to len[k] and ovf[k] (host or device memory, as `kind` says).
+// d_tabs: each frame's tables on the device (launch_huff_tables), used instead of tb in a single pass.
 static int code_records(pixo_b200_ctx *ctx, const CoefLayout &L, uint8_t *c, uint32_t cnt, const FrameGeometry &g,
                         const HuffTables *tb, bool per_frame, uint32_t restart_interval, uint8_t *ent, uint8_t *scan,
-                        uint64_t scan_cap, uint64_t *len, uint32_t *ovf, cudaMemcpyKind kind)
+                        uint64_t scan_cap, uint64_t *len, uint32_t *ovf, cudaMemcpyKind kind,
+                        const void *d_tabs = nullptr)
 {
     const size_t cs = L.stride(), ent_one = per_frame ? entropy_scratch_bytes(1, g, restart_interval) : 0;
     const uint32_t passes = per_frame ? cnt : 1, each = per_frame ? 1 : cnt;   // frames per pass
@@ -797,7 +799,8 @@ static int code_records(pixo_b200_ctx *ctx, const CoefLayout &L, uint8_t *c, uin
         uint64_t *d_len = nullptr;
         uint32_t *d_ovf = nullptr;
         PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, each, g, tb[k], restart_interval, true, &ef,
-                                     ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len, &d_ovf));
+                                     ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len, &d_ovf,
+                                     d_tabs));
         PIXO_CUDA(ctx, cudaMemcpyAsync(len + k, d_len, (size_t)each * 8, kind, ctx->stream));
         PIXO_CUDA(ctx, cudaMemcpyAsync(ovf + k, d_ovf, (size_t)each * 4, kind, ctx->stream));
     }
@@ -1214,14 +1217,14 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
     return 0;
 }
 
-int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
-                              uint32_t n_images, uint32_t width, uint32_t height,
-                              uint32_t color_type, uint32_t quality, uint32_t subsampling,
-                              uint8_t *d_scan, size_t scan_cap_each, uint64_t *d_scan_len,
-                              uint32_t *d_overflow)
+int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                                   uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                   uint32_t quality, uint32_t subsampling, uint32_t restart_interval,
+                                   uint32_t optimize_huffman, uint8_t *d_scan, size_t scan_cap_each,
+                                   uint64_t *d_scan_len, uint32_t *d_overflow, uint8_t *d_dht)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    PIXO_TRY(validate_options(ctx, quality, 0));
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
     PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
     if (!d_pixels || !d_scan || !d_scan_len || !d_overflow)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
@@ -1233,15 +1236,41 @@ int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_
     float lum[64], chr[64];
     quant_tables((int)quality, nullptr, nullptr, lum, chr);
     const CoefLayout L(g);
+    const bool optimize = optimize_huffman != 0;
+    // optimize: every frame's statistics, then its tables in k_huff's form, in d_misc
+    const size_t hist_bytes = align_up((size_t)n_images * kHistWords * sizeof(uint64_t), 256);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)n_images * L.each));
-    PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(n_images, g, 0)));
+    PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(n_images, g, restart_interval)));
+    if (optimize) PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + (size_t)n_images * kHuffDevBytes));
     auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
     PIXO_TRY(transform_records(ctx, d_pixels, pixel_stride, n_images, g, lum, chr, L, c));
     HuffTables t;
     huff_standard(t);
-    return code_records(ctx, L, c, n_images, g, &t, false, 0, reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan,
-                        scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice);
+    void *d_tabs = nullptr;
+    if (optimize) {
+        auto *d_hist = static_cast<uint64_t *>(ctx->d_misc.ptr);
+        d_tabs = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
+        const CoefExtents ec = L.extents(c);
+        const size_t cs = L.stride();
+        PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr,
+                                       cs, n_images, g.ny, g.nc, g.y_per_mcu, restart_interval, false, &ec, d_hist));
+        PIXO_TRY(launch_huff_tables(ctx, d_hist, n_images, g.has_chroma, d_dht, d_tabs));
+    } else if (d_dht) {
+        PIXO_TRY(launch_huff_tables(ctx, nullptr, n_images, g.has_chroma, d_dht, nullptr));
+    }
+    return code_records(ctx, L, c, n_images, g, &t, false, restart_interval, reinterpret_cast<uint8_t *>(ctx->d_ent.ptr),
+                        d_scan, scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice, d_tabs);
+}
+
+int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                              uint32_t n_images, uint32_t width, uint32_t height,
+                              uint32_t color_type, uint32_t quality, uint32_t subsampling,
+                              uint8_t *d_scan, size_t scan_cap_each, uint64_t *d_scan_len,
+                              uint32_t *d_overflow)
+{
+    return pixo_b200_jpeg_encode_dev_opts(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, quality,
+                                          subsampling, 0, 0, d_scan, scan_cap_each, d_scan_len, d_overflow, nullptr);
 }
 
 // Host coefficient arrays: baseline Huffman tables code DC differences of category <= 11 and AC values
@@ -1518,6 +1547,38 @@ int pixo_b200_jpeg_write_headers(uint32_t width, uint32_t height, uint32_t color
     HuffTables t;
     tables_from(hist, g.has_chroma, t);
     *out_len = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
+    return 0;
+}
+
+int pixo_b200_jpeg_write_headers_dht(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                     uint32_t subsampling, uint32_t restart_interval, const uint8_t *dht,
+                                     uint8_t *out, size_t out_cap, size_t *out_len)
+{
+    PIXO_TRY(validate_options(nullptr, quality, restart_interval));
+    PIXO_TRY(validate_jpeg(nullptr, width, height, color_type, subsampling));
+    if (!dht || !out || !out_len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    uint8_t bits[4][16];
+    const uint8_t *vals[4];
+    for (int k = 0; k < 4; ++k) {
+        memcpy(bits[k], dht + k * 272, 16);
+        vals[k] = dht + k * 272 + 16;
+    }
+    ProgTables check;
+    if (!prog_tables(bits, vals, &check))
+        return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "Huffman table: more than 256 values, or a code that does not fit its length");
+    if (out_cap < 1024) return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    uint8_t lum_zz[64], chr_zz[64];
+    quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
+    HuffTables t;
+    huff_from_dht(dht, t);
+    uint8_t hdr[2048];   // 281 bytes + the tables' values (at most 4 x 256)
+    const size_t n = write_headers(hdr, g, lum_zz, chr_zz, t, restart_interval);
+    if (n > out_cap)
+        return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)", out_cap, n);
+    memcpy(out, hdr, n);
+    *out_len = n;
     return 0;
 }
 

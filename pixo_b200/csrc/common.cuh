@@ -21,6 +21,10 @@
 namespace pixo {
 
 constexpr int kHistWords = 536;  // dc_lum[12] dc_chrom[12] ac_lum[256] ac_chrom[256]
+// A frame's four Huffman tables (dc_lum, dc_chrom, ac_lum, ac_chrom) as DHT data, 16 counts + 256 values each,
+// and in the form k_huff reads them (HuffDev, jpeg_entropy.cu)
+constexpr size_t kDhtBytes = 4 * 272;
+constexpr size_t kHuffDevBytes = 1632;
 
 // natural index of zig-zag position i (src/jpeg/quantize.rs:18-22); with a compile-time i the
 // kernels' reorders are static register renaming
@@ -284,12 +288,18 @@ struct FrameGeometry;
 struct HuffTables;
 size_t entropy_scratch_bytes(uint32_t n, const FrameGeometry &g, uint32_t restart_interval);
 // ext: the arrays are the transform's coefficient records; null: the caller's dense natural-order
-// arrays, whose coefficients are checked against the baseline range
+// arrays, whose coefficients are checked against the baseline range.  d_tabs: n frames' own tables as
+// launch_huff_tables writes them (t is then unused); null: t for every frame.
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
                         const HuffTables &t, uint32_t restart_interval, bool allow_segments,
                         const CoefExtents *ext, uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap,
-                        uint64_t **d_out_len, uint32_t **d_overflow);
+                        uint64_t **d_out_len, uint32_t **d_overflow, const void *d_tabs = nullptr);
+// k_huff_tables (jpeg_entropy.cu): the Huffman tables of n frames from their statistics (kHistWords each;
+// d_hist null: the standard tables), as pixo_b200_jpeg_write_headers builds them from a histogram, to d_dht
+// (kDhtBytes each) and d_tabs (kHuffDevBytes each, launch_jpeg_entropy's d_tabs); either may be null
+int launch_huff_tables(pixo_b200_ctx *ctx, const uint64_t *d_hist, uint32_t n, bool has_chroma, uint8_t *d_dht,
+                       void *d_tabs);
 int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                         const FrameGeometry &g, const HuffTables &t, const int dc_seed[3], const int *d_dc_seed,
                         bool allow_segments, uint8_t *d_raw, uint64_t raw_cap, uint64_t *d_bits_tail,

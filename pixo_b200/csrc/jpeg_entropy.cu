@@ -33,6 +33,8 @@
 // (handle_restart, src/jpeg/mod.rs:1423-1445) run here too: every interval is a bit stream of its
 // own (units never straddle one, chain 1 restarts with it, its last unit pads and appends the
 // RSTn marker), while chain 2 - every byte written so far - runs across the whole image.
+#include <type_traits>
+
 #include "common.cuh"
 #include "jpeg_host.hpp"
 
@@ -51,6 +53,15 @@ constexpr int AC_STRIDE = 12, AC_ZRL = 190, AC_EOB = 191, AC_WORDS = 192;
 struct HuffDev {
     uint32_t dc[2][12];
     uint32_t ac[2][AC_WORDS];
+};
+static_assert(sizeof(HuffDev) == kHuffDevBytes, "common.cuh sizes the per-frame tables by kHuffDevBytes");
+// One component's half of a HuffDev (dc[k], ac[k]): what a warp of k_huff<.., TABLES> keeps of its frame's tables
+struct HuffHalf {
+    uint32_t dc[12];
+    uint32_t ac[AC_WORDS];
+};
+struct FrameTables {   // k_huff<.., TABLES>'s tables: frame i's at tabs[i]
+    const HuffDev *tabs;
 };
 
 struct EntParams {
@@ -386,18 +397,24 @@ struct UnitState {
 // bit count and its last 7 bits.  k_seg_* below splice such strings into scan bytes once their
 // bit offsets are known.
 // CHECK: see code_block; a block with a coefficient outside the baseline range sets overflow bit 3.
-template <bool RAW, bool CHECK>
+// TABLES: every frame has tables of its own, Tp.tabs[frame] (k_huff_tables; a segment's frame is q / seg_per_img).  A warp keeps the half of them that its current pass codes with (HuffHalf, 816 bytes) and
+// loads it again when the frame or the component changes: a whole HuffDev per warp would take the CTA to
+// 47.5 KB of shared memory, and five CTAs per SM would no longer fit.
+template <bool RAW, bool CHECK, bool TABLES>
 __global__ void __launch_bounds__(32 * HUFF_WARPS, HUFF_CTAS_PER_SM)
-k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
+k_huff(const __grid_constant__ EntParams P, const __grid_constant__ std::conditional_t<TABLES, FrameTables, HuffDev> Tp)
 {
-    __shared__ HuffDev T;
+    __shared__ std::conditional_t<TABLES, HuffHalf[HUFF_WARPS], HuffDev> T;
     __shared__ __align__(16) WarpMem wmem[HUFF_WARPS];
     static_assert(SBUF_B <= sizeof(((WarpMem *)0)->stage), "the stuffed bytes must fit the stage");
 
     const int lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < (int)(sizeof(HuffDev) / 4); i += blockDim.x)
-        reinterpret_cast<uint32_t *>(&T)[i] = reinterpret_cast<const uint32_t *>(&Tp)[i];
-    __syncthreads();
+    if constexpr (!TABLES) {
+        for (int i = threadIdx.x; i < (int)(sizeof(HuffDev) / 4); i += blockDim.x)
+            reinterpret_cast<uint32_t *>(&T)[i] = reinterpret_cast<const uint32_t *>(&Tp)[i];
+        __syncthreads();
+    }
+    uint32_t tab_key = ~0u;   // TABLES: frame * 2 + half of the warp's copy (uniform)
     WarpMem &M = wmem[threadIdx.x >> 5];
     uint32_t *const obuf = M.obuf;
     uint8_t *const sbuf = M.sbuf;
@@ -465,6 +482,19 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
             uint32_t L = 0, tail7 = 0;
             int nwt = 0;
             if (__any_sync(0xffffffffu, valid)) {   // (a short last unit may leave a whole pass empty)
+                if constexpr (TABLES) {   // the pass's half of its frame's tables (comp ? 1 : 0 is the same in every lane)
+                    const uint32_t half = comp ? 1u : 0u;
+                    const uint32_t key = ((RAW && P.seg_per_img > 1) ? C.img / P.seg_per_img : C.img) * 2u + half;
+                    if (key != tab_key) {
+                        const uint32_t *src = reinterpret_cast<const uint32_t *>(Tp.tabs + (key >> 1));
+                        uint32_t *dst = reinterpret_cast<uint32_t *>(&T[threadIdx.x >> 5]);
+                        __syncwarp();   // every lane is done with the previous half
+                        for (int i = lane; i < 12 + AC_WORDS; i += 32)
+                            dst[i] = __ldg(src + (i < 12 ? half * 12 + i : 24 + half * AC_WORDS + (i - 12)));
+                        __syncwarp();
+                        tab_key = key;
+                    }
+                }
                 const uint32_t m = mu0 + mm;
                 const int16_t *arr;
                 const uint8_t *earr;   // !CHECK: the array's extents (P.e is null otherwise)
@@ -542,13 +572,21 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
                 const int diff = (int)(int16_t)(dc - (from_left ? left : prev_ld));
                 if (valid) {
                     const int tbl = comp ? 1 : 0;   // the same in every lane of the pass
-                    const uint32_t sa_ac = (uint32_t)__cvta_generic_to_shared(&T.ac[tbl][0]);
+                    const uint32_t *dctab;
+                    uint32_t sa_ac;
+                    if constexpr (TABLES) {
+                        dctab = T[threadIdx.x >> 5].dc;
+                        sa_ac = (uint32_t)__cvta_generic_to_shared(&T[threadIdx.x >> 5].ac[0]);
+                    } else {
+                        dctab = T.dc[tbl];
+                        sa_ac = (uint32_t)__cvta_generic_to_shared(&T.ac[tbl][0]);
+                    }
                     const uint32_t sa_slot = (uint32_t)__cvta_generic_to_shared(slot) + 4u * lane;
                     uint32_t acc;
                     bool bad;
-                    L = code_block<false, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
+                    L = code_block<false, CHECK>(M0, M1, diff, dctab, sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
                     if (L > SLOT_W * 32u)  // long block: run again, keeping the words past the slot in local memory
-                        L = code_block<true, CHECK>(M0, M1, diff, T.dc[tbl], sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
+                        L = code_block<true, CHECK>(M0, M1, diff, dctab, sa_ac, sa_stage, sa_slot, spill[p], &acc, &bad);
                     if (CHECK && bad) atomicOr(&P.overflow[C.img], kOvfRange);
                     asm volatile("" ::: "memory");  // slot words were written through st.shared
                     const int nw = (int)(L >> 5), filled = (int)(L & 31u);
@@ -861,6 +899,156 @@ k_huff(const __grid_constant__ EntParams P, const __grid_constant__ HuffDev Tp)
         if (!have) break;
         pend = cur;
         have_pend = true;
+    }
+}
+
+// ---- a frame's Huffman tables from its statistics ---------------------------------------------------
+// huff_from_histogram (jpeg_host.cpp), that is pixo's optimized_from_counts / build_code_lengths /
+// build_bits_vals (src/jpeg/huffman.rs:167-205,288-391), on the device.  One CTA per frame; warp k builds
+// table k (dc_lum, dc_chrom, ac_lum, ac_chrom).  pixo pops a min-heap on (frequency, node index), the
+// leaves numbered in ascending symbol order and merged nodes after them.  Merged frequencies come out
+// non-decreasing with increasing indices, so merging two queues - the leaves sorted by (count, symbol) and
+// the merged nodes in the order they are made, a leaf winning a tie - pops the same nodes.  The warp ranks
+// the leaves; one lane runs the (at most 255) merges and the merged nodes' depths.  A leaf's length is its
+// depth + 1 (pixo's convention) and a table with a length above 16 fails; a single symbol gets length 1.
+// vals are in (length, symbol) order and the codes canonical (assign_codes).  A failed luma table makes
+// all four tables standard, a failed chroma table only itself; gray frames take the standard chroma tables.
+struct HuffStd {   // the standard tables (huff_standard), what a table falls back to
+    uint8_t dht[kDhtBytes];
+    HuffDev dev;
+};
+
+struct TableMem {  // one warp's table
+    unsigned long long cnt[256];   // the statistics, by symbol
+    unsigned long long sf[256];    // the leaves' counts in (count, symbol) order
+    unsigned long long mf[256];    // the merged nodes' frequencies, in the order they are made
+    uint16_t lpar[256], mpar[256], mdep[256];   // parent of a sorted leaf, of a merged node; a merged node's depth
+    uint8_t ssym[256];             // the symbol of a sorted leaf
+    uint8_t len[256];              // code length by symbol, 0: not in the table
+    uint8_t vals[256];
+    uint32_t words[12 + AC_WORDS]; // k_huff's entries (HuffHalf's layout; a DC table fills the first 12)
+    int nlen[17], start[17], first[17], seen[17];   // per length: symbols, first vals index, first code, placed
+};
+
+__global__ void __launch_bounds__(128) k_huff_tables(const unsigned long long *hist, uint32_t has_chroma,
+                                                     const __grid_constant__ HuffStd S, uint8_t *dht, HuffDev *dev)
+{
+    __shared__ TableMem tm[4];
+    __shared__ int ok[4];
+    const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t f = blockIdx.x;
+    const unsigned full = 0xffffffffu, below = (1u << lane) - 1u;
+    TableMem &t = tm[k];
+    const int nsym = k < 2 ? 12 : 256;
+    bool good = hist != nullptr && (has_chroma || k == 0 || k == 2);   // (uniform in the warp)
+    if (good) {
+        const unsigned long long *h = hist + (size_t)f * kHistWords + (k == 0 ? 0 : k == 1 ? 12 : k == 2 ? 24 : 280);
+        for (int s = lane; s < 256; s += 32) {
+            t.cnt[s] = s < nsym ? h[s] : 0ull;
+            t.len[s] = 0;
+            t.vals[s] = 0;
+        }
+        for (int i = lane; i < 12 + AC_WORDS; i += 32) t.words[i] = 0;
+        if (lane < 17) { t.nlen[lane] = 0; t.seen[lane] = 0; }
+        __syncwarp();
+        // each lane ranks symbols lane + 32 j among the leaves by (count, symbol)
+        unsigned long long c[8];
+        int r[8], m = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { c[j] = t.cnt[lane + 32 * j]; r[j] = 0; }
+        for (int s = 0; s < nsym; ++s) {
+            const unsigned long long x = t.cnt[s];
+            if (!x) continue;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) r[j] += (x < c[j] || (x == c[j] && s < lane + 32 * j)) ? 1 : 0;
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            m += __popc(__ballot_sync(full, c[j] != 0));
+            if (c[j]) { t.sf[r[j]] = c[j]; t.ssym[r[j]] = (uint8_t)(lane + 32 * j); }
+        }
+        __syncwarp();
+        if (m == 0) {
+            good = false;
+        } else if (m == 1) {
+            if (lane == 0) t.len[t.ssym[0]] = 1;
+        } else {
+            if (lane == 0) {
+                int li = 0, mi = 0;   // next leaf, next merged node to pop; merged nodes [0, j) exist
+                for (int j = 0; j < m - 1; ++j) {
+                    unsigned long long sum = 0;
+                    for (int two = 0; two < 2; ++two) {
+                        if (li < m && (mi >= j || t.sf[li] <= t.mf[mi])) { sum += t.sf[li]; t.lpar[li++] = (uint16_t)j; }
+                        else { sum += t.mf[mi]; t.mpar[mi++] = (uint16_t)j; }
+                    }
+                    t.mf[j] = sum;
+                }
+                t.mdep[m - 2] = 0;   // the root; a parent is made after its children
+                for (int j = m - 3; j >= 0; --j) t.mdep[j] = (uint16_t)(t.mdep[t.mpar[j]] + 1);
+            }
+            __syncwarp();
+            bool longer = false;
+            for (int i = lane; i < m; i += 32) {
+                const int L = t.mdep[t.lpar[i]] + 2;   // the leaf's depth + 1
+                longer |= L > 16;
+                t.len[t.ssym[i]] = (uint8_t)min(L, 255);
+            }
+            if (__any_sync(full, longer)) good = false;
+        }
+        if (good) {
+            __syncwarp();
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int s = lane + 32 * j;
+                if (s < nsym && t.len[s]) atomicAdd(&t.nlen[t.len[s]], 1);
+            }
+            __syncwarp();
+            if (lane == 0) {
+                int st = 0, code = 0;
+                t.start[0] = t.first[0] = 0;
+                for (int l = 1; l <= 16; ++l) {
+                    t.start[l] = st;
+                    t.first[l] = code;
+                    st += t.nlen[l];
+                    code = (code + t.nlen[l]) << 1;
+                }
+            }
+            __syncwarp();
+#pragma unroll 1
+            for (int j = 0; j < 8; ++j) {   // in symbol order: vals by (length, symbol)
+                const int s = lane + 32 * j;
+                const int L = s < nsym ? t.len[s] : 0;
+                const uint32_t same = __match_any_sync(full, L);
+                const int pos = t.start[L] + t.seen[L] + __popc(same & below);
+                __syncwarp();
+                if (L && (same & below) == 0) t.seen[L] += __popc(same);
+                __syncwarp();
+                if (!L) continue;
+                t.vals[pos] = (uint8_t)s;
+                const uint32_t code = (uint32_t)(t.first[L] + (pos - t.start[L])) << (32 - L);
+                if (k < 2) {
+                    t.words[s] = code | (uint32_t)(L + s);
+                } else {   // make_huff_dev's AC layout
+                    const int cat = s & 15, run = s >> 4;
+                    const int w = s == 0x00 ? AC_EOB : s == 0xF0 ? AC_ZRL : (cat >= 1 && cat <= 10) ? run * AC_STRIDE + cat - 1 : -1;
+                    if (w >= 0) t.words[12 + w] = code | (uint32_t)(L + cat);
+                }
+            }
+        }
+    }
+    if (lane == 0) ok[k] = good;
+    __syncthreads();
+    const bool own = ok[0] && ok[2] && good;
+    if (dht) {
+        uint8_t *o = dht + (size_t)f * kDhtBytes + k * 272;
+        for (int i = lane; i < 272; i += 32)
+            o[i] = own ? (i < 16 ? (uint8_t)t.nlen[i + 1] : t.vals[i - 16]) : S.dht[k * 272 + i];
+    }
+    if (dev) {
+        uint32_t *o = k < 2 ? dev[f].dc[k] : dev[f].ac[k - 2];
+        const uint32_t *std_w = k < 2 ? S.dev.dc[k] : S.dev.ac[k - 2];
+        const uint32_t *own_w = k < 2 ? t.words : t.words + 12;
+        for (int i = lane; i < (k < 2 ? 12 : AC_WORDS); i += 32) o[i] = own ? own_w[i] : std_w[i];
     }
 }
 
@@ -1328,8 +1516,8 @@ static uint64_t mcu_raw_bytes(const FrameGeometry &g) { return (uint64_t)g.y_per
 // to raw_area, each segment's bit count and tail after them (off_bits / off_tails: a band's travel with its
 // strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).  Arrays
 // without extents are the caller's: checked, see code_block.
-static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint32_t n, const FrameGeometry &g,
-                         const SegPlan &sp, uint8_t *seg_scratch, uint8_t *raw_area)
+static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, const HuffDev *tabs, uint32_t n,
+                         const FrameGeometry &g, const SegPlan &sp, uint8_t *seg_scratch, uint8_t *raw_area)
 {
     const bool check = P.e.y == nullptr;
     cudaStream_t st = ctx->stream;
@@ -1354,7 +1542,11 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, uint
     PIXO_CUDA(ctx, cudaMemsetAsync(ent, 0, sp.ent.zero_bytes, st));
     const size_t want = ((size_t)P.nimages * P.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
-    PIXO_TRY(launch(ctx, check ? k_huff<true, true> : k_huff<true, false>, grid, 32 * HUFF_WARPS, 0, P, T));
+    if (tabs)
+        PIXO_TRY(launch(ctx, check ? k_huff<true, true, true> : k_huff<true, false, true>, grid, 32 * HUFF_WARPS, 0, P,
+                        FrameTables{tabs}));
+    else
+        PIXO_TRY(launch(ctx, check ? k_huff<true, true, false> : k_huff<true, false, false>, grid, 32 * HUFF_WARPS, 0, P, T));
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_bits, P.out_len, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_tails, P.out_tail, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -1390,18 +1582,38 @@ static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, ui
     return launch(ctx, k_seg_emit, tiles, SPL_THREADS, 0, Q);
 }
 
+// k_huff_tables over n frames: their statistics (K3, kHistWords each) at d_hist, or null for the standard tables.
+// Each frame's tables go to d_dht as DHT data (kDhtBytes each) and to d_tabs as k_huff reads them (kHuffDevBytes
+// each); either may be null.
+int launch_huff_tables(pixo_b200_ctx *ctx, const uint64_t *d_hist, uint32_t n, bool has_chroma, uint8_t *d_dht,
+                       void *d_tabs)
+{
+    HuffStd S;
+    HuffTables t;
+    huff_standard(t);
+    for (int k = 0; k < 4; ++k) {
+        memcpy(S.dht + k * 272, t.bits[k], 16);
+        memcpy(S.dht + k * 272 + 16, t.vals[k], 256);
+    }
+    make_huff_dev(t, &S.dev);
+    return launch(ctx, k_huff_tables, n, 128, 0, reinterpret_cast<const unsigned long long *>(d_hist),
+                  has_chroma ? 1u : 0u, S, d_dht, static_cast<HuffDev *>(d_tabs));
+}
+
 // Enqueue the entropy stage for n whole images on ctx->stream.  d_scratch: entropy_scratch_bytes.
 // d_out: n * out_cap bytes of scan data; *d_out_len / *d_overflow point into the scratch.
 // allow_segments: few long images may be cut into segments.  ext: the arrays are the transform's
 // coefficient records; null: they are the caller's natural-order arrays, and coefficients outside the
-// baseline range are rejected (overflow bit 3, see code_block).
+// baseline range are rejected (overflow bit 3, see code_block).  d_tabs: every frame's own tables
+// (launch_huff_tables), t is then unused; null: t for every frame.
 int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                         const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
                         const HuffTables &t, uint32_t restart_interval, bool allow_segments,
                         const CoefExtents *ext, uint8_t *d_scratch, uint8_t *d_out, uint64_t out_cap,
-                        uint64_t **d_out_len, uint32_t **d_overflow)
+                        uint64_t **d_out_len, uint32_t **d_overflow, const void *d_tabs)
 {
     const bool check = ext == nullptr;
+    const auto *tabs = static_cast<const HuffDev *>(d_tabs);
     const uint64_t nblocks = g.ny + 2 * g.nc;
     const uint64_t bpm_ = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     uint64_t rst_blocks = (uint64_t)restart_interval * bpm_;
@@ -1445,7 +1657,7 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
         PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total + sp.raw_total));
         auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
         uint8_t *raw_area = seg_scratch + sp.total;
-        PIXO_TRY(code_segments(ctx, P, T, n, g, sp, seg_scratch, raw_area));
+        PIXO_TRY(code_segments(ctx, P, T, tabs, n, g, sp, seg_scratch, raw_area));
         return splice_segments(ctx, n, sp, seg_scratch, raw_area,
                                reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), 0, 0, true,
                                nullptr, d_out, out_cap, P.out_len, P.overflow);
@@ -1454,7 +1666,10 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
     PIXO_TRY(ctx->d_hwin.ensure(ctx, (size_t)grid * HUFF_WARPS * GWIN_B));
     P.win = reinterpret_cast<uint8_t *>(ctx->d_hwin.ptr);
-    return launch(ctx, check ? k_huff<false, true> : k_huff<false, false>, grid, 32 * HUFF_WARPS, 0, P, T);
+    if (tabs)
+        return launch(ctx, check ? k_huff<false, true, true> : k_huff<false, false, true>, grid, 32 * HUFF_WARPS, 0, P,
+                      FrameTables{tabs});
+    return launch(ctx, check ? k_huff<false, true, false> : k_huff<false, false, false>, grid, 32 * HUFF_WARPS, 0, P, T);
 }
 
 size_t band_raw_bytes(const FrameGeometry &g)
@@ -1498,7 +1713,7 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     HuffDev T;
     make_huff_dev(t, &T);
     ctx->bands[d_raw] = sp;
-    PIXO_TRY(code_segments(ctx, P, T, 1, g, sp, seg_scratch, d_raw));   // a band's arrays are the caller's (no extents)
+    PIXO_TRY(code_segments(ctx, P, T, nullptr, 1, g, sp, seg_scratch, d_raw));   // a band's arrays are the caller's (no extents)
     return launch(ctx, k_band_totals, 1, 32, 0, reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
                   reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
                   reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,

@@ -451,6 +451,17 @@ bool huff_from_histogram(const uint64_t hist[536], bool has_chroma, HuffTables &
     return true;
 }
 
+void huff_from_dht(const uint8_t dht[1088], HuffTables &t)
+{
+    for (int k = 0; k < 4; ++k) {
+        const uint8_t *b = dht + k * 272;
+        int n = 0;
+        for (int l = 0; l < 16; ++l) n += b[l];
+        set_spec(t, k, b, b + 16, n);
+        assign_codes(t, k, false);
+    }
+}
+
 // SOI..DRI with the frame header `sof` (0xFFC0 baseline, 0xFFC2 progressive: write_sof_marker,
 // src/jpeg/mod.rs:498-560)
 static size_t write_frame_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],

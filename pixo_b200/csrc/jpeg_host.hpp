@@ -36,6 +36,9 @@ struct HuffTables {
 void huff_standard(HuffTables &t);
 // HuffmanTables::optimized_from_counts, src/jpeg/huffman.rs:167-205.  false == None.
 bool huff_from_histogram(const uint64_t hist[536], bool has_chroma, HuffTables &t);
+// Tables from DHT data: per table 16 counts + 256 values, in the order dc_lum, dc_chrom, ac_lum, ac_chrom.
+// Each table must hold at most 256 values (prog_tables checks that).
+void huff_from_dht(const uint8_t dht[1088], HuffTables &t);
 
 // SOI..SOS (src/jpeg/mod.rs:395-430,449-648).  Returns bytes written (<= 1024).
 size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],

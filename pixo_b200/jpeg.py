@@ -313,6 +313,50 @@ def progressive_scans_dev(d_y, d_cb, d_cr, width, height, color_type=ColorType.R
     return d_out, d_scan_len, d_overflow
 
 
+DHT_BYTES = 4 * 272   # a frame's tables in pixo_b200_jpeg_encode_dev_opts' d_dht
+
+
+def encode_dev(d_frames, pixel_stride, n_images, options: JpegOptions, d_scan, scan_cap_each, d_scan_len,
+               d_overflow, d_dht=None, ctx: Context | None = None) -> None:
+    """pixo_b200_jpeg_encode_dev_opts: n_images device frames (frame i at d_frames + i * pixel_stride bytes)
+    -> frame i's scan bytes at d_scan + i * scan_cap_each, its length in d_scan_len[i], its flags in
+    d_overflow[i] and, when d_dht is given, its tables in d_dht[i] (DHT_BYTES each).  The buffers are
+    anything with .data_ptr() (torch tensors) or device addresses.  options supplies the geometry, quality,
+    restart interval and optimize_huffman; progressive raises ERR_UNSUPPORTED and trellis_quant is ignored,
+    as pixo's baseline encode_scan ignores it.  Queued on the context's stream; nothing is synchronised.
+    jpeg_file(options, dht, scan) makes a frame's file."""
+    if options.progressive:
+        raise _lib.PixoError(_lib.ERR_UNSUPPORTED, "progressive is not a device scan option: use encode_progressive")
+    restart = _restart(options)
+    ctx = ctx or default_context()
+    ptr = lambda t: None if t is None else (int(t) if isinstance(t, int) else int(t.data_ptr()))
+    rc = _lib.load().pixo_b200_jpeg_encode_dev_opts(
+        ctx.handle, ptr(d_frames), int(pixel_stride), int(n_images), int(options.width), int(options.height),
+        int(options.color_type), int(options.quality), int(options.subsampling), restart,
+        int(bool(options.optimize_huffman)), ptr(d_scan), int(scan_cap_each), ptr(d_scan_len), ptr(d_overflow),
+        ptr(d_dht))
+    _lib.check(ctx.handle, rc)
+
+
+def write_headers_dht(options: JpegOptions, dht) -> bytes:
+    """SOI .. SOS of a baseline file whose Huffman tables are `dht` (DHT_BYTES, the layout encode_dev
+    writes per frame)."""
+    d = np.ascontiguousarray(np.asarray(dht, np.uint8).reshape(-1))
+    if d.size != DHT_BYTES:
+        raise _lib.PixoError(_lib.ERR_INVALID_ARGUMENT, f"a DHT block is {DHT_BYTES} bytes, got {d.size}")
+    buf = np.zeros(2048, np.uint8)
+    n = C.c_size_t()
+    _lib.check(None, _lib.load().pixo_b200_jpeg_write_headers_dht(
+        int(options.width), int(options.height), int(options.color_type), int(options.quality),
+        int(options.subsampling), _restart(options), d.ctypes.data, buf.ctypes.data, buf.size, C.byref(n)))
+    return buf[: n.value].tobytes()
+
+
+def jpeg_file(options: JpegOptions, dht, scan) -> bytes:
+    """One frame of encode_dev as a file: headers for its tables, its scan bytes, EOI."""
+    return write_headers_dht(options, dht) + bytes(scan) + b"\xff\xd9"
+
+
 def entropy_encode(y, cb, cr, options: JpegOptions, ctx: Context | None = None) -> bytes:
     """Host entropy stage on its own (no device needed)."""
     y = np.ascontiguousarray(y, np.int16)
