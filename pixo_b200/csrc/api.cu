@@ -455,20 +455,19 @@ static void tables_from(const uint64_t *hist, bool has_chroma, HuffTables &t)
     if (!(hist && huff_from_histogram(hist, has_chroma, t))) huff_standard(t);
 }
 
-// The Huffman tables of `cnt` frames.  optimize: each frame's from its statistics (K3) in d_hist, read
-// back to h_hist (in the pinned h_misc) once the stream has drained; otherwise one set of standard tables.
-static int build_tables(pixo_b200_ctx *ctx, bool optimize, const uint64_t *d_hist, uint64_t *h_hist, uint32_t cnt,
-                        bool has_chroma, std::vector<HuffTables> &tb)
+// A frame's tables as a DHT block (kDhtBytes: per table 16 counts + 256 values, in the order dc_lum, dc_chrom,
+// ac_lum, ac_chrom) in the form the progressive stage reads; a malformed table is refused.
+static int dht_prog_tables(pixo_b200_ctx *ctx, const uint8_t *dht, ProgTables *T)
 {
-    tb.resize(optimize ? cnt : 1);
-    if (!optimize) {
-        tables_from(nullptr, has_chroma, tb[0]);
-        return 0;
+    uint8_t bits[4][16];
+    const uint8_t *vals[4];
+    for (int k = 0; k < 4; ++k) {
+        memcpy(bits[k], dht + k * 272, 16);
+        vals[k] = dht + k * 272 + 16;
     }
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_hist, d_hist, (size_t)cnt * kHistWords * sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                                   ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (uint32_t k = 0; k < cnt; ++k) tables_from(h_hist + (size_t)k * kHistWords, has_chroma, tb[k]);
+    if (!prog_tables(bits, vals, T))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
+                         "Huffman table: more than 256 values, or a code that does not fit its length");
     return 0;
 }
 
@@ -782,36 +781,22 @@ static int transform_records(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t
                                  g.has_chroma ? L.cr(c) : nullptr, L.stride(), 0, &ec);
 }
 
-// k_huff, segments allowed, over the coefficient records of cnt frames at c: one pass with tables tb[0], or with a
-// table per frame one pass per frame, each in its own scratch.  Frame k's scan goes to scan + k * scan_cap, its
-// length and overflow flags to len[k] and ovf[k] (host or device memory, as `kind` says).
-// d_tabs: each frame's tables on the device (launch_huff_tables), used instead of tb in a single pass.
+// k_huff, segments allowed, over the coefficient records of cnt frames at c, in one pass: with tables t, or with
+// each frame's own tables d_tabs (launch_huff_tables) when that is not null.  Frame k's scan goes to
+// scan + k * scan_cap, its length and overflow flags to len[k] and ovf[k] (host or device memory, as `kind` says).
 static int code_records(pixo_b200_ctx *ctx, const CoefLayout &L, uint8_t *c, uint32_t cnt, const FrameGeometry &g,
-                        const HuffTables *tb, bool per_frame, uint32_t restart_interval, uint8_t *ent, uint8_t *scan,
-                        uint64_t scan_cap, uint64_t *len, uint32_t *ovf, cudaMemcpyKind kind,
-                        const void *d_tabs = nullptr)
+                        const HuffTables &t, const void *d_tabs, uint32_t restart_interval, uint8_t *ent, uint8_t *scan,
+                        uint64_t scan_cap, uint64_t *len, uint32_t *ovf, cudaMemcpyKind kind)
 {
-    const size_t cs = L.stride(), ent_one = per_frame ? entropy_scratch_bytes(1, g, restart_interval) : 0;
-    const uint32_t passes = per_frame ? cnt : 1, each = per_frame ? 1 : cnt;   // frames per pass
-    for (uint32_t k = 0; k < passes; ++k) {
-        uint8_t *f = c + (size_t)k * L.each;
-        const CoefExtents ef = L.extents(f);
-        uint64_t *d_len = nullptr;
-        uint32_t *d_ovf = nullptr;
-        PIXO_TRY(launch_jpeg_entropy(ctx, L.y(f), cs, L.cb(f), L.cr(f), cs, each, g, tb[k], restart_interval, true, &ef,
-                                     ent + (size_t)k * ent_one, scan + (size_t)k * scan_cap, scan_cap, &d_len, &d_ovf,
-                                     d_tabs));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(len + k, d_len, (size_t)each * 8, kind, ctx->stream));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(ovf + k, d_ovf, (size_t)each * 4, kind, ctx->stream));
-    }
+    const size_t cs = L.stride();
+    const CoefExtents ec = L.extents(c);
+    uint64_t *d_len = nullptr;
+    uint32_t *d_ovf = nullptr;
+    PIXO_TRY(launch_jpeg_entropy(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g, t, restart_interval, true, &ec, ent, scan,
+                                 scan_cap, &d_len, &d_ovf, d_tabs));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(len, d_len, (size_t)cnt * 8, kind, ctx->stream));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(ovf, d_ovf, (size_t)cnt * 4, kind, ctx->stream));
     return 0;
-}
-
-// k_huff scratch of a baseline group of k frames: with per-frame tables (optimize) each frame has its own
-static size_t group_ent_bytes(uint32_t k, const FrameGeometry &g, uint32_t restart_interval, bool optimize)
-{
-    return optimize ? (size_t)k * entropy_scratch_bytes(1, g, restart_interval)
-                    : entropy_scratch_bytes(k, g, restart_interval);
 }
 
 // What the two group loops of the host encode share: n frames, G per group, each group's pixels uploaded on the
@@ -850,25 +835,26 @@ struct EncodeGroups {
 // no upload can hide - the last group's kernels and the read-back of its scan bytes - stays small.  Fewer while
 // the baseline loop's scratch for two groups would pass 4 GiB; the progressive loop groups its frames the same way.
 static EncodeGroups make_groups(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t n, size_t len_each,
-                                const FrameGeometry &g, uint32_t restart_interval, bool optimize)
+                                const FrameGeometry &g, uint32_t restart_interval)
 {
     const size_t in_stride = align_up(len_each, 256), coef_each = CoefLayout(g).each;
     const uint64_t scan_cap = default_scan_cap(ctx, len_each);
     uint32_t G = (uint32_t)std::min<size_t>(16, std::max<size_t>(1, (((size_t)96 << 20) + len_each / 2) / len_each));
     G = std::min(G, std::max(1u, (n + 1) / 2));
     auto group_bytes = [&](uint32_t k) {
-        return 2 * (size_t)k * (in_stride + coef_each + scan_cap) + group_ent_bytes(k, g, restart_interval, optimize);
+        return 2 * (size_t)k * (in_stride + coef_each + scan_cap) + entropy_scratch_bytes(k, g, restart_interval);
     };
     while (G > 1 && group_bytes(G) > ((size_t)4 << 30)) --G;
     return EncodeGroups{ctx, pixels, len_each, in_stride, n, G};
 }
 
-// Baseline frames.  GPU: colour/DCT/quantise into coefficient records (K1/K2), symbol statistics when optimize
-// (K3), k_huff; host: headers, optimised tables, EOI.  The H2D copy of group g+1 and the D2H copy of group g-1's
-// scan bytes (d2h stream) run under the kernels of group g: the host never drains the compute stream between
-// groups, it waits only for the event behind a group's lengths before it queues that group's D2H of finished
-// scan bytes.  A scan that does not fit is coded again on the GPU with the exact size; the host entropy coder is
-// the last resort for a faulted device stage, counted in ctx->host_fallbacks.
+// Baseline frames.  GPU: colour/DCT/quantise into coefficient records (K1/K2), when optimize symbol statistics
+// (K3) and each frame's tables (k_huff_tables), k_huff; host: headers, EOI.  The H2D copy of group g+1 and the D2H
+// copy of group g-1's scan bytes (d2h stream) run under the kernels of group g: the host never drains the compute
+// stream between groups, it waits only for the event behind a group's lengths and tables before it queues that
+// group's D2H of finished scan bytes.  A scan that does not fit is coded again on the GPU with the exact size; the
+// host entropy coder is the last resort for a faulted device stage, counted in ctx->host_fallbacks.  Both use the
+// frame's tables on the host: by then the next group's k_huff_tables may have overwritten the device copy.
 static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, const FrameGeometry &g,
                                   uint32_t quality, uint32_t restart_interval, bool optimize, uint8_t *out,
                                   size_t out_cap_each, size_t *out_lens)
@@ -880,23 +866,30 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
     const size_t cs = L.stride();
     const uint32_t G = grp.G;
     const uint64_t scan_cap = default_scan_cap(ctx, grp.len_each);
+    // d_misc: a group's statistics, its DHT blocks, its tables in k_huff's form
+    const size_t hist_bytes = align_up((size_t)G * kHistWords * sizeof(uint64_t), 256);
+    const size_t dht_bytes = align_up((size_t)G * kDhtBytes, 256);
     PIXO_TRY(ctx->d_coef.ensure(ctx, 2 * (size_t)G * L.each));
-    PIXO_TRY(ctx->d_ent.ensure(ctx, group_ent_bytes(G, g, restart_interval, optimize)));
+    PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(G, g, restart_interval)));
     PIXO_TRY(ctx->d_out.ensure(ctx, 2 * (size_t)G * scan_cap));
-    PIXO_TRY(ctx->d_misc.ensure(ctx, (size_t)G * kHistWords * sizeof(uint64_t) + 256));
-    const size_t meta_slot = align_up((size_t)G * 12, 256);
-    PIXO_TRY(ctx->h_misc.ensure(ctx, 2 * meta_slot + (size_t)G * kHistWords * sizeof(uint64_t) + 256));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + dht_bytes + (size_t)G * kHuffDevBytes));
+    // h_misc, per slot: a group's lengths, overflow flags and DHT blocks
+    const size_t meta_slot = align_up((size_t)G * (12 + kDhtBytes), 256);
+    PIXO_TRY(ctx->h_misc.ensure(ctx, 2 * meta_slot));
     auto *d_scan = reinterpret_cast<uint8_t *>(ctx->d_out.ptr);
     auto *h_meta = reinterpret_cast<uint8_t *>(ctx->h_misc.ptr);
     auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    auto *h_hist = reinterpret_cast<uint64_t *>(h_meta + 2 * meta_slot);
+    uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
+    void *d_tabs = optimize ? d_dht + dht_bytes : nullptr;
     auto h_len_of = [&](int slot) { return reinterpret_cast<uint64_t *>(h_meta + (size_t)slot * meta_slot); };
     auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
+    auto h_dht_of = [&](int slot) { return h_meta + (size_t)slot * meta_slot + (size_t)G * 12; };
     auto coef_of = [&](int slot) { return reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * L.each; };
-    std::vector<HuffTables> tables[2];
+    HuffTables std_t;
+    huff_from_dht(dht_standard(), std_t);
     const bool out_locked = is_page_locked(out);
 
-    // queue the kernels of group gi and the readback of its lengths
+    // queue the kernels of group gi and the readback of its lengths and tables
     auto compute = [&](uint32_t gi) -> int {
         const uint32_t cnt = grp.size(gi);
         const int slot = (int)(gi & 1);
@@ -905,15 +898,18 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
         PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[slot], 0));
         PIXO_TRY(transform_records(ctx, grp.input(gi), grp.in_stride, cnt, g, lum, chr, L, c));
         PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[slot], ctx->stream));
-        if (optimize)
+        if (optimize) {
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, L.cb(c), L.cr(c), cs, cnt, g.ny, g.nc, g.y_per_mcu,
                                            restart_interval, false, &ec, d_hist));
-        std::vector<HuffTables> &tb = tables[slot];
-        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
+            PIXO_TRY(launch_huff_tables(ctx, d_hist, cnt, g.has_chroma, d_dht, d_tabs));
+        }
         if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out[slot], 0));  // slot's previous D2H drained
-        PIXO_TRY(code_records(ctx, L, c, cnt, g, tb.data(), optimize, restart_interval,
+        PIXO_TRY(code_records(ctx, L, c, cnt, g, std_t, d_tabs, restart_interval,
                               reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan + (size_t)slot * G * scan_cap, scan_cap,
                               h_len_of(slot), h_ovf_of(slot), cudaMemcpyDeviceToHost));
+        if (optimize)
+            PIXO_CUDA(ctx, cudaMemcpyAsync(h_dht_of(slot), d_dht, (size_t)cnt * kDhtBytes, cudaMemcpyDeviceToHost,
+                                           ctx->stream));
         PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_len[slot], ctx->stream));
         return 0;
     };
@@ -923,17 +919,19 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
         const uint32_t first = gi * G, cnt = grp.size(gi);
         const int slot = (int)(gi & 1);
         uint8_t *c = coef_of(slot);
-        const std::vector<HuffTables> &tb = tables[slot];
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
         const uint64_t *h_len = h_len_of(slot);
         const uint32_t *h_ovf = h_ovf_of(slot);
         PIXO_CUDA(ctx, cudaEventSynchronize(ctx->ev_len[slot]));
+        std::vector<HuffTables> tb(optimize ? cnt : 0);   // each frame's tables, from its DHT block
+        for (uint32_t k = 0; k < tb.size(); ++k) huff_from_dht(h_dht_of(slot) + (size_t)k * kDhtBytes, tb[k]);
+        auto tables = [&](uint32_t k) -> const HuffTables & { return optimize ? tb[k] : std_t; };
         std::vector<size_t> hdr(cnt);
         bool redo = false;
         for (uint32_t k = 0; k < cnt; ++k) {
             const uint32_t img = first + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
-            hdr[k] = write_headers(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
+            hdr[k] = write_headers(o, g, lum_zz, chr_zz, tables(k), restart_interval);
             if (h_ovf[k]) { redo = true; continue; }
             const size_t body = (size_t)h_len[k];
             PIXO_TRY(finish_frame(ctx, o, out_cap_each, hdr[k], body, &out_lens[img]));
@@ -952,7 +950,7 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
             const uint32_t img = first + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
             uint8_t *f = c + (size_t)k * L.each;
-            const HuffTables &t = tb[optimize ? k : 0];
+            const HuffTables &t = tables(k);
             // bit 0: the scan did not fit (the kernel reported the size it needs); bit 2: a segment's raw
             // string did not fit its share - either way code the frame again on the GPU, unsegmented, with
             // enough room.  Bit 1 (a faulted chain) goes to the host coder.
@@ -997,9 +995,10 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
 
 // Progressive frames (encode_progressive, src/jpeg/mod.rs:872-927): the transform writes dense natural-order
 // arrays (K3 reads them for the optimised tables, which pixo builds from the plain-rounded coefficients,
-// restart interval included), COEF_TRELLIS then overwrites them with trellis, the progressive stage codes the 7
-// scans, and the host writes SOF2 and each scan's SOS and segment.  The stage's buffers are the context's, so
-// a group is finished before the next is computed: one coefficient slot and one set of tables serve them all.
+// restart interval included, and k_huff_tables builds each frame's tables from them), COEF_TRELLIS then overwrites
+// them with trellis, the progressive stage codes the 7 scans, and the host writes SOF2 and each scan's SOS and
+// segment.  The stage's buffers are the context's, so a group is finished before the next is computed: one
+// coefficient slot and one set of DHT blocks serve them all.
 static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, const FrameGeometry &g,
                                      uint32_t quality, uint32_t restart_interval, bool optimize, bool trellis,
                                      uint8_t *out, size_t out_cap_each, size_t *out_lens)
@@ -1008,15 +1007,18 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, lum, chr);
     const CoefLayout L(g);
-    const size_t cs = L.stride(), hist_bytes = (size_t)grp.G * kHistWords * sizeof(uint64_t) + 256;
+    const size_t cs = L.stride(), hist_bytes = align_up((size_t)grp.G * kHistWords * sizeof(uint64_t), 256);
     PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)grp.G * L.each));
-    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes));
-    PIXO_TRY(ctx->h_misc.ensure(ctx, hist_bytes));
+    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + (size_t)grp.G * kDhtBytes));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, (size_t)grp.G * kDhtBytes));
     auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
     int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
     auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    auto *h_hist = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
-    std::vector<HuffTables> tb;
+    uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
+    auto *h_dht = static_cast<const uint8_t *>(ctx->h_misc.ptr);
+    // frame k's tables: its own (optimize), or the standard ones
+    auto dht_of = [&](uint32_t k) { return optimize ? h_dht + (size_t)k * kDhtBytes : dht_standard(); };
+    HuffTables t;
     ProgResult prog;
     PIXO_TRY(grp.upload(0));
     for (uint32_t gi = 0; gi < grp.count(); ++gi) {
@@ -1028,25 +1030,28 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
         if (optimize || !trellis)
             PIXO_TRY(launch_jpeg_transform(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
                                            lum, chr, L.y(c), cs, cb, cr, cs, 0));
-        if (optimize)
+        if (optimize) {
             PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
                                            false, nullptr, d_hist));
-        PIXO_TRY(build_tables(ctx, optimize, d_hist, h_hist, cnt, g.has_chroma, tb));
-        if (trellis)
+            PIXO_TRY(launch_huff_tables(ctx, d_hist, cnt, g.has_chroma, d_dht, nullptr));
+            PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_misc.ptr, d_dht, (size_t)cnt * kDhtBytes, cudaMemcpyDeviceToHost,
+                                           ctx->stream));
+        }
+        if (trellis)   // waits for the device, the DHT blocks' copy included
             PIXO_TRY(trellis_coefficients(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
                                           lum, chr, L.y(c), cs, cb, cr, cs, false));
+        else if (optimize)
+            PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[gi & 1], ctx->stream));
-        std::vector<ProgTables> pt(tb.size());
-        for (size_t k = 0; k < tb.size(); ++k) {
-            const uint8_t *vals[4] = {tb[k].vals[0], tb[k].vals[1], tb[k].vals[2], tb[k].vals[3]};
-            prog_tables(tb[k].bits, vals, &pt[k]);
-        }
+        std::vector<ProgTables> pt(optimize ? cnt : 1);
+        for (uint32_t k = 0; k < pt.size(); ++k) PIXO_TRY(dht_prog_tables(ctx, dht_of(k), &pt[k]));
         PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, pt.data(), optimize, false, &prog));
         // SOF2 headers, then per scan its SOS and its segment (from the device), EOI
         for (uint32_t k = 0; k < cnt; ++k) {
             const uint32_t img = gi * grp.G + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
-            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, tb[optimize ? k : 0], restart_interval);
+            huff_from_dht(dht_of(k), t);
+            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, t, restart_interval);
             size_t need = pos + 2;
             for (int s = 0; s < 7; ++s) need += 10 + (size_t)prog.len[(size_t)k * 7 + s];
             PIXO_TRY(check_room(ctx, out_cap_each, need));
@@ -1089,7 +1094,7 @@ static int encode_host(pixo_b200_ctx *ctx, const uint8_t *pixels, size_t len_eac
     if (out_cap_each < 1024 + 2)  // before any GPU work is queued
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap_each);
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
-    const EncodeGroups grp = make_groups(ctx, pixels, n_images, len_each, g, restart_interval, optimize);
+    const EncodeGroups grp = make_groups(ctx, pixels, n_images, len_each, g, restart_interval);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_in.ensure(ctx, 2 * (size_t)grp.G * grp.in_stride));
     DrainOnError drain(ctx);
@@ -1175,26 +1180,7 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
                          "coefficient strides must hold a frame's blocks (%zu / %zu elements)", g.ny * 64, g.nc * 64);
     ProgTables T;
-    {
-        HuffTables std_t;
-        uint8_t bits[4][16];
-        const uint8_t *vals[4];
-        if (dht) {
-            for (int k = 0; k < 4; ++k) {
-                memcpy(bits[k], dht + k * 272, 16);
-                vals[k] = dht + k * 272 + 16;
-            }
-        } else {
-            huff_standard(std_t);
-            for (int k = 0; k < 4; ++k) {
-                memcpy(bits[k], std_t.bits[k], 16);
-                vals[k] = std_t.vals[k];
-            }
-        }
-        if (!prog_tables(bits, vals, &T))
-            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
-                             "Huffman table: more than 256 values, or a code that does not fit its length");
-    }
+    PIXO_TRY(dht_prog_tables(ctx, dht ? dht : dht_standard(), &T));
     if (n_frames == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     // The splice kernels take one grid row per segment: at most 8192 frames (57 344 segments) per pass.
@@ -1259,8 +1245,8 @@ int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, 
     } else if (d_dht) {
         PIXO_TRY(launch_huff_tables(ctx, nullptr, n_images, g.has_chroma, d_dht, nullptr));
     }
-    return code_records(ctx, L, c, n_images, g, &t, false, restart_interval, reinterpret_cast<uint8_t *>(ctx->d_ent.ptr),
-                        d_scan, scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice, d_tabs);
+    return code_records(ctx, L, c, n_images, g, t, d_tabs, restart_interval, reinterpret_cast<uint8_t *>(ctx->d_ent.ptr),
+                        d_scan, scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice);
 }
 
 int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
@@ -1331,16 +1317,22 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (optimize_huffman) {
-        PIXO_TRY(ctx->d_misc.ensure(ctx, kHistWords * sizeof(uint64_t) + 256));
-        PIXO_TRY(ctx->h_misc.ensure(ctx, kHistWords * sizeof(uint64_t) + 256));
+    const uint8_t *dht = dht_standard();
+    if (optimize_huffman) {   // K3, k_huff_tables, the DHT block back to the host
+        const size_t hist_bytes = align_up(kHistWords * sizeof(uint64_t), 256);
+        PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + kDhtBytes));
+        PIXO_TRY(ctx->h_misc.ensure(ctx, kDhtBytes));
+        auto *d_hist = static_cast<uint64_t *>(ctx->d_misc.ptr);
+        uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                       false, nullptr, static_cast<uint64_t *>(ctx->d_misc.ptr)));
+                                       false, nullptr, d_hist));
+        PIXO_TRY(launch_huff_tables(ctx, d_hist, 1, g.has_chroma, d_dht, nullptr));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_misc.ptr, d_dht, kDhtBytes, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        dht = static_cast<const uint8_t *>(ctx->h_misc.ptr);
     }
-    std::vector<HuffTables> tb;
-    PIXO_TRY(build_tables(ctx, optimize_huffman != 0, static_cast<uint64_t *>(ctx->d_misc.ptr),
-                          static_cast<uint64_t *>(ctx->h_misc.ptr), 1, g.has_chroma, tb));
-    const HuffTables &t = tb[0];
+    HuffTables t;
+    huff_from_dht(dht, t);
     const size_t hdr = write_headers(out, g, lum_zz, chr_zz, t, restart_interval);
     // The device scan buffer follows the size a JPEG of this geometry normally has, not the caller's
     // worst-case capacity (tens of GB for a gigapixel frame); a scan that needs more is coded again
@@ -1557,16 +1549,8 @@ int pixo_b200_jpeg_write_headers_dht(uint32_t width, uint32_t height, uint32_t c
     PIXO_TRY(validate_options(nullptr, quality, restart_interval));
     PIXO_TRY(validate_jpeg(nullptr, width, height, color_type, subsampling));
     if (!dht || !out || !out_len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    uint8_t bits[4][16];
-    const uint8_t *vals[4];
-    for (int k = 0; k < 4; ++k) {
-        memcpy(bits[k], dht + k * 272, 16);
-        vals[k] = dht + k * 272 + 16;
-    }
     ProgTables check;
-    if (!prog_tables(bits, vals, &check))
-        return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT,
-                         "Huffman table: more than 256 values, or a code that does not fit its length");
+    PIXO_TRY(dht_prog_tables(nullptr, dht, &check));
     if (out_cap < 1024) return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     uint8_t lum_zz[64], chr_zz[64];

@@ -1589,12 +1589,9 @@ int launch_huff_tables(pixo_b200_ctx *ctx, const uint64_t *d_hist, uint32_t n, b
                        void *d_tabs)
 {
     HuffStd S;
+    memcpy(S.dht, dht_standard(), kDhtBytes);
     HuffTables t;
     huff_standard(t);
-    for (int k = 0; k < 4; ++k) {
-        memcpy(S.dht + k * 272, t.bits[k], 16);
-        memcpy(S.dht + k * 272 + 16, t.vals[k], 256);
-    }
     make_huff_dev(t, &S.dev);
     return launch(ctx, k_huff_tables, n, 128, 0, reinterpret_cast<const unsigned long long *>(d_hist),
                   has_chroma ? 1u : 0u, S, d_dht, static_cast<HuffDev *>(d_tabs));

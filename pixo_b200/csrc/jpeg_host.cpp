@@ -462,6 +462,23 @@ void huff_from_dht(const uint8_t dht[1088], HuffTables &t)
     }
 }
 
+const uint8_t *dht_standard()
+{
+    static const struct Block {
+        uint8_t dht[1088];
+        Block()
+        {
+            HuffTables t;
+            huff_standard(t);
+            for (int k = 0; k < 4; ++k) {
+                memcpy(dht + k * 272, t.bits[k], 16);
+                memcpy(dht + k * 272 + 16, t.vals[k], 256);
+            }
+        }
+    } block;
+    return block.dht;
+}
+
 // SOI..DRI with the frame header `sof` (0xFFC0 baseline, 0xFFC2 progressive: write_sof_marker,
 // src/jpeg/mod.rs:498-560)
 static size_t write_frame_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],

@@ -39,6 +39,8 @@ bool huff_from_histogram(const uint64_t hist[536], bool has_chroma, HuffTables &
 // Tables from DHT data: per table 16 counts + 256 values, in the order dc_lum, dc_chrom, ac_lum, ac_chrom.
 // Each table must hold at most 256 values (prog_tables checks that).
 void huff_from_dht(const uint8_t dht[1088], HuffTables &t);
+// The standard tables (huff_standard) as DHT data
+const uint8_t *dht_standard();
 
 // SOI..SOS (src/jpeg/mod.rs:395-430,449-648).  Returns bytes written (<= 1024).
 size_t write_headers(uint8_t *out, const FrameGeometry &g, const uint8_t lum_zz[64],

@@ -48,13 +48,14 @@ def test_encode_batch_over_three_groups(po, frames, ri, opt):
 
 def test_host_fallback_over_three_groups(po, frames):
     """a scan buffer too small for every frame and no GPU retry: the host coder finishes each frame, from the
-    records of its group's slot"""
-    with pixo_b200.Context(0) as ctx:
-        ctx.set_scan_capacity(4096, gpu_retry=False)
-        got = jpeg.encode_batch(frames, JpegOptions(W, H, ColorType.Rgb, Q, Subsampling.S420), ctx=ctx)
-        assert ctx.host_fallbacks == N
-    for k in range(N):
-        assert got[k] == po.jpeg_encode(frames[k], W, H, 2, Q, 1), k
+    records of its group's slot and, with optimised tables, from the frame's tables as the device built them"""
+    for ri, opt in ((None, False), (4, True)):
+        with pixo_b200.Context(0) as ctx:
+            ctx.set_scan_capacity(4096, gpu_retry=False)
+            got = jpeg.encode_batch(frames, JpegOptions(W, H, ColorType.Rgb, Q, Subsampling.S420, ri, opt), ctx=ctx)
+            assert ctx.host_fallbacks == N, (ri, opt)
+        for k in range(N):
+            assert got[k] == po.jpeg_encode(frames[k], W, H, 2, Q, 1, ri or 0, opt), (ri, opt, k)
 
 
 def test_progressive_batch_over_three_groups(frames):

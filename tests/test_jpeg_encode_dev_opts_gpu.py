@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from golden_inputs import make_input
+from oracle import jpeg_progressive as jp
 from pixo_b200 import ColorType, Context, _lib, jpeg
 from pixo_b200.jpeg import JpegOptions, Subsampling
 from test_dev_layouts_gpu import GUARD8, GUARD32, GUARD64, assert_guard, guarded, jpeg_frames, placed, stripes
@@ -175,6 +176,21 @@ def test_every_table_branch(po, gpu_ctx, name):
     for i in range(2):
         assert np.array_equal(tabs[i], want), i
         assert files[i] == oracle_file(po, f, o), i
+    # the host entry points build their tables with the same kernel
+    assert jpeg.encode(f, o, ctx=gpu_ctx) == oracle_file(po, f, o)
+    assert jpeg.encode_batch(np.stack([f, f]), o, ctx=gpu_ctx) == [oracle_file(po, f, o)] * 2
+    ct, ss = int(o.color_type), int(o.subsampling)
+    co = po.jpeg_coefficients(f, o.width, o.height, ct, ss, o.quality)
+    d = [torch.from_numpy(np.ascontiguousarray(a)).cuda() if ct or k == 0 else None for k, a in enumerate(co)]
+    torch.cuda.synchronize()
+    assert jpeg.entropy_encode_dev(*d, o, ctx=gpu_ctx) == po.jpeg_encode_from_coefficients(
+        *co, o.width, o.height, ct, o.quality, ss, o.restart_interval or 0, True)
+    jp.build()
+    for trellis in (False, True):
+        p = JpegOptions(o.width, o.height, o.color_type, o.quality, o.subsampling, o.restart_interval, True, True,
+                        trellis)
+        assert jpeg.encode_progressive(f, p, ctx=gpu_ctx) == jp.encode(f, o.width, o.height, ct, ss, o.quality,
+                                                                        o.restart_interval or 0, True, trellis), trellis
 
 
 # ---- real pixo: the balanced preset's fixtures ---------------------------------------------------------

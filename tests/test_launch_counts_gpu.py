@@ -161,6 +161,8 @@ CASES = {
     "encode_batch_420": lambda ctx: (lambda: jpeg.encode_batch(np.stack([rgb()] * 3),
                                                                JpegOptions(W, H, ColorType.Rgb, 80, Subsampling.S420),
                                                                ctx=ctx)),
+    "encode_batch_420_optimized": lambda ctx: (lambda: jpeg.encode_batch(
+        np.stack([rgb()] * 8), JpegOptions(W, H, ColorType.Rgb, 80, Subsampling.S420, None, True), ctx=ctx)),
     "progressive": progressive(False, False),
     "progressive_optimized_trellis": progressive(True),
     "progressive_batch": lambda ctx: (lambda: jpeg.encode_progressive_batch(
@@ -209,13 +211,15 @@ EXPECTED = {
     "coefficients_gray": 1,
     "coefficients_gray_trellis": 2,
     "encode_420": 2,
-    "encode_420_trellis": 3,
-    "encode_444_optimized_restart": 3,
+    # optimised tables: K1, K3, k_huff_tables, then one k_huff per group (each frame was a k_huff of its own)
+    "encode_420_trellis": 4,
+    "encode_444_optimized_restart": 4,
     "encode_batch_420": 4,
+    "encode_batch_420_optimized": 8,   # two groups of 4: 12 when each frame had a k_huff of its own
     "encode_gray": 2,
     "entropy_dev_420": 1,
     "entropy_dev_420_segments": 5,
-    "entropy_dev_gray_optimized": 2,
+    "entropy_dev_gray_optimized": 3,   # K3, k_huff_tables, k_huff
     "png_adaptive": 1,
     "png_adaptive_fast": 1,
     "png_adaptive_fast_sticky": 2,
@@ -223,8 +227,8 @@ EXPECTED = {
     "png_bigrams": 1,
     "png_small_sub": 1,
     "progressive": 10,
-    "progressive_batch": 30,
-    "progressive_optimized_trellis": 15,
+    "progressive_batch": 32,               # k_huff_tables once per group (two groups of one)
+    "progressive_optimized_trellis": 16,   # k_huff_tables after K3
     "progressive_scans_dev": 10,
     "quantize": 8,
     "quantize_auto": 8,

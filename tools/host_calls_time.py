@@ -1,15 +1,16 @@
 """Times the host-buffer entry points on 4K frames in ordinary (pageable) numpy buffers, as a pixo caller hands
 them over: each call stages its frames to the device, runs its kernels and copies the results back, so a call's
 wall time is what the caller waits for.  One frame per call, except the JPEG batch calls: 8 baseline frames
-(two groups of 4) and 4 progressive frames (two groups of 2).
+(two groups of 4) and 4 progressive frames (two groups of 2).  jpeg_entropy_encode_dev takes the frame's
+coefficients already on the device and returns the file in host memory.
 
     python tools/host_calls_time.py [--reps N]                      (the library PIXO_B200_SO selects)
     python tools/host_calls_time.py --ab A.so B.so [--rounds R] [--out out.json]
 
 --ab runs the two libraries in alternating fresh processes, R rounds each, and reports per call the median
 of each round (milliseconds), the median over the rounds, B / A, and whether both computed the same bytes.
-The card's name, power limit and maximum SM clock are read in the same run.  profiles/h100_host_calls.json
-and profiles/h100_host_encode_calls.json hold such comparisons.
+The card's name, power limit and maximum SM clock are read in the same run.  profiles/h100_host_calls.json,
+profiles/h100_host_encode_calls.json and profiles/h100_host_encode_tables.json hold such comparisons.
 """
 import argparse
 import json
@@ -53,10 +54,15 @@ def calls(ctx):
     from pixo_b200 import resize as rs
     from pixo_b200.jpeg import Subsampling
     from pixo_b200.png import FilterStrategy, PngOptions, QuantizationMode
+    import torch
     rgb, rgba, indexed = frame(3, 1), frame(4, 2), few_colours(4000, 3)
     batch = np.stack([rgb] + [frame(3, 10 + k) for k in range(7)])
     q80 = jpeg.JpegOptions(W, H, ColorType.Rgb, 80, Subsampling.S420)
     pmax = jpeg.JpegOptions.max(W, H, 80)
+    balanced = jpeg.JpegOptions.balanced(W, H, 75)
+    d_coef = [torch.from_numpy(a).cuda() for a in jpeg.compute_all_coefficients(rgb, W, H, ColorType.Rgb,
+                                                                                 Subsampling.S444, 75, ctx=ctx)]
+    torch.cuda.synchronize()
     quant = PngOptions(W, H, ColorType.Rgba, FilterStrategy.Adaptive, True, True, True, QuantizationMode.Force, 256, True)
     lanczos = rs.ResizeOptions.builder(W, H).dst(1920, 1080).color_type(ColorType.Rgba).algorithm(
         rs.ResizeAlgorithm.Lanczos3).build()
@@ -77,6 +83,9 @@ def calls(ctx):
         "jpeg_encode_progressive_max_q80": lambda: jpeg.encode_progressive(rgb, pmax, ctx=ctx),
         "jpeg_encode_progressive_batch_4x_max_q80": lambda: b"".join(
             jpeg.encode_progressive_batch(batch[:4], pmax, ctx=ctx)),
+        "jpeg_encode_balanced_q75": lambda: jpeg.encode(rgb, balanced, ctx=ctx),
+        "jpeg_encode_batch_8x_balanced_q75": lambda: b"".join(jpeg.encode_batch(batch, balanced, ctx=ctx)),
+        "jpeg_entropy_encode_dev_444_q75_optimized": lambda: jpeg.entropy_encode_dev(*d_coef, balanced, ctx=ctx),
     }
 
 
