@@ -196,7 +196,7 @@ static int h2d_copy(pixo_b200_ctx *ctx, void *dst, const void *src, size_t bytes
         if (first_error.load() != (int)cudaSuccess) return;
         cudaError_t e = cudaSetDevice(device);
         const int slot_i = c % NSLOT;
-        uint8_t *slot = reinterpret_cast<uint8_t *>(ctx->h_in.ptr) + (size_t)slot_i * SLOT;
+        uint8_t *slot = ctx->h_in.slot(slot_i, SLOT);
         const size_t off = (size_t)c * SLOT, n = std::min(SLOT, bytes - off);
         if (e == cudaSuccess) e = cudaEventSynchronize(ctx->stage_events[slot_i]);   // the slot's previous DMA (this call's or the last one's) has drained
         if (e == cudaSuccess) {
@@ -238,7 +238,7 @@ static int d2h_copy_sync(pixo_b200_ctx *ctx, void *dst, const void *src, size_t 
     const int n = (int)((bytes + PIECE - 1) / PIECE);
     host_pool(ctx)->run(n, [&](int j) {
         const size_t off = (size_t)j * PIECE, len = std::min(PIECE, bytes - off);
-        memcpy(reinterpret_cast<uint8_t *>(dst) + off, reinterpret_cast<const uint8_t *>(ctx->h_out.ptr) + off, len);
+        memcpy(reinterpret_cast<uint8_t *>(dst) + off, ctx->h_out.slot(j, PIECE), len);
     });
     return 0;
 }
@@ -498,8 +498,8 @@ static int finish_frame(pixo_b200_ctx *ctx, uint8_t *out, size_t out_cap, size_t
 struct CoefLayout {
     size_t yb, cbb, yeb, ceb, each;  // bytes of the Y array, of one chroma array, of their extents, of a frame
     explicit CoefLayout(const FrameGeometry &g)
-        : yb(align_up(g.ny * 64 * sizeof(int16_t), 256)), cbb(align_up(g.nc * 64 * sizeof(int16_t), 256)),
-          yeb(align_up(g.ny, 256)), ceb(align_up(g.nc, 256)), each(yb + 2 * cbb + yeb + 2 * ceb) {}
+        : yb(Layout::round(g.ny * 64 * sizeof(int16_t))), cbb(Layout::round(g.nc * 64 * sizeof(int16_t))),
+          yeb(Layout::round(g.ny)), ceb(Layout::round(g.nc)), each(yb + 2 * cbb + yeb + 2 * ceb) {}
     size_t stride() const { return each / sizeof(int16_t); }
     int16_t *y(void *frame) const { return reinterpret_cast<int16_t *>(frame); }
     int16_t *cb(void *frame) const { return reinterpret_cast<int16_t *>(static_cast<uint8_t *>(frame) + yb); }
@@ -579,9 +579,12 @@ static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, siz
                               ? g.mcus_y
                               : (uint32_t)std::max<size_t>(1, std::min<size_t>(g.mcus_y, kTrellisScratch / row_bytes));
     const size_t piece_bytes = band < g.mcus_y ? row_bytes * band : frame_bytes * group;
-    PIXO_TRY(ctx->d_trellis.ensure(ctx, 256 + piece_bytes));
-    auto *status = static_cast<uint32_t *>(ctx->d_trellis.ptr);
-    float *fy = reinterpret_cast<float *>(static_cast<uint8_t *>(ctx->d_trellis.ptr) + 256);
+    uint32_t *status;
+    float *fy;
+    PIXO_TRY(bind(ctx, ctx->d_trellis, [&](Layout &L) {
+        status = L.take<uint32_t>(1);
+        fy = L.take<float>(piece_bytes / sizeof(float));
+    }));
     PIXO_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(uint32_t), ctx->stream));
     // frames [i0, i0 + nb) from MCU row m0 on, `rows` MCU rows each
     auto piece = [&](uint32_t i0, uint32_t nb, uint32_t m0, uint32_t rows) -> int {
@@ -668,18 +671,15 @@ int pixo_b200_jpeg_coefficients(pixo_b200_ctx *ctx, const uint8_t *pixels, uint3
     const size_t in_bytes = (size_t)width * height * (color_type == PIXO_B200_GRAY ? 1 : 3);
     const size_t yb = g.ny * 64 * sizeof(int16_t), cbb = g.nc * 64 * sizeof(int16_t);
     const size_t hist_bytes = kHistWords * sizeof(uint64_t);
+    int16_t *dy, *dcb = nullptr, *dcr = nullptr;
+    uint64_t *d_hist = nullptr;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
-    PIXO_TRY(ctx->d_y.ensure(ctx, yb));
-    if (cbb) {
-        PIXO_TRY(ctx->d_cb.ensure(ctx, cbb));
-        PIXO_TRY(ctx->d_cr.ensure(ctx, cbb));
-    }
-    if (hist) PIXO_TRY(ctx->d_out.ensure(ctx, hist_bytes));
-    auto *dy = static_cast<int16_t *>(ctx->d_y.ptr);
-    auto *dcb = cbb ? static_cast<int16_t *>(ctx->d_cb.ptr) : nullptr;
-    auto *dcr = cbb ? static_cast<int16_t *>(ctx->d_cr.ptr) : nullptr;
-    auto *d_hist = hist ? static_cast<uint64_t *>(ctx->d_out.ptr) : nullptr;
+    PIXO_TRY(bind(ctx, ctx->d_out, [&](Layout &L) {
+        dy = L.take<int16_t>(g.ny * 64);
+        if (cbb) dcb = L.take<int16_t>(g.nc * 64), dcr = L.take<int16_t>(g.nc * 64);
+        if (hist) d_hist = L.take<uint64_t>(kHistWords);
+    }));
     DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, pixels, in_bytes, ctx->stream));
     PIXO_TRY(pixo_b200_jpeg_coefficients_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
@@ -721,7 +721,7 @@ int pixo_b200_jpeg_trellis_quantize_dev(pixo_b200_ctx *ctx, const float *d_dct, 
 static uint64_t default_scan_cap(const pixo_b200_ctx *ctx, size_t raw_bytes)
 {
     const size_t want = ctx->scan_cap_override ? ctx->scan_cap_override : (raw_bytes / 2 + 65536) / 8 * 9;
-    return align_up(want < 1024 ? 1024 : want, 256);
+    return Layout::round(want < 1024 ? 1024 : want);
 }
 
 constexpr int kGaveUp = -1;  // recode_scan: the device stage did not finish the scan
@@ -744,13 +744,12 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
 {
     const size_t ent = entropy_scratch_bytes(1, g, restart_interval);
     for (int pass = 0;; ++pass) {
-        const size_t scan_bytes = align_up(cap, 256);
-        PIXO_TRY(ctx->d_retry.ensure(ctx, scan_bytes + ent + 256));
-        auto *buf = reinterpret_cast<uint8_t *>(ctx->d_retry.ptr);
+        uint8_t *scan, *scratch;
+        PIXO_TRY(bind(ctx, ctx->d_retry, [&](Layout &L) { scan = L.take(cap), scratch = L.take(ent); }));
         uint64_t *d_len = nullptr;
         uint32_t *d_ovf = nullptr;
-        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments, ext,
-                                     buf + scan_bytes, buf, cap, &d_len, &d_ovf));
+        PIXO_TRY(launch_jpeg_entropy(ctx, d_y, 0, d_cb, d_cr, 0, 1, g, t, restart_interval, segments, ext, scratch, scan,
+                                     cap, &d_len, &d_ovf));
         uint64_t n = 0;
         uint32_t ovf = 0;
         PIXO_CUDA(ctx, cudaMemcpyAsync(&n, d_len, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -767,7 +766,7 @@ static int recode_scan(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_
             continue;
         }
         PIXO_TRY(check_room(ctx, out_cap, hdr + (size_t)n + 2));
-        cap = align_up((size_t)n + 64, 256);
+        cap = Layout::round((size_t)n + 64);
     }
 }
 
@@ -809,7 +808,7 @@ struct EncodeGroups {
 
     uint32_t count() const { return (n + G - 1) / G; }
     uint32_t size(uint32_t gi) const { return std::min(G, n - gi * G); }
-    uint8_t *input(uint32_t gi) const { return static_cast<uint8_t *>(ctx->d_in.ptr) + (gi & 1) * G * in_stride; }
+    uint8_t *input(uint32_t gi) const { return ctx->d_in.slot(gi & 1, (size_t)G * in_stride); }
     // Group gi's frames into its input slot.  Group 0 first makes both copy streams wait for whatever the caller
     // already queued on the context's stream (ev_out[0] is free until group 0's scan bytes are copied back);
     // group gi >= 2 waits until the transform of group gi - 2 has read the slot.
@@ -837,7 +836,7 @@ struct EncodeGroups {
 static EncodeGroups make_groups(pixo_b200_ctx *ctx, const uint8_t *pixels, uint32_t n, size_t len_each,
                                 const FrameGeometry &g, uint32_t restart_interval)
 {
-    const size_t in_stride = align_up(len_each, 256), coef_each = CoefLayout(g).each;
+    const size_t in_stride = Layout::round(len_each), coef_each = CoefLayout(g).each;
     const uint64_t scan_cap = default_scan_cap(ctx, len_each);
     uint32_t G = (uint32_t)std::min<size_t>(16, std::max<size_t>(1, (((size_t)96 << 20) + len_each / 2) / len_each));
     G = std::min(G, std::max(1u, (n + 1) / 2));
@@ -866,25 +865,26 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
     const size_t cs = L.stride();
     const uint32_t G = grp.G;
     const uint64_t scan_cap = default_scan_cap(ctx, grp.len_each);
-    // d_misc: a group's statistics, its DHT blocks, its tables in k_huff's form
-    const size_t hist_bytes = align_up((size_t)G * kHistWords * sizeof(uint64_t), 256);
-    const size_t dht_bytes = align_up((size_t)G * kDhtBytes, 256);
+    uint64_t *d_hist, *h_lens[2];
+    uint8_t *d_dht, *d_own, *h_dhts[2];
+    uint32_t *h_ovfs[2];
     PIXO_TRY(ctx->d_coef.ensure(ctx, 2 * (size_t)G * L.each));
     PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(G, g, restart_interval)));
     PIXO_TRY(ctx->d_out.ensure(ctx, 2 * (size_t)G * scan_cap));
-    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + dht_bytes + (size_t)G * kHuffDevBytes));
-    // h_misc, per slot: a group's lengths, overflow flags and DHT blocks
-    const size_t meta_slot = align_up((size_t)G * (12 + kDhtBytes), 256);
-    PIXO_TRY(ctx->h_misc.ensure(ctx, 2 * meta_slot));
-    auto *d_scan = reinterpret_cast<uint8_t *>(ctx->d_out.ptr);
-    auto *h_meta = reinterpret_cast<uint8_t *>(ctx->h_misc.ptr);
-    auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
-    void *d_tabs = optimize ? d_dht + dht_bytes : nullptr;
-    auto h_len_of = [&](int slot) { return reinterpret_cast<uint64_t *>(h_meta + (size_t)slot * meta_slot); };
-    auto h_ovf_of = [&](int slot) { return reinterpret_cast<uint32_t *>(h_meta + (size_t)slot * meta_slot + (size_t)G * 8); };
-    auto h_dht_of = [&](int slot) { return h_meta + (size_t)slot * meta_slot + (size_t)G * 12; };
-    auto coef_of = [&](int slot) { return reinterpret_cast<uint8_t *>(ctx->d_coef.ptr) + (size_t)slot * G * L.each; };
+    // d_misc: a group's statistics, its DHT blocks, its tables in k_huff's form
+    PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &M) {
+        d_hist = M.take<uint64_t>((size_t)G * kHistWords);
+        d_dht = M.take((size_t)G * kDhtBytes);
+        d_own = M.take((size_t)G * kHuffDevBytes);
+    }));
+    // h_misc, per input slot: a group's lengths, overflow flags and DHT blocks, packed
+    PIXO_TRY(bind(ctx, ctx->h_misc, [&](Layout &H) {
+        for (int s = 0; s < 2; ++s)
+            h_lens[s] = H.take<uint64_t>(G), h_ovfs[s] = H.take<uint32_t>(G), h_dhts[s] = H.take((size_t)G * kDhtBytes);
+    }, 8));
+    auto *d_scan = static_cast<uint8_t *>(ctx->d_out.ptr);
+    void *d_tabs = optimize ? d_own : nullptr;
+    auto coef_of = [&](int slot) { return ctx->d_coef.slot(slot, (size_t)G * L.each); };
     HuffTables std_t;
     huff_from_dht(dht_standard(), std_t);
     const bool out_locked = is_page_locked(out);
@@ -906,9 +906,9 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
         if (gi >= 2) PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out[slot], 0));  // slot's previous D2H drained
         PIXO_TRY(code_records(ctx, L, c, cnt, g, std_t, d_tabs, restart_interval,
                               reinterpret_cast<uint8_t *>(ctx->d_ent.ptr), d_scan + (size_t)slot * G * scan_cap, scan_cap,
-                              h_len_of(slot), h_ovf_of(slot), cudaMemcpyDeviceToHost));
+                              h_lens[slot], h_ovfs[slot], cudaMemcpyDeviceToHost));
         if (optimize)
-            PIXO_CUDA(ctx, cudaMemcpyAsync(h_dht_of(slot), d_dht, (size_t)cnt * kDhtBytes, cudaMemcpyDeviceToHost,
+            PIXO_CUDA(ctx, cudaMemcpyAsync(h_dhts[slot], d_dht, (size_t)cnt * kDhtBytes, cudaMemcpyDeviceToHost,
                                            ctx->stream));
         PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_len[slot], ctx->stream));
         return 0;
@@ -920,11 +920,11 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
         const int slot = (int)(gi & 1);
         uint8_t *c = coef_of(slot);
         uint8_t *scan = d_scan + (size_t)slot * G * scan_cap;
-        const uint64_t *h_len = h_len_of(slot);
-        const uint32_t *h_ovf = h_ovf_of(slot);
+        const uint64_t *h_len = h_lens[slot];
+        const uint32_t *h_ovf = h_ovfs[slot];
         PIXO_CUDA(ctx, cudaEventSynchronize(ctx->ev_len[slot]));
         std::vector<HuffTables> tb(optimize ? cnt : 0);   // each frame's tables, from its DHT block
-        for (uint32_t k = 0; k < tb.size(); ++k) huff_from_dht(h_dht_of(slot) + (size_t)k * kDhtBytes, tb[k]);
+        for (uint32_t k = 0; k < tb.size(); ++k) huff_from_dht(h_dhts[slot] + (size_t)k * kDhtBytes, tb[k]);
         auto tables = [&](uint32_t k) -> const HuffTables & { return optimize ? tb[k] : std_t; };
         std::vector<size_t> hdr(cnt);
         bool redo = false;
@@ -960,7 +960,7 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
                 const size_t need = (h_ovf[k] & kOvfSegment) ? (size_t)scan_cap * 2 : (size_t)h_len[k];
                 if (!(h_ovf[k] & kOvfSegment)) PIXO_TRY(check_room(ctx, out_cap_each, hdr[k] + need + 2));
                 const CoefExtents ef = L.extents(f);
-                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), &ef, g, t, restart_interval, false, align_up(need + 64, 256),
+                rc = recode_scan(ctx, L.y(f), L.cb(f), L.cr(f), &ef, g, t, restart_interval, false, Layout::round(need + 64),
                                  hdr[k], out_cap_each, &body);
                 if (rc != 0 && rc != kGaveUp) return rc;
             }
@@ -1007,14 +1007,18 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, lum, chr);
     const CoefLayout L(g);
-    const size_t cs = L.stride(), hist_bytes = align_up((size_t)grp.G * kHistWords * sizeof(uint64_t), 256);
+    const size_t cs = L.stride();
+    uint64_t *d_hist;
+    uint8_t *d_dht;
     PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)grp.G * L.each));
-    PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + (size_t)grp.G * kDhtBytes));
+    // d_misc: a group's statistics, its DHT blocks
+    PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &M) {
+        d_hist = M.take<uint64_t>((size_t)grp.G * kHistWords);
+        d_dht = M.take((size_t)grp.G * kDhtBytes);
+    }));
     PIXO_TRY(ctx->h_misc.ensure(ctx, (size_t)grp.G * kDhtBytes));
     auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
     int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
-    auto *d_hist = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
     auto *h_dht = static_cast<const uint8_t *>(ctx->h_misc.ptr);
     // frame k's tables: its own (optimize), or the standard ones
     auto dht_of = [&](uint32_t k) { return optimize ? h_dht + (size_t)k * kDhtBytes : dht_standard(); };
@@ -1224,19 +1228,21 @@ int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, 
     const CoefLayout L(g);
     const bool optimize = optimize_huffman != 0;
     // optimize: every frame's statistics, then its tables in k_huff's form, in d_misc
-    const size_t hist_bytes = align_up((size_t)n_images * kHistWords * sizeof(uint64_t), 256);
+    uint64_t *d_hist = nullptr;
+    void *d_tabs = nullptr;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)n_images * L.each));
     PIXO_TRY(ctx->d_ent.ensure(ctx, entropy_scratch_bytes(n_images, g, restart_interval)));
-    if (optimize) PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + (size_t)n_images * kHuffDevBytes));
+    if (optimize)
+        PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &M) {
+            d_hist = M.take<uint64_t>((size_t)n_images * kHistWords);
+            d_tabs = M.take((size_t)n_images * kHuffDevBytes);
+        }));
     auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
     PIXO_TRY(transform_records(ctx, d_pixels, pixel_stride, n_images, g, lum, chr, L, c));
     HuffTables t;
     huff_standard(t);
-    void *d_tabs = nullptr;
     if (optimize) {
-        auto *d_hist = static_cast<uint64_t *>(ctx->d_misc.ptr);
-        d_tabs = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
         const CoefExtents ec = L.extents(c);
         const size_t cs = L.stride();
         PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, g.has_chroma ? L.cb(c) : nullptr, g.has_chroma ? L.cr(c) : nullptr,
@@ -1319,11 +1325,10 @@ int pixo_b200_jpeg_entropy_encode_dev(pixo_b200_ctx *ctx, const int16_t *d_y, co
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     const uint8_t *dht = dht_standard();
     if (optimize_huffman) {   // K3, k_huff_tables, the DHT block back to the host
-        const size_t hist_bytes = align_up(kHistWords * sizeof(uint64_t), 256);
-        PIXO_TRY(ctx->d_misc.ensure(ctx, hist_bytes + kDhtBytes));
+        uint64_t *d_hist;
+        uint8_t *d_dht;
+        PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &M) { d_hist = M.take<uint64_t>(kHistWords), d_dht = M.take(kDhtBytes); }));
         PIXO_TRY(ctx->h_misc.ensure(ctx, kDhtBytes));
-        auto *d_hist = static_cast<uint64_t *>(ctx->d_misc.ptr);
-        uint8_t *d_dht = static_cast<uint8_t *>(ctx->d_misc.ptr) + hist_bytes;
         PIXO_TRY(launch_jpeg_histogram(ctx, d_y, 0, d_cb, d_cr, 0, 1, g.ny, g.nc, g.y_per_mcu, restart_interval,
                                        false, nullptr, d_hist));
         PIXO_TRY(launch_huff_tables(ctx, d_hist, 1, g.has_chroma, d_dht, nullptr));
@@ -1398,28 +1403,31 @@ int pixo_b200_jpeg_band_entropy_dev(pixo_b200_ctx *ctx, const int16_t *d_y, cons
     HuffTables t;
     tables_from(hist, g.has_chroma, t);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    // the stream-ordered flow into a small device scratch: {bits, tail}, then the flags k_band_totals ORs into
-    PIXO_TRY(ctx->d_misc.ensure(ctx, 256));
-    PIXO_TRY(ctx->h_misc.ensure(ctx, 256));
-    auto *d = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    auto *h = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
-    uint32_t ovf = 0;
+    // the stream-ordered flow into a small device scratch, read back
+    struct Totals {
+        uint64_t bits_tail[2];   // the band's bit count, its last 7 bits
+        uint32_t flags;          // k_band_totals ORs into these
+    };
+    PIXO_TRY(ctx->d_misc.ensure(ctx, sizeof(Totals)));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, sizeof(Totals)));
+    auto *d = static_cast<Totals *>(ctx->d_misc.ptr);
+    auto *h = static_cast<Totals *>(ctx->h_misc.ptr);
     // a segment that outgrew its share (bit 0 of a segmented pass): the band again, as one string
     for (bool segments = true;; segments = false) {
-        PIXO_CUDA(ctx, cudaMemsetAsync(d + 2, 0, 4, ctx->stream));
-        PIXO_TRY(launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, dc_seed, nullptr, segments, d_raw, raw_cap, d,
-                                     reinterpret_cast<uint32_t *>(d + 2)));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, 20, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemsetAsync(&d->flags, 0, sizeof d->flags, ctx->stream));
+        PIXO_TRY(launch_band_entropy(ctx, d_y, d_cb, d_cr, g, t, dc_seed, nullptr, segments, d_raw, raw_cap,
+                                     d->bits_tail, &d->flags));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, sizeof(Totals), cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        ovf = *reinterpret_cast<uint32_t *>(h + 2);
-        if (!(segments && ovf == kOvfNoFit && ctx->bands[d_raw].S > 1)) break;
+        if (!(segments && h->flags == kOvfNoFit && ctx->bands[d_raw].S > 1)) break;
     }
-    *nbits = h[0];
-    *tail7 = (uint32_t)h[1];
+    const uint32_t ovf = h->flags;
+    *nbits = h->bits_tail[0];
+    *tail7 = (uint32_t)h->bits_tail[1];
     if (ovf & kOvfRange) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "%s", kOutOfRange);
     if (ovf & kOvfFault) return set_error(ctx, PIXO_B200_ERR_CUDA, "device entropy stage did not finish (flags %u)", ovf);
     if (ovf) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %zu too small (need %llu)", raw_cap,
-                              (unsigned long long)((h[0] + 7) / 8));
+                              (unsigned long long)((h->bits_tail[0] + 7) / 8));
     return 0;
 }
 
@@ -1434,19 +1442,22 @@ int pixo_b200_jpeg_band_splice_dev(pixo_b200_ctx *ctx, const uint8_t *d_raw, uin
         return 0;
     }
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    // the stream-ordered flow into a small device scratch: the length, then the flags (OR-ed into)
-    PIXO_TRY(ctx->d_misc.ensure(ctx, 256));
-    PIXO_TRY(ctx->h_misc.ensure(ctx, 256));
-    auto *d = reinterpret_cast<uint64_t *>(ctx->d_misc.ptr);
-    PIXO_CUDA(ctx, cudaMemsetAsync(d, 0, 16, ctx->stream));
-    PIXO_TRY(launch_band_splice(ctx, d_raw, start_bit, tail_in, is_last_band != 0, nullptr, d_out, out_cap, d,
-                                reinterpret_cast<uint32_t *>(d + 1)));
-    auto *h = reinterpret_cast<uint64_t *>(ctx->h_misc.ptr);
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, 12, cudaMemcpyDeviceToHost, ctx->stream));
+    // the stream-ordered flow into a small device scratch, read back
+    struct Spliced {
+        uint64_t len;
+        uint32_t flags;   // OR-ed into
+    };
+    PIXO_TRY(ctx->d_misc.ensure(ctx, sizeof(Spliced)));
+    PIXO_TRY(ctx->h_misc.ensure(ctx, sizeof(Spliced)));
+    auto *d = static_cast<Spliced *>(ctx->d_misc.ptr);
+    auto *h = static_cast<Spliced *>(ctx->h_misc.ptr);
+    PIXO_CUDA(ctx, cudaMemsetAsync(d, 0, sizeof(Spliced), ctx->stream));
+    PIXO_TRY(launch_band_splice(ctx, d_raw, start_bit, tail_in, is_last_band != 0, nullptr, d_out, out_cap, &d->len,
+                                &d->flags));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h, d, sizeof(Spliced), cudaMemcpyDeviceToHost, ctx->stream));
     PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*reinterpret_cast<uint32_t *>(h + 1))
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "splice output capacity %zu too small", out_cap);
-    *out_len = h[0];
+    if (h->flags) return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "splice output capacity %zu too small", out_cap);
+    *out_len = h->len;
     return 0;
 }
 
@@ -1628,10 +1639,10 @@ int pixo_b200_png_filter(pixo_b200_ctx *ctx, const uint8_t *data, uint32_t width
     const size_t in_bytes = row_bytes * height, out_bytes = (row_bytes + 1) * (size_t)height;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
-    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
-    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
-    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
-    uint32_t *d_adler = adler32_out ? static_cast<uint32_t *>(ctx->d_y.ptr) : nullptr;
+    uint8_t *d_out;
+    uint32_t *d_adler;   // the Adler word after the filtered stream
+    PIXO_TRY(bind(ctx, ctx->d_out, [&](Layout &L) { d_out = L.take(out_bytes + 16), d_adler = L.take<uint32_t>(1); }));
+    if (!adler32_out) d_adler = nullptr;
     DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
     PIXO_TRY(pixo_b200_png_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width, height,
@@ -1702,10 +1713,9 @@ int pixo_b200_png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_t 
     const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
-    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
-    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
-    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
-    auto *d_adler = static_cast<uint32_t *>(ctx->d_y.ptr);
+    uint8_t *d_out;
+    uint32_t *d_adler;   // the Adler word after the filtered stream
+    PIXO_TRY(bind(ctx, ctx->d_out, [&](Layout &L) { d_out = L.take(out_bytes + 16), d_adler = L.take<uint32_t>(1); }));
     DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
     PIXO_TRY(pixo_b200_png_reduce_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
@@ -1773,10 +1783,9 @@ int pixo_b200_png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *data, size_
     const size_t out_bytes = (size_t)height * ((size_t)width * (color_type + 1) + 1);
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     PIXO_TRY(ctx->d_in.ensure(ctx, in_bytes));
-    PIXO_TRY(ctx->d_out.ensure(ctx, out_bytes + 16));
-    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
-    auto *d_out = static_cast<uint8_t *>(ctx->d_out.ptr);
-    auto *d_adler = static_cast<uint32_t *>(ctx->d_y.ptr);
+    uint8_t *d_out;
+    uint32_t *d_adler;   // the Adler word after the filtered stream
+    PIXO_TRY(bind(ctx, ctx->d_out, [&](Layout &L) { d_out = L.take(out_bytes + 16), d_adler = L.take<uint32_t>(1); }));
     DrainOnError drain(ctx);
     PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, in_bytes, ctx->stream));
     PIXO_TRY(pixo_b200_png_quantize_filter_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), in_bytes, 1, width,
@@ -1814,12 +1823,12 @@ int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint3
     if (!ctx || !out || (!data && len))
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ctx->d_in.ensure(ctx, len + 16));
-    PIXO_TRY(ctx->d_y.ensure(ctx, 64));
-    auto *d_sum = static_cast<uint32_t *>(ctx->d_y.ptr);
+    uint8_t *d_data;
+    uint32_t *d_sum;
+    PIXO_TRY(bind(ctx, ctx->d_in, [&](Layout &L) { d_data = L.take(len + 16), d_sum = L.take<uint32_t>(1); }));
     DrainOnError drain(ctx);
-    if (len) PIXO_TRY(h2d_copy(ctx, ctx->d_in.ptr, data, len, ctx->stream));
-    PIXO_TRY(pixo_b200_adler32_dev(ctx, static_cast<const uint8_t *>(ctx->d_in.ptr), len, d_sum));
+    if (len) PIXO_TRY(h2d_copy(ctx, d_data, data, len, ctx->stream));
+    PIXO_TRY(pixo_b200_adler32_dev(ctx, d_data, len, d_sum));
     PIXO_TRY(d2h_copy_sync(ctx, out, d_sum, 4, ctx->stream));
     drain.armed = false;
     return 0;

@@ -73,6 +73,8 @@ struct Buffer {
     // at least `bytes`: a smaller buffer is freed, once the context's stream has drained, and
     // allocated again with room to grow
     int ensure(pixo_b200_ctx *ctx, size_t bytes);
+    // slot i of a buffer used as an array of equal slots, `stride` bytes each
+    uint8_t *slot(size_t i, size_t stride) const { return static_cast<uint8_t *>(ptr) + i * stride; }
 };
 using DevBuf = Buffer<false>;
 using PinnedBuf = Buffer<true>;
@@ -99,22 +101,41 @@ private:
     bool stop_ = false;
 };
 
-// Device scratch layout of the entropy stage for n images (all sizes in bytes, 256-aligned)
-struct EntropyPlan {
-    size_t nunits;                 // k_huff work units per image
-    size_t off_st1, off_st2, off_ticket, off_ovf, zero_bytes, off_outlen, off_tail, total;
+// The layout of a scratch buffer: regions appended in order, each taking whole 256-byte units, so that
+// every region starts 256-byte aligned.  A stage describes its regions once and runs that description
+// twice: without a base, to count the bytes to ensure, and on the buffer, to bind its pointers (see bind).
+// Small host read-back areas pack their regions in 8-byte units instead (`unit`).
+class Layout {
+public:
+    explicit Layout(void *base = nullptr, size_t unit = 256) : base_(static_cast<uint8_t *>(base)), unit_(unit) {}
+    // the next region, room for `count` T; null while counting
+    template <class T = uint8_t>
+    T *take(size_t count)
+    {
+        T *p = base_ ? reinterpret_cast<T *>(base_ + size_) : nullptr;
+        end_ = size_ + count * sizeof(T);
+        size_ = (end_ + unit_ - 1) / unit_ * unit_;
+        return p;
+    }
+    size_t size() const { return size_; }   // bytes taken so far, the last region's too
+    size_t end() const { return end_; }     // where the last region's own bytes end: what a buffer must hold
+    // the bytes a region of `bytes` takes, and the most whole units `bytes` holds
+    static size_t round(size_t bytes) { return (bytes + 255) / 256 * 256; }
+    static size_t floor(size_t bytes) { return bytes / 256 * 256; }
+
+private:
+    uint8_t *base_;
+    size_t unit_;
+    size_t size_ = 0, end_ = 0;
 };
 
 // Images cut into S segments, each coded as a raw bit string of its own and spliced afterwards
-// (see jpeg_entropy.cu, k_seg_*)
+// (see jpeg_entropy.cu, k_seg_*).  Sizes only: the scratch and the raw area are bound where they are used.
 struct SegPlan {
-    uint32_t S;
-    uint64_t seg_mcus, last_mcus;
+    uint32_t n, S;
+    uint64_t seg_mcus, last_mcus, bpm;
     size_t raw_cap;                 // bytes per segment
     uint32_t max_tiles;             // per image
-    EntropyPlan ent;                // status words etc. for n * S pseudo images
-    size_t off_ent, off_rec, off_ntiles, off_cnt, total;   // offsets into the context's segment scratch
-    size_t raw_bytes, off_bits, off_tails, raw_total;      // layout of the raw area: strings, then the segments' bit counts and tails
 };
 
 // Huffman tables of the progressive scans as get_code_from_table sees them: (code << 8) | length per
@@ -122,14 +143,6 @@ struct SegPlan {
 struct ProgTables {
     uint32_t dc[2][16];
     uint32_t ac[2][256];
-};
-
-// Device scratch of the progressive stage for n frames (jpeg_progressive.cu), offsets in bytes
-struct ProgLayout {
-    uint64_t nb[7];
-    uint32_t tile_base[8];
-    uint64_t blk_base[8];
-    size_t off_status, off_blen, off_flag, off_tile_last, off_tile_carry, off_tile_bits, off_tile_off, off_bits, off_tables, total;
 };
 
 // The 7 stuffed segments of each of n frames: segment q = frame * 7 + scan at stage + q * stage_cap, its
@@ -165,7 +178,7 @@ struct pixo_b200_ctx {
     bool gpu_retry = true;         // re-run k_huff with the exact size when the heuristic was too small
     std::string err;
     // reusable scratch
-    pixo::DevBuf d_in, d_y, d_cb, d_cr, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
+    pixo::DevBuf d_in, d_misc, d_out, d_ent, d_coef, d_retry, d_raw;
     pixo::DevBuf d_hwin;                        // k_huff: every warp's assembled unit, from its phase A to its phase B
     pixo::DevBuf d_red, d_red_idx, d_red_img;   // PNG reduction: statistics, palette indices, reduced rows
     pixo::DevBuf d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
@@ -209,7 +222,18 @@ int cuda_fail(pixo_b200_ctx *ctx, cudaError_t e, const char *what);
         if (rc__ != 0) return rc__;    \
     } while (0)
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// Ensure `buf` holds the regions `describe(Layout &)` takes, then bind them: describe runs twice, without a
+// base to count them and on the buffer to set the pointers it assigns.
+template <bool Pinned, class F>
+int bind(pixo_b200_ctx *ctx, Buffer<Pinned> &buf, F &&describe, size_t unit = 256)
+{
+    Layout count(nullptr, unit);
+    describe(count);
+    PIXO_TRY(buf.ensure(ctx, count.end()));
+    Layout L(buf.ptr, unit);
+    describe(L);
+    return 0;
+}
 
 // Dynamic shared memory of a launch: `bytes`, and `limit`, what the kernel's maximum is raised to.  A
 // kernel launched with varying sizes passes one fixed limit, so that no context lowers it under another.
@@ -309,15 +333,21 @@ int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_b
                        uint32_t *d_flags);
 // bytes a band's raw buffer needs for the band as one string of the usual size, with its trailer
 size_t band_raw_bytes(const FrameGeometry &g);
-// n whole raw strings of raw_cap bytes each, spliced on their own (no segments): the raw area holds the
-// strings, then their bit counts (off_bits) and tails (off_tails); the splice scratch is `total` bytes
+// The raw area of a SegPlan: the segments' strings, then their bit counts and tails (the trailer)
+struct SegRaw {
+    uint8_t *strings;
+    unsigned long long *bits, *tails;
+    size_t total, trailer;   // bytes of the area, of the trailer
+};
+SegRaw seg_raw(const SegPlan &p, void *base);
+size_t seg_scratch_bytes(const SegPlan &p);   // the device scratch of its coding and splice
+// n whole raw strings of raw_cap bytes each, spliced on their own (no segments)
 SegPlan splice_plan(uint32_t n, size_t raw_cap);
-int launch_splice(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
-                  uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow);
+int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area, uint8_t *d_out,
+                  uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow);
 
 // progressive scans (jpeg_progressive.cu)
 bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
-ProgLayout prog_layout(const FrameGeometry &g, uint32_t n);
 int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                        const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
                        const ProgTables *T, bool per_frame, bool check_only, ProgResult *res);

@@ -1054,7 +1054,17 @@ __global__ void __launch_bounds__(128) k_huff_tables(const unsigned long long *h
 
 }  // namespace
 
-static EntropyPlan plan_entropy(uint32_t n, uint64_t nblocks, uint64_t rst_blocks)
+// Scratch of the entropy stage for n images: k_huff's status words, appended to L
+struct EntropyPlan {
+    size_t nunits;                 // k_huff work units per image
+    unsigned long long *st1, *st2;
+    uint32_t *ticket, *ovf;
+    size_t zero_bytes;             // the regions above, from st1 on: cleared per launch
+    uint64_t *out_len;
+    unsigned long long *tail;
+};
+
+static EntropyPlan plan_entropy(Layout &L, uint32_t n, uint64_t nblocks, uint64_t rst_blocks)
 {
     EntropyPlan p;
     p.nunits = (size_t)((nblocks + UB - 1) / UB);
@@ -1063,22 +1073,23 @@ static EntropyPlan plan_entropy(uint32_t n, uint64_t nblocks, uint64_t rst_block
         const uint64_t last = nblocks - (n_int - 1) * rst_blocks;
         p.nunits = (size_t)((n_int - 1) * upi + (last + UB - 1) / UB);
     }
-    size_t o = 0;
-    p.off_st1 = o; o += align_up((size_t)n * p.nunits * 8, 256);
-    p.off_st2 = o; o += align_up((size_t)n * p.nunits * 8, 256);
-    p.off_ticket = o; o += 256;
-    p.off_ovf = o; o += align_up((size_t)n * 4, 256);
-    p.zero_bytes = o;  // everything up to here is cleared per launch
-    p.off_outlen = o; o += align_up((size_t)n * 8, 256);
-    p.off_tail = o; o += align_up((size_t)n * 8, 256);
-    p.total = o;
+    const size_t start = L.size();
+    p.st1 = L.take<unsigned long long>((size_t)n * p.nunits);
+    p.st2 = L.take<unsigned long long>((size_t)n * p.nunits);
+    p.ticket = L.take<uint32_t>(1);
+    p.ovf = L.take<uint32_t>(n);
+    p.zero_bytes = L.size() - start;
+    p.out_len = L.take<uint64_t>(n);
+    p.tail = L.take<unsigned long long>(n);
     return p;
 }
 
 size_t entropy_scratch_bytes(uint32_t n, const FrameGeometry &g, uint32_t restart_interval)
 {
     const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
-    return plan_entropy(n, g.ny + 2 * g.nc, (uint64_t)restart_interval * bpm).total;
+    Layout L;
+    plan_entropy(L, n, g.ny + 2 * g.nc, (uint64_t)restart_interval * bpm);
+    return L.size();
 }
 
 // ---- splicing a raw bit string into the stream's scan bytes -------------------------------------
@@ -1476,28 +1487,55 @@ static uint32_t segments_for(uint32_t n, uint64_t total_mcus, uint64_t bpm)
     return S < 2 ? 1 : S;
 }
 
-// Segments of raw_cap string bytes each: the offsets of the plan's scratch and raw area
-static void lay_out(SegPlan &p, uint32_t n, uint64_t bpm, size_t raw_cap)
+// Segments of raw_cap string bytes each
+static void set_raw_cap(SegPlan &p, size_t raw_cap)
 {
-    const uint32_t S = p.S;
     p.raw_cap = raw_cap;
-    p.max_tiles = (uint32_t)(S * (p.raw_cap / SPL_TILE + 2));
-    p.ent = plan_entropy(n * S, p.seg_mcus * bpm, 0);
-    size_t o = 0;
-    p.off_ent = o; o += align_up(p.ent.total, 256);
-    p.raw_bytes = align_up((size_t)n * S * p.raw_cap, 256);
-    p.off_bits = p.raw_bytes;
-    p.off_tails = p.off_bits + align_up((size_t)n * S * 8, 256);
-    p.raw_total = p.off_tails + align_up((size_t)n * S * 8, 256);
-    p.off_rec = o; o += align_up((size_t)n * S * sizeof(SegRec), 256);
-    p.off_ntiles = o; o += align_up((size_t)n * 4, 256);
-    p.off_cnt = o; o += align_up((size_t)n * p.max_tiles * 4, 256);
-    p.total = o;
+    p.max_tiles = (uint32_t)(p.S * (raw_cap / SPL_TILE + 2));
+}
+
+// The segment scratch of a plan: the entropy stage's status words for its n * S pseudo images, then the
+// splice's records
+struct SegScratch {
+    EntropyPlan ent;
+    SegRec *rec;
+    uint32_t *ntiles, *cnt;
+    size_t total;
+};
+
+static SegScratch seg_scratch(const SegPlan &p, void *base)
+{
+    Layout L(base);
+    SegScratch s;
+    s.ent = plan_entropy(L, p.n * p.S, p.seg_mcus * p.bpm, 0);
+    s.rec = L.take<SegRec>((size_t)p.n * p.S);
+    s.ntiles = L.take<uint32_t>(p.n);
+    s.cnt = L.take<uint32_t>((size_t)p.n * p.max_tiles);
+    s.total = L.size();
+    return s;
+}
+
+size_t seg_scratch_bytes(const SegPlan &p) { return seg_scratch(p, nullptr).total; }
+
+SegRaw seg_raw(const SegPlan &p, void *base)
+{
+    Layout L(base);
+    SegRaw r;
+    const size_t strings = (size_t)p.n * p.S;
+    r.strings = L.take(strings * p.raw_cap);
+    const size_t strings_bytes = L.size();
+    r.bits = L.take<unsigned long long>(strings);
+    r.tails = L.take<unsigned long long>(strings);
+    r.total = L.size();
+    r.trailer = r.total - strings_bytes;
+    return r;
 }
 
 static SegPlan plan_segments(uint32_t n, uint32_t S, uint64_t total_mcus, uint64_t bpm, uint64_t mcu_raw_bytes)
 {
     SegPlan p;
+    p.n = n;
+    p.bpm = bpm;
     p.seg_mcus = (total_mcus + S - 1) / S;
     S = (uint32_t)((total_mcus + p.seg_mcus - 1) / p.seg_mcus);   // no empty last segment
     p.S = S;
@@ -1506,40 +1544,40 @@ static SegPlan plan_segments(uint32_t n, uint32_t S, uint64_t total_mcus, uint64
     // that), at most what its blocks can possibly need (64 x 26 bits + DC < 216 bytes per block).  It
     // does not depend on the caller's output capacity, so an output that is too small is still measured.
     const uint64_t fair = p.seg_mcus * mcu_raw_bytes + 4096, worst = p.seg_mcus * bpm * 216 + 64;
-    lay_out(p, n, bpm, (size_t)align_up(std::min(fair, worst), 256));
+    set_raw_cap(p, Layout::round((size_t)std::min(fair, worst)));
     return p;
 }
 
 static uint64_t mcu_raw_bytes(const FrameGeometry &g) { return (uint64_t)g.y_per_mcu * 64 * (g.has_chroma ? 3 : 1); }
 
 // k_huff<RAW> over the n * S segments of sp (P: the coefficient arrays and DC predictors).  The strings go
-// to raw_area, each segment's bit count and tail after them (off_bits / off_tails: a band's travel with its
-// strings to a later splice); the segments' flags stay in seg_scratch (off_ent + ent.off_ovf).  Arrays
-// without extents are the caller's: checked, see code_block.
-static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, const HuffDev *tabs, uint32_t n,
-                         const FrameGeometry &g, const SegPlan &sp, uint8_t *seg_scratch, uint8_t *raw_area)
+// to raw_area, each segment's bit count and tail after them (seg_raw: a band's travel with its strings to a
+// later splice); the segments' flags stay in seg_scratch (its ent.ovf).  Arrays without extents are the
+// caller's: checked, see code_block.
+static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, const HuffDev *tabs,
+                         const FrameGeometry &g, const SegPlan &sp, uint8_t *scratch, uint8_t *raw_area)
 {
     const bool check = P.e.y == nullptr;
     cudaStream_t st = ctx->stream;
-    const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
-    uint8_t *ent = seg_scratch + sp.off_ent;
-    P.nimages = n * sp.S;
+    const EntropyPlan ent = seg_scratch(sp, scratch).ent;
+    const SegRaw raw = seg_raw(sp, raw_area);
+    P.nimages = sp.n * sp.S;
     P.seg_per_img = sp.S;
-    P.nblocks = (uint32_t)(sp.seg_mcus * bpm);
-    P.nblocks_last = (uint32_t)(sp.last_mcus * bpm);
-    P.nunits = (uint32_t)sp.ent.nunits;
+    P.nblocks = (uint32_t)(sp.seg_mcus * sp.bpm);
+    P.nblocks_last = (uint32_t)(sp.last_mcus * sp.bpm);
+    P.nunits = (uint32_t)ent.nunits;
     P.seg_y_stride = (size_t)sp.seg_mcus * g.y_per_mcu * 64;
     P.seg_c_stride = (size_t)sp.seg_mcus * 64;
     P.rst_blocks = P.rst_mcus = P.upi = 0;
-    P.st_bits = reinterpret_cast<unsigned long long *>(ent + sp.ent.off_st1);
-    P.st_ff = reinterpret_cast<unsigned long long *>(ent + sp.ent.off_st2);
-    P.ticket = reinterpret_cast<uint32_t *>(ent + sp.ent.off_ticket);
-    P.overflow = reinterpret_cast<uint32_t *>(ent + sp.ent.off_ovf);
-    P.out_len = reinterpret_cast<uint64_t *>(ent + sp.ent.off_outlen);
-    P.out_tail = reinterpret_cast<unsigned long long *>(ent + sp.ent.off_tail);
-    P.out = raw_area;
+    P.st_bits = ent.st1;
+    P.st_ff = ent.st2;
+    P.ticket = ent.ticket;
+    P.overflow = ent.ovf;
+    P.out_len = ent.out_len;
+    P.out_tail = ent.tail;
+    P.out = raw.strings;
     P.out_cap = sp.raw_cap;
-    PIXO_CUDA(ctx, cudaMemsetAsync(ent, 0, sp.ent.zero_bytes, st));
+    PIXO_CUDA(ctx, cudaMemsetAsync(ent.st1, 0, ent.zero_bytes, st));
     const size_t want = ((size_t)P.nimages * P.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
     if (tabs)
@@ -1547,8 +1585,8 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, cons
                         FrameTables{tabs}));
     else
         PIXO_TRY(launch(ctx, check ? k_huff<true, true, false> : k_huff<true, false, false>, grid, 32 * HUFF_WARPS, 0, P, T));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_bits, P.out_len, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(raw_area + sp.off_tails, P.out_tail, (size_t)n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(raw.bits, P.out_len, (size_t)sp.n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(raw.tails, P.out_tail, (size_t)sp.n * sp.S * 8, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
@@ -1556,21 +1594,24 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, cons
 // raw_area: final bytes in d_out (out_cap per image), byte counts and flags in d_out_len / d_overflow.
 // raw_overflow: the coding kernel's flags per segment, or null.  base_bit / base_tail / last / base_dev:
 // see SegParams (a band of a tiled frame passes its place in the stream; a whole image passes 0, 0, true).
-static int splice_segments(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, uint8_t *seg_scratch,
-                           const uint8_t *raw_area, const uint32_t *raw_overflow, uint64_t base_bit, uint32_t base_tail,
-                           bool last, const uint64_t *base_dev, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
+static int splice_segments(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *scratch, const uint8_t *raw_area,
+                           const uint32_t *raw_overflow, uint64_t base_bit, uint32_t base_tail, bool last,
+                           const uint64_t *base_dev, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
                            uint32_t *d_overflow)
 {
+    const uint32_t n = sp.n;
+    const SegScratch s = seg_scratch(sp, scratch);
+    const SegRaw raw = seg_raw(sp, const_cast<uint8_t *>(raw_area));
     SegParams Q;
     Q.raw = raw_area; Q.raw_cap = sp.raw_cap;
-    Q.bits = reinterpret_cast<const unsigned long long *>(raw_area + sp.off_bits);
-    Q.tails = reinterpret_cast<const unsigned long long *>(raw_area + sp.off_tails);
+    Q.bits = raw.bits;
+    Q.tails = raw.tails;
     Q.S = sp.S; Q.max_tiles = sp.max_tiles;
     Q.base_bit = base_bit; Q.base_tail = base_tail; Q.last_band = last ? 1u : 0u;
     Q.base_dev = reinterpret_cast<const unsigned long long *>(base_dev);
-    Q.rec = reinterpret_cast<SegRec *>(seg_scratch + sp.off_rec);
-    Q.ntiles = reinterpret_cast<uint32_t *>(seg_scratch + sp.off_ntiles);
-    Q.cnt = reinterpret_cast<uint32_t *>(seg_scratch + sp.off_cnt);
+    Q.rec = s.rec;
+    Q.ntiles = s.ntiles;
+    Q.cnt = s.cnt;
     Q.out = d_out; Q.out_cap = out_cap;
     Q.out_len = reinterpret_cast<unsigned long long *>(d_out_len);
     Q.overflow = d_overflow;
@@ -1615,7 +1656,8 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     const uint64_t bpm_ = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     uint64_t rst_blocks = (uint64_t)restart_interval * bpm_;
     if (rst_blocks >= nblocks) rst_blocks = 0;  // a single interval: no marker is ever written
-    const EntropyPlan pl = plan_entropy(n, nblocks, rst_blocks);
+    Layout L(d_scratch);
+    const EntropyPlan pl = plan_entropy(L, n, nblocks, rst_blocks);
     if (nblocks > 0xFFFFFFFFull || (uint64_t)n * pl.nunits > 0x7FFFFFFFull)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "entropy stage: too many blocks per call");
     EntParams P;
@@ -1629,13 +1671,13 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     P.rst_mcus = rst_blocks ? restart_interval : 0u;
     P.upi = rst_blocks ? (uint32_t)((rst_blocks + UB - 1) / UB) : 0u;
     P.nimages = n;
-    P.st_bits = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_st1);
-    P.st_ff = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_st2);
-    P.ticket = reinterpret_cast<uint32_t *>(d_scratch + pl.off_ticket);
-    P.overflow = reinterpret_cast<uint32_t *>(d_scratch + pl.off_ovf);
-    P.out_len = reinterpret_cast<uint64_t *>(d_scratch + pl.off_outlen);
+    P.st_bits = pl.st1;
+    P.st_ff = pl.st2;
+    P.ticket = pl.ticket;
+    P.overflow = pl.ovf;
+    P.out_len = pl.out_len;
     P.out = d_out; P.out_cap = out_cap;
-    P.out_tail = reinterpret_cast<unsigned long long *>(d_scratch + pl.off_tail);
+    P.out_tail = pl.tail;
     P.dc_seed[0] = P.dc_seed[1] = P.dc_seed[2] = 0;
     P.dc_seed_dev = nullptr;
     P.win = nullptr;   // set below; k_huff<RAW> has no phase B
@@ -1645,19 +1687,19 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
     HuffDev T;
     make_huff_dev(t, &T);
     cudaStream_t st = ctx->stream;
-    PIXO_CUDA(ctx, cudaMemsetAsync(d_scratch, 0, pl.zero_bytes, st));
+    PIXO_CUDA(ctx, cudaMemsetAsync(pl.st1, 0, pl.zero_bytes, st));
     P.seg_per_img = 1; P.nblocks_last = P.nblocks; P.seg_y_stride = P.seg_c_stride = 0;
     // few images: cut each into segments (short look-back chains) and splice - see k_seg_*
     const uint32_t S = (rst_blocks == 0 && allow_segments) ? segments_for(n, g.total_mcus(), bpm_) : 1;
     const SegPlan sp = plan_segments(n, S, g.total_mcus(), bpm_, mcu_raw_bytes(g));
-    if (sp.S > 1) {
-        PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total + sp.raw_total));
-        auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
-        uint8_t *raw_area = seg_scratch + sp.total;
-        PIXO_TRY(code_segments(ctx, P, T, tabs, n, g, sp, seg_scratch, raw_area));
-        return splice_segments(ctx, n, sp, seg_scratch, raw_area,
-                               reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), 0, 0, true,
-                               nullptr, d_out, out_cap, P.out_len, P.overflow);
+    if (sp.S > 1) {   // d_raw: the segment scratch, then the raw area
+        uint8_t *scratch, *raw_area;
+        PIXO_TRY(bind(ctx, ctx->d_raw, [&](Layout &R) {
+            scratch = R.take(seg_scratch_bytes(sp)), raw_area = R.take(seg_raw(sp, nullptr).total);
+        }));
+        PIXO_TRY(code_segments(ctx, P, T, tabs, g, sp, scratch, raw_area));
+        return splice_segments(ctx, sp, scratch, raw_area, seg_scratch(sp, scratch).ent.ovf, 0, 0, true, nullptr, d_out,
+                               out_cap, P.out_len, P.overflow);
     }
     const size_t want = ((size_t)n * pl.nunits + HUFF_WARPS - 1) / HUFF_WARPS;
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * HUFF_CTAS_PER_SM);
@@ -1671,7 +1713,8 @@ int launch_jpeg_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
 
 size_t band_raw_bytes(const FrameGeometry &g)
 {
-    return plan_segments(1, 1, g.total_mcus(), g.y_per_mcu + (g.has_chroma ? 2 : 0), mcu_raw_bytes(g)).raw_total;
+    return seg_raw(plan_segments(1, 1, g.total_mcus(), g.y_per_mcu + (g.has_chroma ? 2 : 0), mcu_raw_bytes(g)), nullptr)
+        .total;
 }
 
 // Code one band of a frame tiled over several GPUs into the caller's buffer d_raw (k_huff<RAW> over S >= 1
@@ -1691,16 +1734,16 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     const uint64_t bpm = g.y_per_mcu + (g.has_chroma ? 2 : 0);
     SegPlan sp = plan_segments(1, allow_segments ? segments_for(1, g.total_mcus(), bpm) : 1, g.total_mcus(), bpm,
                                mcu_raw_bytes(g));
-    if (sp.S == 1 || sp.raw_total > raw_cap) {
+    if (sp.S == 1 || seg_raw(sp, nullptr).total > raw_cap) {
         sp = plan_segments(1, 1, g.total_mcus(), bpm, mcu_raw_bytes(g));
-        const size_t trailer = sp.raw_total - sp.raw_bytes;
-        if (raw_cap < trailer)
+        const SegRaw need = seg_raw(sp, nullptr);
+        if (raw_cap < need.trailer)
             return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %llu too small (need %zu)",
-                             (unsigned long long)raw_cap, sp.raw_total);
-        lay_out(sp, 1, bpm, (size_t)(raw_cap - trailer) / 256 * 256);
+                             (unsigned long long)raw_cap, need.total);
+        set_raw_cap(sp, Layout::floor((size_t)(raw_cap - need.trailer)));
     }
-    PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total));
-    auto *seg_scratch = reinterpret_cast<uint8_t *>(ctx->d_raw.ptr);
+    PIXO_TRY(ctx->d_raw.ensure(ctx, seg_scratch_bytes(sp)));
+    auto *scratch = static_cast<uint8_t *>(ctx->d_raw.ptr);
     EntParams P;
     memset(&P, 0, sizeof P);
     P.y = d_y; P.cb = d_cb; P.cr = d_cr;
@@ -1710,10 +1753,9 @@ int launch_band_entropy(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d
     HuffDev T;
     make_huff_dev(t, &T);
     ctx->bands[d_raw] = sp;
-    PIXO_TRY(code_segments(ctx, P, T, nullptr, 1, g, sp, seg_scratch, d_raw));   // a band's arrays are the caller's (no extents)
-    return launch(ctx, k_band_totals, 1, 32, 0, reinterpret_cast<const unsigned long long *>(d_raw + sp.off_bits),
-                  reinterpret_cast<const unsigned long long *>(d_raw + sp.off_tails),
-                  reinterpret_cast<const uint32_t *>(seg_scratch + sp.off_ent + sp.ent.off_ovf), sp.S,
+    PIXO_TRY(code_segments(ctx, P, T, nullptr, g, sp, scratch, d_raw));   // a band's arrays are the caller's (no extents)
+    const SegRaw raw = seg_raw(sp, d_raw);
+    return launch(ctx, k_band_totals, 1, 32, 0, raw.bits, raw.tails, seg_scratch(sp, scratch).ent.ovf, sp.S,
                   reinterpret_cast<unsigned long long *>(d_bits_tail), d_flags);
 }
 
@@ -1728,25 +1770,27 @@ int launch_band_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint64_t base_b
     if (it == ctx->bands.end())
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "this raw buffer was not coded by pixo_b200_jpeg_band_entropy_dev");
     const SegPlan sp = it->second;
-    PIXO_TRY(ctx->d_raw.ensure(ctx, sp.total));
-    return splice_segments(ctx, 1, sp, reinterpret_cast<uint8_t *>(ctx->d_raw.ptr), d_raw, nullptr, base_bit, base_tail,
-                           last, d_base, d_out, out_cap, d_out_len, d_flags);
+    PIXO_TRY(ctx->d_raw.ensure(ctx, seg_scratch_bytes(sp)));
+    return splice_segments(ctx, sp, static_cast<uint8_t *>(ctx->d_raw.ptr), d_raw, nullptr, base_bit, base_tail, last,
+                           d_base, d_out, out_cap, d_out_len, d_flags);
 }
 
 SegPlan splice_plan(uint32_t n, size_t raw_cap)
 {
     SegPlan p;
+    p.n = n;
     p.S = 1;
     p.seg_mcus = p.last_mcus = 0;
-    lay_out(p, n, 1, raw_cap);
+    p.bpm = 1;
+    set_raw_cap(p, raw_cap);
     return p;
 }
 
 // The progressive scans' strings: each a whole stream of its own (base bit 0, 1-padded at its end)
-int launch_splice(pixo_b200_ctx *ctx, uint32_t n, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
-                  uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow)
+int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area, uint8_t *d_out,
+                  uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow)
 {
-    return splice_segments(ctx, n, sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap, d_out_len,
+    return splice_segments(ctx, sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap, d_out_len,
                            d_overflow);
 }
 

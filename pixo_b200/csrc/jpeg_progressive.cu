@@ -440,33 +440,20 @@ bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTa
     return true;
 }
 
-ProgLayout prog_layout(const FrameGeometry &g, uint32_t n)
+// The scans' block and tile counts of one frame into P
+static void prog_counts(const FrameGeometry &g, ProgParams &P)
 {
-    ProgLayout L;
     uint32_t tb = 0;
     uint64_t bb = 0;
     for (int s = 0; s < NSCAN; ++s) {
-        L.nb[s] = kComp[s] == 0 ? g.ny : g.nc;
-        L.tile_base[s] = tb;
-        L.blk_base[s] = bb;
-        tb += (uint32_t)((L.nb[s] + PT - 1) / PT);
-        bb += L.nb[s];
+        P.nb[s] = kComp[s] == 0 ? g.ny : g.nc;
+        P.tile_base[s] = tb;
+        P.blk_base[s] = bb;
+        tb += (uint32_t)((P.nb[s] + PT - 1) / PT);
+        bb += P.nb[s];
     }
-    L.tile_base[NSCAN] = tb;
-    L.blk_base[NSCAN] = bb;
-    const size_t tiles = (size_t)n * tb, blocks = (size_t)n * bb;
-    size_t o = 0;
-    L.off_status = o; o += 256;
-    L.off_blen = o; o += align_up(blocks * 4, 256);
-    L.off_flag = o; o += align_up(blocks, 256);
-    L.off_tile_last = o; o += align_up(tiles * 4, 256);
-    L.off_tile_carry = o; o += align_up(tiles * 4, 256);
-    L.off_tile_bits = o; o += align_up(tiles * 4, 256);
-    L.off_tile_off = o; o += align_up(tiles * 8, 256);
-    L.off_bits = o; o += align_up((size_t)n * NSCAN * 8, 256);
-    L.off_tables = o; o += align_up((size_t)n * sizeof(ProgTables), 256);
-    L.total = o;
-    return L;
+    P.tile_base[NSCAN] = tb;
+    P.blk_base[NSCAN] = bb;
 }
 
 // Measure (and with !check_only, code) the 7 scans of n frames.  Waits for the device twice: after the
@@ -476,40 +463,44 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
                        const ProgTables *T, bool per_frame, bool check_only, ProgResult *res)
 {
     cudaStream_t st = ctx->stream;
-    const ProgLayout L = prog_layout(g, n);
-    PIXO_TRY(ctx->d_prog.ensure(ctx, L.total));
-    auto *base = static_cast<uint8_t *>(ctx->d_prog.ptr);
     ProgParams P;
     memset(&P, 0, sizeof P);
+    prog_counts(g, P);
+    const size_t tiles = (size_t)n * P.tile_base[NSCAN], blocks = (size_t)n * P.blk_base[NSCAN];
+    ProgTables *d_tables;
+    PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
+        P.status = L.take<uint32_t>(1);
+        P.blen = L.take<uint32_t>(blocks);
+        P.flag = L.take(blocks);
+        P.tile_last = L.take<uint32_t>(tiles);
+        P.tile_carry = L.take<uint32_t>(tiles);
+        P.tile_bits = L.take<uint32_t>(tiles);
+        P.tile_off = L.take<unsigned long long>(tiles);
+        P.bits = L.take<unsigned long long>((size_t)n * NSCAN);
+        P.tables = d_tables = L.take<ProgTables>(n);
+    }));
     P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
     P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
-    for (int s = 0; s < NSCAN; ++s) P.nb[s] = L.nb[s];
-    for (int s = 0; s <= NSCAN; ++s) { P.tile_base[s] = L.tile_base[s]; P.blk_base[s] = L.blk_base[s]; }
     P.n = n;
-    P.status = reinterpret_cast<uint32_t *>(base + L.off_status);
-    P.blen = reinterpret_cast<uint32_t *>(base + L.off_blen);
-    P.flag = base + L.off_flag;
-    P.tile_last = reinterpret_cast<uint32_t *>(base + L.off_tile_last);
-    P.tile_carry = reinterpret_cast<uint32_t *>(base + L.off_tile_carry);
-    P.tile_bits = reinterpret_cast<uint32_t *>(base + L.off_tile_bits);
-    P.tile_off = reinterpret_cast<unsigned long long *>(base + L.off_tile_off);
-    P.bits = reinterpret_cast<unsigned long long *>(base + L.off_bits);
-    P.tables = reinterpret_cast<const ProgTables *>(base + L.off_tables);
     P.tables_per_frame = per_frame ? 1u : 0u;
-    const uint64_t tiles = (uint64_t)n * L.tile_base[NSCAN];
     if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive stage: too many blocks per call");
     PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(base + L.off_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(d_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
     if (tiles) {
         PIXO_TRY(launch(ctx, k_prog_measure, (unsigned)tiles, PT, 0, P));
         PIXO_TRY(launch(ctx, k_prog_carry, n * NSCAN, PT, 0, P));
         PIXO_TRY(launch(ctx, k_prog_count, (unsigned)tiles, PT, 0, P));
     }
     PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
+    // h_prog: the status word, every stream's bit count (then its segment's length), the splice's flags
     const size_t nstream = (size_t)n * NSCAN;
-    PIXO_TRY(ctx->h_prog.ensure(ctx, 256 + nstream * 8));
-    auto *h_status = static_cast<uint32_t *>(ctx->h_prog.ptr);
-    auto *h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
+    uint32_t *h_status, *h_ovf = nullptr;
+    uint64_t *h_bits;
+    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
+        h_status = L.take<uint32_t>(1);
+        h_bits = L.take<uint64_t>(nstream);
+        if (!check_only) h_ovf = L.take<uint32_t>(nstream);
+    }, 8));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, nstream * 8, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaStreamSynchronize(st));
@@ -521,34 +512,35 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     // raw strings, sized by the longest stream
     uint64_t max_bytes = 0;
     for (size_t q = 0; q < nstream; ++q) max_bytes = std::max<uint64_t>(max_bytes, (h_bits[q] + 7) / 8);
-    const size_t raw_cap = (size_t)((max_bytes + 16 + 255) / 256 * 256);
-    SegPlan sp = splice_plan(n * NSCAN, raw_cap);
-    const size_t stage_cap = (2 * raw_cap + 256) / 256 * 256;   // every byte 0xFF still fits
-    const size_t off_len = sp.total, off_ovf = off_len + (nstream * 8 + 255) / 256 * 256;
-    const size_t off_stage = off_ovf + (nstream * 4 + 255) / 256 * 256;
-    PIXO_TRY(ctx->d_prog_raw.ensure(ctx, sp.raw_total));
-    PIXO_TRY(ctx->d_prog_out.ensure(ctx, off_stage + nstream * stage_cap));
-    auto *raw = static_cast<uint8_t *>(ctx->d_prog_raw.ptr);
-    auto *outb = static_cast<uint8_t *>(ctx->d_prog_out.ptr);
-    PIXO_CUDA(ctx, cudaMemsetAsync(raw, 0, sp.raw_total, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(raw + sp.off_bits, P.bits, nstream * 8, cudaMemcpyDeviceToDevice, st));
-    PIXO_CUDA(ctx, cudaMemsetAsync(outb + off_ovf, 0, nstream * 4, st));
-    P.raw = reinterpret_cast<uint32_t *>(raw);
+    const size_t raw_cap = Layout::round((size_t)max_bytes + 16);
+    const SegPlan sp = splice_plan(n * NSCAN, raw_cap);
+    const size_t stage_cap = Layout::round(2 * raw_cap + 1);   // every byte 0xFF still fits
+    // d_prog_out: the splice's scratch, every segment's length and flags, the segments
+    uint8_t *scratch, *stage;
+    uint64_t *d_len;
+    uint32_t *d_ovf;
+    PIXO_TRY(bind(ctx, ctx->d_prog_out, [&](Layout &L) {
+        scratch = L.take(seg_scratch_bytes(sp));
+        d_len = L.take<uint64_t>(nstream);
+        d_ovf = L.take<uint32_t>(nstream);
+        stage = L.take(nstream * stage_cap);
+    }));
+    PIXO_TRY(ctx->d_prog_raw.ensure(ctx, seg_raw(sp, nullptr).total));
+    const SegRaw raw = seg_raw(sp, ctx->d_prog_raw.ptr);
+    PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, raw.total, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(raw.bits, P.bits, nstream * 8, cudaMemcpyDeviceToDevice, st));
+    PIXO_CUDA(ctx, cudaMemsetAsync(d_ovf, 0, nstream * 4, st));
+    P.raw = reinterpret_cast<uint32_t *>(raw.strings);
     P.raw_words = raw_cap / 4;
     if (tiles) PIXO_TRY(launch(ctx, k_prog_emit, (unsigned)tiles, PT, 0, P));
-    auto *d_len = reinterpret_cast<uint64_t *>(outb + off_len);
-    auto *d_ovf = reinterpret_cast<uint32_t *>(outb + off_ovf);
-    PIXO_TRY(launch_splice(ctx, n * NSCAN, sp, outb, raw, outb + off_stage, stage_cap, d_len, d_ovf));
-    PIXO_TRY(ctx->h_prog.ensure(ctx, 256 + nstream * 12));
-    h_bits = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(ctx->h_prog.ptr) + 256);
-    auto *h_ovf = reinterpret_cast<uint32_t *>(h_bits + nstream);
+    PIXO_TRY(launch_splice(ctx, sp, scratch, raw.strings, stage, stage_cap, d_len, d_ovf));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, d_len, nstream * 8, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, nstream * 4, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaStreamSynchronize(st));
     res->len.assign(h_bits, h_bits + nstream);
     for (size_t q = 0; q < nstream; ++q)
         if (h_ovf[q]) return set_error(ctx, PIXO_B200_ERR_CUDA, "progressive splice overflowed its exact-size buffer");
-    res->stage = outb + off_stage;
+    res->stage = stage;
     res->stage_cap = stage_cap;
     res->d_len = d_len;
     return 0;

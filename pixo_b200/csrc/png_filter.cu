@@ -992,13 +992,16 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
     const size_t segcap = row_bytes + 15 < (size_t)SEG_BYTES ? ((row_bytes + 15) & ~(size_t)15) : (size_t)SEG_BYTES;
     const Smem smem{2 * (16 + segcap) + segcap + 32 + 8192,   // + bigram "seen" bitmap
                     2 * (16 + (size_t)SEG_BYTES) + SEG_BYTES + 32 + 8192};
-    // misc scratch: per image {accA, accB} u64, counter u32, decided u8
-    const size_t per = 2 * sizeof(unsigned long long) + sizeof(uint32_t) + 4;
-    PIXO_TRY(ctx->d_misc.ensure(ctx, (size_t)n_images * per + 64));
-    auto *acc = reinterpret_cast<unsigned long long *>(ctx->d_misc.ptr);
-    auto *counter = reinterpret_cast<uint32_t *>(acc + 2 * (size_t)n_images);
-    auto *decided = reinterpret_cast<uint8_t *>(counter + n_images);
-    PIXO_CUDA(ctx, cudaMemsetAsync(ctx->d_misc.ptr, 0, (size_t)n_images * per + 64, ctx->stream));
+    // misc scratch, cleared: per image {accA, accB}, a counter and the decided filter
+    unsigned long long *acc;
+    uint32_t *counter;
+    uint8_t *decided;
+    size_t misc_bytes;
+    PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &L) {
+        acc = L.take<unsigned long long>(2 * (size_t)n_images), counter = L.take<uint32_t>(n_images);
+        decided = L.take(n_images), misc_bytes = L.end();
+    }, 8));
+    PIXO_CUDA(ctx, cudaMemsetAsync(acc, 0, misc_bytes, ctx->stream));
 
     if (use_band) {
         const auto band = oa == 4 ? k_png_band<4> : oa == 2 ? k_png_band<2> : k_png_band<0>;
@@ -1055,10 +1058,10 @@ int launch_png_filter_rows(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_
 
 int launch_adler32(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32_t *d_out)
 {
-    PIXO_TRY(ctx->d_misc.ensure(ctx, 64));
-    auto *acc = reinterpret_cast<unsigned long long *>(ctx->d_misc.ptr);
-    auto *counter = reinterpret_cast<uint32_t *>(acc + 2);
-    PIXO_CUDA(ctx, cudaMemsetAsync(ctx->d_misc.ptr, 0, 64, ctx->stream));
+    unsigned long long *acc;   // {accA, accB}, then the counter, cleared
+    uint32_t *counter;
+    PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &L) { acc = L.take<unsigned long long>(2), counter = L.take<uint32_t>(1); }, 8));
+    PIXO_CUDA(ctx, cudaMemsetAsync(acc, 0, 2 * sizeof *acc + sizeof *counter, ctx->stream));
     size_t nvec = len / 16 + 1;
     uint32_t grid = (uint32_t)((nvec + 256 * 8 - 1) / (256 * 8));
     const uint32_t cap = (uint32_t)ctx->sm_count * 8;

@@ -396,17 +396,19 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         PIXO_CUDA(ctx, cub::DeviceRunLengthEncode::Encode(nullptr, tmp_rle, (const unsigned long long *)nullptr,
                                                           (unsigned long long *)nullptr, (uint32_t *)nullptr,
                                                           (uint32_t *)nullptr, (int)maxk, ctx->stream));
-        const size_t off_b = align_up(maxk * 8, 256), off_u = off_b + align_up(maxk * 8, 256), off_c = off_u + align_up(maxk * 8, 256);
-        const size_t off_n = off_c + align_up(maxk * 4, 256), off_t = off_n + 256;
-        PIXO_TRY(ctx->d_quant.ensure(ctx, off_t + std::max(tmp_sort, tmp_rle)));
-        PIXO_TRY(ctx->h_quant.ensure(ctx, maxk * 12 + 16));
-        auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant.ptr);
-        auto *ka = reinterpret_cast<unsigned long long *>(base), *kb = reinterpret_cast<unsigned long long *>(base + off_b);
-        auto *uq = reinterpret_cast<unsigned long long *>(base + off_u);
-        auto *cn = reinterpret_cast<uint32_t *>(base + off_c), *nr = reinterpret_cast<uint32_t *>(base + off_n);
-        auto *h_uq = reinterpret_cast<unsigned long long *>(ctx->h_quant.ptr);
-        auto *h_cn = reinterpret_cast<uint32_t *>(h_uq + maxk);
-        auto *h_nr = h_cn + maxk;
+        // d_quant: the sample keys, sorted, the runs' keys and counts, the run count, cub's temporary storage;
+        // h_quant: the runs' keys and counts, the run count
+        unsigned long long *ka, *kb, *uq, *h_uq;
+        uint32_t *cn, *nr, *h_cn, *h_nr;
+        uint8_t *tmp;
+        PIXO_TRY(bind(ctx, ctx->d_quant, [&](Layout &L) {
+            ka = L.take<unsigned long long>(maxk), kb = L.take<unsigned long long>(maxk);
+            uq = L.take<unsigned long long>(maxk), cn = L.take<uint32_t>(maxk), nr = L.take<uint32_t>(1);
+            tmp = L.take(std::max(tmp_sort, tmp_rle));
+        }));
+        PIXO_TRY(bind(ctx, ctx->h_quant, [&](Layout &L) {
+            h_uq = L.take<unsigned long long>(maxk), h_cn = L.take<uint32_t>(maxk), h_nr = L.take<uint32_t>(1);
+        }, 8));
         for (uint32_t i0 = 0; i0 < n_images; i0 += chunk) {
             const uint32_t nb = std::min(chunk, n_images - i0);
             const int nk = (int)(nb * per);
@@ -416,9 +418,9 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
             const uint32_t ctas = (uint32_t)std::min<uint64_t>(((uint64_t)nk + Q_THREADS - 1) / Q_THREADS, (uint64_t)ctx->sm_count * 16);
             PIXO_TRY(launch(ctx, k_quant_sample, ctas, Q_THREADS, 0, S));
             size_t tb = tmp_sort;
-            PIXO_CUDA(ctx, cub::DeviceRadixSort::SortKeys(base + off_t, tb, ka, kb, nk, 0, 39, ctx->stream));
+            PIXO_CUDA(ctx, cub::DeviceRadixSort::SortKeys(tmp, tb, ka, kb, nk, 0, 39, ctx->stream));
             tb = tmp_rle;
-            PIXO_CUDA(ctx, cub::DeviceRunLengthEncode::Encode(base + off_t, tb, kb, uq, cn, nr, nk, ctx->stream));
+            PIXO_CUDA(ctx, cub::DeviceRunLengthEncode::Encode(tmp, tb, kb, uq, cn, nr, nk, ctx->stream));
             PIXO_CUDA(ctx, cudaMemcpyAsync(h_nr, nr, 4, cudaMemcpyDeviceToHost, ctx->stream));
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             const uint32_t runs = *h_nr;
@@ -465,24 +467,31 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
 
     std::vector<uint32_t> qall;
     for (uint32_t i = 0; i < n_images; ++i) if (kind[i] != LOSSLESS) qall.push_back(i);
-    const size_t idx_stride = align_up(npix, 256);
+    const size_t idx_stride = Layout::round(npix);
     // steps 3-5 in passes of at most QUANT_PASS quantised images: every grid.y stays within CUDA's limit
     // and the scratch (about 330 KB per image besides its indices) does not grow with the batch
     for (size_t q0 = 0; q0 < qall.size(); q0 += QUANT_PASS) {
         const std::vector<uint32_t> qids(qall.begin() + q0, qall.begin() + std::min(qall.size(), q0 + QUANT_PASS));
         const size_t nq = qids.size();
         // 3. k-means, tables, map / dither on the device
-        const size_t o_jobs = 0, jobs_bytes = align_up(nq * (sizeof(KmeansJob) + sizeof(LutJob) + sizeof(MapJob) + sizeof(DitherJob)) + 1024, 256);
-        const size_t o_pal = jobs_bytes, o_acc = o_pal + align_up(nq * 256 * 4, 256), o_col = o_acc + align_up(nq * 256 * 5 * 8, 256);
-        const size_t o_lut = o_col + align_up(nq * MAX_HIST_COLORS * 8, 256), groups = (height + 31) / 32;
-        const size_t o_edge = o_lut + align_up(nq * LUT_CELLS, 256), o_prog = o_edge + align_up(nq * (groups - 1 + 1) * width * 4, 256);
-        const size_t o_tick = o_prog + align_up(nq * groups * 4, 256), o_idx = o_tick + 256;
-        PIXO_TRY(ctx->d_quant_img.ensure(ctx, o_idx + nq * idx_stride));
-        auto *base = reinterpret_cast<uint8_t *>(ctx->d_quant_img.ptr);
-        auto *d_pal = reinterpret_cast<uint32_t *>(base + o_pal);
-        auto *d_acc = reinterpret_cast<unsigned long long *>(base + o_acc);
-        auto *d_col = reinterpret_cast<uint32_t *>(base + o_col);
-        uint8_t *d_idx = base + o_idx;
+        const size_t jobs_bytes = nq * (sizeof(KmeansJob) + sizeof(LutJob) + sizeof(MapJob) + sizeof(DitherJob)) + 1024;
+        const size_t groups = (height + 31) / 32;
+        // d_quant_img: the jobs, palettes, k-means sums, histogram colours, tables, dither edges and progress, the
+        // dither ticket, the indices
+        uint8_t *d_jobs, *d_lut, *d_idx;
+        uint32_t *d_pal, *d_col, *d_edge, *d_prog, *d_tick;
+        unsigned long long *d_acc;
+        PIXO_TRY(bind(ctx, ctx->d_quant_img, [&](Layout &L) {
+            d_jobs = L.take(jobs_bytes);
+            d_pal = L.take<uint32_t>(nq * 256);
+            d_acc = L.take<unsigned long long>(nq * 256 * 5);
+            d_col = L.take<uint32_t>(nq * MAX_HIST_COLORS * 2);
+            d_lut = L.take(nq * LUT_CELLS);
+            d_edge = L.take<uint32_t>(nq * groups * width);
+            d_prog = L.take<uint32_t>(nq * groups);
+            d_tick = L.take<uint32_t>(1);
+            d_idx = L.take(nq * idx_stride);
+        }));
         std::vector<uint32_t> h_pal(nq * 256, 0);
         std::vector<uint32_t> h_col;   // each k-means job's histogram colours then counts, packed
         std::vector<KmeansJob> km;
@@ -501,17 +510,17 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
                 km.push_back({cc, cc + hcol[i].size(), (uint32_t)hcol[i].size(), (uint32_t)pal[i].size(), dp, d_acc + k * 256 * 5});
                 max_cols = std::max(max_cols, (uint32_t)hcol[i].size());
             }
-            uint8_t *lut = base + o_lut + k * LUT_CELLS;
+            uint8_t *lut = d_lut + k * LUT_CELLS;
             if (kind[i] == LUT) lj.push_back({dp, (uint32_t)pal[i].size(), lut});
             MapJob M{d_data + (size_t)i * in_stride, d_idx + k * idx_stride, kind[i] == LUT ? lut : nullptr, dp,
                      (uint32_t)pal[i].size()};
             if (kind[i] == LUT && dither)
-                dj.push_back({M.src, M.idx, lut, dp, M.npal, reinterpret_cast<uint32_t *>(base + o_edge) + k * groups * width,
-                              reinterpret_cast<uint32_t *>(base + o_prog) + k * groups});
+                dj.push_back({M.src, M.idx, lut, dp, M.npal, d_edge + k * groups * width,
+                              d_prog + k * groups});
             else
                 mj.push_back(M);
         }
-        auto *d_km = reinterpret_cast<KmeansJob *>(base + o_jobs);
+        auto *d_km = reinterpret_cast<KmeansJob *>(d_jobs);
         auto *d_lj = reinterpret_cast<LutJob *>(d_km + km.size());
         auto *d_mj = reinterpret_cast<MapJob *>(d_lj + lj.size());
         auto *d_dj = reinterpret_cast<DitherJob *>(d_mj + mj.size());
@@ -522,7 +531,7 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
         put(lj.data(), lj.size() * sizeof(LutJob));
         put(mj.data(), mj.size() * sizeof(MapJob));
         put(dj.data(), dj.size() * sizeof(DitherJob));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(base, jobs.data(), o, cudaMemcpyHostToDevice, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs.data(), o, cudaMemcpyHostToDevice, ctx->stream));
         PIXO_CUDA(ctx, cudaMemcpyAsync(d_pal, h_pal.data(), nq * 256 * 4, cudaMemcpyHostToDevice, ctx->stream));
         if (!km.empty()) {
             PIXO_CUDA(ctx, cudaMemcpyAsync(d_col, h_col.data(), h_col.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -541,9 +550,8 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
             const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, (npix + Q_THREADS * MAP_PX - 1) / (Q_THREADS * MAP_PX)));
             PIXO_TRY(launch(ctx, k_quant_map, dim3(ctas, (uint32_t)mj.size()), Q_THREADS, 0, d_mj, npix, bpp));
         }
-        uint32_t *d_tick = reinterpret_cast<uint32_t *>(base + o_tick);
         if (!dj.empty()) {
-            PIXO_CUDA(ctx, cudaMemsetAsync(base + o_prog, 0, nq * groups * 4, ctx->stream));
+            PIXO_CUDA(ctx, cudaMemsetAsync(d_prog, 0, nq * groups * 4, ctx->stream));
             PIXO_CUDA(ctx, cudaMemsetAsync(d_tick, 0, 8, ctx->stream));
             bool &carveout_set = ctx->kernels[reinterpret_cast<const void *>(k_quant_dither)].carveout_set;
             if (!carveout_set) {

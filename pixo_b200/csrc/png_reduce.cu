@@ -396,14 +396,15 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
     }
     const size_t cnt_words = 256 + TRI_MAX;
     std::vector<uint8_t> maps(pal_ids.size() * 256, 0);
+    uint8_t *d_idx = nullptr;   // every palette image's indices, npix each
     if (!pal_ids.empty()) {
         const size_t np = pal_ids.size();
-        const size_t jobs_off = (np * npix + 255) & ~(size_t)255;
-        const size_t cnt_off = jobs_off + ((np * sizeof(IndexJob) + 255) & ~(size_t)255);
-        PIXO_TRY(ctx->d_red_idx.ensure(ctx, cnt_off + np * cnt_words * 4));
-        auto *base = reinterpret_cast<uint8_t *>(ctx->d_red_idx.ptr);
-        auto *d_jobs = reinterpret_cast<IndexJob *>(base + jobs_off);
-        auto *d_cnt = reinterpret_cast<uint32_t *>(base + cnt_off);
+        // d_red_idx: the indices, the jobs, the counts
+        IndexJob *d_jobs;
+        uint32_t *d_cnt;
+        PIXO_TRY(bind(ctx, ctx->d_red_idx, [&](Layout &L) {
+            d_idx = L.take(np * npix), d_jobs = L.take<IndexJob>(np), d_cnt = L.take<uint32_t>(np * cnt_words);
+        }));
         std::vector<IndexJob> jobs(np);
         uint32_t nmax = 0;
         bool any_stats = false;
@@ -412,7 +413,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
             IndexJob &J = jobs[k];
             memset(&J, 0, sizeof J);
             J.src = d_data + (size_t)i * in_stride;
-            J.idx = base + k * npix;
+            J.idx = d_idx + k * npix;
             J.counts = d_cnt + k * cnt_words;
             J.n = (uint32_t)keys[i].size();
             J.stats = J.n > 2;
@@ -478,7 +479,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         switch (kind[i]) {
         case PALETTE:
             J.mode = PACK_PALETTE; J.bits = bits[i];
-            J.src = reinterpret_cast<const uint8_t *>(ctx->d_red_idx.ptr) + pal_k * npix;
+            J.src = d_idx + pal_k * npix;
             memcpy(J.map, &maps[pal_k * 256], 256);
             ++pal_k;
             r.color_type_byte = 3; r.effective_color_type = PIXO_B200_RGB; r.bytes_per_pixel = 1;
@@ -505,14 +506,15 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
     }
     if (!pack.empty()) {
         const size_t jobs_bytes = pack.size() * sizeof(PackJob);
-        const size_t img_off = (jobs_bytes + 255) & ~(size_t)255;
-        PIXO_TRY(ctx->d_red_img.ensure(ctx, img_off + (size_t)n_images * red_stride));
-        auto *base = reinterpret_cast<uint8_t *>(ctx->d_red_img.ptr);
-        d_red_img = base + img_off;
+        // d_red_img: the jobs, the reduced rows
+        PackJob *d_jobs;
+        PIXO_TRY(bind(ctx, ctx->d_red_img, [&](Layout &L) {
+            d_jobs = L.take<PackJob>(pack.size()), d_red_img = L.take((size_t)n_images * red_stride);
+        }));
         for (size_t k = 0; k < pack.size(); ++k) pack[k].dst = d_red_img + (size_t)pack_img[k] * red_stride;
-        PIXO_CUDA(ctx, cudaMemcpyAsync(base, pack.data(), jobs_bytes, cudaMemcpyHostToDevice, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(d_jobs, pack.data(), jobs_bytes, cudaMemcpyHostToDevice, ctx->stream));
         PackParams K;
-        K.jobs = reinterpret_cast<const PackJob *>(base);
+        K.jobs = d_jobs;
         K.width = width; K.height = height; K.bpp = bpp;
         uint64_t most = 0;
         for (const PackJob &J : pack) most = std::max<uint64_t>(most, J.row_bytes * height);
@@ -521,7 +523,7 @@ int png_reduce_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_strid
         ctas = std::max(ctas, 1u);
         for (size_t k0 = 0; k0 < pack.size(); k0 += 65535) {
             const uint32_t nb = (uint32_t)std::min<size_t>(pack.size() - k0, 65535);
-            K.jobs = reinterpret_cast<const PackJob *>(base) + k0;
+            K.jobs = d_jobs + k0;
             PIXO_TRY(launch(ctx, k_reduce_pack, dim3(ctas, nb), RED_THREADS, 0, K));
         }
     }

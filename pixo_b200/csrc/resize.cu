@@ -254,41 +254,49 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
     ResizeAxis h, v;
     resize_axis(sw, dw, true, h);
     resize_axis(sh, dh, true, v);
-    // tables: h start/count, v start/count (u32), h/v offsets (u64), h/v weights (f32), each 256-aligned
-    const size_t o_hs = 0, o_hc = o_hs + align_up(4 * (size_t)dw, 256), o_vs = o_hc + align_up(4 * (size_t)dw, 256),
-                 o_vc = o_vs + align_up(4 * (size_t)dh, 256), o_ho = o_vc + align_up(4 * (size_t)dh, 256), o_vo = o_ho + align_up(8 * (size_t)dw, 256),
-                 o_hw = o_vo + align_up(8 * (size_t)dh, 256), o_vw = o_hw + align_up(4 * h.w.size() + 4, 256),
-                 total = o_vw + align_up(4 * v.w.size() + 4, 256);
-    PIXO_TRY(ctx->d_resize.ensure(ctx, total));
-    uint8_t *T = reinterpret_cast<uint8_t *>(ctx->d_resize.ptr);
-    const struct { size_t off; const void *p; size_t bytes; } up[] = {
-        {o_hs, h.start.data(), 4 * (size_t)dw}, {o_hc, h.count.data(), 4 * (size_t)dw},
-        {o_vs, v.start.data(), 4 * (size_t)dh}, {o_vc, v.count.data(), 4 * (size_t)dh},
-        {o_ho, h.offset.data(), 8 * (size_t)dw}, {o_vo, v.offset.data(), 8 * (size_t)dh},
-        {o_hw, h.w.data(), 4 * h.w.size()},      {o_vw, v.w.data(), 4 * v.w.size()}};
+    // tables: h start/count, v start/count (u32), h/v offsets (u64), h/v weights (f32), laid out alike in the
+    // pinned upload buffer (H) and on the device (T)
+    struct Tables {
+        uint32_t *hs, *hc, *vs, *vc;
+        uint64_t *ho, *vo;
+        float *hw, *vw;
+        size_t bytes;
+    } T, H;
+    auto tables = [&](Tables &t) {
+        return [&](Layout &L) {
+            t.hs = L.take<uint32_t>(dw), t.hc = L.take<uint32_t>(dw), t.vs = L.take<uint32_t>(dh), t.vc = L.take<uint32_t>(dh);
+            t.ho = L.take<uint64_t>(dw), t.vo = L.take<uint64_t>(dh);
+            t.hw = L.take<float>(h.w.size() + 1), t.vw = L.take<float>(v.w.size() + 1);
+            t.bytes = L.end();
+        };
+    };
+    PIXO_TRY(bind(ctx, ctx->d_resize, tables(T)));
     // One copy from one of the context's two pinned buffers, in turn.  A copy from the pageable vectors
     // lets the driver wait for the stream before the call returns (it does for some MB of tables); a
     // pinned one is only queued.  A buffer is rewritten once the copy out of it, two uploads back, has run.
     const int slot = (int)(ctx->resize_uploads % 2);
     PIXO_CUDA(ctx, cudaEventSynchronize(ctx->resize_events[slot]));
-    PIXO_TRY(ctx->h_resize[slot].ensure(ctx, total));
-    uint8_t *H = reinterpret_cast<uint8_t *>(ctx->h_resize[slot].ptr);
+    PIXO_TRY(bind(ctx, ctx->h_resize[slot], tables(H)));
+    const struct { void *dst; const void *src; size_t bytes; } up[] = {
+        {H.hs, h.start.data(), 4 * (size_t)dw}, {H.hc, h.count.data(), 4 * (size_t)dw},
+        {H.vs, v.start.data(), 4 * (size_t)dh}, {H.vc, v.count.data(), 4 * (size_t)dh},
+        {H.ho, h.offset.data(), 8 * (size_t)dw}, {H.vo, v.offset.data(), 8 * (size_t)dh},
+        {H.hw, h.w.data(), 4 * h.w.size()},      {H.vw, v.w.data(), 4 * v.w.size()}};
     for (const auto &u : up)
-        if (u.bytes) memcpy(H + u.off, u.p, u.bytes);
-    PIXO_CUDA(ctx, cudaMemcpyAsync(T, H, total, cudaMemcpyHostToDevice, ctx->stream));
+        if (u.bytes) memcpy(u.dst, u.src, u.bytes);
+    PIXO_CUDA(ctx, cudaMemcpyAsync(T.hs, H.hs, T.bytes, cudaMemcpyHostToDevice, ctx->stream));
     PIXO_CUDA(ctx, cudaEventRecord(ctx->resize_events[slot], ctx->stream));
     ctx->resize_uploads++;
-    const uint32_t *hs = reinterpret_cast<const uint32_t *>(T + o_hs), *hc = reinterpret_cast<const uint32_t *>(T + o_hc);
-    const uint32_t *vs = reinterpret_cast<const uint32_t *>(T + o_vs), *vc = reinterpret_cast<const uint32_t *>(T + o_vc);
-    const uint64_t *ho = reinterpret_cast<const uint64_t *>(T + o_ho), *vo = reinterpret_cast<const uint64_t *>(T + o_vo);
-    const float *hw = reinterpret_cast<const float *>(T + o_hw), *vw = reinterpret_cast<const float *>(T + o_vw);
+    const uint32_t *hs = T.hs, *hc = T.hc, *vs = T.vs, *vc = T.vc;
+    const uint64_t *ho = T.ho, *vo = T.vo;
+    const float *hw = T.hw, *vw = T.vw;
 
     const std::vector<Band> bands = lanczos_bands(v, sh, dw, dh, BPP, kResizeScratch);
     size_t most = 1;  // intermediate bytes of the largest band
     for (const Band &b : bands) most = std::max(most, (size_t)(b.re - b.rs) * b.cw * BPP);
     // frames per pass: as many whole intermediates as the cap holds (only when one band covers the frame)
     const uint32_t per_pass = bands.size() == 1 ? (uint32_t)std::min<size_t>({n, 65535, std::max<size_t>(1, kResizeScratch / most)}) : 1;
-    const size_t tstride = (most + 255) / 256 * 256;
+    const size_t tstride = Layout::round(most);
     PIXO_TRY(ctx->d_resize_tmp.ensure(ctx, tstride * per_pass));
     uint8_t *tmp = reinterpret_cast<uint8_t *>(ctx->d_resize_tmp.ptr);
     for (uint32_t f0 = 0; f0 < n; f0 += per_pass) {

@@ -127,4 +127,71 @@ for ct in range(4):
             ctx.sync()
 tall = rng.integers(0, 256, 16 * 70000 * 4, dtype=np.uint8)
 rs.resize(tall, rs.ResizeOptions.builder(16, 70000).dst(1000, 3).algorithm(rs.ResizeAlgorithm.Lanczos3).build(), ctx=ctx)
+# ---- the stages whose scratch layouts go through pixo::Layout and no earlier part reaches: PNG quantisation
+# (Auto, Force, dither, a given palette; host and device entry points), COEF_TRELLIS and the trellis entry
+# point, device encodes with optimised tables and a restart interval, the device entropy entry point with
+# optimised tables, and the stream-ordered band flow on one rank ---------------------------------------------
+from pixo_b200.png import QuantizationMode  # noqa: E402
+for (ww, hh) in ((70, 33), (300, 40)):
+    cols = rng.integers(0, 256, (500, 4), dtype=np.uint8)
+    px = cols[rng.integers(0, 500, ww * hh)].reshape(-1)
+    pal = rng.integers(0, 256, (16, 4), dtype=np.uint8)
+    for mode, dith in ((QuantizationMode.Auto, False), (QuantizationMode.Force, False), (QuantizationMode.Force, True)):
+        o = PngOptions(ww, hh, ColorType.Rgba, FilterStrategy.Adaptive, True, True, True, mode, 64, dith)
+        png.quantize_and_filter(px, o, ctx=ctx)
+        png.quantize_and_filter(px, o, palette=pal, ctx=ctx)
+    d_px = torch.from_numpy(np.concatenate([px, px])).to(dev)
+    d_out = torch.empty(2 * hh * (ww * 4 + 1), dtype=torch.uint8, device=dev)
+    d_ad = torch.zeros(2, dtype=torch.int32, device=dev)
+    torch.cuda.synchronize(dev)
+    o = PngOptions(ww, hh, ColorType.Rgba, FilterStrategy.Adaptive, True, True, True, QuantizationMode.Force, 64, True)
+    png.quantize_and_filter_dev(d_px, px.size, 2, o, d_out, hh * (ww * 4 + 1), d_ad, palettes=[None, pal], ctx=ctx)
+    ctx.sync()
+im = synthetic.noise(333, 222, 3, 6)
+jpeg.compute_all_coefficients(im, 333, 222, ColorType.Rgb, Subsampling.S420, 80, ctx=ctx, use_trellis=True)
+jpeg.compute_all_coefficients(im[: 333 * 222], 333, 222, ColorType.Gray, Subsampling.S444, 90, ctx=ctx, use_trellis=True)
+d_dct = torch.from_numpy(rng.normal(0, 200, (5000, 64)).astype(np.float32)).to(dev)
+torch.cuda.synchronize(dev)
+jpeg.trellis_quantize_dev(d_dct, np.full(64, 16, np.float32), ctx=ctx)
+ctx.sync()
+ww, hh, nf, cap = 640, 480, 3, 2 << 20
+d_fr = torch.from_numpy(np.stack([synthetic.noise(ww, hh, 3, k) for k in range(nf)]).reshape(-1)).to(dev)
+d_scan = torch.empty(nf * cap, dtype=torch.uint8, device=dev)
+d_len = torch.zeros(nf, dtype=torch.int64, device=dev)
+d_ovf = torch.zeros(nf, dtype=torch.int32, device=dev)
+d_dht = torch.empty(nf * jpeg.DHT_BYTES, dtype=torch.uint8, device=dev)
+torch.cuda.synchronize(dev)
+for rst, opt in ((5, True), (None, True), (5, False)):
+    jpeg.encode_dev(d_fr, ww * hh * 3, nf, JpegOptions(ww, hh, ColorType.Rgb, 80, Subsampling.S420, rst, opt), d_scan, cap,
+                    d_len, d_ovf, d_dht, ctx=ctx)
+ctx.sync()
+coef = [torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        for a in jpeg.compute_all_coefficients(im, 333, 222, ColorType.Rgb, Subsampling.S420, 80, ctx=ctx)]
+torch.cuda.synchronize(dev)
+for rst in (None, 4):
+    jpeg.entropy_encode_dev(*coef, JpegOptions(333, 222, ColorType.Rgb, 80, Subsampling.S420, rst, True), ctx=ctx)
+fw, fh = 1024, 512
+frame = synthetic.noise(fw, fh, 3, 12)
+want = jpeg.encode(frame, JpegOptions(fw, fh, ColorType.Rgb, 80, Subsampling.S420), ctx=ctx)
+for S in ("1", "3"):
+    os.environ["PIXO_B200_SEGMENTS"] = S
+    b = parallel.plan_bands(fw, fh, 1)[0]
+    d_y = torch.empty((b.y_blocks, 64), dtype=torch.int16, device=dev)
+    d_cb = torch.empty((b.c_blocks, 64), dtype=torch.int16, device=dev)
+    d_cr = torch.empty_like(d_cb)
+    px = torch.from_numpy(np.ascontiguousarray(frame).reshape(-1)).to(dev)
+    stream = torch.cuda.Stream(dev)
+    torch.cuda.synchronize(dev)
+    with torch.cuda.stream(stream):
+        ctx.set_stream(stream.cuda_stream)
+        _lib.check(ctx.handle, lib.pixo_b200_jpeg_coefficients_dev(
+            ctx.handle, px.data_ptr(), px.numel(), 1, fw, fh, 2, 1, lq.ctypes.data_as(_lib.f32p), cq.ctypes.data_as(_lib.f32p),
+            d_y.data_ptr(), b.y_blocks * 64, d_cb.data_ptr(), d_cr.data_ptr(), b.c_blocks * 64, 0, None))
+        coder = parallel.DeviceBandCoder(ctx, d_y, d_cb, d_cr, fw, fh, 2, 1, b.y_blocks, b.c_blocks)
+        parts, _ = parallel.tiled_scan_parts_async(coder, [True], 0, 1)
+        got = parallel.assemble_tiled(parts, None, fw, fh, 2, 80, 1)
+        stream.synchronize()
+    ctx.set_stream(None)
+    assert got == want, ("stream-ordered band", S)
+del os.environ["PIXO_B200_SEGMENTS"]
 print("tour done")
