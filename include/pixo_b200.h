@@ -14,7 +14,8 @@
  *    context's stream: after the work queued on it before the call, before the work queued after.
  *    These return with their work still queued (a call that grows the context's scratch first
  *    waits for the stream once, to free the smaller buffer):
- *      jpeg_coefficients_dev (without PIXO_B200_COEF_TRELLIS), jpeg_encode_dev, jpeg_encode_dev_opts, png_filter_dev,
+ *      jpeg_coefficients_dev (without PIXO_B200_COEF_TRELLIS), jpeg_encode_dev, jpeg_encode_dev_opts,
+ *      jpeg_encode_dev_progressive, png_filter_dev,
  *      png_filter_rows_dev, adler32_dev, resize_dev, jpeg_band_histogram_dev,
  *      jpeg_band_entropy_dev_async, jpeg_band_splice_dev_async.
  *    (resize_dev with Lanczos3 stages its weight tables in one of the context's two pinned buffers,
@@ -274,6 +275,34 @@ int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, 
                                    uint32_t optimize_huffman, uint8_t *d_scan, size_t scan_cap_each,
                                    uint64_t *d_scan_len, uint32_t *d_overflow, uint8_t *d_dht);
 
+/* pixo's max preset for device frames: pixo_b200_jpeg_encode_progressive_batch's scans without a host in the
+ * loop.  Frame i at d_pixels + i*pixel_stride -> its 7 stuffed, 1-padded segments (simple_progressive_script's
+ * scans, in order) back to back at d_out + i*out_cap_each, their lengths in d_scan_len[i*7 + s] and, when d_dht
+ * (device, may be NULL) is given, the tables they were coded with at d_dht + i*1088 (pixo_b200_jpeg_encode_dev_opts'
+ * layout; standard ones unless optimize_huffman).  Segments and tables are exactly what
+ * pixo_b200_jpeg_encode_progressive_batch writes for the same pixels and options, quirks included (see
+ * pixo_b200_jpeg_encode_progressive); pixo_b200_jpeg_progressive_file(frame i's tables, its segments, its
+ * lengths) is that call's file.
+ * Queued on the context's stream like pixo_b200_jpeg_encode_dev_opts: nothing waits for the device except growth
+ * of the context's scratch.  What the host entry point learns by waiting is a bit of d_overflow[i]:
+ *   bit 0   the segments did not fit out_cap_each; nothing was written in the frame's slot, and d_scan_len holds
+ *           lengths whose sum is enough for a second call (the exact ones when the frame's raw bits fit the slot,
+ *           twice each segment's unstuffed bytes otherwise)
+ *   bit 4   input the trellis or the progressive stage cannot carry (a frame of 8-bit pixels never reaches it); set on
+ *           every frame coded in the same pass, with nothing written in their slots
+ * Checks, in this order, each before anything is launched: quality and restart_interval (as pixo_b200_jpeg_encode),
+ * the geometry, null d_pixels / d_out / d_scan_len / d_overflow (PIXO_B200_ERR_INVALID_ARGUMENT), n_images 0 returns
+ * at once, more than 65535 frames and a d_scan_len not 8-byte aligned or a d_overflow not 4-byte aligned are
+ * PIXO_B200_ERR_INVALID_ARGUMENT.  d_pixels and d_out may sit at any byte.  Frames go through in passes of at most
+ * 8192, each holding a raw string of out_cap_each + 16 bytes per frame and the frames' coefficients in the context's
+ * scratch, at most 512 MiB of each (one frame at least); see DESIGN.md section 7. */
+int pixo_b200_jpeg_encode_dev_progressive(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                                          uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                          uint32_t quality, uint32_t subsampling, uint32_t restart_interval,
+                                          uint32_t optimize_huffman, uint32_t trellis_quant, uint8_t *d_out,
+                                          size_t out_cap_each, uint64_t *d_scan_len, uint32_t *d_overflow,
+                                          uint8_t *d_dht);
+
 /* Entropy-code caller-provided coefficient arrays (host) into a baseline JPEG: the host half of
  * pixo_b200_jpeg_encode on its own (src/jpeg/mod.rs:395-447,1408-1563 consuming arrays shaped
  * like compute_all_coefficients' result).  Host-only, no device needed.
@@ -390,6 +419,18 @@ int pixo_b200_jpeg_write_headers(uint32_t width, uint32_t height, uint32_t color
 int pixo_b200_jpeg_write_headers_dht(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
                                      uint32_t subsampling, uint32_t restart_interval, const uint8_t *dht,
                                      uint8_t *out, size_t out_cap, size_t *out_len);
+
+/* A whole progressive file from one frame's scans (host memory): SOI, APP0, DQT, SOF2, DHT of `dht` (1088 bytes in
+ * pixo_b200_jpeg_encode_dev_opts' layout, NULL = the standard tables), DRI when restart_interval != 0, then per
+ * scan s of simple_progressive_script its SOS and scan_len[s] bytes of `segments` (the 7 segments back to back, as
+ * pixo_b200_jpeg_encode_dev_progressive and pixo_b200_jpeg_progressive_scans_dev leave them in a slot), then EOI.
+ * For the segments and tables of pixo_b200_jpeg_encode_progressive it is the file that call writes.  The tables are
+ * checked as pixo_b200_jpeg_write_headers_dht checks them; PIXO_B200_ERR_OUTPUT_TOO_SMALL when out_cap is below the
+ * file's length.  Host-only. */
+int pixo_b200_jpeg_progressive_file(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                    uint32_t subsampling, uint32_t restart_interval, const uint8_t *dht,
+                                    const uint8_t *segments, const uint64_t scan_len[7], uint8_t *out, size_t out_cap,
+                                    size_t *out_len);
 
 /* ---- PNG -------------------------------------------------------------------------------- */
 

@@ -73,6 +73,9 @@ SYMBOLS = {
     "pixo_b200_jpeg_encode_dev_opts": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, C.c_size_t, vp,
                                                  vp, vp]),
+    "pixo_b200_jpeg_encode_dev_progressive": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                        C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                        C.c_uint32, vp, C.c_size_t, vp, vp, vp]),
     "pixo_b200_jpeg_entropy_encode": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32,
                                                 C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp,
                                                 C.c_size_t, szp]),
@@ -98,6 +101,8 @@ SYMBOLS = {
                                                u64p, vp, C.c_size_t, szp]),
     "pixo_b200_jpeg_write_headers_dht": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                    C.c_uint32, vp, vp, C.c_size_t, szp]),
+    "pixo_b200_jpeg_progressive_file": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                  C.c_uint32, vp, vp, u64p, vp, C.c_size_t, szp]),
     "pixo_b200_png_filter_rows_dev": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_size_t,
                                                 C.c_uint32, C.c_uint32, vp, vp]),
     "pixo_b200_adler32_combine": (C.c_uint32, [C.c_uint32, C.c_uint32, C.c_uint64]),

@@ -562,11 +562,11 @@ static constexpr size_t kTrellisScratch = (size_t)256 << 20;
 
 // COEF_TRELLIS: compute_all_coefficients(.., use_trellis = true).  Per piece the transform writes each
 // block's f32 DCT to the context's scratch, then k_trellis quantises each component's blocks into the
-// caller's arrays.  Waits for the device (the input check is reported by the call).
-static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
-                                uint32_t width, uint32_t height, uint32_t color_type, uint32_t subsampling,
-                                const float lum_q[64], const float chr_q[64], int16_t *d_y, size_t y_stride,
-                                int16_t *d_cb, int16_t *d_cr, size_t c_stride, bool zigzag)
+// caller's arrays.  Queued; *d_status (the context's scratch) gets bit 0 for input k_trellis rejects.
+static int trellis_pieces(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
+                          uint32_t width, uint32_t height, uint32_t color_type, uint32_t subsampling,
+                          const float lum_q[64], const float chr_q[64], int16_t *d_y, size_t y_stride,
+                          int16_t *d_cb, int16_t *d_cr, size_t c_stride, bool zigzag, uint32_t **d_status)
 {
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     const bool chroma = g.has_chroma;
@@ -611,6 +611,19 @@ static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, siz
         for (uint32_t i = 0; i < n_images; ++i)
             for (uint32_t m0 = 0; m0 < g.mcus_y; m0 += band) PIXO_TRY(piece(i, 1, m0, band));
     }
+    *d_status = status;
+    return 0;
+}
+
+// trellis_pieces, then waits for the device: the input check is reported by the call
+static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
+                                uint32_t width, uint32_t height, uint32_t color_type, uint32_t subsampling,
+                                const float lum_q[64], const float chr_q[64], int16_t *d_y, size_t y_stride,
+                                int16_t *d_cb, int16_t *d_cr, size_t c_stride, bool zigzag)
+{
+    uint32_t *status;
+    PIXO_TRY(trellis_pieces(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling, lum_q, chr_q,
+                            d_y, y_stride, d_cb, d_cr, c_stride, zigzag, &status));
     return trellis_status(ctx, status);
 }
 
@@ -1255,6 +1268,72 @@ int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, 
                         d_scan, scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice);
 }
 
+// The frames of one pass of pixo_b200_jpeg_encode_dev_progressive: at most the splice grid's 8192, and as many as
+// keep the pass's raw strings (out_cap + 16 bytes per frame) and its coefficient arrays each within kProgPass
+// (at least one frame).
+static constexpr size_t kProgPass = (size_t)512 << 20;
+static constexpr uint32_t kProgPassFrames = 8192;
+
+int pixo_b200_jpeg_encode_dev_progressive(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
+                                          uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
+                                          uint32_t quality, uint32_t subsampling, uint32_t restart_interval,
+                                          uint32_t optimize_huffman, uint32_t trellis_quant, uint8_t *d_out,
+                                          size_t out_cap_each, uint64_t *d_scan_len, uint32_t *d_overflow,
+                                          uint8_t *d_dht)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_TRY(validate_options(ctx, quality, restart_interval));
+    PIXO_TRY(validate_jpeg(ctx, width, height, color_type, subsampling));
+    if (!d_pixels || !d_out || !d_scan_len || !d_overflow)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (n_images == 0) return 0;
+    if (n_images > 65535) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "at most 65535 frames per call");
+    if ((reinterpret_cast<uintptr_t>(d_scan_len) & 7) || (reinterpret_cast<uintptr_t>(d_overflow) & 3))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "d_scan_len must be 8-byte aligned, d_overflow 4-byte aligned");
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    const bool optimize = optimize_huffman != 0, trellis = trellis_quant != 0;
+    float lum[64], chr[64];
+    quant_tables((int)quality, nullptr, nullptr, lum, chr);
+    const CoefLayout L(g);
+    const size_t cs = L.stride();
+    const size_t raw_each = Layout::round(out_cap_each + 16);
+    const uint32_t pass = (uint32_t)std::min<size_t>(
+        std::min<size_t>(n_images, kProgPassFrames), std::max<size_t>(1, std::min(kProgPass / raw_each, kProgPass / L.each)));
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ctx->d_coef.ensure(ctx, (size_t)pass * L.each));
+    // d_misc: a pass's statistics (optimize), its DHT blocks when the caller keeps none
+    uint64_t *d_hist = nullptr;
+    uint8_t *dht_own = nullptr;
+    if (optimize || !d_dht)
+        PIXO_TRY(bind(ctx, ctx->d_misc, [&](Layout &M) {
+            if (optimize) d_hist = M.take<uint64_t>((size_t)pass * kHistWords);
+            if (!d_dht) dht_own = M.take((size_t)pass * kDhtBytes);
+        }));
+    auto *c = reinterpret_cast<uint8_t *>(ctx->d_coef.ptr);
+    int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
+    for (uint32_t i0 = 0; i0 < n_images; i0 += pass) {
+        const uint32_t cnt = std::min(pass, n_images - i0);
+        const uint8_t *px = d_pixels + (size_t)i0 * pixel_stride;
+        uint8_t *dht = d_dht ? d_dht + (size_t)i0 * kDhtBytes : dht_own;
+        // encode_progressive_groups' sequence: plain coefficients for the statistics, the tables, COEF_TRELLIS
+        if (optimize || !trellis)
+            PIXO_TRY(launch_jpeg_transform(ctx, px, pixel_stride, cnt, width, height, color_type, subsampling, lum, chr,
+                                           L.y(c), cs, cb, cr, cs, 0));
+        if (optimize)
+            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
+                                           false, nullptr, d_hist));
+        PIXO_TRY(launch_huff_tables(ctx, d_hist, cnt, g.has_chroma, dht, nullptr));
+        uint32_t *status = nullptr;
+        if (trellis)
+            PIXO_TRY(trellis_pieces(ctx, px, pixel_stride, cnt, width, height, color_type, subsampling, lum, chr, L.y(c),
+                                    cs, cb, cr, cs, false, &status));
+        PIXO_TRY(launch_progressive_queued(ctx, L.y(c), cs, cb, cr, cs, cnt, g, dht, status,
+                                           d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7,
+                                           d_overflow + i0));
+    }
+    return 0;
+}
+
 int pixo_b200_jpeg_encode_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
                               uint32_t n_images, uint32_t width, uint32_t height,
                               uint32_t color_type, uint32_t quality, uint32_t subsampling,
@@ -1574,6 +1653,46 @@ int pixo_b200_jpeg_write_headers_dht(uint32_t width, uint32_t height, uint32_t c
         return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small (need %zu)", out_cap, n);
     memcpy(out, hdr, n);
     *out_len = n;
+    return 0;
+}
+
+int pixo_b200_jpeg_progressive_file(uint32_t width, uint32_t height, uint32_t color_type, uint32_t quality,
+                                    uint32_t subsampling, uint32_t restart_interval, const uint8_t *dht,
+                                    const uint8_t *segments, const uint64_t scan_len[7], uint8_t *out, size_t out_cap,
+                                    size_t *out_len)
+{
+    PIXO_TRY(validate_options(nullptr, quality, restart_interval));
+    PIXO_TRY(validate_jpeg(nullptr, width, height, color_type, subsampling));
+    if (!scan_len || !out || !out_len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (!dht) dht = dht_standard();
+    ProgTables check;
+    PIXO_TRY(dht_prog_tables(nullptr, dht, &check));
+    uint64_t body = 0;
+    for (int s = 0; s < 7; ++s) {
+        if (scan_len[s] > out_cap)
+            return set_error(nullptr, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu too small", out_cap);
+        body += scan_len[s];
+    }
+    if (body && !segments) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
+    uint8_t lum_zz[64], chr_zz[64];
+    quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
+    HuffTables t;
+    huff_from_dht(dht, t);
+    uint8_t hdr[2048];   // 281 bytes + the tables' values (at most 4 x 256)
+    const size_t n = write_headers_progressive(hdr, g, lum_zz, chr_zz, t, restart_interval);
+    PIXO_TRY(check_room(nullptr, out_cap, n + 7 * 10 + (size_t)body + 2));
+    memcpy(out, hdr, n);
+    size_t pos = n;
+    for (int s = 0; s < 7; ++s) {
+        pos += write_sos_progressive(out + pos, s);
+        if (scan_len[s]) memcpy(out + pos, segments, (size_t)scan_len[s]);
+        segments += scan_len[s];
+        pos += (size_t)scan_len[s];
+    }
+    out[pos] = 0xFF;
+    out[pos + 1] = 0xD9;
+    *out_len = pos + 2;
     return 0;
 }
 

@@ -55,6 +55,7 @@ constexpr uint32_t kOvfNoFit = 1u;     // the scan did not fit its capacity; its
 constexpr uint32_t kOvfFault = 2u;     // a look-back chain timed out
 constexpr uint32_t kOvfSegment = 4u;   // a segment's raw string outgrew its share
 constexpr uint32_t kOvfRange = 8u;     // a coefficient outside the baseline range
+constexpr uint32_t kOvfInput = 16u;    // input the trellis or the progressive stage cannot carry
 
 // Reusable scratch of a context: device memory (Buffer<false>, DevBuf) or page-locked host memory
 // (Buffer<true>, PinnedBuf), two types so that one cannot be passed where the other is meant.  Freed
@@ -345,6 +346,13 @@ size_t seg_scratch_bytes(const SegPlan &p);   // the device scratch of its codin
 SegPlan splice_plan(uint32_t n, size_t raw_cap);
 int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area, uint8_t *d_out,
                   uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow);
+// launch_splice for whole-string plans (S == 1) that writes an image only when all of it fits: a string whose
+// stuffed bytes exceed out_cap gets overflow bit 0, its length in d_out_len and nothing in d_out.  bounds:
+// [n][nr + 1] bit offsets into each string, multiples of 8, the last its bit count; range_len ([n][nr]) receives
+// the stuffed bytes between consecutive bounds of every string that has bytes.
+int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
+                          uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow,
+                          const unsigned long long *bounds, uint32_t nr, uint64_t *range_len);
 
 // progressive scans (jpeg_progressive.cu)
 bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
@@ -353,5 +361,11 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
                        const ProgTables *T, bool per_frame, bool check_only, ProgResult *res);
 int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
                             uint64_t *d_scan_len, uint32_t *d_overflow);
+// the stage of pixo_b200_jpeg_encode_dev_progressive, without a wait: frame i's tables from d_dht + i * kDhtBytes,
+// d_trellis_status (or null) folded into the frames' flags (jpeg_progressive.cu)
+int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
+                              const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
+                              const uint8_t *d_dht, const uint32_t *d_trellis_status, uint8_t *d_out, uint64_t out_cap,
+                              uint64_t *d_scan_len, uint32_t *d_overflow);
 
 }  // namespace pixo

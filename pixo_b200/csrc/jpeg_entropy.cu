@@ -1447,6 +1447,47 @@ __global__ void __launch_bounds__(SPL_THREADS) k_seg_emit(const __grid_constant_
     }
 }
 
+// Whole strings (S == 1) only, one CTA per image, after k_seg_scan: the stuffed offset of every bound of the
+// image's string (its byte offset + the 0xFF bytes before it: the prefix of its tile, and the tile's bytes up to
+// it counted here), the stuffed length of each range between bounds, and the image's total.  An image whose total
+// does not fit out_cap gets overflow bit 0 and no tiles, so that k_seg_emit writes nothing of it.
+__global__ void __launch_bounds__(SPL_THREADS) k_seg_fit(const __grid_constant__ SegParams P,
+                                                         const unsigned long long *bounds, uint32_t nr,
+                                                         unsigned long long *range_len)
+{
+    __shared__ uint32_t wsum[SPL_THREADS / 32];
+    const uint32_t i = blockIdx.x, nt = P.ntiles[i];
+    if (nt == 0) return;
+    const SegRec r = P.rec[i];
+    const uint8_t *raw = P.raw + (size_t)i * P.raw_cap;
+    const unsigned long long *b = bounds + (size_t)i * (nr + 1);
+    // stuffed offset of byte m (0 <= m <= nbytes) of the string (whole CTA)
+    auto stuffed = [&](unsigned long long m) {
+        const uint32_t t = m == r.nbytes ? nt - 1 : (uint32_t)(m / SPL_TILE);
+        uint32_t c = 0;
+        for (unsigned long long j = (unsigned long long)t * SPL_TILE + threadIdx.x; j < m; j += SPL_THREADS)
+            c += seg_byte(raw, r, j) == 0xFFu;
+        c = __reduce_add_sync(0xffffffffu, c);
+        __syncthreads();   // wsum may still be read from the previous bound
+        if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
+        __syncthreads();
+        unsigned long long tot = m + P.cnt[(size_t)i * P.max_tiles + t];
+        for (int w = 0; w < SPL_THREADS / 32; ++w) tot += wsum[w];
+        return tot;
+    };
+    unsigned long long prev = stuffed(b[0] >> 3);
+    for (uint32_t k = 0; k < nr; ++k) {
+        const unsigned long long next = stuffed(b[k + 1] >> 3);
+        if (threadIdx.x == 0) range_len[(size_t)i * nr + k] = next - prev;
+        prev = next;
+    }
+    if (threadIdx.x == 0 && prev > P.out_cap) {
+        atomicOr(&P.overflow[i], kOvfNoFit);
+        P.ntiles[i] = 0;
+        P.out_len[i] = prev;
+    }
+}
+
 }  // namespace
 
 static void make_huff_dev(const HuffTables &t, HuffDev *Tp)
@@ -1590,16 +1631,11 @@ static int code_segments(pixo_b200_ctx *ctx, EntParams P, const HuffDev &T, cons
     return 0;
 }
 
-// The four splice kernels over the n images of sp whose segment strings, bit counts and tails are in
-// raw_area: final bytes in d_out (out_cap per image), byte counts and flags in d_out_len / d_overflow.
-// raw_overflow: the coding kernel's flags per segment, or null.  base_bit / base_tail / last / base_dev:
-// see SegParams (a band of a tiled frame passes its place in the stream; a whole image passes 0, 0, true).
-static int splice_segments(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *scratch, const uint8_t *raw_area,
-                           const uint32_t *raw_overflow, uint64_t base_bit, uint32_t base_tail, bool last,
-                           const uint64_t *base_dev, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
-                           uint32_t *d_overflow)
+// The splice kernels' parameters (see splice_segments)
+static SegParams splice_params(const SegPlan &sp, uint8_t *scratch, const uint8_t *raw_area, const uint32_t *raw_overflow,
+                               uint64_t base_bit, uint32_t base_tail, bool last, const uint64_t *base_dev, uint8_t *d_out,
+                               uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow)
 {
-    const uint32_t n = sp.n;
     const SegScratch s = seg_scratch(sp, scratch);
     const SegRaw raw = seg_raw(sp, const_cast<uint8_t *>(raw_area));
     SegParams Q;
@@ -1616,10 +1652,24 @@ static int splice_segments(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *scrat
     Q.out_len = reinterpret_cast<unsigned long long *>(d_out_len);
     Q.overflow = d_overflow;
     Q.raw_overflow = raw_overflow;
-    const dim3 tiles((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, n);
-    PIXO_TRY(launch(ctx, k_seg_prefix, n, SPL_THREADS, 0, Q));
+    return Q;
+}
+
+// The four splice kernels over the n images of sp whose segment strings, bit counts and tails are in
+// raw_area: final bytes in d_out (out_cap per image), byte counts and flags in d_out_len / d_overflow.
+// raw_overflow: the coding kernel's flags per segment, or null.  base_bit / base_tail / last / base_dev:
+// see SegParams (a band of a tiled frame passes its place in the stream; a whole image passes 0, 0, true).
+static int splice_segments(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *scratch, const uint8_t *raw_area,
+                           const uint32_t *raw_overflow, uint64_t base_bit, uint32_t base_tail, bool last,
+                           const uint64_t *base_dev, uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len,
+                           uint32_t *d_overflow)
+{
+    const SegParams Q = splice_params(sp, scratch, raw_area, raw_overflow, base_bit, base_tail, last, base_dev, d_out,
+                                      out_cap, d_out_len, d_overflow);
+    const dim3 tiles((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, sp.n);
+    PIXO_TRY(launch(ctx, k_seg_prefix, sp.n, SPL_THREADS, 0, Q));
     PIXO_TRY(launch(ctx, k_seg_count, tiles, SPL_THREADS, 0, Q));
-    PIXO_TRY(launch(ctx, k_seg_scan, n, 1024, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_scan, sp.n, 1024, 0, Q));
     return launch(ctx, k_seg_emit, tiles, SPL_THREADS, 0, Q);
 }
 
@@ -1792,6 +1842,24 @@ int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, c
 {
     return splice_segments(ctx, sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap, d_out_len,
                            d_overflow);
+}
+
+// The progressive scans of pixo_b200_jpeg_encode_dev_progressive: every frame one string, its scans byte-aligned in it.
+// k_seg_fit runs between the prefix of the tiles' 0xFF counts and the emission, so that a frame is written whole or
+// not at all.  d_overflow must be set before (k_seg_emit only ORs into it).
+int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,
+                          uint8_t *d_out, uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow,
+                          const unsigned long long *bounds, uint32_t nr, uint64_t *range_len)
+{
+    const SegParams Q = splice_params(sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap,
+                                      d_out_len, d_overflow);
+    const dim3 tiles((sp.max_tiles + SPL_TPC - 1) / SPL_TPC, sp.n);
+    PIXO_TRY(launch(ctx, k_seg_prefix, sp.n, SPL_THREADS, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_count, tiles, SPL_THREADS, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_scan, sp.n, 1024, 0, Q));
+    PIXO_TRY(launch(ctx, k_seg_fit, sp.n, SPL_THREADS, 0, Q, bounds, nr,
+                    reinterpret_cast<unsigned long long *>(range_len)));
+    return launch(ctx, k_seg_emit, tiles, SPL_THREADS, 0, Q);
 }
 
 }  // namespace pixo

@@ -29,6 +29,10 @@
 //                   zeroed raw string (MSB first)
 //   k_seg_*         (jpeg_entropy.cu) splice every raw string into stuffed, 1-padded bytes
 //   k_prog_pack     (device entry) the 7 segments of a frame back to back in the caller's slot
+// The queued stage (pixo_b200_jpeg_encode_dev_progressive) reads nothing back: k_prog_dht_tables builds each
+// frame's tables from its DHT block, k_prog_place lays the frame's 7 streams out byte-aligned in ONE string of
+// out_cap + 16 bytes and decides the fit from the raw bytes, k_prog_emit_at codes into it, and the splice (with
+// k_seg_fit, which decides the fit from the stuffed bytes) writes the 7 segments straight into the caller's slot.
 // Nothing spins on another CTA, so no step can hang: a fault is a CUDA error.
 #include <string.h>
 
@@ -339,13 +343,29 @@ __global__ void __launch_bounds__(PT) k_prog_offsets(const __grid_constant__ Pro
 
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
 
-// Per block: flushes and symbols OR-ed into the stream's zeroed raw words at the block's bit offset
-__global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgParams P)
+// Where the queued stage puts a frame's 7 streams: one string per frame in P.raw (P.raw_words words per
+// frame), stream s from bit start[frame * 8 + s] on, each padded with 1s to a whole byte, so that the splice of
+// the frame's string is its 7 segments back to back.  start[frame * 8 + 7]: the string's bits.
+struct ProgPlace {
+    unsigned long long *start;       // [n][8]
+    unsigned long long *str_bits;    // [n]: the string's bits for the splice, 0 = the frame is skipped
+    unsigned long long *str_tails;   // [n]: 0 (every string starts on a byte)
+    const uint32_t *trellis_status;  // bit 0: COEF_TRELLIS rejected its input, or null
+    unsigned long long out_cap;
+    unsigned long long *scan_len;    // [n][7] the caller's
+    uint32_t *overflow;              // [n] the caller's
+};
+
+// Per block: flushes and symbols OR-ed into the stream's zeroed raw words at the block's bit offset.
+// AT: into the frame's string at the stream's start (ProgPlace), skipping frames that are not spliced.
+template <bool AT>
+__device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &Q)
 {
     __shared__ ProgTables T;
     __shared__ uint32_t sh[PT / 32];
     __shared__ unsigned long long sh64[PT / 32];
     const TileId id = tile_id(P, blockIdx.x);
+    if (AT && Q.str_bits[id.frame] == 0) return;   // (uniform per CTA)
     load_tables(P, id.frame, T);
     const int comp = scan_comp(id.scan), ss = scan_ss(id.scan), se = scan_se(id.scan);
     const bool dc_scan = ss == 0;
@@ -362,7 +382,8 @@ __global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgPa
     unsigned long long all;
     unsigned long long pos = P.tile_off[tix] + cta_scan_excl<unsigned long long>(len, 0ull, sh64, &all, AddOp());
     if (!live || len == 0) return;
-    uint32_t *words = P.raw + (size_t)(id.frame * NSCAN + id.scan) * P.raw_words;
+    uint32_t *words = P.raw + (size_t)(AT ? id.frame : id.frame * NSCAN + id.scan) * P.raw_words;
+    if (AT) pos += Q.start[(size_t)id.frame * 8 + id.scan];
     auto put = [&](uint32_t val, uint32_t n) {
         if (n == 0) return;
         const uint32_t al = val << (32u - n);
@@ -381,6 +402,77 @@ __global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgPa
     if (f.before) code_eobrun(f.before, T.ac[lum], put);
     if (dc_scan || last >= ss) code_own(v, prev, ss, last, dc_scan, T.dc[lum], T.ac[lum], put);
     if (f.after) code_eobrun(f.after, T.ac[lum], put);
+}
+
+__global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgParams P)
+{
+    prog_emit<false>(P, ProgPlace{});
+}
+
+__global__ void __launch_bounds__(PT) k_prog_emit_at(const __grid_constant__ ProgParams P, const __grid_constant__ ProgPlace Q)
+{
+    prog_emit<true>(P, Q);
+}
+
+// Per frame (one thread): the streams' places in the frame's string (ProgPlace), whether the string can fit
+// the caller's slot, and the 1-padding of each stream's last byte (the raw area is zeroed, k_prog_emit_at ORs
+// its bits in afterwards).  Raw bytes never exceed the stuffed ones, so a string longer than out_cap cannot fit
+// (overflow bit 0), and one that is not longer fits its raw area (out_cap + 16 bytes).  A frame of a pass whose
+// coefficients the trellis or this stage rejected gets kOvfInput.  scan_len: each stream's bytes x 2, room for any
+// stuffing; the splice overwrites it with the exact lengths of the frames it splices.
+__global__ void __launch_bounds__(128) k_prog_place(const __grid_constant__ ProgParams P, const __grid_constant__ ProgPlace Q)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const bool bad = *P.status || (Q.trellis_status && *Q.trellis_status);
+    const unsigned long long *bits = P.bits + (size_t)i * NSCAN;
+    unsigned long long off = 0;
+    for (int s = 0; s < NSCAN; ++s) {
+        Q.start[(size_t)i * 8 + s] = off;
+        Q.scan_len[(size_t)i * NSCAN + s] = 2 * ((bits[s] + 7) >> 3);
+        off += (bits[s] + 7) & ~7ull;
+    }
+    Q.start[(size_t)i * 8 + NSCAN] = off;
+    const bool fit = !bad && (off >> 3) <= Q.out_cap;
+    Q.overflow[i] = bad ? kOvfInput : (fit ? 0u : kOvfNoFit);
+    Q.str_bits[i] = fit ? off : 0ull;
+    Q.str_tails[i] = 0;
+    if (!fit) return;
+    uint8_t *raw = reinterpret_cast<uint8_t *>(P.raw + (size_t)i * P.raw_words);
+    for (int s = 0; s < NSCAN; ++s) {
+        const uint32_t r = (uint32_t)(bits[s] & 7);
+        if (r) raw[(Q.start[(size_t)i * 8 + s] + bits[s]) >> 3] |= (uint8_t)(0xFFu >> r);
+    }
+}
+
+// Per frame (one CTA): a DHT block (kDhtBytes: per table 16 counts + 256 values) as prog_tables makes it on the
+// host - get_code_from_table's (code << 8) | length, the first entry of a symbol winning, (0, 4) for a missing
+// symbol.  The blocks come from k_huff_tables, so every table is well formed.
+__global__ void __launch_bounds__(128) k_prog_dht_tables(const uint8_t *dht, ProgTables *out)
+{
+    __shared__ uint8_t seen[4][256];
+    const uint8_t *d = dht + (size_t)blockIdx.x * kDhtBytes;
+    ProgTables &T = out[blockIdx.x];
+    uint32_t *w = reinterpret_cast<uint32_t *>(&T);
+    for (int k = threadIdx.x; k < (int)(sizeof(ProgTables) / 4); k += blockDim.x) w[k] = 4u;
+    for (int k = threadIdx.x; k < 4 * 256; k += blockDim.x) seen[k >> 8][k & 255] = 0;
+    __syncthreads();
+    if (threadIdx.x >= 4) return;
+    const int k = threadIdx.x;
+    uint32_t *dst = k < 2 ? T.dc[k] : T.ac[k - 2];
+    const int nsym = k < 2 ? 16 : 256;
+    const uint8_t *bits = d + k * 272, *vals = bits + 16;
+    uint32_t code = 0;
+    int idx = 0;
+    for (int l = 0; l < 16; ++l) {
+        for (int c = 0; c < bits[l] && idx < 256; ++c, ++idx, ++code) {
+            const uint8_t sym = vals[idx];
+            if (seen[k][sym]) continue;
+            seen[k][sym] = 1;
+            if (sym < nsym) dst[sym] = (code << 8) | (uint32_t)(l + 1);
+        }
+        code <<= 1;
+    }
 }
 
 // Per frame: the 7 spliced segments back to back at out + frame * out_cap, their lengths, and
@@ -555,6 +647,70 @@ int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t 
     return launch(ctx, k_prog_pack, dim3(NSCAN * ctas, n), PT, 0, ctas, res.stage, res.stage_cap,
                   reinterpret_cast<const unsigned long long *>(res.d_len), d_out, out_cap,
                   reinterpret_cast<unsigned long long *>(d_scan_len), d_overflow);
+}
+
+// The stage of a pass of n frames, queued without a wait (pixo_b200_jpeg_encode_dev_progressive): frame i's tables
+// from its DHT block at d_dht + i * kDhtBytes, its 7 segments back to back at d_out + i * out_cap, their lengths
+// and the frame's flags in d_scan_len / d_overflow.  The raw area holds one string of out_cap + 16 bytes per frame,
+// so nothing has to be read back to size it.  12 launches: k_prog_dht_tables, the four measuring kernels,
+// k_prog_place, k_prog_emit_at and the splice (launch_splice_bounded: five).
+int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
+                              const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
+                              const uint8_t *d_dht, const uint32_t *d_trellis_status, uint8_t *d_out, uint64_t out_cap,
+                              uint64_t *d_scan_len, uint32_t *d_overflow)
+{
+    cudaStream_t st = ctx->stream;
+    ProgParams P;
+    memset(&P, 0, sizeof P);
+    prog_counts(g, P);
+    const size_t tiles = (size_t)n * P.tile_base[NSCAN], blocks = (size_t)n * P.blk_base[NSCAN];
+    ProgTables *d_tables;
+    ProgPlace Q;
+    PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
+        P.status = L.take<uint32_t>(1);
+        P.blen = L.take<uint32_t>(blocks);
+        P.flag = L.take(blocks);
+        P.tile_last = L.take<uint32_t>(tiles);
+        P.tile_carry = L.take<uint32_t>(tiles);
+        P.tile_bits = L.take<uint32_t>(tiles);
+        P.tile_off = L.take<unsigned long long>(tiles);
+        P.bits = L.take<unsigned long long>((size_t)n * NSCAN);
+        P.tables = d_tables = L.take<ProgTables>(n);
+        Q.start = L.take<unsigned long long>((size_t)n * 8);
+    }));
+    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
+    P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
+    P.n = n;
+    P.tables_per_frame = 1;
+    const size_t raw_cap = Layout::round((size_t)out_cap + 16);
+    const SegPlan sp = splice_plan(n, raw_cap);
+    uint8_t *scratch;
+    uint64_t *d_len;
+    PIXO_TRY(bind(ctx, ctx->d_prog_out, [&](Layout &L) {
+        scratch = L.take(seg_scratch_bytes(sp));
+        d_len = L.take<uint64_t>(n);
+    }));
+    PIXO_TRY(ctx->d_prog_raw.ensure(ctx, seg_raw(sp, nullptr).total));
+    const SegRaw raw = seg_raw(sp, ctx->d_prog_raw.ptr);
+    P.raw = reinterpret_cast<uint32_t *>(raw.strings);
+    P.raw_words = raw_cap / 4;
+    Q.str_bits = raw.bits;
+    Q.str_tails = raw.tails;
+    Q.trellis_status = d_trellis_status;
+    Q.out_cap = out_cap;
+    Q.scan_len = reinterpret_cast<unsigned long long *>(d_scan_len);
+    Q.overflow = d_overflow;
+    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
+    PIXO_TRY(launch(ctx, k_prog_dht_tables, n, 128, 0, d_dht, d_tables));
+    PIXO_TRY(launch(ctx, k_prog_measure, (unsigned)tiles, PT, 0, P));   // (every frame has a Y block)
+    PIXO_TRY(launch(ctx, k_prog_carry, n * NSCAN, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_count, (unsigned)tiles, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
+    PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, (size_t)n * raw_cap, st));
+    PIXO_TRY(launch(ctx, k_prog_place, (n + 127) / 128, 128, 0, P, Q));
+    PIXO_TRY(launch(ctx, k_prog_emit_at, (unsigned)tiles, PT, 0, P, Q));
+    return launch_splice_bounded(ctx, sp, scratch, raw.strings, d_out, out_cap, d_len, d_overflow, Q.start, NSCAN,
+                                 d_scan_len);
 }
 
 }  // namespace pixo

@@ -357,6 +357,49 @@ def jpeg_file(options: JpegOptions, dht, scan) -> bytes:
     return write_headers_dht(options, dht) + bytes(scan) + b"\xff\xd9"
 
 
+def encode_progressive_dev(d_frames, pixel_stride, n_images, options: JpegOptions, d_out, out_cap_each, d_scan_len,
+                           d_overflow, d_dht=None, ctx: Context | None = None) -> None:
+    """pixo_b200_jpeg_encode_dev_progressive: pixo's progressive scans (options.optimize_huffman and
+    options.trellis_quant as given; options.progressive is not read) of n_images device frames (frame i at
+    d_frames + i * pixel_stride bytes) -> frame i's 7 segments back to back at d_out + i * out_cap_each, their
+    lengths in d_scan_len[i] (7 int64), its flags in d_overflow[i] (bit 0: did not fit, bit 4: input the stage
+    cannot carry) and, when d_dht is given, its tables in d_dht[i] (DHT_BYTES).  The buffers are anything with
+    .data_ptr() (torch tensors) or device addresses.  Queued on the context's stream; nothing is synchronised.
+    progressive_file(options, dht, segments, lens) makes a frame's file."""
+    restart = _restart(options)
+    ctx = ctx or default_context()
+    ptr = lambda t: None if t is None else (int(t) if isinstance(t, int) else int(t.data_ptr()))
+    rc = _lib.load().pixo_b200_jpeg_encode_dev_progressive(
+        ctx.handle, ptr(d_frames), int(pixel_stride), int(n_images), int(options.width), int(options.height),
+        int(options.color_type), int(options.quality), int(options.subsampling), restart,
+        int(bool(options.optimize_huffman)), int(bool(options.trellis_quant)), ptr(d_out), int(out_cap_each),
+        ptr(d_scan_len), ptr(d_overflow), ptr(d_dht))
+    _lib.check(ctx.handle, rc)
+
+
+def progressive_file(options: JpegOptions, dht, segments, lens) -> bytes:
+    """A whole progressive file from one frame's tables (DHT_BYTES, or None for the standard ones), its 7
+    segments back to back (bytes or a uint8 array, at least sum(lens) long) and their 7 lengths."""
+    ln = np.ascontiguousarray(np.asarray(lens, np.uint64).reshape(-1))
+    if ln.size != 7:
+        raise _lib.PixoError(_lib.ERR_INVALID_ARGUMENT, f"a progressive file has 7 scans, got {ln.size} lengths")
+    seg = _as_u8(segments)
+    if seg.size < int(ln.sum()):
+        raise _lib.PixoError(_lib.ERR_INVALID_ARGUMENT, f"segments hold {seg.size} bytes, the lengths {int(ln.sum())}")
+    d = None
+    if dht is not None:
+        d = np.ascontiguousarray(np.asarray(dht, np.uint8).reshape(-1))
+        if d.size != DHT_BYTES:
+            raise _lib.PixoError(_lib.ERR_INVALID_ARGUMENT, f"a DHT block is {DHT_BYTES} bytes, got {d.size}")
+    buf = np.zeros(4096 + int(ln.sum()), np.uint8)
+    n = C.c_size_t()
+    _lib.check(None, _lib.load().pixo_b200_jpeg_progressive_file(
+        int(options.width), int(options.height), int(options.color_type), int(options.quality),
+        int(options.subsampling), _restart(options), None if d is None else d.ctypes.data,
+        seg.ctypes.data if seg.size else None, ln.ctypes.data_as(_lib.u64p), buf.ctypes.data, buf.size, C.byref(n)))
+    return buf[: n.value].tobytes()
+
+
 def entropy_encode(y, cb, cr, options: JpegOptions, ctx: Context | None = None) -> bytes:
     """Host entropy stage on its own (no device needed)."""
     y = np.ascontiguousarray(y, np.int16)

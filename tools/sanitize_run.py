@@ -110,6 +110,18 @@ yb[7, 63] = -3
 d_yb = torch.from_numpy(yb).to(dev)
 jpeg.progressive_scans_dev(d_yb, None, None, 8 * 400, 8 * 100, ColorType.Gray, Subsampling.S444, ctx=ctx)
 ctx.sync()
+# the queued progressive stage (encode_progressive_dev): k_prog_dht_tables, k_prog_place, k_prog_emit_at and
+# k_seg_fit, with a frame that fits, one whose stuffed bytes do not and one whose raw bytes do not
+d_fr = torch.from_numpy(np.stack([np.full(64 * 48 * 3, 90, np.uint8), synthetic.noise(64, 48, 3, 6),
+                                  synthetic.noise(64, 48, 3, 7)])).to(dev)
+for cap, (opt, tr) in ((16384, (True, True)), (16384, (False, False)), (2048, (True, False))):
+    d_o = torch.empty(3 * cap, dtype=torch.uint8, device=dev)
+    d_l = torch.empty((3, 7), dtype=torch.int64, device=dev)
+    d_f = torch.empty(3, dtype=torch.int32, device=dev)
+    d_t = torch.empty((3, jpeg.DHT_BYTES), dtype=torch.uint8, device=dev)
+    jpeg.encode_progressive_dev(d_fr, 64 * 48 * 3, 3, JpegOptions(64, 48, ColorType.Rgb, 100, Subsampling.S420, None,
+                                                                  opt, True, tr), d_o, cap, d_l, d_f, d_t, ctx=ctx)
+    ctx.sync()
 # resize: every kernel at every pixel size, the wide and byte nearest copies, and Lanczos3 in one band and,
 # for a tall frame whose one destination row needs 280 MB of intermediate, in column chunks
 from pixo_b200 import resize as rs  # noqa: E402
