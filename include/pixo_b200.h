@@ -26,7 +26,8 @@
  *    still queued when they return):
  *      jpeg_coefficients_dev with PIXO_B200_COEF_TRELLIS, jpeg_trellis_quantize_dev,
  *      jpeg_progressive_scans_dev, jpeg_entropy_encode_dev, jpeg_band_last_dc,
- *      jpeg_band_entropy_dev, jpeg_band_splice_dev, png_reduce_filter_dev,
+ *      jpeg_band_entropy_dev, jpeg_band_splice_dev, jpeg_band_dev_progressive_summary,
+ *      jpeg_band_dev_progressive, jpeg_band_dev_progressive_splice, png_reduce_filter_dev,
  *      png_quantize_filter_dev.
  *    The others take host pointers and return after the result is in `out`.
  *  - every function returns a pixo_b200_status (0 = ok).  pixo_b200_last_error(ctx) gives the
@@ -398,6 +399,52 @@ int pixo_b200_jpeg_band_entropy_dev_async(pixo_b200_ctx *ctx, const int16_t *d_y
 int pixo_b200_jpeg_band_splice_dev_async(pixo_b200_ctx *ctx, const uint8_t *d_raw, const uint64_t *d_offset,
                                          uint8_t *d_out, size_t out_cap, uint64_t *d_out_len,
                                          uint32_t *d_flags);
+/* The progressive scans of one band (pixo's max preset, pixo_b200_jpeg_encode_progressive's scans and quirks).  A band
+ * of whole MCU rows is a contiguous range of each component's array (4:2:0 Y in MCU order too), so it is given as
+ * ny Y and nc chroma blocks starting at the frame's Y block y_base and chroma block c_base (the blocks of the bands
+ * before it).  Per scan a band needs from the bands before it:
+ *   - DC scans: the DC predictor of its first block, the last DC of the nearest earlier band with blocks of that
+ *     component in the arrays being coded (0 for none; predictors are never reset);
+ *   - AC scans (Y 1-10, Y 11-63, Cb 1-63, Cr 1-63): the EOB run pending at its start, given as the carry
+ *     max((index + 1) << 1 | init) over the earlier bands' last_enc (0 for none): init is 1 when that block's last
+ *     non-zero lies below the scan's Se.  0x7FFF flushes then fall where pixo's frame-wide count puts them, and the
+ *     flush at the scan's end belongs to the band that holds the scan's last block;
+ *   - its start bit in each scan's stream, and the bits it inherits in the stream's first byte (see below).
+ * Every array is natural order, 16-byte aligned where the band has blocks of it; d_cb / d_cr are ignored when nc
+ * is 0.  Coefficients outside -16383..16383 return PIXO_B200_ERR_INVALID_ARGUMENT, with nothing written.  These
+ * calls wait for the device.  No restart interval on this path (pixo's max preset sets none).
+ *
+ * summary: the band's last DC per component (0 without blocks) and, per AC scan, its largest
+ * ((frame index + 1) << 1 | init) over its non-empty blocks (0: none), from the arrays being coded. */
+int pixo_b200_jpeg_band_dev_progressive_summary(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
+                                                const int16_t *d_cr, size_t ny, size_t nc, uint64_t y_base,
+                                                uint64_t c_base, int32_t last_dc[3], uint32_t last_enc[4]);
+/* The band's 7 scans as raw bit strings (no 0xFF stuffing, no padding) in d_raw, their bit counts in nbits and their
+ * last 7 bits (fewer when the string is shorter; the last bit in bit 0) in tail7.  frame_ny / frame_nc: the frame's
+ * block counts (frame_nc 0: a gray frame, whose chroma scans are empty).  dc_seed / ac_carry: see above (ac_carry in
+ * the order Y 1-10, Y 11-63, Cb, Cr).  d_hist (device, may be NULL): the frame's 536 summed statistics of the
+ * PLAIN-rounded coefficients (pixo_b200_jpeg_band_histogram_dev of every band, seeded with the plain arrays' DC
+ * predictors) -> optimised tables built on the device as pixo_b200_jpeg_encode_dev_progressive builds them; NULL:
+ * the standard tables.  d_dht (device, may be NULL) receives those tables (1088 bytes, the layout
+ * pixo_b200_jpeg_progressive_file takes), also for a band without blocks.  d_raw: 16-byte aligned, untouched by
+ * other work until the band's scans have been spliced; NULL allowed for a band without blocks.  *raw_need receives
+ * the bytes d_raw must hold (0 without blocks); below that the call returns PIXO_B200_ERR_OUTPUT_TOO_SMALL with
+ * nbits set and nothing else written, and a second call with raw_cap >= *raw_need succeeds. */
+int pixo_b200_jpeg_band_dev_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
+                                        const int16_t *d_cr, size_t ny, size_t nc, uint64_t y_base, uint64_t c_base,
+                                        uint64_t frame_ny, uint64_t frame_nc, const int32_t dc_seed[3],
+                                        const uint32_t ac_carry[4], const uint64_t *d_hist, uint8_t *d_dht,
+                                        uint8_t *d_raw, size_t raw_cap, size_t *raw_need, uint64_t nbits[7],
+                                        uint32_t tail7[7]);
+/* Scan `scan` (0..6, simple_progressive_script's order) of a band coded into d_raw, as
+ * pixo_b200_jpeg_band_splice_dev splices a baseline band: nbits = that scan's count (0: the band owns no byte of the
+ * scan; d_raw may then be NULL), start_bit = the scan's bits in the bands before it, tail_in = the last
+ * (start_bit % 8) of those bits (they may come from several bands when some wrote fewer than 7), is_last_band = no
+ * later band writes a bit of this scan (this band 1-pads its end).  The 7 segments of pixo_b200_jpeg_progressive_file
+ * are, per scan, the bands' spliced bytes in band order. */
+int pixo_b200_jpeg_band_dev_progressive_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint32_t scan, uint64_t nbits,
+                                               uint64_t start_bit, uint32_t tail_in, uint32_t is_last_band,
+                                               uint8_t *d_out, size_t out_cap, uint64_t *out_len);
 int pixo_b200_jpeg_band_entropy(const int16_t *y, const int16_t *cb, const int16_t *cr, uint32_t width,
                                 uint32_t band_height, uint32_t color_type, uint32_t subsampling,
                                 const int32_t dc_seed[3], const uint64_t *hist, uint8_t *raw,

@@ -92,6 +92,13 @@ SYMBOLS = {
     "pixo_b200_jpeg_band_entropy_dev_async": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                         vp, u64p, vp, C.c_size_t, vp, vp]),
     "pixo_b200_jpeg_band_splice_dev_async": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp, vp]),
+    "pixo_b200_jpeg_band_dev_progressive_summary": (C.c_int, [vp, vp, vp, vp, C.c_size_t, C.c_size_t, C.c_uint64,
+                                                              C.c_uint64, C.POINTER(C.c_int32), u32p]),
+    "pixo_b200_jpeg_band_dev_progressive": (C.c_int, [vp, vp, vp, vp, C.c_size_t, C.c_size_t, C.c_uint64, C.c_uint64,
+                                                      C.c_uint64, C.c_uint64, C.POINTER(C.c_int32), u32p, vp, vp, vp,
+                                                      C.c_size_t, szp, u64p, u32p]),
+    "pixo_b200_jpeg_band_dev_progressive_splice": (C.c_int, [vp, vp, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32,
+                                                             C.c_uint32, vp, C.c_size_t, u64p]),
     "pixo_b200_jpeg_band_entropy": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                               C.POINTER(C.c_int32), u64p, vp, C.c_size_t, u64p, u32p]),
     "pixo_b200_jpeg_band_histogram": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,

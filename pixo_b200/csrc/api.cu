@@ -1574,6 +1574,87 @@ int pixo_b200_jpeg_band_splice_dev_async(pixo_b200_ctx *ctx, const uint8_t *d_ra
     return launch_band_splice(ctx, d_raw, 0, 0, false, d_offset, d_out, out_cap, d_out_len, d_flags);
 }
 
+// The progressive scans of one band (pixo_b200_jpeg_band_dev_progressive*): a band's arrays, 16-byte aligned where it
+// has blocks, inside the frame's
+static int check_prog_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr, size_t ny,
+                           size_t nc, uint64_t y_base, uint64_t c_base)
+{
+    if ((ny && !d_y) || (nc && (!d_cb || !d_cr))) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    PIXO_TRY(check_coef_alignment(ctx, ny ? d_y : nullptr, d_cb, d_cr, nc > 0));
+    // enc_of ((index + 1) << 1 | init) must fit 32 bits
+    if (y_base + ny >= 0x7FFFFFFFull || c_base + nc >= 0x7FFFFFFFull || y_base > 0x7FFFFFFFull || c_base > 0x7FFFFFFFull)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive band: too many blocks per component");
+    return 0;
+}
+
+int pixo_b200_jpeg_band_dev_progressive_summary(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
+                                                const int16_t *d_cr, size_t ny, size_t nc, uint64_t y_base,
+                                                uint64_t c_base, int32_t last_dc[3], uint32_t last_enc[4])
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (!last_dc || !last_enc) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
+    PIXO_TRY(check_prog_band(ctx, d_y, d_cb, d_cr, ny, nc, y_base, c_base));
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    ProgBandSummary sum;
+    PIXO_TRY(launch_progressive_band_summary(ctx, d_y, d_cb, d_cr, ny, nc, y_base, c_base, &sum));
+    for (int k = 0; k < 3; ++k) last_dc[k] = sum.last_dc[k];
+    for (int k = 0; k < 4; ++k) last_enc[k] = sum.last_enc[k];
+    return 0;
+}
+
+int pixo_b200_jpeg_band_dev_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb,
+                                        const int16_t *d_cr, size_t ny, size_t nc, uint64_t y_base, uint64_t c_base,
+                                        uint64_t frame_ny, uint64_t frame_nc, const int32_t dc_seed[3],
+                                        const uint32_t ac_carry[4], const uint64_t *d_hist, uint8_t *d_dht,
+                                        uint8_t *d_raw, size_t raw_cap, size_t *raw_need, uint64_t nbits[7],
+                                        uint32_t tail7[7])
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (!dc_seed || !ac_carry || !raw_need || !nbits || !tail7)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
+    PIXO_TRY(check_prog_band(ctx, d_y, d_cb, d_cr, ny, nc, y_base, c_base));
+    if (y_base + ny > frame_ny || c_base + nc > frame_nc)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive band: blocks outside the frame");
+    if ((ny || nc) && !d_raw) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if ((reinterpret_cast<uintptr_t>(d_raw) & 15) || (reinterpret_cast<uintptr_t>(d_hist) & 7))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "d_raw must be 16-byte aligned, d_hist 8-byte aligned");
+    ProgBand B;
+    B.ny = ny; B.nc = nc; B.y_base = y_base; B.c_base = c_base; B.frame_ny = frame_ny; B.frame_nc = frame_nc;
+    for (int k = 0; k < 3; ++k) {
+        if (dc_seed[k] < -16383 || dc_seed[k] > 16383)
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "DC seed %d out of the progressive range", dc_seed[k]);
+        B.dc_seed[k] = dc_seed[k];
+    }
+    for (int k = 0; k < 4; ++k) {   // a carry names a block before the band: (index + 1) <= the band's first index
+        if ((ac_carry[k] >> 1) > (k < 2 ? y_base : c_base))
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "AC carry %u lies past the band's first block", ac_carry[k]);
+        B.ac_carry[k] = ac_carry[k];
+    }
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return launch_progressive_band(ctx, d_y, d_cb, d_cr, B, d_hist, d_dht, d_raw, raw_cap, raw_need, nbits, tail7);
+}
+
+int pixo_b200_jpeg_band_dev_progressive_splice(pixo_b200_ctx *ctx, const uint8_t *d_raw, uint32_t scan, uint64_t nbits,
+                                               uint64_t start_bit, uint32_t tail_in, uint32_t is_last_band,
+                                               uint8_t *d_out, size_t out_cap, uint64_t *out_len)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (scan >= 7) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "scan %u: a progressive frame has 7", scan);
+    if (nbits == 0) {   // the band owns no byte of this scan; it still returns with the stream drained, as the
+                        // other band calls do
+        if (!d_out || !out_len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
+        PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        *out_len = 0;
+        return 0;
+    }
+    const auto it = ctx->prog_bands.find(d_raw);
+    if (it == ctx->prog_bands.end())
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "this raw buffer was not coded by pixo_b200_jpeg_band_dev_progressive");
+    return pixo_b200_jpeg_band_splice_dev(ctx, d_raw + (size_t)scan * it->second, nbits, start_bit, tail_in, is_last_band,
+                                          d_out, out_cap, out_len);
+}
+
 int pixo_b200_jpeg_band_entropy(const int16_t *y, const int16_t *cb, const int16_t *cr, uint32_t width,
                                 uint32_t band_height, uint32_t color_type, uint32_t subsampling,
                                 const int32_t dc_seed[3], const uint64_t *hist, uint8_t *raw,

@@ -155,6 +155,23 @@ struct ProgResult {
     std::vector<uint64_t> len;
 };
 
+// One band of a frame's MCU rows for the progressive scans (pixo_b200_jpeg_band_dev_progressive): its blocks of
+// each component, the frame index of its first, the frame's blocks (frame_nc 0: gray), and what the frame's earlier
+// bands leave - the DC predictors and, per AC scan (Y 1-10, Y 11-63, Cb, Cr), the carry of the EOB run
+struct ProgBand {
+    uint64_t ny, nc, y_base, c_base, frame_ny, frame_nc;
+    int dc_seed[3];
+    uint32_t ac_carry[4];
+};
+
+// What a band leaves the later ones: its last DC per component, its largest enc_of per AC scan, and status bit 0
+// for a coefficient outside -16383..16383
+struct ProgBandSummary {
+    uint32_t last_enc[4];
+    int32_t last_dc[3];
+    uint32_t status;
+};
+
 // What a context has set on one kernel.  Function attributes belong to the device, and every context
 // sets the same values, so contexts sharing a device never undo each other's settings.
 struct KernelAttrs {
@@ -200,6 +217,9 @@ struct pixo_b200_ctx {
     // How the bands coded by pixo_b200_jpeg_band_entropy_dev(_async) were cut into segments, keyed by
     // the caller's raw buffer (which holds the segments' strings, bit counts and tails until the splice).
     std::unordered_map<const void *, pixo::SegPlan> bands;
+    // The bands coded by pixo_b200_jpeg_band_dev_progressive: bytes between their scans' splice areas (each one of
+    // `bands`), keyed by the caller's raw buffer
+    std::unordered_map<const void *, size_t> prog_bands;
     std::unordered_map<const void *, pixo::KernelAttrs> kernels;   // keyed by the kernel's host function
 
     pixo_b200_ctx() = default;
@@ -361,6 +381,12 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
                        const ProgTables *T, bool per_frame, bool check_only, ProgResult *res);
 int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
                             uint64_t *d_scan_len, uint32_t *d_overflow);
+// one band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive, _summary)
+int launch_progressive_band_summary(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                                    uint64_t ny, uint64_t nc, uint64_t y_base, uint64_t c_base, ProgBandSummary *out);
+int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                            const ProgBand &B, const uint64_t *d_hist, uint8_t *d_dht_out, uint8_t *d_raw,
+                            size_t raw_cap, size_t *raw_need, uint64_t nbits[7], uint32_t tail7[7]);
 // the stage of pixo_b200_jpeg_encode_dev_progressive, without a wait: frame i's tables from d_dht + i * kDhtBytes,
 // d_trellis_status (or null) folded into the frames' flags (jpeg_progressive.cu)
 int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,

@@ -34,6 +34,9 @@
 // out_cap + 16 bytes and decides the fit from the raw bytes, k_prog_emit_at codes into it, and the splice (with
 // k_seg_fit, which decides the fit from the stuffed bytes) writes the 7 segments straight into the caller's slot.
 // Nothing spins on another CTA, so no step can hang: a fault is a CUDA error.
+// One band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive*) runs measure / carry / count /
+// offsets / emit in their band mode (BAND = true, see ProgParams), then k_prog_band_trailer; k_prog_band_last is
+// the band's summary for the bands after it.
 #include <string.h>
 
 #include <algorithm>
@@ -68,6 +71,12 @@ struct ProgParams {
     uint32_t *status;                // bit 0: a coefficient outside -16383..16383
     const ProgTables *tables;        // [n] per frame, or [1] for every frame
     uint32_t tables_per_frame;       // 1 or 0
+    // band mode (the kernels' BAND = true, one frame): the band's blocks are a contiguous range of each scan's
+    // array, and what the frame's earlier bands leave crosses into it
+    uint64_t gbase[NSCAN];           // frame index of the band's first block of each scan
+    uint64_t gnb[NSCAN];             // the frame's blocks of each scan
+    uint32_t carry_in[NSCAN];        // AC scans: enc_of (frame index) of the last non-empty block before the band
+    int dc_seed[3];                  // DC predictors before the band's first block, per component
 };
 
 // tile t of the batch -> frame, scan, tile inside the scan
@@ -87,6 +96,10 @@ __device__ __forceinline__ TileId tile_id(const ProgParams &P, uint32_t t)
     id.tile = r - P.tile_base[id.scan];
     return id;
 }
+
+// frame index of the band's first block of scan s (0 for a whole frame)
+template <bool BAND>
+__device__ __forceinline__ uint64_t scan_base(const ProgParams &P, uint32_t s) { return BAND ? P.gbase[s] : 0; }
 
 __device__ __forceinline__ int scan_comp(uint32_t s) { return s == 0 || s == 3 || s == 4 ? 0 : (s == 1 || s == 5 ? 1 : 2); }
 __device__ __forceinline__ int scan_ss(uint32_t s) { return s < 3 ? 0 : (s == 4 ? 11 : 1); }
@@ -239,6 +252,7 @@ __device__ __forceinline__ int load_block(const int16_t *blk, int ss, int se, bo
     return last;
 }
 
+template <bool BAND>
 __global__ void __launch_bounds__(PT) k_prog_measure(const __grid_constant__ ProgParams P)
 {
     __shared__ ProgTables T;
@@ -256,7 +270,7 @@ __global__ void __launch_bounds__(PT) k_prog_measure(const __grid_constant__ Pro
         const int16_t *blk = P.arr[comp] + (size_t)id.frame * P.stride[comp] + b * 64;
         uint32_t v[32];
         const int last = load_block(blk, ss, se, dc_scan, v);
-        const int prev = (dc_scan && b) ? blk[-64] : 0;
+        const int prev = (dc_scan && b) ? blk[-64] : (BAND && dc_scan ? P.dc_seed[comp] : 0);
         bool ok = true;
         if (dc_scan || last >= ss)
             ok = code_own(v, prev, ss, last, dc_scan, T.dc[lum], T.ac[lum], [&](uint32_t, uint32_t n) { len += n; });
@@ -265,21 +279,22 @@ __global__ void __launch_bounds__(PT) k_prog_measure(const __grid_constant__ Pro
         const size_t r = (size_t)id.frame * P.blk_base[NSCAN] + P.blk_base[id.scan] + b;
         P.blen[r] = len;
         P.flag[r] = flag;
-        enc = enc_of(b, flag);
+        enc = enc_of(b + scan_base<BAND>(P, id.scan), flag);
     }
     uint32_t tot;
     cta_scan_excl<uint32_t>(enc, 0u, sh, &tot, MaxOp());
     if (threadIdx.x == 0) P.tile_last[(size_t)id.frame * P.tile_base[NSCAN] + P.tile_base[id.scan] + id.tile] = tot;
 }
 
-// One CTA per stream: exclusive running maximum of tile_last over the stream's tiles
+// One CTA per stream: exclusive running maximum of tile_last over the stream's tiles (from the band's carry)
+template <bool BAND>
 __global__ void __launch_bounds__(PT) k_prog_carry(const __grid_constant__ ProgParams P)
 {
     __shared__ uint32_t sh[PT / 32];
     const uint32_t frame = blockIdx.x / NSCAN, s = blockIdx.x % NSCAN;
     const uint32_t nt = P.tile_base[s + 1] - P.tile_base[s];
     const size_t base = (size_t)frame * P.tile_base[NSCAN] + P.tile_base[s];
-    uint32_t run = 0;
+    uint32_t run = BAND ? P.carry_in[s] : 0u;
     for (uint32_t t0 = 0; t0 < nt; t0 += PT) {
         const uint32_t t = t0 + threadIdx.x;
         const uint32_t x = t < nt ? P.tile_last[base + t] : 0u;
@@ -291,6 +306,7 @@ __global__ void __launch_bounds__(PT) k_prog_carry(const __grid_constant__ ProgP
 }
 
 // Per block: own bits + its flushes (AC scans) -> blen; tile totals
+template <bool BAND>
 __global__ void __launch_bounds__(PT) k_prog_count(const __grid_constant__ ProgParams P)
 {
     __shared__ ProgTables T;
@@ -308,9 +324,10 @@ __global__ void __launch_bounds__(PT) k_prog_count(const __grid_constant__ ProgP
     const uint8_t flag = live ? P.flag[r] : 0;
     uint32_t len = live ? P.blen[r] : 0u, tot;
     if (!dc_scan) {   // (uniform per CTA)
-        const uint32_t ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(b, flag), 0u, sh, &tot, MaxOp()));
+        const uint64_t gb = b + scan_base<BAND>(P, id.scan);
+        const uint32_t ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(gb, flag), 0u, sh, &tot, MaxOp()));
         if (live) {
-            const Flushes f = flushes_of(b, nb, flag, ex);
+            const Flushes f = flushes_of(gb, BAND ? P.gnb[id.scan] : nb, flag, ex);
             auto add = [&](uint32_t, uint32_t n) { len += n; };
             if (f.before) code_eobrun(f.before, T.ac[lum], add);
             if (f.after) code_eobrun(f.after, T.ac[lum], add);
@@ -358,7 +375,8 @@ struct ProgPlace {
 
 // Per block: flushes and symbols OR-ed into the stream's zeroed raw words at the block's bit offset.
 // AT: into the frame's string at the stream's start (ProgPlace), skipping frames that are not spliced.
-template <bool AT>
+// BAND: one band of a frame (see ProgParams).
+template <bool AT, bool BAND>
 __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &Q)
 {
     __shared__ ProgTables T;
@@ -376,8 +394,9 @@ __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &
     const size_t r = (size_t)id.frame * P.blk_base[NSCAN] + P.blk_base[id.scan] + b;
     const bool live = b < nb;
     const uint8_t flag = live ? P.flag[r] : 0;
+    const uint64_t gb = b + scan_base<BAND>(P, id.scan);
     uint32_t ex = 0, tot;
-    if (!dc_scan) ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(b, flag), 0u, sh, &tot, MaxOp()));
+    if (!dc_scan) ex = max(P.tile_carry[tix], cta_scan_excl<uint32_t>(enc_of(gb, flag), 0u, sh, &tot, MaxOp()));
     const unsigned long long len = live ? P.blen[r] : 0ull;
     unsigned long long all;
     unsigned long long pos = P.tile_off[tix] + cta_scan_excl<unsigned long long>(len, 0ull, sh64, &all, AddOp());
@@ -396,22 +415,23 @@ __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &
     const int16_t *blk = P.arr[comp] + (size_t)id.frame * P.stride[comp] + b * 64;
     uint32_t v[32];
     const int last = load_block(blk, ss, se, dc_scan, v);
-    const int prev = (dc_scan && b) ? blk[-64] : 0;
+    const int prev = (dc_scan && b) ? blk[-64] : (BAND && dc_scan ? P.dc_seed[comp] : 0);
     Flushes f{0, 0};
-    if (!dc_scan) f = flushes_of(b, nb, flag, ex);
+    if (!dc_scan) f = flushes_of(gb, BAND ? P.gnb[id.scan] : nb, flag, ex);
     if (f.before) code_eobrun(f.before, T.ac[lum], put);
     if (dc_scan || last >= ss) code_own(v, prev, ss, last, dc_scan, T.dc[lum], T.ac[lum], put);
     if (f.after) code_eobrun(f.after, T.ac[lum], put);
 }
 
+template <bool BAND>
 __global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgParams P)
 {
-    prog_emit<false>(P, ProgPlace{});
+    prog_emit<false, BAND>(P, ProgPlace{});
 }
 
 __global__ void __launch_bounds__(PT) k_prog_emit_at(const __grid_constant__ ProgParams P, const __grid_constant__ ProgPlace Q)
 {
-    prog_emit<true>(P, Q);
+    prog_emit<true, false>(P, Q);
 }
 
 // Per frame (one thread): the streams' places in the frame's string (ProgPlace), whether the string can fit
@@ -501,6 +521,87 @@ __global__ void __launch_bounds__(PT) k_prog_pack(uint32_t ctas, const uint8_t *
         dst[j] = src[j];
 }
 
+// ---- one band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive*) ----------------------------
+// A band of whole MCU rows is a contiguous range of every scan's array, so the band mode of the kernels above codes
+// it with frame indices (gbase), the frame's block counts (gnb: the end-of-scan flush falls in the band that holds
+// the scan's last block) and what the earlier bands leave: the DC predictors and, per AC scan, the running maximum
+// of enc_of over their non-empty blocks (carry_in).  The band's summary gives the later bands those values.
+
+struct ProgBandLast {
+    const int16_t *arr[3];
+    uint64_t nb[3], base[3];         // the band's blocks of each component, the frame index of its first
+    ProgBandSummary *out;            // zeroed by the caller
+};
+
+// One thread per block of the component blockIdx.y: the block's enc_of in each AC scan of its component (Y: 1-10 and
+// 11-63, chroma: 1-63), the largest of the band to out->last_enc, the last block's DC to out->last_dc, status bit 0
+// for a coefficient outside -16383..16383
+__global__ void __launch_bounds__(PT) k_prog_band_last(const __grid_constant__ ProgBandLast A)
+{
+    const uint32_t comp = blockIdx.y;
+    const uint64_t nb = A.nb[comp];
+    const uint64_t b = (uint64_t)blockIdx.x * PT + threadIdx.x;
+    if ((uint64_t)blockIdx.x * PT >= nb) return;   // (uniform per CTA)
+    uint32_t lo = 0, hi = 0;   // Y: scans 1-10 and 11-63; chroma: scan 1-63 in lo
+    bool ok = true;
+    if (b < nb) {
+        const uint4 *q = reinterpret_cast<const uint4 *>(A.arr[comp] + b * 64);
+        uint32_t v[32];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const uint4 w = q[k];
+            v[4 * k] = w.x; v[4 * k + 1] = w.y; v[4 * k + 2] = w.z; v[4 * k + 3] = w.w;
+        }
+        int last_a = 0, last_b = 0;   // last non-zero zig-zag position in 1..10, in 11..63 (0: none)
+#pragma unroll
+        for (int k = 0; k < 64; ++k) {
+            const int nat = zz_nat(k);
+            const int c = (int16_t)(v[nat >> 1] >> (16 * (nat & 1)));
+            ok &= c >= -16383 && c <= 16383;
+            if (k >= 1 && c != 0) (k <= 10 ? last_a : last_b) = k;
+        }
+        const uint64_t gb = b + A.base[comp];
+        auto flag = [](int last, int se) { return (uint8_t)(last ? 1u | (last < se ? 2u : 0u) : 0u); };
+        if (comp == 0) {
+            lo = enc_of(gb, flag(last_a, 10));
+            hi = enc_of(gb, flag(last_b, 63));
+        } else {
+            lo = enc_of(gb, flag(last_b ? last_b : last_a, 63));
+        }
+        if (b + 1 == nb) A.out->last_dc[comp] = (int16_t)v[0];
+    }
+    lo = __reduce_max_sync(0xffffffffu, lo);
+    hi = __reduce_max_sync(0xffffffffu, hi);
+    const bool bad = __any_sync(0xffffffffu, !ok);
+    if ((threadIdx.x & 31) == 0) {
+        if (lo) atomicMax(&A.out->last_enc[comp == 0 ? 0 : 1 + comp], lo);
+        if (hi) atomicMax(&A.out->last_enc[1], hi);
+        if (bad) atomicOr(&A.out->status, 1u);
+    }
+}
+
+// Where a coded band's 7 strings live: scan s's string at P.raw + s * P.raw_words (a splice area of its own, see
+// SegRaw), its bit count and tail to that area's trailer, the tails also to tail7 for the host
+struct ProgBandRaw {
+    unsigned long long *bits[NSCAN], *tails[NSCAN];
+    unsigned long long *tail7;       // [NSCAN]
+};
+
+// Thread s: scan s's bit count and last (up to) 7 bits, the last one in bit 0
+__global__ void __launch_bounds__(32) k_prog_band_trailer(const __grid_constant__ ProgParams P,
+                                                          const __grid_constant__ ProgBandRaw R)
+{
+    const uint32_t s = threadIdx.x;
+    if (s >= NSCAN) return;
+    const unsigned long long n = P.bits[s];
+    const uint8_t *raw = reinterpret_cast<const uint8_t *>(P.raw + (size_t)s * P.raw_words);
+    unsigned long long t = 0;
+    for (unsigned long long i = n > 7 ? n - 7 : 0; i < n; ++i) t = (t << 1) | ((raw[i >> 3] >> (7 - (i & 7))) & 1u);
+    *R.bits[s] = n;
+    *R.tails[s] = t;
+    R.tail7[s] = t;
+}
+
 }  // namespace
 
 // get_code_from_table over each table: (code << 8) | length per symbol, pixo's (0, 4) for a symbol the
@@ -579,9 +680,9 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(d_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
     if (tiles) {
-        PIXO_TRY(launch(ctx, k_prog_measure, (unsigned)tiles, PT, 0, P));
-        PIXO_TRY(launch(ctx, k_prog_carry, n * NSCAN, PT, 0, P));
-        PIXO_TRY(launch(ctx, k_prog_count, (unsigned)tiles, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_measure<false>, (unsigned)tiles, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_carry<false>, n * NSCAN, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_count<false>, (unsigned)tiles, PT, 0, P));
     }
     PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
     // h_prog: the status word, every stream's bit count (then its segment's length), the splice's flags
@@ -624,7 +725,7 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     PIXO_CUDA(ctx, cudaMemsetAsync(d_ovf, 0, nstream * 4, st));
     P.raw = reinterpret_cast<uint32_t *>(raw.strings);
     P.raw_words = raw_cap / 4;
-    if (tiles) PIXO_TRY(launch(ctx, k_prog_emit, (unsigned)tiles, PT, 0, P));
+    if (tiles) PIXO_TRY(launch(ctx, k_prog_emit<false>, (unsigned)tiles, PT, 0, P));
     PIXO_TRY(launch_splice(ctx, sp, scratch, raw.strings, stage, stage_cap, d_len, d_ovf));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, d_len, nstream * 8, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, nstream * 4, cudaMemcpyDeviceToHost, st));
@@ -702,15 +803,141 @@ int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_s
     Q.overflow = d_overflow;
     PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
     PIXO_TRY(launch(ctx, k_prog_dht_tables, n, 128, 0, d_dht, d_tables));
-    PIXO_TRY(launch(ctx, k_prog_measure, (unsigned)tiles, PT, 0, P));   // (every frame has a Y block)
-    PIXO_TRY(launch(ctx, k_prog_carry, n * NSCAN, PT, 0, P));
-    PIXO_TRY(launch(ctx, k_prog_count, (unsigned)tiles, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_measure<false>, (unsigned)tiles, PT, 0, P));   // (every frame has a Y block)
+    PIXO_TRY(launch(ctx, k_prog_carry<false>, n * NSCAN, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_count<false>, (unsigned)tiles, PT, 0, P));
     PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
     PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, (size_t)n * raw_cap, st));
     PIXO_TRY(launch(ctx, k_prog_place, (n + 127) / 128, 128, 0, P, Q));
     PIXO_TRY(launch(ctx, k_prog_emit_at, (unsigned)tiles, PT, 0, P, Q));
     return launch_splice_bounded(ctx, sp, scratch, raw.strings, d_out, out_cap, d_len, d_overflow, Q.start, NSCAN,
                                  d_scan_len);
+}
+
+// The band summary: the last DC of each component, the largest enc_of (frame index) of each AC scan.  Waits for
+// the device.
+int launch_progressive_band_summary(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                                    uint64_t ny, uint64_t nc, uint64_t y_base, uint64_t c_base, ProgBandSummary *out)
+{
+    cudaStream_t st = ctx->stream;
+    ProgBandLast A;
+    A.arr[0] = d_y; A.arr[1] = d_cb; A.arr[2] = d_cr;
+    A.nb[0] = ny; A.nb[1] = A.nb[2] = nc;
+    A.base[0] = y_base; A.base[1] = A.base[2] = c_base;
+    PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) { A.out = L.take<ProgBandSummary>(1); }));
+    ProgBandSummary *h;
+    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) { h = L.take<ProgBandSummary>(1); }, 8));
+    PIXO_CUDA(ctx, cudaMemsetAsync(A.out, 0, sizeof(ProgBandSummary), st));
+    const uint64_t tiles = (std::max(ny, nc) + PT - 1) / PT;
+    if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive band: too many blocks");
+    if (tiles) PIXO_TRY(launch(ctx, k_prog_band_last, dim3((unsigned)tiles, nc ? 3 : 1), PT, 0, A));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h, A.out, sizeof(ProgBandSummary), cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+    if (h->status)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    *out = *h;
+    return 0;
+}
+
+// Code one band of a frame: its tables from d_hist (k_huff_tables, the standard ones when null; to d_dht_out when
+// it is not null), the band mode of measure / carry / count / offsets, a wait for the bit counts, then the 7
+// strings, each in a splice area of its own in d_raw (registered in ctx->bands, so launch_band_splice takes it),
+// and their tails.  Nothing is written for a coefficient out of range or a raw_cap below *raw_need.
+int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
+                            const ProgBand &B, const uint64_t *d_hist, uint8_t *d_dht_out, uint8_t *d_raw,
+                            size_t raw_cap, size_t *raw_need, uint64_t nbits[NSCAN], uint32_t tail7[NSCAN])
+{
+    cudaStream_t st = ctx->stream;
+    ProgParams P;
+    memset(&P, 0, sizeof P);
+    uint32_t tb = 0;
+    uint64_t bb = 0;
+    for (int s = 0; s < NSCAN; ++s) {
+        const bool y = kComp[s] == 0;
+        P.nb[s] = y ? B.ny : B.nc;
+        P.gbase[s] = y ? B.y_base : B.c_base;
+        P.gnb[s] = y ? B.frame_ny : B.frame_nc;
+        P.carry_in[s] = s >= 3 ? B.ac_carry[s - 3] : 0u;
+        P.tile_base[s] = tb;
+        P.blk_base[s] = bb;
+        tb += (uint32_t)((P.nb[s] + PT - 1) / PT);
+        bb += P.nb[s];
+    }
+    P.tile_base[NSCAN] = tb;
+    P.blk_base[NSCAN] = bb;
+    for (int k = 0; k < 3; ++k) P.dc_seed[k] = B.dc_seed[k];
+    const size_t tiles = P.tile_base[NSCAN], blocks = P.blk_base[NSCAN];
+    if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive band: too many blocks");
+    ProgTables *d_tables;
+    uint8_t *dht;
+    ProgBandRaw R;
+    PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
+        P.status = L.take<uint32_t>(1);
+        P.blen = L.take<uint32_t>(blocks);
+        P.flag = L.take(blocks);
+        P.tile_last = L.take<uint32_t>(tiles);
+        P.tile_carry = L.take<uint32_t>(tiles);
+        P.tile_bits = L.take<uint32_t>(tiles);
+        P.tile_off = L.take<unsigned long long>(tiles);
+        P.bits = L.take<unsigned long long>(NSCAN);
+        P.tables = d_tables = L.take<ProgTables>(1);
+        dht = L.take(kDhtBytes);
+        R.tail7 = L.take<unsigned long long>(NSCAN);
+    }));
+    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
+    P.n = 1;
+    uint32_t *h_status;
+    uint64_t *h_bits, *h_tails;
+    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
+        h_status = L.take<uint32_t>(1);
+        h_bits = L.take<uint64_t>(NSCAN);
+        h_tails = L.take<uint64_t>(NSCAN);
+    }, 8));
+    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
+    PIXO_TRY(launch_huff_tables(ctx, d_hist, 1, B.frame_nc > 0, dht, nullptr));
+    PIXO_TRY(launch(ctx, k_prog_dht_tables, 1, 128, 0, dht, d_tables));
+    if (tiles) {
+        PIXO_TRY(launch(ctx, k_prog_measure<true>, (unsigned)tiles, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_carry<true>, NSCAN, PT, 0, P));
+        PIXO_TRY(launch(ctx, k_prog_count<true>, (unsigned)tiles, PT, 0, P));
+    }
+    PIXO_TRY(launch(ctx, k_prog_offsets, NSCAN, PT, 0, P));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, NSCAN * 8, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+    if (*h_status)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    // every scan's splice area as large as the longest string needs, so that scan s starts at s * stride
+    uint64_t max_bytes = 0;
+    for (int s = 0; s < NSCAN; ++s) max_bytes = std::max<uint64_t>(max_bytes, (h_bits[s] + 7) / 8);
+    const SegPlan sp = splice_plan(1, Layout::round((size_t)max_bytes + 16));
+    const size_t stride = seg_raw(sp, nullptr).total;
+    *raw_need = blocks ? NSCAN * stride : 0;
+    for (int s = 0; s < NSCAN; ++s) nbits[s] = h_bits[s], tail7[s] = 0;
+    if (raw_cap < *raw_need)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "raw capacity %zu too small (need %zu)", raw_cap, *raw_need);
+    if (d_dht_out) PIXO_CUDA(ctx, cudaMemcpyAsync(d_dht_out, dht, kDhtBytes, cudaMemcpyDeviceToDevice, st));
+    if (!blocks) {   // an empty band: no string
+        PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+        return 0;
+    }
+    PIXO_CUDA(ctx, cudaMemsetAsync(d_raw, 0, *raw_need, st));
+    P.raw = reinterpret_cast<uint32_t *>(d_raw);
+    P.raw_words = stride / 4;
+    for (int s = 0; s < NSCAN; ++s) {
+        uint8_t *area = d_raw + (size_t)s * stride;
+        const SegRaw r = seg_raw(sp, area);
+        R.bits[s] = r.bits;
+        R.tails[s] = r.tails;
+        ctx->bands[area] = sp;
+    }
+    ctx->prog_bands[d_raw] = stride;
+    PIXO_TRY(launch(ctx, k_prog_emit<true>, (unsigned)tiles, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_band_trailer, 1, 32, 0, P, R));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_tails, R.tail7, NSCAN * 8, cudaMemcpyDeviceToHost, st));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
+    for (int s = 0; s < NSCAN; ++s) tail7[s] = (uint32_t)h_tails[s];
+    return 0;
 }
 
 }  // namespace pixo

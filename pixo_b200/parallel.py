@@ -317,6 +317,9 @@ class ThreadComm:
         allv = self.all_gather(rank, t)
         return [allv[r] for r in range(self.world)] if rank == dst else None
 
+    def all_reduce_sum(self, rank, t):
+        return self.all_gather(rank, t).sum(0)
+
 
 class _DistComm:
     def __init__(self, world):
@@ -339,6 +342,12 @@ class _DistComm:
         bufs = [torch.empty_like(t) for _ in range(self.world)] if rank == dst else None
         dist.gather(t, bufs, dst=dst)
         return bufs
+
+    def all_reduce_sum(self, rank, t):
+        import torch.distributed as dist
+        if self.world > 1:
+            dist.all_reduce(t, op=dist.ReduceOp.SUM)
+        return t
 
 
 def tiled_scan_parts_async(coder, nonempty: list[bool], rank: int, world: int, dst: int = 0, comm=None):
@@ -432,6 +441,279 @@ def tiled_scan_parts_local(coders: list, optimize_huffman: bool = False):
         start, tail_in, is_last = bit_offsets(nbits, tails, r)
         parts.append(c.splice(nbits[r], start, tail_in, is_last))
     return parts, hist
+
+
+# ---- the progressive scans of one tiled frame (pixo's max preset) -------------------------------------
+# A band of whole MCU rows is a contiguous range of every component's array (4:2:0 Y in MCU order too), so each of
+# the 7 scans of simple_progressive_script codes the band's range on its own once three things cross in from the
+# bands before it: the DC predictors (DC scans), the EOB run pending at the band's start (AC scans) and the bit
+# offset in the scan's stream.  Each rank codes its band into 7 raw strings (pixo_b200_jpeg_band_dev_progressive),
+# splices every scan at its offset (k_seg_*), and dst writes the file with the segments in scan-major order.
+
+PROG_SCANS = 7
+PROG_SCAN_COMP = (0, 1, 2, 0, 0, 1, 2)   # the component of each scan: Y DC, Cb DC, Cr DC, Y 1-10, Y 11-63, Cb, Cr
+
+
+def prog_dc_seeds(last_dcs, counts, rank: int) -> np.ndarray:
+    """DC predictors band `rank` starts from, per component: the last DC of the nearest earlier band that has
+    blocks of that component (0 for none; pixo never resets them).  last_dcs, counts: [world, 3] (blocks of Y, Cb,
+    Cr)."""
+    seed = np.zeros(3, np.int32)
+    for c in range(3):
+        for r in range(rank - 1, -1, -1):
+            if int(counts[r][c]):
+                seed[c] = int(last_dcs[r][c])
+                break
+    return seed
+
+
+def ac_carries(last_encs, rank: int) -> np.ndarray:
+    """The EOB-run carry of band `rank` in each AC scan (Y 1-10, Y 11-63, Cb, Cr): the largest
+    ((frame index + 1) << 1 | init) over the earlier bands' last non-empty blocks, 0 for none.  last_encs: [world, 4]
+    (pixo_b200_jpeg_band_dev_progressive_summary's last_enc of every band)."""
+    out = np.zeros(4, np.uint32)
+    for r in range(rank):
+        out = np.maximum(out, np.asarray(last_encs[r], np.uint32))
+    return out
+
+
+def scan_bit_offsets(nbits, tails, rank: int) -> tuple[int, int, bool]:
+    """(start_bit, tail_in, is_last) of band `rank` in ONE scan's stream: `bit_offsets` for bands that may write fewer
+    than 7 bits of a scan (a tail then holds all of its band's bits), so the bits inherited in the first byte can
+    come from several bands.  is_last: the band writes the scan's last bit (and 1-pads it)."""
+    start = int(sum(int(n) for n in nbits[:rank]))
+    need = start & 7
+    tail_in = have = 0
+    for r in range(rank - 1, -1, -1):
+        if have >= need:
+            break
+        take = min(int(nbits[r]), need - have)
+        tail_in |= (int(tails[r]) & ((1 << take) - 1)) << have
+        have += take
+    is_last = bool(int(nbits[rank])) and not any(int(n) for n in nbits[rank + 1:])
+    return start, tail_in, is_last
+
+
+def band_bases(bands: list[Band], rank: int) -> tuple[int, int]:
+    """Frame index of band `rank`'s first Y block and first chroma block."""
+    return sum(b.y_blocks for b in bands[:rank]), sum(b.c_blocks for b in bands[:rank])
+
+
+class ProgressiveBandCoder:
+    """One rank's band of a progressive frame on its device (pixo_b200_jpeg_band_dev_progressive*).  coded: the band's
+    (y, cb, cr) int16 device arrays to code (natural order, the trellis arrays under trellis_quant); plain: the
+    plain-rounded arrays the optimised tables are counted from (None: the coded ones).  ny / nc: the band's blocks,
+    y_base / c_base the frame index of its first ones, frame_ny / frame_nc the frame's (frame_nc 0: gray).
+    geometry (width, band_height, color_type, subsampling) is needed for the table statistics only."""
+
+    def __init__(self, ctx, coded, ny, nc, y_base, c_base, frame_ny, frame_nc, plain=None, geometry=None):
+        import torch
+        self.ctx, self.lib, self.torch = ctx, _lib.load(), torch
+        self.coded = tuple(coded)
+        self.plain = tuple(plain) if plain is not None else None
+        self.ny, self.nc = int(ny), int(nc)
+        self.y_base, self.c_base = int(y_base), int(c_base)
+        self.frame_ny, self.frame_nc = int(frame_ny), int(frame_nc)
+        self.geometry = geometry
+        self.dev = self.coded[0].device
+        self.raw = None
+        self.dht = torch.empty(1088, dtype=torch.uint8, device=self.dev)
+
+    @staticmethod
+    def _p(t):
+        return None if t is None else int(t.data_ptr())
+
+    def _arrays(self, arrs):
+        y, cb, cr = arrs
+        return self._p(y), self._p(cb) if self.nc else None, self._p(cr) if self.nc else None
+
+    def summary(self) -> list[int]:
+        """[plain last DC x 3, coded last DC x 3, last_enc x 4, ny, nc]: what the later bands need from this one."""
+        dc, enc = (C.c_int32 * 3)(), (C.c_uint32 * 4)()
+        _lib.check(self.ctx.handle, self.lib.pixo_b200_jpeg_band_dev_progressive_summary(
+            self.ctx.handle, *self._arrays(self.coded), self.ny, self.nc, self.y_base, self.c_base, dc, enc))
+        plain = list(dc)
+        if self.plain is not None:
+            pdc = (C.c_int32 * 3)()
+            _lib.check(self.ctx.handle, self.lib.pixo_b200_jpeg_band_last_dc(
+                self.ctx.handle, *self._arrays(self.plain), self.ny, self.nc, pdc))
+            plain = list(pdc)
+        return plain + list(dc) + list(enc) + [self.ny, self.nc]
+
+    def histogram(self, seed):
+        """536 baseline counters of the plain arrays from DC predictors `seed` (torch int64 on the device)."""
+        hist = self.torch.zeros(536, dtype=self.torch.int64, device=self.dev)
+        if self.ny:
+            if self.geometry is None:
+                raise _lib.PixoError(_lib.ERR_INVALID_ARGUMENT, "optimised tables need the band's geometry")
+            self.torch.cuda.current_stream(self.dev).synchronize()
+            s = (C.c_int32 * 3)(*[int(v) for v in seed])
+            _lib.check(self.ctx.handle, self.lib.pixo_b200_jpeg_band_histogram_dev(
+                self.ctx.handle, *self._arrays(self.plain or self.coded), *[int(v) for v in self.geometry], s,
+                int(hist.data_ptr())))
+            self.ctx.sync()
+        return hist
+
+    def code(self, seed, carry, hist=None) -> tuple[list[int], list[int]]:
+        """The band's 7 raw strings from DC predictors `seed`, EOB-run carries `carry` and the frame's summed
+        statistics `hist` (device int64 [536]; None: standard tables) -> (bits, tails) per scan.  self.dht then
+        holds the tables."""
+        if hist is not None:
+            self.torch.cuda.current_stream(self.dev).synchronize()   # (an all-reduce on torch's stream)
+        s = (C.c_int32 * 3)(*[int(v) for v in seed])
+        cy = (C.c_uint32 * 4)(*[int(v) for v in carry])
+        need, nbits, tails = C.c_size_t(), (C.c_uint64 * 7)(), (C.c_uint32 * 7)()
+        if self.raw is None and (self.ny or self.nc):
+            self.raw = self.torch.empty(((self.ny + 2 * self.nc) * 48 + 7 * 4096) // 16 * 16, dtype=self.torch.uint8,
+                                        device=self.dev)
+        for _ in range(2):
+            rc = self.lib.pixo_b200_jpeg_band_dev_progressive(
+                self.ctx.handle, *self._arrays(self.coded), self.ny, self.nc, self.y_base, self.c_base, self.frame_ny,
+                self.frame_nc, s, cy, self._p(hist), self._p(self.dht), self._p(self.raw),
+                0 if self.raw is None else self.raw.numel(), C.byref(need), nbits, tails)
+            if rc != _lib.ERR_OUTPUT_TOO_SMALL:
+                break
+            self.raw = self.torch.empty(need.value, dtype=self.torch.uint8, device=self.dev)
+        _lib.check(self.ctx.handle, rc)
+        return list(nbits), list(tails)
+
+    def splice(self, scan, nbits, start_bit, tail_in, is_last):
+        """-> uint8 device tensor: this band's finished bytes of scan `scan`."""
+        out = self.torch.empty((nbits + 7) // 8 * 2 + 64, dtype=self.torch.uint8, device=self.dev)
+        n = C.c_uint64()
+        _lib.check(self.ctx.handle, self.lib.pixo_b200_jpeg_band_dev_progressive_splice(
+            self.ctx.handle, self._p(self.raw), int(scan), int(nbits), int(start_bit), int(tail_in), int(is_last),
+            int(out.data_ptr()), out.numel(), C.byref(n)))
+        return out[: n.value]
+
+
+def band_coefficients(ctx, d_pixels, width: int, band_height: int, color_type: int, subsampling: int, quality: int,
+                      trellis: bool):
+    """The band's coefficient arrays from its pixel rows (device uint8, band_height x width x bpp): (plain, coded),
+    each (y, cb, cr) int16 device tensors [max(n, 1), 64] - plain-rounded, and COEF_TRELLIS ones when `trellis`
+    (coded is plain otherwise)."""
+    import torch
+    from . import jpeg
+    lib = _lib.load()
+    dev = d_pixels.device
+    ny, nc = jpeg.block_counts(width, band_height, color_type, subsampling) if band_height else (0, 0)
+    _, _, lq, cq = jpeg.quant_tables(quality)
+
+    def arrays(flags):
+        a = [torch.empty((max(n, 1), 64), dtype=torch.int16, device=dev) for n in (ny, nc, nc)]
+        if ny:
+            torch.cuda.current_stream(dev).synchronize()   # torch's stream is not the context's
+            _lib.check(ctx.handle, lib.pixo_b200_jpeg_coefficients_dev(
+                ctx.handle, int(d_pixels.data_ptr()), d_pixels.numel(), 1, width, band_height, color_type, subsampling,
+                lq.ctypes.data_as(_lib.f32p), cq.ctypes.data_as(_lib.f32p), int(a[0].data_ptr()), ny * 64,
+                int(a[1].data_ptr()), int(a[2].data_ptr()), nc * 64, flags, None))
+            ctx.sync()
+        return tuple(a)
+
+    plain = arrays(0)
+    return plain, (arrays(2) if trellis else plain)   # 2: COEF_TRELLIS
+
+
+def progressive_band_coder(ctx, d_pixels, width: int, height: int, color_type: int, subsampling: int, quality: int,
+                           trellis: bool, bands: list[Band], rank: int) -> ProgressiveBandCoder:
+    """Band `rank` of plan_bands(width, height, ...) from its pixel rows on its device: transform (and trellis),
+    then its coder."""
+    b = bands[rank]
+    bh = b.px_row1 - b.px_row0
+    plain, coded = band_coefficients(ctx, d_pixels, width, bh, color_type, subsampling, quality, trellis)
+    yb, cb = band_bases(bands, rank)
+    return ProgressiveBandCoder(ctx, coded, b.y_blocks, b.c_blocks, yb, cb, sum(x.y_blocks for x in bands),
+                                sum(x.c_blocks for x in bands), plain if trellis else None,
+                                (width, max(bh, 1), color_type, subsampling))
+
+
+def _check_progressive_options(options):
+    from . import jpeg
+    if jpeg._restart(options):
+        raise _lib.PixoError(_lib.ERR_UNSUPPORTED, "a restart interval on a tiled progressive frame")
+
+
+def tiled_progressive_parts(coder, optimize_huffman: bool, rank: int, world: int, dst: int = 0, comm=None):
+    """The progressive scans of one tiled frame, this rank's band in `coder` (ProgressiveBandCoder).  Returns, on
+    dst, (the 7 segments back to back as a uint8 tensor on dst's device, their 7 lengths, the tables as 1088 bytes)
+    and None elsewhere.  Collectives (through `comm`: torch.distributed by default, or ThreadComm): all-gather of
+    the summaries, [all-reduce of the 536 counters], all-gather of 7 x (bits, tail), all-gather of 7 byte counts,
+    gather of the bytes to dst."""
+    import torch
+    comm = comm or _DistComm(world)
+    dev = coder.dev
+
+    def all_gather(vals):
+        return comm.all_gather(rank, torch.tensor([int(v) for v in vals], dtype=torch.int64, device=dev)).cpu().numpy()
+
+    s = all_gather(coder.summary())
+    counts = s[:, [10, 11, 11]]
+    hist = None
+    if optimize_huffman:
+        hist = comm.all_reduce_sum(rank, coder.histogram(prog_dc_seeds(s[:, 0:3], counts, rank)))
+    nbits, tails = coder.code(prog_dc_seeds(s[:, 3:6], counts, rank), ac_carries(s[:, 6:10], rank), hist)
+    bt = all_gather(nbits + tails).reshape(world, 2, PROG_SCANS)
+    bodies = []
+    for k in range(PROG_SCANS):
+        start, tail_in, is_last = scan_bit_offsets(bt[:, 0, k], bt[:, 1, k], rank)
+        bodies.append(coder.splice(k, nbits[k], start, tail_in, is_last))
+    sizes = all_gather([b.numel() for b in bodies])            # [world, 7]
+    pad = torch.zeros(max(int(sizes.sum(1).max()), 1), dtype=torch.uint8, device=dev)
+    body = torch.cat(bodies)
+    pad[: body.numel()] = body
+    bufs = comm.gather(rank, pad, dst)
+    if rank != dst:
+        return None
+    segs = []
+    for k in range(PROG_SCANS):                                 # scan-major: every band's bytes of scan k
+        for r in range(world):
+            off = int(sizes[r, :k].sum())
+            segs.append(bufs[r][off: off + int(sizes[r, k])])
+    return torch.cat(segs), [int(v) for v in sizes.sum(0)], coder.dht.cpu().numpy()
+
+
+def encode_progressive_tiled(coder, options, rank: int, world: int, dst: int = 0, comm=None):
+    """One frame tiled over `world` ranks as the progressive file pixo writes for `options` (JpegOptions; its
+    geometry, quality and optimize_huffman; trellis_quant decides the coder's arrays): the file on dst, None
+    elsewhere.  A restart interval raises ERR_UNSUPPORTED."""
+    from . import jpeg
+    _check_progressive_options(options)
+    parts = tiled_progressive_parts(coder, bool(options.optimize_huffman), rank, world, dst, comm)
+    if parts is None:
+        return None
+    seg, lens, dht = parts
+    return jpeg.progressive_file(options, dht, seg.cpu().numpy(), lens)
+
+
+def tiled_progressive_parts_local(coders: list, optimize_huffman: bool = False):
+    """tiled_progressive_parts with every band in THIS process (one device): (segments, lengths, tables)."""
+    import torch
+    world = len(coders)
+    s = np.array([c.summary() for c in coders], np.int64)
+    counts = s[:, [10, 11, 11]]
+    hist = None
+    if optimize_huffman:
+        hist = sum(c.histogram(prog_dc_seeds(s[:, 0:3], counts, r)) for r, c in enumerate(coders))
+    coded = [c.code(prog_dc_seeds(s[:, 3:6], counts, r), ac_carries(s[:, 6:10], r), hist) for r, c in enumerate(coders)]
+    nb = np.array([n for n, _ in coded], np.int64)
+    tl = np.array([t for _, t in coded], np.int64)
+    segs, lens = [], [0] * PROG_SCANS
+    for k in range(PROG_SCANS):
+        for r, c in enumerate(coders):
+            start, tail_in, is_last = scan_bit_offsets(nb[:, k], tl[:, k], r)
+            part = c.splice(k, int(nb[r, k]), start, tail_in, is_last)
+            segs.append(part)
+            lens[k] += part.numel()
+    dev = coders[0].dev
+    return torch.cat(segs) if segs else torch.empty(0, dtype=torch.uint8, device=dev), lens, coders[0].dht.cpu().numpy()
+
+
+def encode_progressive_tiled_local(coders: list, options) -> bytes:
+    """encode_progressive_tiled with every band in this process."""
+    from . import jpeg
+    _check_progressive_options(options)
+    seg, lens, dht = tiled_progressive_parts_local(coders, bool(options.optimize_huffman))
+    return jpeg.progressive_file(options, dht, seg.cpu().numpy(), lens)
 
 
 # ---- Adler-32 of a stream held in pieces (PNG filter stage in row bands) ----------------------------
