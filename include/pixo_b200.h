@@ -238,7 +238,7 @@ int pixo_b200_jpeg_encode_progressive_batch(pixo_b200_ctx *ctx, const uint8_t *p
  * the standard tables.  PIXO_B200_ERR_INVALID_ARGUMENT, with nothing written, for a coefficient outside
  * -16383..16383 (every DC difference then fits int16 and every category is <= 15), a table with more
  * than 256 values or a code that does not fit its length, or a layout above.  Waits for the device to
- * measure the scans; the final copy into d_out is queued on the context's stream. */
+ * measure the scans; the splice into d_out is queued on the context's stream. */
 int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                                          const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
                                          uint32_t n_frames, uint32_t width, uint32_t height, uint32_t color_type,

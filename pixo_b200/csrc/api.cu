@@ -1036,7 +1036,6 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
     // frame k's tables: its own (optimize), or the standard ones
     auto dht_of = [&](uint32_t k) { return optimize ? h_dht + (size_t)k * kDhtBytes : dht_standard(); };
     HuffTables t;
-    ProgResult prog;
     PIXO_TRY(grp.upload(0));
     for (uint32_t gi = 0; gi < grp.count(); ++gi) {
         if (gi + 1 < grp.count()) PIXO_TRY(grp.upload(gi + 1));
@@ -1062,21 +1061,36 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
         PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[gi & 1], ctx->stream));
         std::vector<ProgTables> pt(optimize ? cnt : 1);
         for (uint32_t k = 0; k < pt.size(); ++k) PIXO_TRY(dht_prog_tables(ctx, dht_of(k), &pt[k]));
-        PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, pt.data(), optimize, false, &prog));
+        ProgSlots slots;   // in d_prog_out, sized from the measured strings
+        PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, nullptr, pt.data(), optimize, nullptr, &slots));
+        // every segment's length and every frame's flags to h_prog
+        uint64_t *h_len;
+        uint32_t *h_ovf;
+        PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &H) {
+            h_len = H.take<uint64_t>((size_t)cnt * 7);
+            h_ovf = H.take<uint32_t>(cnt);
+        }, 8));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, slots.scan_len, (size_t)cnt * 7 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, slots.overflow, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         // SOF2 headers, then per scan its SOS and its segment (from the device), EOI
         for (uint32_t k = 0; k < cnt; ++k) {
+            if (h_ovf[k]) return set_error(ctx, PIXO_B200_ERR_CUDA, "progressive splice overflowed its slot");
             const uint32_t img = gi * grp.G + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
+            const uint64_t *len = h_len + (size_t)k * 7;
             huff_from_dht(dht_of(k), t);
             size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, t, restart_interval);
             size_t need = pos + 2;
-            for (int s = 0; s < 7; ++s) need += 10 + (size_t)prog.len[(size_t)k * 7 + s];
+            for (int s = 0; s < 7; ++s) need += 10 + (size_t)len[s];
             PIXO_TRY(check_room(ctx, out_cap_each, need));
+            const uint8_t *seg = slots.out + (size_t)k * slots.cap;
             for (int s = 0; s < 7; ++s) {
                 pos += write_sos_progressive(o + pos, s);
-                const size_t n = (size_t)prog.len[(size_t)k * 7 + s];
-                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, prog.stage + ((size_t)k * 7 + s) * prog.stage_cap, n, ctx->stream));
+                const size_t n = (size_t)len[s];
+                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, seg, n, ctx->stream));
                 pos += n;
+                seg += n;
             }
             o[pos] = 0xFF;
             o[pos + 1] = 0xD9;
@@ -1200,22 +1214,20 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
     PIXO_TRY(dht_prog_tables(ctx, dht ? dht : dht_standard(), &T));
     if (n_frames == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    // The splice kernels take one grid row per segment: at most 8192 frames (57 344 segments) per pass.
-    // More frames are checked first, so that a rejected coefficient leaves every output untouched.
+    // At most 8192 frames per pass, as pixo_b200_jpeg_encode_dev_progressive codes them.  More frames are
+    // checked first (the measuring half alone), so that a rejected coefficient leaves every output untouched.
     constexpr uint32_t kPass = 8192;
     const int16_t *cb = chroma ? d_cb : nullptr, *cr = chroma ? d_cr : nullptr;
     auto at = [](const int16_t *a, size_t stride, uint32_t i0) { return a ? a + (size_t)i0 * stride : nullptr; };
-    ProgResult res;
     if (n_frames > kPass)
         for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass)
             PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
-                                        c_stride, std::min(kPass, n_frames - i0), g, &T, false, true, &res));
+                                        c_stride, std::min(kPass, n_frames - i0), g, nullptr, &T, false, nullptr,
+                                        nullptr));
     for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass) {
-        const uint32_t cnt = std::min(kPass, n_frames - i0);
+        ProgSlots dst{d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7, d_overflow + i0};
         PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
-                                    c_stride, cnt, g, &T, false, false, &res));
-        PIXO_TRY(launch_progressive_pack(ctx, res, cnt, d_out + (size_t)i0 * out_cap_each, out_cap_each,
-                                         d_scan_len + (size_t)i0 * 7, d_overflow + i0));
+                                    c_stride, std::min(kPass, n_frames - i0), g, nullptr, &T, false, nullptr, &dst));
     }
     return 0;
 }
@@ -1327,9 +1339,8 @@ int pixo_b200_jpeg_encode_dev_progressive(pixo_b200_ctx *ctx, const uint8_t *d_p
         if (trellis)
             PIXO_TRY(trellis_pieces(ctx, px, pixel_stride, cnt, width, height, color_type, subsampling, lum, chr, L.y(c),
                                     cs, cb, cr, cs, false, &status));
-        PIXO_TRY(launch_progressive_queued(ctx, L.y(c), cs, cb, cr, cs, cnt, g, dht, status,
-                                           d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7,
-                                           d_overflow + i0));
+        ProgSlots dst{d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7, d_overflow + i0};
+        PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, dht, nullptr, false, status, &dst));
     }
     return 0;
 }

@@ -146,13 +146,13 @@ struct ProgTables {
     uint32_t ac[2][256];
 };
 
-// The 7 stuffed segments of each of n frames: segment q = frame * 7 + scan at stage + q * stage_cap, its
-// length in len[q] (host) and d_len[q] (device)
-struct ProgResult {
-    uint8_t *stage = nullptr;
-    size_t stage_cap = 0;
-    uint64_t *d_len = nullptr;
-    std::vector<uint64_t> len;
+// Where the progressive scans of n frames go: frame i's 7 stuffed segments back to back at out + i * cap, their
+// lengths at scan_len + i * 7, its flags at overflow[i] (device memory)
+struct ProgSlots {
+    uint8_t *out = nullptr;
+    uint64_t cap = 0;
+    uint64_t *scan_len = nullptr;
+    uint32_t *overflow = nullptr;
 };
 
 // One band of a frame's MCU rows for the progressive scans (pixo_b200_jpeg_band_dev_progressive): its blocks of
@@ -202,7 +202,7 @@ struct pixo_b200_ctx {
     pixo::DevBuf d_quant, d_quant_img;          // PNG quantisation: sample sort, then palettes / tables / indices
     pixo::DevBuf d_trellis;                     // JPEG trellis: status word + f32 DCT blocks
     pixo::DevBuf d_prog, d_prog_raw, d_prog_out;   // JPEG progressive scans: per-block state, raw strings,
-                                                   // stuffed segments
+                                                   // the splice's scratch (and the host loop's frame slots)
     pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
@@ -364,9 +364,7 @@ SegRaw seg_raw(const SegPlan &p, void *base);
 size_t seg_scratch_bytes(const SegPlan &p);   // the device scratch of its coding and splice
 // n whole raw strings of raw_cap bytes each, spliced on their own (no segments)
 SegPlan splice_plan(uint32_t n, size_t raw_cap);
-int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area, uint8_t *d_out,
-                  uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow);
-// launch_splice for whole-string plans (S == 1) that writes an image only when all of it fits: a string whose
+// The splice of a whole-string plan (S == 1) that writes an image only when all of it fits: a string whose
 // stuffed bytes exceed out_cap gets overflow bit 0, its length in d_out_len and nothing in d_out.  bounds:
 // [n][nr + 1] bit offsets into each string, multiples of 8, the last its bit count; range_len ([n][nr]) receives
 // the stuffed bytes between consecutive bounds of every string that has bytes.
@@ -376,22 +374,22 @@ int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_sc
 
 // progressive scans (jpeg_progressive.cu)
 bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
+// The 7 scans of n whole frames into *dst.  Tables and the raw strings:
+//  - d_dht: frame i's from its DHT block at d_dht + i * kDhtBytes, queued without a wait; a frame's raw string
+//    is as long as its slot (dst->cap + 16 bytes), and a frame whose raw bytes exceed dst->cap is left out
+//    (overflow bit 0).  d_trellis_status (or null) is folded into the frames' flags.
+//  - otherwise the host's T (n when per_frame, else 1), and a wait for the bit counts: a coefficient out of
+//    range is refused before anything is written, and each raw string is as long as the longest frame's, so
+//    only the splice decides the fit.  dst null: nothing is coded; dst->out null: per-frame slots of twice the
+//    longest string, which every frame fits, in d_prog_out, set in *dst.
 int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
-                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                       const ProgTables *T, bool per_frame, bool check_only, ProgResult *res);
-int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
-                            uint64_t *d_scan_len, uint32_t *d_overflow);
+                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g, const uint8_t *d_dht,
+                       const ProgTables *T, bool per_frame, const uint32_t *d_trellis_status, ProgSlots *dst);
 // one band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive, _summary)
 int launch_progressive_band_summary(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                                     uint64_t ny, uint64_t nc, uint64_t y_base, uint64_t c_base, ProgBandSummary *out);
 int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_t *d_cb, const int16_t *d_cr,
                             const ProgBand &B, const uint64_t *d_hist, uint8_t *d_dht_out, uint8_t *d_raw,
                             size_t raw_cap, size_t *raw_need, uint64_t nbits[7], uint32_t tail7[7]);
-// the stage of pixo_b200_jpeg_encode_dev_progressive, without a wait: frame i's tables from d_dht + i * kDhtBytes,
-// d_trellis_status (or null) folded into the frames' flags (jpeg_progressive.cu)
-int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
-                              const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                              const uint8_t *d_dht, const uint32_t *d_trellis_status, uint8_t *d_out, uint64_t out_cap,
-                              uint64_t *d_scan_len, uint32_t *d_overflow);
 
 }  // namespace pixo

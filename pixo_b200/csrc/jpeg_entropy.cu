@@ -1836,15 +1836,7 @@ SegPlan splice_plan(uint32_t n, size_t raw_cap)
     return p;
 }
 
-// The progressive scans' strings: each a whole stream of its own (base bit 0, 1-padded at its end)
-int launch_splice(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area, uint8_t *d_out,
-                  uint64_t out_cap, uint64_t *d_out_len, uint32_t *d_overflow)
-{
-    return splice_segments(ctx, sp, seg_scratch, raw_area, nullptr, 0, 0, true, nullptr, d_out, out_cap, d_out_len,
-                           d_overflow);
-}
-
-// The progressive scans of pixo_b200_jpeg_encode_dev_progressive: every frame one string, its scans byte-aligned in it.
+// The progressive scans of whole frames: every frame one string, its scans byte-aligned in it.
 // k_seg_fit runs between the prefix of the tiles' 0xFF counts and the emission, so that a frame is written whole or
 // not at all.  d_overflow must be set before (k_seg_emit only ORs into it).
 int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_scratch, const uint8_t *raw_area,

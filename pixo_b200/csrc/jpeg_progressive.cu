@@ -23,20 +23,20 @@
 //   k_prog_carry    per stream: exclusive running maximum of the tiles' last non-empty blocks
 //   k_prog_count    per block: the EOB-run flushes it emits, added to its length; tile bit totals
 //   k_prog_offsets  per stream: exclusive prefix of the tile totals (u64) and the stream's bit count
-//   (host)          reads the bit counts back: the raw area is then sized exactly, so no string can
-//                   outgrow it
-//   k_prog_emit     per block: its bit offset (tile prefix + CTA scan), its bits OR-ed into the
-//                   zeroed raw string (MSB first)
-//   k_seg_*         (jpeg_entropy.cu) splice every raw string into stuffed, 1-padded bytes
-//   k_prog_pack     (device entry) the 7 segments of a frame back to back in the caller's slot
-// The queued stage (pixo_b200_jpeg_encode_dev_progressive) reads nothing back: k_prog_dht_tables builds each
-// frame's tables from its DHT block, k_prog_place lays the frame's 7 streams out byte-aligned in ONE string of
-// out_cap + 16 bytes and decides the fit from the raw bytes, k_prog_emit_at codes into it, and the splice (with
-// k_seg_fit, which decides the fit from the stuffed bytes) writes the 7 segments straight into the caller's slot.
+//   k_prog_place    per frame: its 7 streams laid out byte-aligned in ONE zeroed raw string, whether the
+//                   frame is coded (see the capacity below), the 1-padding of each stream's last byte
+//   k_prog_emit_at  per block: its bit offset (stream start + tile prefix + CTA scan), its bits OR-ed into
+//                   the frame's string (MSB first)
+//   k_seg_*         (jpeg_entropy.cu) splice each frame's string into its 7 stuffed, 1-padded segments
+//                   back to back in the caller's slot; k_seg_fit writes a frame whole or not at all
+// The tables come from the frames' DHT blocks (k_prog_dht_tables) or from the host.  A frame's raw string
+// is sized from the slot's capacity (out_cap + 16 bytes, nothing read back; k_prog_place leaves out a frame
+// whose raw bytes exceed out_cap), or from the bit counts read back after k_prog_offsets, so that every
+// frame is coded and k_seg_fit alone decides the fit.
 // Nothing spins on another CTA, so no step can hang: a fault is a CUDA error.
 // One band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive*) runs measure / carry / count /
-// offsets / emit in their band mode (BAND = true, see ProgParams), then k_prog_band_trailer; k_prog_band_last is
-// the band's summary for the bands after it.
+// offsets / emit in their band mode (BAND = true, see ProgParams), each stream a string of its own, then
+// k_prog_band_trailer; k_prog_band_last is the band's summary for the bands after it.
 #include <string.h>
 
 #include <algorithm>
@@ -66,8 +66,9 @@ struct ProgParams {
     uint32_t *tile_bits;             // [n][tiles]
     unsigned long long *tile_off;    // [n][tiles]: bits of the stream before the tile
     unsigned long long *bits;        // [n * NSCAN]: bits of each stream
-    uint32_t *raw;                   // [n * NSCAN][raw_cap / 4] big-endian words, zeroed before k_prog_emit
-    unsigned long long raw_words;    // words per stream
+    uint32_t *raw;                   // big-endian words, zeroed before the emission: one string per frame (see
+                                     // ProgPlace), or per stream of a band
+    unsigned long long raw_words;    // words per string
     uint32_t *status;                // bit 0: a coefficient outside -16383..16383
     const ProgTables *tables;        // [n] per frame, or [1] for every frame
     uint32_t tables_per_frame;       // 1 or 0
@@ -360,30 +361,30 @@ __global__ void __launch_bounds__(PT) k_prog_offsets(const __grid_constant__ Pro
 
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
 
-// Where the queued stage puts a frame's 7 streams: one string per frame in P.raw (P.raw_words words per
-// frame), stream s from bit start[frame * 8 + s] on, each padded with 1s to a whole byte, so that the splice of
-// the frame's string is its 7 segments back to back.  start[frame * 8 + 7]: the string's bits.
+// Where whole frames' 7 streams go: one string per frame in P.raw (P.raw_words words per frame), stream s
+// from bit start[frame * 8 + s] on, each padded with 1s to a whole byte, so that the splice of the frame's
+// string is its 7 segments back to back.  start[frame * 8 + 7]: the string's bits.
 struct ProgPlace {
     unsigned long long *start;       // [n][8]
     unsigned long long *str_bits;    // [n]: the string's bits for the splice, 0 = the frame is skipped
     unsigned long long *str_tails;   // [n]: 0 (every string starts on a byte)
     const uint32_t *trellis_status;  // bit 0: COEF_TRELLIS rejected its input, or null
-    unsigned long long out_cap;
+    unsigned long long out_cap;      // the raw bytes a coded frame may have, at most the string's
     unsigned long long *scan_len;    // [n][7] the caller's
     uint32_t *overflow;              // [n] the caller's
 };
 
-// Per block: flushes and symbols OR-ed into the stream's zeroed raw words at the block's bit offset.
-// AT: into the frame's string at the stream's start (ProgPlace), skipping frames that are not spliced.
-// BAND: one band of a frame (see ProgParams).
-template <bool AT, bool BAND>
+// Per block: flushes and symbols OR-ed into the zeroed raw words at the block's bit offset.  Whole frames:
+// into the frame's string at the stream's start (ProgPlace), skipping frames that are not spliced.  BAND:
+// one band of a frame (see ProgParams), each stream a string of its own.
+template <bool BAND>
 __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &Q)
 {
     __shared__ ProgTables T;
     __shared__ uint32_t sh[PT / 32];
     __shared__ unsigned long long sh64[PT / 32];
     const TileId id = tile_id(P, blockIdx.x);
-    if (AT && Q.str_bits[id.frame] == 0) return;   // (uniform per CTA)
+    if (!BAND && Q.str_bits[id.frame] == 0) return;   // (uniform per CTA)
     load_tables(P, id.frame, T);
     const int comp = scan_comp(id.scan), ss = scan_ss(id.scan), se = scan_se(id.scan);
     const bool dc_scan = ss == 0;
@@ -401,8 +402,8 @@ __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &
     unsigned long long all;
     unsigned long long pos = P.tile_off[tix] + cta_scan_excl<unsigned long long>(len, 0ull, sh64, &all, AddOp());
     if (!live || len == 0) return;
-    uint32_t *words = P.raw + (size_t)(AT ? id.frame : id.frame * NSCAN + id.scan) * P.raw_words;
-    if (AT) pos += Q.start[(size_t)id.frame * 8 + id.scan];
+    uint32_t *words = P.raw + (size_t)(BAND ? id.frame * NSCAN + id.scan : id.frame) * P.raw_words;
+    if (!BAND) pos += Q.start[(size_t)id.frame * 8 + id.scan];
     auto put = [&](uint32_t val, uint32_t n) {
         if (n == 0) return;
         const uint32_t al = val << (32u - n);
@@ -423,23 +424,26 @@ __device__ __forceinline__ void prog_emit(const ProgParams &P, const ProgPlace &
     if (f.after) code_eobrun(f.after, T.ac[lum], put);
 }
 
+// One band of a frame (its streams' strings, see launch_progressive_band); whole frames go through k_prog_emit_at
 template <bool BAND>
 __global__ void __launch_bounds__(PT) k_prog_emit(const __grid_constant__ ProgParams P)
 {
-    prog_emit<false, BAND>(P, ProgPlace{});
+    static_assert(BAND, "whole frames are coded by k_prog_emit_at");
+    prog_emit<true>(P, ProgPlace{});
 }
 
 __global__ void __launch_bounds__(PT) k_prog_emit_at(const __grid_constant__ ProgParams P, const __grid_constant__ ProgPlace Q)
 {
-    prog_emit<true, false>(P, Q);
+    prog_emit<false>(P, Q);
 }
 
-// Per frame (one thread): the streams' places in the frame's string (ProgPlace), whether the string can fit
-// the caller's slot, and the 1-padding of each stream's last byte (the raw area is zeroed, k_prog_emit_at ORs
-// its bits in afterwards).  Raw bytes never exceed the stuffed ones, so a string longer than out_cap cannot fit
-// (overflow bit 0), and one that is not longer fits its raw area (out_cap + 16 bytes).  A frame of a pass whose
-// coefficients the trellis or this stage rejected gets kOvfInput.  scan_len: each stream's bytes x 2, room for any
-// stuffing; the splice overwrites it with the exact lengths of the frames it splices.
+// Per frame (one thread): the streams' places in the frame's string (ProgPlace), whether the frame is coded,
+// and the 1-padding of each stream's last byte (the raw area is zeroed, k_prog_emit_at ORs its bits in
+// afterwards).  A string of more than Q.out_cap raw bytes is left out (overflow bit 0): with the caller's slot
+// capacity there, raw bytes never exceed the stuffed ones, so it could not fit, and one that is not longer fits
+// its raw area (out_cap + 16 bytes).  A frame of a pass whose coefficients the trellis or this stage rejected
+// gets kOvfInput.  scan_len: each stream's bytes x 2, room for any stuffing; the splice overwrites it with the
+// exact lengths of the frames it splices.
 __global__ void __launch_bounds__(128) k_prog_place(const __grid_constant__ ProgParams P, const __grid_constant__ ProgPlace Q)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -493,32 +497,6 @@ __global__ void __launch_bounds__(128) k_prog_dht_tables(const uint8_t *dht, Pro
         }
         code <<= 1;
     }
-}
-
-// Per frame: the 7 spliced segments back to back at out + frame * out_cap, their lengths, and
-// overflow bit 0 (nothing copied) when they do not fit
-// (ctas CTAs per segment, sized by the host from the longest segment)
-__global__ void __launch_bounds__(PT) k_prog_pack(uint32_t ctas, const uint8_t *stage, unsigned long long stage_cap,
-                                                  const unsigned long long *seg_len, uint8_t *out,
-                                                  unsigned long long out_cap, unsigned long long *scan_len,
-                                                  uint32_t *overflow)
-{
-    const uint32_t frame = blockIdx.y, s = blockIdx.x / ctas, part = blockIdx.x % ctas;
-    const unsigned long long *L = seg_len + (size_t)frame * NSCAN;
-    unsigned long long off = 0, total = 0;
-    for (uint32_t k = 0; k < NSCAN; ++k) {
-        if (k < s) off += L[k];
-        total += L[k];
-    }
-    if (part == 0 && threadIdx.x == 0) {
-        scan_len[(size_t)frame * NSCAN + s] = L[s];
-        if (s == 0) overflow[frame] = total > out_cap ? 1u : 0u;
-    }
-    if (total > out_cap) return;
-    const uint8_t *src = stage + ((size_t)frame * NSCAN + s) * stage_cap;
-    uint8_t *dst = out + (size_t)frame * out_cap + off;
-    for (unsigned long long j = (unsigned long long)part * PT + threadIdx.x; j < L[s]; j += (unsigned long long)ctas * PT)
-        dst[j] = src[j];
 }
 
 // ---- one band of a frame tiled over several GPUs (pixo_b200_jpeg_band_dev_progressive*) ----------------------------
@@ -633,13 +611,18 @@ bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTa
     return true;
 }
 
-// The scans' block and tile counts of one frame into P
-static void prog_counts(const FrameGeometry &g, ProgParams &P)
+// The scans' block and tile counts of one band of a frame into P (a whole frame is the band of all its blocks),
+// and what the frame's earlier bands leave it
+static void prog_counts(const ProgBand &B, ProgParams &P)
 {
     uint32_t tb = 0;
     uint64_t bb = 0;
     for (int s = 0; s < NSCAN; ++s) {
-        P.nb[s] = kComp[s] == 0 ? g.ny : g.nc;
+        const bool y = kComp[s] == 0;
+        P.nb[s] = y ? B.ny : B.nc;
+        P.gbase[s] = y ? B.y_base : B.c_base;
+        P.gnb[s] = y ? B.frame_ny : B.frame_nc;
+        P.carry_in[s] = s >= 3 ? B.ac_carry[s - 3] : 0u;
         P.tile_base[s] = tb;
         P.blk_base[s] = bb;
         tb += (uint32_t)((P.nb[s] + PT - 1) / PT);
@@ -647,171 +630,127 @@ static void prog_counts(const FrameGeometry &g, ProgParams &P)
     }
     P.tile_base[NSCAN] = tb;
     P.blk_base[NSCAN] = bb;
+    for (int k = 0; k < 3; ++k) P.dc_seed[k] = B.dc_seed[k];
 }
 
-// Measure (and with !check_only, code) the 7 scans of n frames.  Waits for the device twice: after the
-// bit counts (to size the raw strings exactly) and after the splice (segment lengths to the host).
-int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
-                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                       const ProgTables *T, bool per_frame, bool check_only, ProgResult *res)
+// The per-block state of P.n frames (or of one band) in L, and room for P.n tables, which it returns
+static ProgTables *take_state(Layout &L, ProgParams &P)
+{
+    const size_t tiles = (size_t)P.n * P.tile_base[NSCAN], blocks = (size_t)P.n * P.blk_base[NSCAN];
+    P.status = L.take<uint32_t>(1);
+    P.blen = L.take<uint32_t>(blocks);
+    P.flag = L.take(blocks);
+    P.tile_last = L.take<uint32_t>(tiles);
+    P.tile_carry = L.take<uint32_t>(tiles);
+    P.tile_bits = L.take<uint32_t>(tiles);
+    P.tile_off = L.take<unsigned long long>(tiles);
+    P.bits = L.take<unsigned long long>((size_t)P.n * NSCAN);
+    ProgTables *tables = L.take<ProgTables>(P.n);
+    P.tables = tables;
+    return tables;
+}
+
+// The measuring half of a whole-frame pass: the per-block state and the streams' places in d_prog, the tables
+// (from the frames' DHT blocks when d_dht is not null, else the host's T), k_prog_measure / carry / count / offsets
+static int prog_measure(pixo_b200_ctx *ctx, ProgParams &P, ProgPlace &Q, const uint8_t *d_dht, const ProgTables *T,
+                        bool per_frame)
 {
     cudaStream_t st = ctx->stream;
-    ProgParams P;
-    memset(&P, 0, sizeof P);
-    prog_counts(g, P);
-    const size_t tiles = (size_t)n * P.tile_base[NSCAN], blocks = (size_t)n * P.blk_base[NSCAN];
+    const uint32_t n = P.n;
+    const unsigned tiles = n * P.tile_base[NSCAN];   // (every frame has a Y block)
     ProgTables *d_tables;
     PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
-        P.status = L.take<uint32_t>(1);
-        P.blen = L.take<uint32_t>(blocks);
-        P.flag = L.take(blocks);
-        P.tile_last = L.take<uint32_t>(tiles);
-        P.tile_carry = L.take<uint32_t>(tiles);
-        P.tile_bits = L.take<uint32_t>(tiles);
-        P.tile_off = L.take<unsigned long long>(tiles);
-        P.bits = L.take<unsigned long long>((size_t)n * NSCAN);
-        P.tables = d_tables = L.take<ProgTables>(n);
-    }));
-    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
-    P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
-    P.n = n;
-    P.tables_per_frame = per_frame ? 1u : 0u;
-    if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive stage: too many blocks per call");
-    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(d_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
-    if (tiles) {
-        PIXO_TRY(launch(ctx, k_prog_measure<false>, (unsigned)tiles, PT, 0, P));
-        PIXO_TRY(launch(ctx, k_prog_carry<false>, n * NSCAN, PT, 0, P));
-        PIXO_TRY(launch(ctx, k_prog_count<false>, (unsigned)tiles, PT, 0, P));
-    }
-    PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
-    // h_prog: the status word, every stream's bit count (then its segment's length), the splice's flags
-    const size_t nstream = (size_t)n * NSCAN;
-    uint32_t *h_status, *h_ovf = nullptr;
-    uint64_t *h_bits;
-    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
-        h_status = L.take<uint32_t>(1);
-        h_bits = L.take<uint64_t>(nstream);
-        if (!check_only) h_ovf = L.take<uint32_t>(nstream);
-    }, 8));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, nstream * 8, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
-    if (*h_status)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
-                         "coefficient out of the progressive range (-16383..16383)");
-    if (check_only) return 0;
-
-    // raw strings, sized by the longest stream
-    uint64_t max_bytes = 0;
-    for (size_t q = 0; q < nstream; ++q) max_bytes = std::max<uint64_t>(max_bytes, (h_bits[q] + 7) / 8);
-    const size_t raw_cap = Layout::round((size_t)max_bytes + 16);
-    const SegPlan sp = splice_plan(n * NSCAN, raw_cap);
-    const size_t stage_cap = Layout::round(2 * raw_cap + 1);   // every byte 0xFF still fits
-    // d_prog_out: the splice's scratch, every segment's length and flags, the segments
-    uint8_t *scratch, *stage;
-    uint64_t *d_len;
-    uint32_t *d_ovf;
-    PIXO_TRY(bind(ctx, ctx->d_prog_out, [&](Layout &L) {
-        scratch = L.take(seg_scratch_bytes(sp));
-        d_len = L.take<uint64_t>(nstream);
-        d_ovf = L.take<uint32_t>(nstream);
-        stage = L.take(nstream * stage_cap);
-    }));
-    PIXO_TRY(ctx->d_prog_raw.ensure(ctx, seg_raw(sp, nullptr).total));
-    const SegRaw raw = seg_raw(sp, ctx->d_prog_raw.ptr);
-    PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, raw.total, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(raw.bits, P.bits, nstream * 8, cudaMemcpyDeviceToDevice, st));
-    PIXO_CUDA(ctx, cudaMemsetAsync(d_ovf, 0, nstream * 4, st));
-    P.raw = reinterpret_cast<uint32_t *>(raw.strings);
-    P.raw_words = raw_cap / 4;
-    if (tiles) PIXO_TRY(launch(ctx, k_prog_emit<false>, (unsigned)tiles, PT, 0, P));
-    PIXO_TRY(launch_splice(ctx, sp, scratch, raw.strings, stage, stage_cap, d_len, d_ovf));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, d_len, nstream * 8, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, d_ovf, nstream * 4, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
-    res->len.assign(h_bits, h_bits + nstream);
-    for (size_t q = 0; q < nstream; ++q)
-        if (h_ovf[q]) return set_error(ctx, PIXO_B200_ERR_CUDA, "progressive splice overflowed its exact-size buffer");
-    res->stage = stage;
-    res->stage_cap = stage_cap;
-    res->d_len = d_len;
-    return 0;
-}
-
-int launch_progressive_pack(pixo_b200_ctx *ctx, const ProgResult &res, uint32_t n, uint8_t *d_out, uint64_t out_cap,
-                            uint64_t *d_scan_len, uint32_t *d_overflow)
-{
-    uint64_t longest = 0;
-    for (uint64_t l : res.len) longest = std::max(longest, l);
-    const uint32_t ctas = (uint32_t)std::min<uint64_t>(2048, std::max<uint64_t>(1, (longest + PT * 64 - 1) / (PT * 64)));
-    return launch(ctx, k_prog_pack, dim3(NSCAN * ctas, n), PT, 0, ctas, res.stage, res.stage_cap,
-                  reinterpret_cast<const unsigned long long *>(res.d_len), d_out, out_cap,
-                  reinterpret_cast<unsigned long long *>(d_scan_len), d_overflow);
-}
-
-// The stage of a pass of n frames, queued without a wait (pixo_b200_jpeg_encode_dev_progressive): frame i's tables
-// from its DHT block at d_dht + i * kDhtBytes, its 7 segments back to back at d_out + i * out_cap, their lengths
-// and the frame's flags in d_scan_len / d_overflow.  The raw area holds one string of out_cap + 16 bytes per frame,
-// so nothing has to be read back to size it.  12 launches: k_prog_dht_tables, the four measuring kernels,
-// k_prog_place, k_prog_emit_at and the splice (launch_splice_bounded: five).
-int launch_progressive_queued(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
-                              const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g,
-                              const uint8_t *d_dht, const uint32_t *d_trellis_status, uint8_t *d_out, uint64_t out_cap,
-                              uint64_t *d_scan_len, uint32_t *d_overflow)
-{
-    cudaStream_t st = ctx->stream;
-    ProgParams P;
-    memset(&P, 0, sizeof P);
-    prog_counts(g, P);
-    const size_t tiles = (size_t)n * P.tile_base[NSCAN], blocks = (size_t)n * P.blk_base[NSCAN];
-    ProgTables *d_tables;
-    ProgPlace Q;
-    PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
-        P.status = L.take<uint32_t>(1);
-        P.blen = L.take<uint32_t>(blocks);
-        P.flag = L.take(blocks);
-        P.tile_last = L.take<uint32_t>(tiles);
-        P.tile_carry = L.take<uint32_t>(tiles);
-        P.tile_bits = L.take<uint32_t>(tiles);
-        P.tile_off = L.take<unsigned long long>(tiles);
-        P.bits = L.take<unsigned long long>((size_t)n * NSCAN);
-        P.tables = d_tables = L.take<ProgTables>(n);
+        d_tables = take_state(L, P);
         Q.start = L.take<unsigned long long>((size_t)n * 8);
     }));
-    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
-    P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
-    P.n = n;
-    P.tables_per_frame = 1;
-    const size_t raw_cap = Layout::round((size_t)out_cap + 16);
-    const SegPlan sp = splice_plan(n, raw_cap);
+    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
+    if (d_dht)
+        PIXO_TRY(launch(ctx, k_prog_dht_tables, n, 128, 0, d_dht, d_tables));
+    else
+        PIXO_CUDA(ctx, cudaMemcpyAsync(d_tables, T, (per_frame ? n : 1) * sizeof(ProgTables), cudaMemcpyHostToDevice, st));
+    PIXO_TRY(launch(ctx, k_prog_measure<false>, tiles, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_carry<false>, n * NSCAN, PT, 0, P));
+    PIXO_TRY(launch(ctx, k_prog_count<false>, tiles, PT, 0, P));
+    return launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P);
+}
+
+// The coding half: every frame's string of raw_each bytes in d_prog_raw, k_prog_place (a frame of more than
+// place_cap raw bytes is left out), k_prog_emit_at and the splice into dst (launch_splice_bounded: five launches).
+// dst.out null: slots of dst.cap bytes, their lengths and flags in d_prog_out, to dst.
+static int prog_code(pixo_b200_ctx *ctx, ProgParams &P, ProgPlace &Q, size_t raw_each, uint64_t place_cap,
+                     const uint32_t *d_trellis_status, ProgSlots &dst)
+{
+    const uint32_t n = P.n;
+    const SegPlan sp = splice_plan(n, raw_each);
+    const bool own = dst.out == nullptr;
     uint8_t *scratch;
     uint64_t *d_len;
+    // d_prog_out: the splice's scratch, every frame's spliced length, and the slots the pass owns
     PIXO_TRY(bind(ctx, ctx->d_prog_out, [&](Layout &L) {
         scratch = L.take(seg_scratch_bytes(sp));
         d_len = L.take<uint64_t>(n);
+        if (own) {
+            dst.out = L.take((size_t)n * dst.cap);
+            dst.scan_len = L.take<uint64_t>((size_t)n * NSCAN);
+            dst.overflow = L.take<uint32_t>(n);
+        }
     }));
     PIXO_TRY(ctx->d_prog_raw.ensure(ctx, seg_raw(sp, nullptr).total));
     const SegRaw raw = seg_raw(sp, ctx->d_prog_raw.ptr);
     P.raw = reinterpret_cast<uint32_t *>(raw.strings);
-    P.raw_words = raw_cap / 4;
+    P.raw_words = raw_each / 4;
     Q.str_bits = raw.bits;
     Q.str_tails = raw.tails;
     Q.trellis_status = d_trellis_status;
-    Q.out_cap = out_cap;
-    Q.scan_len = reinterpret_cast<unsigned long long *>(d_scan_len);
-    Q.overflow = d_overflow;
-    PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
-    PIXO_TRY(launch(ctx, k_prog_dht_tables, n, 128, 0, d_dht, d_tables));
-    PIXO_TRY(launch(ctx, k_prog_measure<false>, (unsigned)tiles, PT, 0, P));   // (every frame has a Y block)
-    PIXO_TRY(launch(ctx, k_prog_carry<false>, n * NSCAN, PT, 0, P));
-    PIXO_TRY(launch(ctx, k_prog_count<false>, (unsigned)tiles, PT, 0, P));
-    PIXO_TRY(launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P));
-    PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, (size_t)n * raw_cap, st));
+    Q.out_cap = place_cap;
+    Q.scan_len = reinterpret_cast<unsigned long long *>(dst.scan_len);
+    Q.overflow = dst.overflow;
+    PIXO_CUDA(ctx, cudaMemsetAsync(raw.strings, 0, (size_t)n * raw_each, ctx->stream));
     PIXO_TRY(launch(ctx, k_prog_place, (n + 127) / 128, 128, 0, P, Q));
-    PIXO_TRY(launch(ctx, k_prog_emit_at, (unsigned)tiles, PT, 0, P, Q));
-    return launch_splice_bounded(ctx, sp, scratch, raw.strings, d_out, out_cap, d_len, d_overflow, Q.start, NSCAN,
-                                 d_scan_len);
+    PIXO_TRY(launch(ctx, k_prog_emit_at, n * P.tile_base[NSCAN], PT, 0, P, Q));
+    return launch_splice_bounded(ctx, sp, scratch, raw.strings, dst.out, dst.cap, d_len, dst.overflow, Q.start, NSCAN,
+                                 dst.scan_len);
+}
+
+int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
+                       const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g, const uint8_t *d_dht,
+                       const ProgTables *T, bool per_frame, const uint32_t *d_trellis_status, ProgSlots *dst)
+{
+    ProgParams P;
+    memset(&P, 0, sizeof P);
+    prog_counts(ProgBand{g.ny, g.nc, 0, 0, g.ny, g.nc, {}, {}}, P);
+    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
+    P.stride[0] = y_stride; P.stride[1] = P.stride[2] = c_stride;
+    P.n = n;
+    P.tables_per_frame = d_dht || per_frame ? 1u : 0u;
+    if ((size_t)n * P.tile_base[NSCAN] > 0x7FFFFFFFull)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive stage: too many blocks per call");
+    ProgPlace Q;
+    PIXO_TRY(prog_measure(ctx, P, Q, d_dht, T, per_frame));
+    if (d_dht) return prog_code(ctx, P, Q, Layout::round(dst->cap + 16), dst->cap, d_trellis_status, *dst);
+
+    // measured: the status word and every stream's bit count to h_prog
+    uint32_t *h_status;
+    uint64_t *h_bits;
+    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
+        h_status = L.take<uint32_t>(1);
+        h_bits = L.take<uint64_t>((size_t)n * NSCAN);
+    }, 8));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, (size_t)n * NSCAN * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (*h_status)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    if (!dst) return 0;
+    uint64_t longest = 0;   // raw bytes of the longest frame string (its streams byte-aligned, see k_prog_place)
+    for (uint32_t i = 0; i < n; ++i) {
+        uint64_t bytes = 0;
+        for (int s = 0; s < NSCAN; ++s) bytes += (h_bits[(size_t)i * NSCAN + s] + 7) / 8;
+        longest = std::max(longest, bytes);
+    }
+    if (!dst->out) dst->cap = Layout::round(2 * longest);   // stuffing at most doubles a byte: every frame fits
+    const size_t raw_each = Layout::round(longest + 16);
+    return prog_code(ctx, P, Q, raw_each, raw_each, nullptr, *dst);
 }
 
 // The band summary: the last DC of each component, the largest enc_of (frame index) of each AC scan.  Waits for
@@ -850,42 +789,19 @@ int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_
     cudaStream_t st = ctx->stream;
     ProgParams P;
     memset(&P, 0, sizeof P);
-    uint32_t tb = 0;
-    uint64_t bb = 0;
-    for (int s = 0; s < NSCAN; ++s) {
-        const bool y = kComp[s] == 0;
-        P.nb[s] = y ? B.ny : B.nc;
-        P.gbase[s] = y ? B.y_base : B.c_base;
-        P.gnb[s] = y ? B.frame_ny : B.frame_nc;
-        P.carry_in[s] = s >= 3 ? B.ac_carry[s - 3] : 0u;
-        P.tile_base[s] = tb;
-        P.blk_base[s] = bb;
-        tb += (uint32_t)((P.nb[s] + PT - 1) / PT);
-        bb += P.nb[s];
-    }
-    P.tile_base[NSCAN] = tb;
-    P.blk_base[NSCAN] = bb;
-    for (int k = 0; k < 3; ++k) P.dc_seed[k] = B.dc_seed[k];
+    prog_counts(B, P);
+    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
+    P.n = 1;
     const size_t tiles = P.tile_base[NSCAN], blocks = P.blk_base[NSCAN];
     if (tiles > 0x7FFFFFFFull) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "progressive band: too many blocks");
     ProgTables *d_tables;
     uint8_t *dht;
     ProgBandRaw R;
     PIXO_TRY(bind(ctx, ctx->d_prog, [&](Layout &L) {
-        P.status = L.take<uint32_t>(1);
-        P.blen = L.take<uint32_t>(blocks);
-        P.flag = L.take(blocks);
-        P.tile_last = L.take<uint32_t>(tiles);
-        P.tile_carry = L.take<uint32_t>(tiles);
-        P.tile_bits = L.take<uint32_t>(tiles);
-        P.tile_off = L.take<unsigned long long>(tiles);
-        P.bits = L.take<unsigned long long>(NSCAN);
-        P.tables = d_tables = L.take<ProgTables>(1);
+        d_tables = take_state(L, P);
         dht = L.take(kDhtBytes);
         R.tail7 = L.take<unsigned long long>(NSCAN);
     }));
-    P.arr[0] = d_y; P.arr[1] = d_cb; P.arr[2] = d_cr;
-    P.n = 1;
     uint32_t *h_status;
     uint64_t *h_bits, *h_tails;
     PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {

@@ -286,7 +286,8 @@ def progressive_scans_dev(d_y, d_cb, d_cr, width, height, color_type=ColorType.R
     """The progressive scan stage on device coefficient arrays (int16 torch tensors in
     compute_all_coefficients' layout, natural order, 16-byte aligned; frame i at i * stride elements).
     tables: None for the standard tables, a uint8 [4, 272] array (dht_array) or a DHT dict.
-    Returns (d_out, d_scan_len [n, 7], d_overflow [n]) - new tensors when not given."""
+    Returns (d_out, d_scan_len [n, 7], d_overflow [n]) - new tensors when not given - once the context's stream
+    has written them, so that they can be read on any stream."""
     import torch
     ctx = ctx or default_context()
     ny, nc = block_counts(width, height, color_type, subsampling)
@@ -310,6 +311,7 @@ def progressive_scans_dev(d_y, d_cb, d_cr, width, height, color_type=ColorType.R
         int(color_type), int(subsampling), None if dht is None else dht.ctypes.data, ptr(d_out), int(out_cap_each),
         ptr(d_scan_len), ptr(d_overflow))
     _lib.check(ctx.handle, rc)
+    ctx.sync()   # the call itself waits only for the bit counts; its splice into d_out is queued
     return d_out, d_scan_len, d_overflow
 
 

@@ -226,10 +226,12 @@ EXPECTED = {
     "png_adaptive_optimize_alpha": 1,
     "png_bigrams": 1,
     "png_small_sub": 1,
-    "progressive": 10,
-    "progressive_batch": 32,               # k_huff_tables once per group (two groups of one)
-    "progressive_optimized_trellis": 16,   # k_huff_tables after K3
-    "progressive_scans_dev": 10,
+    # progressive scans: k_prog_place and k_seg_fit in, k_prog_pack out (one splice per frame string, written
+    # straight into the slot): 10, 32, 16 and 10 with a string per scan and a copy out of a stage buffer
+    "progressive": 12,
+    "progressive_batch": 36,               # k_huff_tables once per group (two groups of one)
+    "progressive_optimized_trellis": 18,   # k_huff_tables after K3
+    "progressive_scans_dev": 11,
     "quantize": 8,
     "quantize_auto": 8,
     "quantize_dither": 8,

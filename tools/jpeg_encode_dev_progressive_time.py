@@ -6,7 +6,7 @@ profiles/h100_jpeg_encode_dev_progressive.json: the card's name and power limit,
     the call returns with its files in host memory);
   - the scan stage alone on the same frames' coefficients: the queued stage (encode_dev_progressive without
     trellis and with the standard tables, minus the transform and k_huff_tables, timed on their own) against
-    pixo_b200_jpeg_progressive_scans_dev, which waits for the device twice;
+    pixo_b200_jpeg_progressive_scans_dev, which waits for the device for the bit counts;
   - a small-batch pipeline: CALLS calls of FEW 1080p frames each, queued back to back with one synchronisation
     at the end, against the same files through the waiting routes (encode_progressive_batch per call, from pinned
     memory), host clock around each whole pipeline;
@@ -176,7 +176,7 @@ def main():
          "transform_device_ms": events_ms(transform, stream),
          "progressive_scans_dev_host_ms": host_ms(lambda: (scans_dev(), ctx.sync())),
          "note": "the queued stage is encode_dev_progressive minus the transform and k_huff_tables (see kernels_ms); "
-                 "progressive_scans_dev waits for the device twice, so it is timed by the host clock to its end"}
+                 "progressive_scans_dev waits for the device, so it is timed by the host clock to its end"}
     rec["configs"]["scan_stage_420_q80_32x4k"] = r
     print("stage", json.dumps(r), flush=True)
     rec["kernels_ms"] = {"max_420_q80_32x4k": kernel_ms(lambda: d.call(ctx, px, each, mx), ctx),

@@ -74,8 +74,9 @@ def kernel_ms(fn, ctx, names):
     return {k: round(v, 3) for k, v in sorted(kt.items())}
 
 
-PROG_KERNELS = ("k_prog_measure", "k_prog_carry", "k_prog_count", "k_prog_offsets", "k_prog_emit", "k_prog_pack",
-                "k_seg_prefix", "k_seg_count", "k_seg_scan", "k_seg_emit")
+# (a kernel's time goes to the first name it contains: k_prog_emit_at before k_prog_emit)
+PROG_KERNELS = ("k_prog_measure", "k_prog_carry", "k_prog_count", "k_prog_offsets", "k_prog_place", "k_prog_emit_at",
+                "k_prog_emit", "k_seg_prefix", "k_seg_count", "k_seg_scan", "k_seg_fit", "k_seg_emit")
 
 
 def main():

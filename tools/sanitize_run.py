@@ -94,7 +94,8 @@ d_ad = torch.zeros(4, dtype=torch.int32, device=dev)
 torch.cuda.synchronize(dev)
 png.reduce_and_filter_dev(d_in, 300 * 40 * 4, 4, PngOptions.from_preset(300, 40, 1), d_out, 40 * (300 * 4 + 1), d_ad, ctx=ctx)
 ctx.sync()
-# JPEG progressive scans: every k_prog_* kernel, the splice and k_prog_pack, with trellis and plain
+# JPEG progressive scans with the tables and raw strings from the host (the wait for the bit counts): the
+# measuring kernels, k_prog_place, k_prog_emit_at and the splice with k_seg_fit, with trellis and plain
 # coefficients, optimised and standard tables, gray / 4:4:4 / 4:2:0, a batch and caller arrays
 for (ww, hh) in ((333, 222), (17, 9)):
     for ct, ss in ((2, Subsampling.S420), (2, Subsampling.S444), (0, Subsampling.S444)):
