@@ -66,7 +66,9 @@ typedef enum {
     PIXO_B200_ERR_OUTPUT_TOO_SMALL = 8,    /* caller's output capacity insufficient */
     PIXO_B200_ERR_UNSUPPORTED = 9,         /* option outside the hot path (progressive) */
     PIXO_B200_ERR_CUDA = 10,               /* CUDA runtime/driver failure (no device, launch) */
-    PIXO_B200_ERR_OOM = 11                 /* device or pinned allocation failed */
+    PIXO_B200_ERR_OOM = 11,                /* device or pinned allocation failed */
+    PIXO_B200_ERR_INVALID_DECODE = 12,     /* Error::InvalidDecode: malformed or corrupt input to a decoder */
+    PIXO_B200_ERR_UNSUPPORTED_DECODE = 13  /* Error::UnsupportedDecode: valid input a decoder does not handle */
 } pixo_b200_status;
 
 /* pixo::ColorType repr(u8) — src/color.rs:8-18 */
@@ -646,6 +648,40 @@ int pixo_b200_resize_dev(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_st
  * arrays are written.  Host-only, no device needed. */
 int pixo_b200_resize_weights(uint32_t src_size, uint32_t dst_size, uint32_t *start, uint32_t *count,
                              uint64_t *offset, float *weights, size_t weights_cap, size_t *n_weights);
+
+/* ---- baseline JPEG decoding ------------------------------------------------------------ */
+
+/* Replaces pixo::decode::decode_jpeg — src/decode/jpeg.rs:214-740 with bit_reader.rs:141-256 and idct.rs — pixel for
+ * pixel, on every input it accepts: truncated, corrupt and RSTn-bearing scans included (a read failure ends the scan,
+ * and the blocks never stored stay 0 in the component planes, as there).  Errors are pixo's, decided in pixo's order:
+ * PIXO_B200_ERR_INVALID_DECODE (Error::InvalidDecode) or PIXO_B200_ERR_UNSUPPORTED_DECODE (Error::UnsupportedDecode,
+ * e.g. "progressive JPEG not supported"), with pixo's Display text ("Decode error: ...", "Unsupported: ...") as the
+ * error string.  One difference: an SOS with no components before any SOF0, on which pixo panics, is
+ * PIXO_B200_ERR_INVALID_DECODE ("SOS with no frame components").  The output is packed Gray (color_type
+ * PIXO_B200_GRAY) or RGB (PIXO_B200_RGB), width * height * (1 or 3) bytes. */
+
+/* Host only, no device needed: the geometry and colour type decode_jpeg would return, or its error (the string is
+ * pixo_b200_last_error(NULL) on this thread).  Returns 0 exactly when decode_jpeg returns Ok.  width, height and
+ * color_type may be NULL. */
+int pixo_b200_jpeg_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
+                               uint32_t *color_type);
+/* One file to host memory.  pixels_cap below the frame returns PIXO_B200_ERR_OUTPUT_TOO_SMALL with the geometry
+ * set.  Waits for the device. */
+int pixo_b200_jpeg_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                          uint32_t *width, uint32_t *height, uint32_t *color_type);
+/* n files in host memory -> decoded frames in device memory: file i's frame at d_out + out_offsets[i] (the caller
+ * sizes them with pixo_b200_jpeg_decode_info; any byte alignment).  status[i] receives 0 or file i's error code
+ * before the call returns; a file that fails is skipped and nothing is written for it.  The headers are parsed on
+ * the host; the scans are uploaded and decoded on the context's stream, and the call returns with that work queued
+ * (the files may be reused at once).  Every file's scan is decoded sequentially by one GPU thread; the files of a
+ * batch run in parallel, one per warp.  3 launches per pass (scan, IDCT, colour); passes hold at most 65 536 files
+ * and about 1 GiB of device scratch.  A file needs 192 bytes of scratch per 8x8 block of its component planes (the
+ * frame as its SOF0 declares it, rounded up to whole MCUs, i.e. about 3 bytes per sample) plus its scan bytes; a
+ * file larger than the pass limit goes alone, and one larger than the device can hold returns PIXO_B200_ERR_OOM
+ * (frames of earlier passes may then have been written).  Null arrays, or a null d_out with n > 0, return
+ * PIXO_B200_ERR_INVALID_ARGUMENT before anything is read. */
+int pixo_b200_jpeg_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                                    uint8_t *d_out, const size_t *out_offsets, int32_t *status);
 
 /* Replaces compress::adler32::adler32 — src/compress/adler32.rs:11-47 (dispatch
  * src/simd/mod.rs:72-90).  Host buffer in, checksum out. */

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "jpeg_decode_host.hpp"
 #include "jpeg_host.hpp"
 #include "resize_host.hpp"
 
@@ -2132,6 +2133,90 @@ int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, u
     PIXO_TRY(d2h_copy_sync(ctx, out, ctx->d_out.ptr, out_bytes, ctx->stream));
     drain.armed = false;
     return 0;
+}
+
+// ---- baseline JPEG decoding ------------------------------------------------------------------
+
+static int jdec_error(pixo_b200_ctx *ctx, const JdecParsed &p)
+{
+    if (p.status == kJdecUnsupported)
+        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED_DECODE, "Unsupported: %s", p.msg.c_str());
+    return set_error(ctx, PIXO_B200_ERR_INVALID_DECODE, "Decode error: %s", p.msg.c_str());
+}
+
+static void jdec_geometry(const JdecParsed &p, uint32_t *width, uint32_t *height, uint32_t *color_type)
+{
+    if (width) *width = p.width;
+    if (height) *height = p.height;
+    if (color_type) *color_type = p.ncomp == 1 ? PIXO_B200_GRAY : PIXO_B200_RGB;
+}
+
+int pixo_b200_jpeg_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
+                               uint32_t *color_type)
+{
+    if (!data && len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
+    JdecParsed p;
+    jdec_parse(data, len, p);
+    if (p.status != kJdecOk) return jdec_error(nullptr, p);
+    jdec_geometry(p, width, height, color_type);
+    return 0;
+}
+
+int pixo_b200_jpeg_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                          uint32_t *width, uint32_t *height, uint32_t *color_type)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (!data && len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
+    JdecParsed p;
+    jdec_parse(data, len, p);
+    if (p.status != kJdecOk) return jdec_error(ctx, p);
+    jdec_geometry(p, width, height, color_type);
+    const size_t bytes = p.out_bytes();
+    if (pixels_cap < bytes)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", pixels_cap, bytes);
+    if (bytes == 0) return 0;
+    if (!pixels) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "pixels is null");
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    PIXO_TRY(ctx->d_out.ensure(ctx, bytes));
+    DrainOnError drain(ctx);
+    const JdecParsed *files[1] = {&p};
+    const uint64_t off[1] = {0};
+    PIXO_TRY(launch_jpeg_decode(ctx, files, &data, 1, off, static_cast<uint8_t *>(ctx->d_out.ptr)));
+    PIXO_TRY(d2h_copy_sync(ctx, pixels, ctx->d_out.ptr, bytes, ctx->stream));
+    drain.armed = false;
+    return 0;
+}
+
+int pixo_b200_jpeg_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                                    uint8_t *d_out, const size_t *out_offsets, int32_t *status)
+{
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    if (n == 0) return 0;
+    if (!files || !lens || !out_offsets || !status || !d_out)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null array");
+    std::vector<JdecParsed> parsed(n);
+    std::vector<const JdecParsed *> ok;
+    std::vector<const uint8_t *> data;
+    std::vector<uint64_t> off;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (!files[i] && lens[i]) {
+            status[i] = PIXO_B200_ERR_INVALID_ARGUMENT;
+            continue;
+        }
+        jdec_parse(files[i], lens[i], parsed[i]);
+        if (parsed[i].status != kJdecOk) {
+            status[i] = parsed[i].status == kJdecUnsupported ? PIXO_B200_ERR_UNSUPPORTED_DECODE
+                                                             : PIXO_B200_ERR_INVALID_DECODE;
+            continue;
+        }
+        status[i] = 0;
+        ok.push_back(&parsed[i]);
+        data.push_back(files[i]);
+        off.push_back(out_offsets[i]);
+    }
+    if (ok.empty()) return 0;
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return launch_jpeg_decode(ctx, ok.data(), data.data(), (uint32_t)ok.size(), off.data(), d_out);
 }
 
 }  // extern "C"

@@ -204,6 +204,7 @@ struct pixo_b200_ctx {
     pixo::DevBuf d_prog, d_prog_raw, d_prog_out;   // JPEG progressive scans: per-block state, raw strings,
                                                    // the splice's scratch (and the host loop's frame slots)
     pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
+    pixo::DevBuf d_jdec;                   // JPEG decode: a pass's records, tables and scans, coefficients, planes
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn

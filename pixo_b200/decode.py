@@ -1,0 +1,98 @@
+"""Mirror of pixo::decode for baseline JPEGs (src/decode/jpeg.rs), decoded on the GPU.
+
+  JpegImage                 pixo::decode::JpegImage (width, height, pixels, color_type)
+  decode_jpeg               pixo::decode::decode_jpeg: pixel-identical, pixo's errors and messages
+  jpeg_info                 the geometry and colour type decode_jpeg would return, host only
+  decode_jpeg_batch_dev     many files -> frames in one device tensor, queued on the context's stream
+"""
+from __future__ import annotations
+
+import ctypes as C
+import dataclasses
+
+import numpy as np
+
+from . import _lib
+from .color import ColorType
+from .context import Context, default_context
+
+
+@dataclasses.dataclass
+class JpegImage:
+    width: int
+    height: int
+    pixels: np.ndarray
+    color_type: ColorType
+
+
+def _bytes(data) -> bytes:
+    return data.tobytes() if isinstance(data, np.ndarray) else bytes(data)
+
+
+def jpeg_info(data) -> tuple[int, int, ColorType]:
+    """(width, height, color_type) of the image decode_jpeg would return; raises PixoError with pixo's error."""
+    b = _bytes(data)
+    w, h, ct = C.c_uint32(), C.c_uint32(), C.c_uint32()
+    _lib.check(None, _lib.load().pixo_b200_jpeg_decode_info(b, len(b), C.byref(w), C.byref(h), C.byref(ct)))
+    return w.value, h.value, ColorType(ct.value)
+
+
+def decode_jpeg(data, ctx: Context | None = None) -> JpegImage:
+    """pixo::decode::decode_jpeg on the GPU: packed Gray or RGB pixels."""
+    ctx = ctx or default_context()
+    b = _bytes(data)
+    w, h, ct = jpeg_info(b)
+    out = np.empty(max(w * h * ColorType(ct).bytes_per_pixel(), 1), np.uint8)
+    rw, rh, rct = C.c_uint32(), C.c_uint32(), C.c_uint32()
+    _lib.check(ctx.handle, _lib.load().pixo_b200_jpeg_decode(ctx.handle, b, len(b), out.ctypes.data, out.size,
+                                                             C.byref(rw), C.byref(rh), C.byref(rct)))
+    return JpegImage(w, h, out[:w * h * ColorType(ct).bytes_per_pixel()], ct)
+
+
+@dataclasses.dataclass
+class DecodedBatch:
+    """Frames of a batch decode: frame i is frames[offsets[i] : offsets[i] + nbytes(i)], packed, with geometry
+    geometries[i] = (width, height, color_type); a file pixo rejects has geometry None and its PixoError in errors."""
+    frames: object                     # torch.uint8 tensor on the context's device
+    offsets: list
+    geometries: list
+    errors: list
+
+
+def decode_jpeg_batch_dev(files, ctx: Context | None = None, align: int = 256) -> DecodedBatch:
+    """Decodes the files into one device tensor (pixo_b200_jpeg_decode_to_device); the decode is queued on the
+    context's stream when this returns, and the tensor belongs to that stream (work on another stream must wait for
+    it, e.g. through ctx.sync()).  Each frame starts on an `align`-byte boundary."""
+    import torch
+    ctx = ctx or default_context()
+    blobs = [_bytes(f) for f in files]
+    geoms, errors, offsets, total = [], [], [], 0
+    for b in blobs:
+        try:
+            w, h, ct = jpeg_info(b)
+            geoms.append((w, h, ct))
+            errors.append(None)
+        except _lib.PixoError as e:
+            geoms.append(None)
+            errors.append(e)
+        offsets.append(total)
+        if geoms[-1]:
+            total += -(-geoms[-1][0] * geoms[-1][1] * ColorType(geoms[-1][2]).bytes_per_pixel() // align) * align
+    # allocated on the stream that writes it: torch's caching allocator then neither hands the memory out while the
+    # decode is still writing it nor lets the decode write memory that earlier work on another stream still reads
+    dev = torch.device("cuda", ctx.device)
+    sp = _lib.load().pixo_b200_ctx_stream(ctx.handle)
+    stream = torch.cuda.ExternalStream(sp, device=dev) if sp else torch.cuda.default_stream(dev)
+    with torch.cuda.stream(stream):
+        frames = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    n = len(blobs)
+    ptrs = (C.c_char_p * max(n, 1))(*blobs)
+    lens = (C.c_size_t * max(n, 1))(*[len(b) for b in blobs])
+    offs = (C.c_size_t * max(n, 1))(*offsets)
+    status = (C.c_int32 * max(n, 1))()
+    _lib.check(ctx.handle, _lib.load().pixo_b200_jpeg_decode_to_device(
+        ctx.handle, C.cast(ptrs, C.c_void_p), lens, n, frames.data_ptr(), offs, status))
+    for i in range(n):
+        if status[i] and errors[i] is None:
+            errors[i] = _lib.PixoError(status[i], "invalid argument")
+    return DecodedBatch(frames, offsets, geoms, errors)

@@ -207,4 +207,16 @@ for S in ("1", "3"):
     ctx.set_stream(None)
     assert got == want, ("stream-ordered band", S)
 del os.environ["PIXO_B200_SEGMENTS"]
+# ---- baseline JPEG decoding: k_jdec_scan / k_jdec_idct / k_jdec_color over real, truncated, corrupt and constructed
+# files, gray, 4:4:4, 4:2:0 and odd sampling factors ----------------------------------------------------------
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+from pixo_b200 import decode as jdec  # noqa: E402
+from jpeg_decode_corpus import constructed, corrupted, truncations  # noqa: E402
+small = jpeg.encode(synthetic.noise(37, 21, 3, 2), JpegOptions(37, 21, ColorType.Rgb, 90, Subsampling.S420, 3), ctx=ctx)
+gray = jpeg.encode(synthetic.noise(w, h, 1, 4), JpegOptions(w, h, ColorType.Gray, 85, Subsampling.S444), ctx=ctx)
+files = [plain, small, gray]
+files += truncations(small) + corrupted(small, 5, 50) + [constructed(k) for k in range(100)]
+jdec.decode_jpeg_batch_dev(files, ctx=ctx)
+jdec.decode_jpeg(plain, ctx=ctx)
+ctx.sync()
 print("tour done")
