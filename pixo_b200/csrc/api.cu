@@ -616,18 +616,6 @@ static int trellis_pieces(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pi
     return 0;
 }
 
-// trellis_pieces, then waits for the device: the input check is reported by the call
-static int trellis_coefficients(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride, uint32_t n_images,
-                                uint32_t width, uint32_t height, uint32_t color_type, uint32_t subsampling,
-                                const float lum_q[64], const float chr_q[64], int16_t *d_y, size_t y_stride,
-                                int16_t *d_cb, int16_t *d_cr, size_t c_stride, bool zigzag)
-{
-    uint32_t *status;
-    PIXO_TRY(trellis_pieces(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling, lum_q, chr_q,
-                            d_y, y_stride, d_cb, d_cr, c_stride, zigzag, &status));
-    return trellis_status(ctx, status);
-}
-
 int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
                                     size_t pixel_stride, uint32_t n_images, uint32_t width,
                                     uint32_t height, uint32_t color_type, uint32_t subsampling,
@@ -650,11 +638,14 @@ int pixo_b200_jpeg_coefficients_dev(pixo_b200_ctx *ctx, const uint8_t *d_pixels,
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT,
                          "coefficient buffers must be 16-byte aligned with strides multiple of 8");
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (flags & PIXO_B200_COEF_TRELLIS)
-        return trellis_coefficients(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling,
-                                    lum_q, chr_q, d_y, y_stride, color_type == PIXO_B200_GRAY ? nullptr : d_cb,
-                                    color_type == PIXO_B200_GRAY ? nullptr : d_cr, c_stride,
-                                    (flags & PIXO_B200_COEF_ZIGZAG) != 0);
+    if (flags & PIXO_B200_COEF_TRELLIS) {   // waits for the device: the input check is reported by the call
+        uint32_t *status;
+        PIXO_TRY(trellis_pieces(ctx, d_pixels, pixel_stride, n_images, width, height, color_type, subsampling, lum_q,
+                                chr_q, d_y, y_stride, color_type == PIXO_B200_GRAY ? nullptr : d_cb,
+                                color_type == PIXO_B200_GRAY ? nullptr : d_cr, c_stride,
+                                (flags & PIXO_B200_COEF_ZIGZAG) != 0, &status));
+        return trellis_status(ctx, status);
+    }
     PIXO_TRY(launch_jpeg_transform(ctx, d_pixels, pixel_stride, n_images, width, height,
                                    color_type, subsampling, lum_q, chr_q, d_y, y_stride, d_cb,
                                    d_cr, c_stride, flags));
@@ -1007,12 +998,58 @@ static int encode_baseline_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, c
     return finish(grp.count() - 1);
 }
 
-// Progressive frames (encode_progressive, src/jpeg/mod.rs:872-927): the transform writes dense natural-order
-// arrays (K3 reads them for the optimised tables, which pixo builds from the plain-rounded coefficients,
-// restart interval included, and k_huff_tables builds each frame's tables from them), COEF_TRELLIS then overwrites
-// them with trellis, the progressive stage codes the 7 scans, and the host writes SOF2 and each scan's SOS and
-// segment.  The stage's buffers are the context's, so a group is finished before the next is computed: one
-// coefficient slot and one set of DHT blocks serve them all.
+// A progressive pass's coefficients and tables, queued in pixo's order (encode_progressive, src/jpeg/mod.rs:872-927),
+// which builds the tables from the plain-rounded coefficients before trellis overwrites them: the plain transform into
+// dense arrays at c when the tables need it or no trellis follows, K3 with the restart interval (optimize),
+// k_huff_tables into d_dht unless it is null, COEF_TRELLIS (*d_trellis_status: its status word, null without it).
+static int progressive_coefficients(pixo_b200_ctx *ctx, const uint8_t *px, size_t pixel_stride, uint32_t cnt,
+                                    const FrameGeometry &g, const float *lum, const float *chr, const CoefLayout &L,
+                                    uint8_t *c, uint32_t restart_interval, bool optimize, bool trellis,
+                                    uint64_t *d_hist, uint8_t *d_dht, uint32_t **d_trellis_status)
+{
+    const size_t cs = L.stride();
+    int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
+    if (optimize || !trellis)
+        PIXO_TRY(launch_jpeg_transform(ctx, px, pixel_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum,
+                                       chr, L.y(c), cs, cb, cr, cs, 0));
+    if (optimize)
+        PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
+                                       false, nullptr, d_hist));
+    if (d_dht) PIXO_TRY(launch_huff_tables(ctx, optimize ? d_hist : nullptr, cnt, g.has_chroma, d_dht, nullptr));
+    *d_trellis_status = nullptr;
+    if (trellis)
+        PIXO_TRY(trellis_pieces(ctx, px, pixel_stride, cnt, g.width, g.height, g.color_type, g.subsampling, lum, chr,
+                                L.y(c), cs, cb, cr, cs, false, d_trellis_status));
+    return 0;
+}
+
+// A progressive file around its 7 segments of len[s] bytes: SOF2 headers with DHT block dht's tables, per scan its SOS
+// and segment, EOI.  Checks the room, then writes all but the segments (out + at[s]) and the length to *out_len.
+static int progressive_layout(pixo_b200_ctx *ctx, const FrameGeometry &g, const uint8_t lum_zz[64],
+                              const uint8_t chr_zz[64], const uint8_t *dht, uint32_t restart_interval,
+                              const uint64_t len[7], uint8_t *out, size_t out_cap, size_t at[7], size_t *out_len)
+{
+    HuffTables t;
+    huff_from_dht(dht, t);
+    uint8_t hdr[2048];   // 281 bytes + the tables' values (at most 4 x 256)
+    size_t pos = write_headers_progressive(hdr, g, lum_zz, chr_zz, t, restart_interval);
+    size_t need = pos + 7 * 10 + 2;
+    for (int s = 0; s < 7; ++s) need += (size_t)len[s];
+    PIXO_TRY(check_room(ctx, out_cap, need));
+    memcpy(out, hdr, pos);
+    for (int s = 0; s < 7; ++s) {
+        pos += write_sos_progressive(out + pos, s);
+        at[s] = pos;
+        pos += (size_t)len[s];
+    }
+    out[pos] = 0xFF;
+    out[pos + 1] = 0xD9;
+    *out_len = pos + 2;
+    return 0;
+}
+
+// Progressive frames: progressive_coefficients, the 7 scans, each file around them (progressive_layout).  The stage's
+// buffers are the context's, so each group is finished before the next: one coefficient slot and DHT set serve all.
 static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp, const FrameGeometry &g,
                                      uint32_t quality, uint32_t restart_interval, bool optimize, bool trellis,
                                      uint8_t *out, size_t out_cap_each, size_t *out_lens)
@@ -1036,30 +1073,24 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
     auto *h_dht = static_cast<const uint8_t *>(ctx->h_misc.ptr);
     // frame k's tables: its own (optimize), or the standard ones
     auto dht_of = [&](uint32_t k) { return optimize ? h_dht + (size_t)k * kDhtBytes : dht_standard(); };
-    HuffTables t;
     PIXO_TRY(grp.upload(0));
     for (uint32_t gi = 0; gi < grp.count(); ++gi) {
         if (gi + 1 < grp.count()) PIXO_TRY(grp.upload(gi + 1));
         // coefficients, tables and the 7 segments of every frame of the group (waits for the device)
         const uint32_t cnt = grp.size(gi);
-        const uint8_t *px = grp.input(gi);
         PIXO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi & 1], 0));
-        if (optimize || !trellis)
-            PIXO_TRY(launch_jpeg_transform(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
-                                           lum, chr, L.y(c), cs, cb, cr, cs, 0));
-        if (optimize) {
-            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                           false, nullptr, d_hist));
-            PIXO_TRY(launch_huff_tables(ctx, d_hist, cnt, g.has_chroma, d_dht, nullptr));
+        // DHT blocks only when optimised: the host has the standard tables without a k_huff_tables launch
+        uint32_t *status;
+        PIXO_TRY(progressive_coefficients(ctx, grp.input(gi), grp.in_stride, cnt, g, lum, chr, L, c, restart_interval,
+                                          optimize, trellis, d_hist, optimize ? d_dht : nullptr, &status));
+        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[gi & 1], ctx->stream));
+        if (optimize)
             PIXO_CUDA(ctx, cudaMemcpyAsync(ctx->h_misc.ptr, d_dht, (size_t)cnt * kDhtBytes, cudaMemcpyDeviceToHost,
                                            ctx->stream));
-        }
         if (trellis)   // waits for the device, the DHT blocks' copy included
-            PIXO_TRY(trellis_coefficients(ctx, px, grp.in_stride, cnt, g.width, g.height, g.color_type, g.subsampling,
-                                          lum, chr, L.y(c), cs, cb, cr, cs, false));
+            PIXO_TRY(trellis_status(ctx, status));
         else if (optimize)
             PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        PIXO_CUDA(ctx, cudaEventRecord(ctx->ev_used[gi & 1], ctx->stream));
         std::vector<ProgTables> pt(optimize ? cnt : 1);
         for (uint32_t k = 0; k < pt.size(); ++k) PIXO_TRY(dht_prog_tables(ctx, dht_of(k), &pt[k]));
         ProgSlots slots;   // in d_prog_out, sized from the measured strings
@@ -1074,28 +1105,20 @@ static int encode_progressive_groups(pixo_b200_ctx *ctx, const EncodeGroups &grp
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_len, slots.scan_len, (size_t)cnt * 7 * 8, cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaMemcpyAsync(h_ovf, slots.overflow, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ctx->stream));
         PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        // SOF2 headers, then per scan its SOS and its segment (from the device), EOI
+        // each file around its segments, which come from the device
         for (uint32_t k = 0; k < cnt; ++k) {
             if (h_ovf[k]) return set_error(ctx, PIXO_B200_ERR_CUDA, "progressive splice overflowed its slot");
             const uint32_t img = gi * grp.G + k;
             uint8_t *o = out + (size_t)img * out_cap_each;
             const uint64_t *len = h_len + (size_t)k * 7;
-            huff_from_dht(dht_of(k), t);
-            size_t pos = write_headers_progressive(o, g, lum_zz, chr_zz, t, restart_interval);
-            size_t need = pos + 2;
-            for (int s = 0; s < 7; ++s) need += 10 + (size_t)len[s];
-            PIXO_TRY(check_room(ctx, out_cap_each, need));
+            size_t at[7];
+            PIXO_TRY(progressive_layout(ctx, g, lum_zz, chr_zz, dht_of(k), restart_interval, len, o, out_cap_each, at,
+                                        &out_lens[img]));
             const uint8_t *seg = slots.out + (size_t)k * slots.cap;
             for (int s = 0; s < 7; ++s) {
-                pos += write_sos_progressive(o + pos, s);
-                const size_t n = (size_t)len[s];
-                if (n) PIXO_TRY(d2h_copy_sync(ctx, o + pos, seg, n, ctx->stream));
-                pos += n;
-                seg += n;
+                if (len[s]) PIXO_TRY(d2h_copy_sync(ctx, o + at[s], seg, (size_t)len[s], ctx->stream));
+                seg += len[s];
             }
-            o[pos] = 0xFF;
-            o[pos + 1] = 0xD9;
-            out_lens[img] = pos + 2;
         }
     }
     return 0;
@@ -1193,6 +1216,11 @@ static int check_coef_alignment(pixo_b200_ctx *ctx, const int16_t *d_y, const in
     return 0;
 }
 
+// A pass of the progressive stage: at most the splice grid's 8192 frames, and in encode_dev_progressive no more than
+// keep its raw strings (out_cap + 16 bytes per frame) and coefficient arrays each within kProgPass (one at least).
+static constexpr size_t kProgPass = (size_t)512 << 20;
+static constexpr uint32_t kProgPassFrames = 8192;
+
 int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride,
                                          const int16_t *d_cb, const int16_t *d_cr, size_t c_stride,
                                          uint32_t n_frames, uint32_t width, uint32_t height, uint32_t color_type,
@@ -1215,20 +1243,19 @@ int pixo_b200_jpeg_progressive_scans_dev(pixo_b200_ctx *ctx, const int16_t *d_y,
     PIXO_TRY(dht_prog_tables(ctx, dht ? dht : dht_standard(), &T));
     if (n_frames == 0) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    // At most 8192 frames per pass, as pixo_b200_jpeg_encode_dev_progressive codes them.  More frames are
-    // checked first (the measuring half alone), so that a rejected coefficient leaves every output untouched.
-    constexpr uint32_t kPass = 8192;
+    // The pass from frame i0 on.  A call of more than one pass is checked first (dst null: the measuring half alone),
+    // so that a rejected coefficient leaves every output untouched.
     const int16_t *cb = chroma ? d_cb : nullptr, *cr = chroma ? d_cr : nullptr;
-    auto at = [](const int16_t *a, size_t stride, uint32_t i0) { return a ? a + (size_t)i0 * stride : nullptr; };
-    if (n_frames > kPass)
-        for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass)
-            PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
-                                        c_stride, std::min(kPass, n_frames - i0), g, nullptr, &T, false, nullptr,
-                                        nullptr));
-    for (uint32_t i0 = 0; i0 < n_frames; i0 += kPass) {
+    auto pass = [&](uint32_t i0, ProgSlots *dst) {
+        auto at = [&](const int16_t *a, size_t stride) { return a ? a + (size_t)i0 * stride : nullptr; };
+        return launch_progressive(ctx, at(d_y, y_stride), y_stride, at(cb, c_stride), at(cr, c_stride), c_stride,
+                                  std::min(kProgPassFrames, n_frames - i0), g, nullptr, &T, false, nullptr, dst);
+    };
+    if (n_frames > kProgPassFrames)
+        for (uint32_t i0 = 0; i0 < n_frames; i0 += kProgPassFrames) PIXO_TRY(pass(i0, nullptr));
+    for (uint32_t i0 = 0; i0 < n_frames; i0 += kProgPassFrames) {
         ProgSlots dst{d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7, d_overflow + i0};
-        PIXO_TRY(launch_progressive(ctx, at(d_y, y_stride, i0), y_stride, at(cb, c_stride, i0), at(cr, c_stride, i0),
-                                    c_stride, std::min(kPass, n_frames - i0), g, nullptr, &T, false, nullptr, &dst));
+        PIXO_TRY(pass(i0, &dst));
     }
     return 0;
 }
@@ -1281,12 +1308,6 @@ int pixo_b200_jpeg_encode_dev_opts(pixo_b200_ctx *ctx, const uint8_t *d_pixels, 
                         d_scan, scan_cap_each, d_scan_len, d_overflow, cudaMemcpyDeviceToDevice);
 }
 
-// The frames of one pass of pixo_b200_jpeg_encode_dev_progressive: at most the splice grid's 8192, and as many as
-// keep the pass's raw strings (out_cap + 16 bytes per frame) and its coefficient arrays each within kProgPass
-// (at least one frame).
-static constexpr size_t kProgPass = (size_t)512 << 20;
-static constexpr uint32_t kProgPassFrames = 8192;
-
 int pixo_b200_jpeg_encode_dev_progressive(pixo_b200_ctx *ctx, const uint8_t *d_pixels, size_t pixel_stride,
                                           uint32_t n_images, uint32_t width, uint32_t height, uint32_t color_type,
                                           uint32_t quality, uint32_t subsampling, uint32_t restart_interval,
@@ -1326,20 +1347,10 @@ int pixo_b200_jpeg_encode_dev_progressive(pixo_b200_ctx *ctx, const uint8_t *d_p
     int16_t *cb = g.has_chroma ? L.cb(c) : nullptr, *cr = g.has_chroma ? L.cr(c) : nullptr;
     for (uint32_t i0 = 0; i0 < n_images; i0 += pass) {
         const uint32_t cnt = std::min(pass, n_images - i0);
-        const uint8_t *px = d_pixels + (size_t)i0 * pixel_stride;
         uint8_t *dht = d_dht ? d_dht + (size_t)i0 * kDhtBytes : dht_own;
-        // encode_progressive_groups' sequence: plain coefficients for the statistics, the tables, COEF_TRELLIS
-        if (optimize || !trellis)
-            PIXO_TRY(launch_jpeg_transform(ctx, px, pixel_stride, cnt, width, height, color_type, subsampling, lum, chr,
-                                           L.y(c), cs, cb, cr, cs, 0));
-        if (optimize)
-            PIXO_TRY(launch_jpeg_histogram(ctx, L.y(c), cs, cb, cr, cs, cnt, g.ny, g.nc, g.y_per_mcu, restart_interval,
-                                           false, nullptr, d_hist));
-        PIXO_TRY(launch_huff_tables(ctx, d_hist, cnt, g.has_chroma, dht, nullptr));
-        uint32_t *status = nullptr;
-        if (trellis)
-            PIXO_TRY(trellis_pieces(ctx, px, pixel_stride, cnt, width, height, color_type, subsampling, lum, chr, L.y(c),
-                                    cs, cb, cr, cs, false, &status));
+        uint32_t *status;
+        PIXO_TRY(progressive_coefficients(ctx, d_pixels + (size_t)i0 * pixel_stride, pixel_stride, cnt, g, lum, chr, L, c,
+                                          restart_interval, optimize, trellis, d_hist, dht, &status));
         ProgSlots dst{d_out + (size_t)i0 * out_cap_each, out_cap_each, d_scan_len + (size_t)i0 * 7, d_overflow + i0};
         PIXO_TRY(launch_progressive(ctx, L.y(c), cs, cb, cr, cs, cnt, g, dht, nullptr, false, status, &dst));
     }
@@ -1770,22 +1781,12 @@ int pixo_b200_jpeg_progressive_file(uint32_t width, uint32_t height, uint32_t co
     const FrameGeometry g = make_geometry(width, height, color_type, subsampling);
     uint8_t lum_zz[64], chr_zz[64];
     quant_tables((int)quality, lum_zz, chr_zz, nullptr, nullptr);
-    HuffTables t;
-    huff_from_dht(dht, t);
-    uint8_t hdr[2048];   // 281 bytes + the tables' values (at most 4 x 256)
-    const size_t n = write_headers_progressive(hdr, g, lum_zz, chr_zz, t, restart_interval);
-    PIXO_TRY(check_room(nullptr, out_cap, n + 7 * 10 + (size_t)body + 2));
-    memcpy(out, hdr, n);
-    size_t pos = n;
+    size_t at[7];
+    PIXO_TRY(progressive_layout(nullptr, g, lum_zz, chr_zz, dht, restart_interval, scan_len, out, out_cap, at, out_len));
     for (int s = 0; s < 7; ++s) {
-        pos += write_sos_progressive(out + pos, s);
-        if (scan_len[s]) memcpy(out + pos, segments, (size_t)scan_len[s]);
+        if (scan_len[s]) memcpy(out + at[s], segments, (size_t)scan_len[s]);
         segments += scan_len[s];
-        pos += (size_t)scan_len[s];
     }
-    out[pos] = 0xFF;
-    out[pos + 1] = 0xD9;
-    *out_len = pos + 2;
     return 0;
 }
 

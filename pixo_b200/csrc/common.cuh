@@ -375,14 +375,16 @@ int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_sc
 
 // progressive scans (jpeg_progressive.cu)
 bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
-// The 7 scans of n whole frames into *dst.  Tables and the raw strings:
+// The 7 scans of n whole frames into *dst (the coefficients, DHT blocks and trellis status of an encode come from
+// api.cu's progressive_coefficients).  Tables and the raw strings:
 //  - d_dht: frame i's from its DHT block at d_dht + i * kDhtBytes, queued without a wait; a frame's raw string
 //    is as long as its slot (dst->cap + 16 bytes), and a frame whose raw bytes exceed dst->cap is left out
 //    (overflow bit 0).  d_trellis_status (or null) is folded into the frames' flags.
-//  - otherwise the host's T (n when per_frame, else 1), and a wait for the bit counts: a coefficient out of
-//    range is refused before anything is written, and each raw string is as long as the longest frame's, so
-//    only the splice decides the fit.  dst null: nothing is coded; dst->out null: per-frame slots of twice the
-//    longest string, which every frame fits, in d_prog_out, set in *dst.
+//  - otherwise the host's T (n when per_frame, else 1), and one wait for the bit counts, read back as
+//    launch_progressive_band reads its own: a coefficient out of range is refused before anything is written,
+//    and each raw string is as long as the longest frame's, so only the splice decides the fit.  dst null:
+//    nothing is coded; dst->out null: per-frame slots of twice the longest string, which every frame fits, in
+//    d_prog_out, set in *dst.
 int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, const int16_t *d_cb,
                        const int16_t *d_cr, size_t c_stride, uint32_t n, const FrameGeometry &g, const uint8_t *d_dht,
                        const ProgTables *T, bool per_frame, const uint32_t *d_trellis_status, ProgSlots *dst);

@@ -674,6 +674,23 @@ static int prog_measure(pixo_b200_ctx *ctx, ProgParams &P, ProgPlace &Q, const u
     return launch(ctx, k_prog_offsets, n * NSCAN, PT, 0, P);
 }
 
+// The measuring half's status word and the bit counts of its P.n x 7 streams to h_prog, after one wait; a
+// coefficient out of range is refused.  *h_bits: the counts, valid until h_prog is bound again.
+static int prog_read_bits(pixo_b200_ctx *ctx, const ProgParams &P, uint64_t **h_bits)
+{
+    uint32_t *h_status;
+    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
+        h_status = L.take<uint32_t>(1);
+        *h_bits = L.take<uint64_t>((size_t)P.n * NSCAN);
+    }, 8));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaMemcpyAsync(*h_bits, P.bits, (size_t)P.n * NSCAN * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (*h_status)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    return 0;
+}
+
 // The coding half: every frame's string of raw_each bytes in d_prog_raw, k_prog_place (a frame of more than
 // place_cap raw bytes is left out), k_prog_emit_at and the splice into dst (launch_splice_bounded: five launches).
 // dst.out null: slots of dst.cap bytes, their lengths and flags in d_prog_out, to dst.
@@ -729,18 +746,8 @@ int launch_progressive(pixo_b200_ctx *ctx, const int16_t *d_y, size_t y_stride, 
     PIXO_TRY(prog_measure(ctx, P, Q, d_dht, T, per_frame));
     if (d_dht) return prog_code(ctx, P, Q, Layout::round(dst->cap + 16), dst->cap, d_trellis_status, *dst);
 
-    // measured: the status word and every stream's bit count to h_prog
-    uint32_t *h_status;
     uint64_t *h_bits;
-    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
-        h_status = L.take<uint32_t>(1);
-        h_bits = L.take<uint64_t>((size_t)n * NSCAN);
-    }, 8));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, (size_t)n * NSCAN * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*h_status)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    PIXO_TRY(prog_read_bits(ctx, P, &h_bits));
     if (!dst) return 0;
     uint64_t longest = 0;   // raw bytes of the longest frame string (its streams byte-aligned, see k_prog_place)
     for (uint32_t i = 0; i < n; ++i) {
@@ -802,13 +809,6 @@ int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_
         dht = L.take(kDhtBytes);
         R.tail7 = L.take<unsigned long long>(NSCAN);
     }));
-    uint32_t *h_status;
-    uint64_t *h_bits, *h_tails;
-    PIXO_TRY(bind(ctx, ctx->h_prog, [&](Layout &L) {
-        h_status = L.take<uint32_t>(1);
-        h_bits = L.take<uint64_t>(NSCAN);
-        h_tails = L.take<uint64_t>(NSCAN);
-    }, 8));
     PIXO_CUDA(ctx, cudaMemsetAsync(P.status, 0, 4, st));
     PIXO_TRY(launch_huff_tables(ctx, d_hist, 1, B.frame_nc > 0, dht, nullptr));
     PIXO_TRY(launch(ctx, k_prog_dht_tables, 1, 128, 0, dht, d_tables));
@@ -818,11 +818,8 @@ int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_
         PIXO_TRY(launch(ctx, k_prog_count<true>, (unsigned)tiles, PT, 0, P));
     }
     PIXO_TRY(launch(ctx, k_prog_offsets, NSCAN, PT, 0, P));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_status, P.status, 4, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaMemcpyAsync(h_bits, P.bits, NSCAN * 8, cudaMemcpyDeviceToHost, st));
-    PIXO_CUDA(ctx, cudaStreamSynchronize(st));
-    if (*h_status)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "coefficient out of the progressive range (-16383..16383)");
+    uint64_t *h_bits;
+    PIXO_TRY(prog_read_bits(ctx, P, &h_bits));
     // every scan's splice area as large as the longest string needs, so that scan s starts at s * stride
     uint64_t max_bytes = 0;
     for (int s = 0; s < NSCAN; ++s) max_bytes = std::max<uint64_t>(max_bytes, (h_bits[s] + 7) / 8);
@@ -850,6 +847,7 @@ int launch_progressive_band(pixo_b200_ctx *ctx, const int16_t *d_y, const int16_
     ctx->prog_bands[d_raw] = stride;
     PIXO_TRY(launch(ctx, k_prog_emit<true>, (unsigned)tiles, PT, 0, P));
     PIXO_TRY(launch(ctx, k_prog_band_trailer, 1, 32, 0, P, R));
+    uint64_t *h_tails = h_bits;   // in h_prog, over the bit counts, which nbits holds by now
     PIXO_CUDA(ctx, cudaMemcpyAsync(h_tails, R.tail7, NSCAN * 8, cudaMemcpyDeviceToHost, st));
     PIXO_CUDA(ctx, cudaStreamSynchronize(st));
     for (int s = 0; s < NSCAN; ++s) tail7[s] = (uint32_t)h_tails[s];
