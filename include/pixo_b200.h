@@ -683,6 +683,51 @@ int pixo_b200_jpeg_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, u
 int pixo_b200_jpeg_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
                                     uint8_t *d_out, const size_t *out_offsets, int32_t *status);
 
+/* ---- PNG decoding ------------------------------------------------------------------------- */
+
+/* Replaces pixo::decode::decode_png — src/decode/png.rs:101-626 with inflate.rs:46-513 and bit_reader.rs:10-135 —
+ * pixel for pixel, with pixo's error for every file it refuses, decided in pixo's order: the chunk walk (truncated
+ * chunk, then each chunk's CRC, IHDR length and colour type), the checks after it, the zlib header, inflate with
+ * pixo's Huffman tables as from_lengths builds them (no completeness check; later symbols win the 9-bit lookup),
+ * Adler-32 over every byte produced, the size, the first row with an invalid filter type, then a missing PLTE.
+ * Errors: PIXO_B200_ERR_INVALID_DECODE (Error::InvalidDecode), PIXO_B200_ERR_UNSUPPORTED_DECODE (Adam7, preset
+ * dictionary), PIXO_B200_ERR_INVALID_DIMENSIONS (a zero side) and PIXO_B200_ERR_IMAGE_TOO_LARGE (a side above
+ * 2^24), with pixo's Display text as the error string.  The frame is packed: Gray, GrayAlpha, RGB or RGBA as pixo
+ * returns it (16-bit samples keep their high byte, sub-8-bit gray is bit-replicated, tRNS is ignored for gray and
+ * RGB, and indexed is RGBA only when tRNS holds a value other than 255), width * height * channels bytes: the layout
+ * pixo_b200_resize_dev and the device encoders read.  A chunk type that is not valid UTF-8 is shown as pixo shows
+ * it (U+FFFD); a NUL in it ends the C string. */
+
+/* Host only, no device needed: the geometry and colour type decode_png would return, or the error it decides
+ * before inflating (the string is pixo_b200_last_error(NULL) on this thread).  One exception: the IDAT chunks' CRCs
+ * are checked only in a file the host refuses for another reason, so a file whose only fault is an IDAT CRC (or is
+ * found while inflating) returns 0 here.  *producible is 0 when the IDAT data cannot produce the frame's rows
+ * (height * (1 + scanline bytes) above 1032 bytes per DEFLATE byte plus 65 535: every symbol takes a bit, a 258-byte
+ * match two), so that decoding is certain to fail and no frame need be allocated for the file.  width, height,
+ * color_type and producible may be NULL. */
+int pixo_b200_png_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
+                              uint32_t *color_type, int32_t *producible);
+/* One file to host memory.  pixels_cap below the frame returns PIXO_B200_ERR_OUTPUT_TOO_SMALL with the geometry
+ * set, except for a file that is not producible (see above): it is decoded for its error alone, with no frame
+ * allocated and no output capacity needed.  Waits for the device. */
+int pixo_b200_png_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                         uint32_t *width, uint32_t *height, uint32_t *color_type);
+/* n files in host memory -> decoded frames in device memory: file i's frame at d_out + out_offsets[i] (sized with
+ * pixo_b200_png_decode_info; any byte alignment).  status[i] receives 0 or file i's error code; a file that fails
+ * is skipped and nothing is written for it.  The chunks are walked on the host; the IDAT payloads are uploaded and
+ * decoded on the context's stream, and the call waits for the device once per pass, so status is final and the
+ * frames are written (in stream order) when it returns.  Per pass: k_png_crc (every IDAT chunk's CRC-32, over many
+ * CTAs), k_png_inflate (one warp per zlib stream, longest first), k_png_unfilter (a wavefront of 32-row groups,
+ * writing 8-bit Gray / GrayAlpha / RGB / RGBA frames directly) and, when the pass holds sub-8-bit, 16-bit or indexed
+ * files, k_png_expand: 3 or 4 launches.  Passes hold at most 65 536 files and about 1 GiB of device scratch; a file
+ * needs its IDAT bytes plus min(expected size, 1032 * DEFLATE bytes + 65 535) for its inflated rows (a header that
+ * claims more than its stream can produce costs only what the stream can produce), and one larger than the pass
+ * limit goes alone; one larger than the device can hold returns PIXO_B200_ERR_OOM (frames of earlier passes may
+ * then have been written).  Null arrays, or a null d_out with n > 0, return PIXO_B200_ERR_INVALID_ARGUMENT before
+ * anything is read. */
+int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                                   uint8_t *d_out, const size_t *out_offsets, int32_t *status);
+
 /* Replaces compress::adler32::adler32 — src/compress/adler32.rs:11-47 (dispatch
  * src/simd/mod.rs:72-90).  Host buffer in, checksum out. */
 int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t *out);

@@ -5,7 +5,7 @@ Python mirror of the reference's public API for this path:
   pixo_b200.png   <->  pixo::png    (filter::apply_filters*, FilterStrategy, PngOptions) and
                        pixo::compress::adler32
   pixo_b200.resize <-> pixo::resize (resize, resize_into, ResizeOptions, ResizeAlgorithm)
-  pixo_b200.decode <-> pixo::decode (decode_jpeg, JpegImage)
+  pixo_b200.decode <-> pixo::decode (decode_jpeg, JpegImage, decode_png, PngImage)
 All arithmetic happens in libpixo_b200.so (hand-written CUDA behind a C ABI, include/pixo_b200.h).
 """
 from ._lib import PixoError, SO_PATH, load  # noqa: F401

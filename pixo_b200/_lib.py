@@ -134,6 +134,9 @@ SYMBOLS = {
     "pixo_b200_jpeg_decode_info": (C.c_int, [vp, C.c_size_t, u32p, u32p, u32p]),
     "pixo_b200_jpeg_decode": (C.c_int, [vp, vp, C.c_size_t, vp, C.c_size_t, u32p, u32p, u32p]),
     "pixo_b200_jpeg_decode_to_device": (C.c_int, [vp, vp, szp, C.c_uint32, vp, szp, C.POINTER(C.c_int32)]),
+    "pixo_b200_png_decode_info": (C.c_int, [vp, C.c_size_t, u32p, u32p, u32p, C.POINTER(C.c_int32)]),
+    "pixo_b200_png_decode": (C.c_int, [vp, vp, C.c_size_t, vp, C.c_size_t, u32p, u32p, u32p]),
+    "pixo_b200_png_decode_to_device": (C.c_int, [vp, vp, szp, C.c_uint32, vp, szp, C.POINTER(C.c_int32)]),
     "pixo_b200_resize_weights": (C.c_int, [C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_size_t, szp]),
     "pixo_b200_adler32": (C.c_int, [vp, vp, C.c_size_t, u32p]),
     "pixo_b200_adler32_dev": (C.c_int, [vp, vp, C.c_size_t, vp]),

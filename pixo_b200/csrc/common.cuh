@@ -205,6 +205,7 @@ struct pixo_b200_ctx {
                                                    // the splice's scratch (and the host loop's frame slots)
     pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
     pixo::DevBuf d_jdec;                   // JPEG decode: a pass's records, tables and scans, coefficients, planes
+    pixo::DevBuf d_pdec;                   // PNG decode: a pass's records, chunks and streams, rings, inflated rows
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn

@@ -1,0 +1,70 @@
+// png_decode_host.hpp — host half of the PNG decoder (pixo::decode::decode_png): the chunk walk with pixo's checks,
+// messages and order, the zlib header, and the per-file records the kernels read (png_decode_host.cpp).  The IDAT
+// CRCs, inflate, unfiltering and sample expansion run on the device (png_decode.cu).
+#pragma once
+
+#include <stddef.h>
+#include <stdint.h>
+
+#include <string>
+#include <vector>
+
+namespace pixo {
+
+// Error kinds of decode_png (src/error.rs)
+enum PdecKind { kPdecOk = 0, kPdecInvalid = 1, kPdecUnsupported = 2, kPdecDimensions = 3, kPdecTooLarge = 4 };
+
+// The CRC-32 of PNG chunks (reflected 0xEDB88320).  crc32_update runs the register over bytes without the final
+// inversion; crc32_shift(r, n) is the register r advanced over n zero bytes, so that the register over A || B
+// from any start s is crc32_shift(reg(s, A), |B|) ^ reg(0, B).
+uint32_t crc32_update(uint32_t reg, const uint8_t *p, size_t n);
+uint32_t crc32_shift(uint32_t reg, uint64_t nbytes);
+
+// One file after the host's share of decode_png (src/decode/png.rs:101-263 and the zlib header of
+// inflate_zlib_with_size, src/decode/inflate.rs:294-320)
+struct PdecParsed {
+    int kind = kPdecOk;
+    std::string msg;            // pixo's Display text of the error
+    uint32_t width = 0, height = 0;
+    uint8_t depth = 0, ctype = 0;   // IHDR bit depth and PNG colour type (0, 2, 3, 4, 6)
+    bool has_plte = false;
+    std::vector<uint8_t> plte, trns;
+    // IDAT chunks met before the walk stopped: byte offset of each payload in the file, its length and stored CRC
+    std::vector<uint64_t> idat_off;
+    std::vector<uint32_t> idat_len, idat_crc;
+    uint64_t idat_total = 0;
+    uint64_t expected = 0;      // calculate_expected_size: height * (1 + scanline bytes)
+    uint64_t sb = 0;            // scanline bytes (without the filter byte)
+    uint32_t bpp = 0;           // the unfilter's bytes per pixel (1 for indexed and sub-8-bit gray)
+    uint32_t out_channels = 0;  // of the decoded frame
+    uint32_t out_ct = 0;        // pixo_b200 colour type of the decoded frame
+    uint64_t out_bytes() const { return (uint64_t)width * height * out_channels; }
+    // the most bytes the DEFLATE data (IDAT bytes less the 2-byte header and the 4-byte Adler-32) can produce:
+    // every symbol takes at least one bit, so a match of 258 bytes takes at least 2
+    uint64_t produce_bound() const { return 1032 * (idat_total - 6) + 65535; }
+    // false when the stream cannot produce the rows: decode_png is then certain to fail (size mismatch, or an
+    // earlier inflate error), and no frame need be allocated for the file
+    bool producible() const { return expected <= produce_bound(); }
+    uint64_t scratch() const { return producible() ? expected : produce_bound(); }
+    // frames of 8-bit Gray, GrayAlpha, RGB and RGBA are the unfiltered rows themselves
+    bool direct() const { return depth == 8 && ctype != 3; }
+};
+
+// Everything decode_png decides before it inflates, IDAT CRCs excepted: p.kind is kPdecOk when the file reaches
+// the DEFLATE data.  With check_idat_crc the IDAT CRCs are checked here as well, each at its place in the walk.
+void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_crc);
+
+}  // namespace pixo
+
+struct pixo_b200_ctx;
+namespace pixo {
+// What the device decided for one file: 0, or the first failure in pixo's order after the host's checks
+struct PdecResult {
+    int kind;          // PdecKind
+    std::string msg;
+};
+// Decodes n parsed files (all kPdecOk) on the context's stream: file i's frame to d_out + out_off[i].  data[i] is
+// the file.  Waits for the device once per pass and fills res[i].  Passes of bounded scratch.
+int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const uint8_t *const *data, uint32_t n,
+                      const uint64_t *out_off, uint8_t *d_out, PdecResult *res);
+}  // namespace pixo

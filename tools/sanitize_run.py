@@ -219,4 +219,16 @@ files += truncations(small) + corrupted(small, 5, 50) + [constructed(k) for k in
 jdec.decode_jpeg_batch_dev(files, ctx=ctx)
 jdec.decode_jpeg(plain, ctx=ctx)
 ctx.sync()
+# ---- PNG decoding: k_png_crc / k_png_inflate / k_png_unfilter / k_png_expand over real, truncated, bit-flipped and
+# constructed files: every colour type and depth, hand-built DEFLATE, failing files between good ones ------------------
+import glob  # noqa: E402
+from png_decode_corpus import bit_flips, corpus  # noqa: E402
+from png_decode_corpus import truncations as png_truncations  # noqa: E402
+gold = sorted(glob.glob(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                                     "p*.png")))[:12]
+pngs = [open(p, "rb").read() for p in gold]
+pngs += [f for n, f in corpus() if n != "huge_claim_small_idat"] + png_truncations(pngs[0]) + bit_flips(pngs[1], 20, 3)
+jdec.decode_png_batch_dev(pngs, ctx=ctx)
+jdec.decode_png(pngs[0], ctx=ctx)
+ctx.sync()
 print("tour done")
