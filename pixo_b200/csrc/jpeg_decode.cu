@@ -353,11 +353,16 @@ void describe_pass(Layout &L, const PassSizes &s, JdecPass &P)
     P.planes = L.take<uint8_t>(s.blocks * 64);
 }
 
-// Device scratch of one pass: more files go in further passes; a file larger than this goes alone
+// Device scratch of one pass: more files go in further passes; a file larger than this goes alone.  The scratch
+// bound is the only one: every file is charged at least kJdecFileTables, so a pass holds fewer than 65 536 files.
 constexpr uint64_t kJdecPassBytes = (uint64_t)1 << 30;
-constexpr uint32_t kJdecPassFiles = 1u << 16;
+constexpr uint64_t kJdecFileTables = 8 * 2048;   // a file's tables, values, order and prefix entries, rounded up
+static_assert(kJdecPassBytes / (kJdecFileTables + sizeof(JdecFile)) < (1u << 16), "a pass's file count stays small");
 
-uint64_t file_scratch(const JdecParsed &p) { return p.blocks() * 192 + p.entropy_len + sizeof(JdecFile) + 8 * 2048; }
+uint64_t file_scratch(const JdecParsed &p)
+{
+    return p.blocks() * 192 + p.entropy_len + sizeof(JdecFile) + kJdecFileTables;
+}
 
 }  // namespace
 
@@ -368,7 +373,7 @@ int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const
         // the pass: files p0 .. p1-1
         uint32_t p1 = p0;
         uint64_t need = 0;
-        while (p1 < n && p1 - p0 < kJdecPassFiles && (p1 == p0 || need + file_scratch(*files[p1]) <= kJdecPassBytes))
+        while (p1 < n && (p1 == p0 || need + file_scratch(*files[p1]) <= kJdecPassBytes))
             need += file_scratch(*files[p1++]);
         const uint32_t m = p1 - p0;
         PassSizes s;

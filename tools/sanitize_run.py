@@ -231,4 +231,14 @@ pngs += [f for n, f in corpus() if n != "huge_claim_small_idat"] + png_truncatio
 jdec.decode_png_batch_dev(pngs, ctx=ctx)
 jdec.decode_png(pngs[0], ctx=ctx)
 ctx.sync()
+# ---- well-formed files past one row group and with odd sampling: a tall Paeth RGBA16 PNG (bpp 8 at every group's
+# first row) and a 3x2-sampled JPEG with restart intervals ------------------------------------------------------
+from decode_inputs import geometry, jfif, png_image, qtable, safe_tails, sparse_coefs  # noqa: E402
+tall, _ = png_image(45, 200, 16, 6, 1, filters=(4,))
+jdec.decode_png(tall, ctx=ctx)
+comps = [(3, 2, qtable(1)), (1, 1, qtable(2)), (2, 1, qtable(3))]
+mw, mh, bpm = geometry(101, 53, comps)
+odd = jfif(101, 53, comps, safe_tails(sparse_coefs(mw * mh * bpm, 4), bpm, 3, mw * mh), restart=3)
+jdec.decode_jpeg(odd, ctx=ctx)
+ctx.sync()
 print("tour done")
