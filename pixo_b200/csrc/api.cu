@@ -2137,167 +2137,80 @@ int pixo_b200_resize(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, u
     return 0;
 }
 
-// ---- baseline JPEG decoding ------------------------------------------------------------------
+}  // extern "C"
 
-static int jdec_error(pixo_b200_ctx *ctx, const JdecParsed &p)
+// ---- JPEG and PNG decoding ------------------------------------------------------------------------------
+// One set of entry points for both decoders, over the parsed file (JdecParsed, PdecParsed); parse and launch_decode
+// are overloaded on it.
+
+static int decode_error(pixo_b200_ctx *ctx, const DecodeStatus &s)
 {
-    if (p.status == kJdecUnsupported)
-        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED_DECODE, "Unsupported: %s", p.msg.c_str());
-    return set_error(ctx, PIXO_B200_ERR_INVALID_DECODE, "Decode error: %s", p.msg.c_str());
+    return set_error(ctx, s.code, "%s", s.msg.c_str());
 }
 
-static void jdec_geometry(const JdecParsed &p, uint32_t *width, uint32_t *height, uint32_t *color_type)
-{
-    if (width) *width = p.width;
-    if (height) *height = p.height;
-    if (color_type) *color_type = p.ncomp == 1 ? PIXO_B200_GRAY : PIXO_B200_RGB;
-}
-
-int pixo_b200_jpeg_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
-                               uint32_t *color_type)
-{
-    if (!data && len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
-    JdecParsed p;
-    jdec_parse(data, len, p);
-    if (p.status != kJdecOk) return jdec_error(nullptr, p);
-    jdec_geometry(p, width, height, color_type);
-    return 0;
-}
-
-int pixo_b200_jpeg_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
-                          uint32_t *width, uint32_t *height, uint32_t *color_type)
-{
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    if (!data && len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
-    JdecParsed p;
-    jdec_parse(data, len, p);
-    if (p.status != kJdecOk) return jdec_error(ctx, p);
-    jdec_geometry(p, width, height, color_type);
-    const size_t bytes = p.out_bytes();
-    if (pixels_cap < bytes)
-        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", pixels_cap, bytes);
-    if (bytes == 0) return 0;
-    if (!pixels) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "pixels is null");
-    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    PIXO_TRY(ctx->d_out.ensure(ctx, bytes));
-    DrainOnError drain(ctx);
-    const JdecParsed *files[1] = {&p};
-    const uint64_t off[1] = {0};
-    PIXO_TRY(launch_jpeg_decode(ctx, files, &data, 1, off, static_cast<uint8_t *>(ctx->d_out.ptr)));
-    PIXO_TRY(d2h_copy_sync(ctx, pixels, ctx->d_out.ptr, bytes, ctx->stream));
-    drain.armed = false;
-    return 0;
-}
-
-int pixo_b200_jpeg_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
-                                    uint8_t *d_out, const size_t *out_offsets, int32_t *status)
-{
-    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
-    if (n == 0) return 0;
-    if (!files || !lens || !out_offsets || !status || !d_out)
-        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null array");
-    std::vector<JdecParsed> parsed(n);
-    std::vector<const JdecParsed *> ok;
-    std::vector<const uint8_t *> data;
-    std::vector<uint64_t> off;
-    for (uint32_t i = 0; i < n; ++i) {
-        if (!files[i] && lens[i]) {
-            status[i] = PIXO_B200_ERR_INVALID_ARGUMENT;
-            continue;
-        }
-        jdec_parse(files[i], lens[i], parsed[i]);
-        if (parsed[i].status != kJdecOk) {
-            status[i] = parsed[i].status == kJdecUnsupported ? PIXO_B200_ERR_UNSUPPORTED_DECODE
-                                                             : PIXO_B200_ERR_INVALID_DECODE;
-            continue;
-        }
-        status[i] = 0;
-        ok.push_back(&parsed[i]);
-        data.push_back(files[i]);
-        off.push_back(out_offsets[i]);
-    }
-    if (ok.empty()) return 0;
-    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    return launch_jpeg_decode(ctx, ok.data(), data.data(), (uint32_t)ok.size(), off.data(), d_out);
-}
-
-// ---- PNG decoding ----------------------------------------------------------------------------------------
-
-static int pdec_status(int kind)
-{
-    switch (kind) {
-    case kPdecUnsupported: return PIXO_B200_ERR_UNSUPPORTED_DECODE;
-    case kPdecDimensions: return PIXO_B200_ERR_INVALID_DIMENSIONS;
-    case kPdecTooLarge: return PIXO_B200_ERR_IMAGE_TOO_LARGE;
-    default: return PIXO_B200_ERR_INVALID_DECODE;
-    }
-}
-
-// The host's share of decode_png.  A file the host refuses is walked again with its IDAT CRCs checked, so that an
-// IDAT chunk that fails before the host's error is reported first, as pixo reports it.
-static void pdec_parse_file(const uint8_t *data, size_t len, PdecParsed &p)
-{
-    pdec_parse(data, len, p, false);
-    if (p.kind != kPdecOk) pdec_parse(data, len, p, true);
-}
-
-static void pdec_geometry(const PdecParsed &p, uint32_t *width, uint32_t *height, uint32_t *color_type)
+template <class Parsed>
+static void decode_geometry(const Parsed &p, uint32_t *width, uint32_t *height, uint32_t *color_type)
 {
     if (width) *width = p.width;
     if (height) *height = p.height;
     if (color_type) *color_type = p.out_ct;
 }
 
-int pixo_b200_png_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
-                              uint32_t *color_type, int32_t *producible)
+template <class Parsed>
+static int decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height, uint32_t *color_type,
+                       int32_t *producible)
 {
     if (!data && len) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
-    PdecParsed p;
-    pdec_parse_file(data, len, p);
-    if (p.kind != kPdecOk) return set_error(nullptr, pdec_status(p.kind), "%s", p.msg.c_str());
-    pdec_geometry(p, width, height, color_type);
+    Parsed p;
+    parse(data, len, p);
+    if (p.status.code) return decode_error(nullptr, p.status);
+    decode_geometry(p, width, height, color_type);
     if (producible) *producible = p.producible();
     return 0;
 }
 
-int pixo_b200_png_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
-                         uint32_t *width, uint32_t *height, uint32_t *color_type)
+template <class Parsed>
+static int decode_one(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                      uint32_t *width, uint32_t *height, uint32_t *color_type)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     if (!data && len) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "data is null");
-    PdecParsed p;
-    pdec_parse_file(data, len, p);
-    if (p.kind != kPdecOk) return set_error(ctx, pdec_status(p.kind), "%s", p.msg.c_str());
-    pdec_geometry(p, width, height, color_type);
+    Parsed p;
+    parse(data, len, p);
+    if (p.status.code) return decode_error(ctx, p.status);
+    decode_geometry(p, width, height, color_type);
     // a file whose stream cannot produce its rows is decoded for its error only: no frame, no output capacity
     const bool producible = p.producible();
     const size_t bytes = p.out_bytes();
     if (producible && pixels_cap < bytes)
         return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", pixels_cap, bytes);
+    if (producible && bytes == 0) return 0;   // a JPEG frame 0 rows high: nothing to decode
     if (producible && !pixels) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "pixels is null");
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
     if (producible) PIXO_TRY(ctx->d_out.ensure(ctx, bytes));
     DrainOnError drain(ctx);
-    const PdecParsed *files[1] = {&p};
+    const Parsed *files[1] = {&p};
     const uint64_t off[1] = {0};
-    PdecResult res;
-    PIXO_TRY(launch_png_decode(ctx, files, &data, 1, off, producible ? static_cast<uint8_t *>(ctx->d_out.ptr) : nullptr,
-                               &res));
-    drain.armed = false;
-    if (res.kind != kPdecOk) return set_error(ctx, pdec_status(res.kind), "%s", res.msg.c_str());
+    DecodeStatus res;
+    PIXO_TRY(launch_decode(ctx, files, &data, 1, off, producible ? static_cast<uint8_t *>(ctx->d_out.ptr) : nullptr,
+                           &res));
+    if (res.code) return decode_error(ctx, res);
     if (!producible) return set_error(ctx, PIXO_B200_ERR_CUDA, "png decode: a stream produced more than its bound");
-    return d2h_copy_sync(ctx, pixels, ctx->d_out.ptr, bytes, ctx->stream);
+    PIXO_TRY(d2h_copy_sync(ctx, pixels, ctx->d_out.ptr, bytes, ctx->stream));
+    drain.armed = false;
+    return 0;
 }
 
-int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
-                                   uint8_t *d_out, const size_t *out_offsets, int32_t *status)
+template <class Parsed>
+static int decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                            uint8_t *d_out, const size_t *out_offsets, int32_t *status)
 {
     if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
     if (n == 0) return 0;
     if (!files || !lens || !out_offsets || !status || !d_out)
         return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null array");
-    std::vector<PdecParsed> parsed(n);
-    std::vector<const PdecParsed *> ok;
+    std::vector<Parsed> parsed(n);
+    std::vector<const Parsed *> ok;
     std::vector<const uint8_t *> data;
     std::vector<uint64_t> off;
     std::vector<uint32_t> idx;
@@ -2306,12 +2219,9 @@ int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *fil
             status[i] = PIXO_B200_ERR_INVALID_ARGUMENT;
             continue;
         }
-        pdec_parse_file(files[i], lens[i], parsed[i]);
-        if (parsed[i].kind != kPdecOk) {
-            status[i] = pdec_status(parsed[i].kind);
-            continue;
-        }
-        status[i] = 0;
+        parse(files[i], lens[i], parsed[i]);
+        status[i] = parsed[i].status.code;
+        if (status[i]) continue;
         ok.push_back(&parsed[i]);
         data.push_back(files[i]);
         off.push_back(out_offsets[i]);
@@ -2319,11 +2229,49 @@ int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *fil
     }
     if (ok.empty()) return 0;
     PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
-    std::vector<PdecResult> res(ok.size());
-    PIXO_TRY(launch_png_decode(ctx, ok.data(), data.data(), (uint32_t)ok.size(), off.data(), d_out, res.data()));
+    std::vector<DecodeStatus> res(ok.size());
+    PIXO_TRY(launch_decode(ctx, ok.data(), data.data(), (uint32_t)ok.size(), off.data(), d_out, res.data()));
     for (size_t k = 0; k < ok.size(); ++k)
-        if (res[k].kind != kPdecOk) status[idx[k]] = pdec_status(res[k].kind);
+        if (res[k].code) status[idx[k]] = res[k].code;
     return 0;
+}
+
+extern "C" {
+
+int pixo_b200_jpeg_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
+                               uint32_t *color_type)
+{
+    return decode_info<JdecParsed>(data, len, width, height, color_type, nullptr);
+}
+
+int pixo_b200_jpeg_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                          uint32_t *width, uint32_t *height, uint32_t *color_type)
+{
+    return decode_one<JdecParsed>(ctx, data, len, pixels, pixels_cap, width, height, color_type);
+}
+
+int pixo_b200_jpeg_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                                    uint8_t *d_out, const size_t *out_offsets, int32_t *status)
+{
+    return decode_to_device<JdecParsed>(ctx, files, lens, n, d_out, out_offsets, status);
+}
+
+int pixo_b200_png_decode_info(const uint8_t *data, size_t len, uint32_t *width, uint32_t *height,
+                              uint32_t *color_type, int32_t *producible)
+{
+    return decode_info<PdecParsed>(data, len, width, height, color_type, producible);
+}
+
+int pixo_b200_png_decode(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint8_t *pixels, size_t pixels_cap,
+                         uint32_t *width, uint32_t *height, uint32_t *color_type)
+{
+    return decode_one<PdecParsed>(ctx, data, len, pixels, pixels_cap, width, height, color_type);
+}
+
+int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *files, const size_t *lens, uint32_t n,
+                                   uint8_t *d_out, const size_t *out_offsets, int32_t *status)
+{
+    return decode_to_device<PdecParsed>(ctx, files, lens, n, d_out, out_offsets, status);
 }
 
 }  // extern "C"

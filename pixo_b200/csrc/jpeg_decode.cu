@@ -8,10 +8,8 @@
 // Arithmetic follows pixo's release build: integer overflow wraps, shift counts are masked, casts truncate.
 #include <string.h>
 
-#include <algorithm>
-#include <numeric>
-
 #include "common.cuh"
+#include "decode_host.hpp"
 #include "jpeg_decode_host.hpp"
 
 namespace pixo {
@@ -181,18 +179,6 @@ done:
     stored[f] = count;
 }
 
-// the file holding item g of a pass, from the pass's prefix sums (prefix[0] = 0, prefix[n] = total)
-__device__ uint32_t file_of(const uint64_t *__restrict__ prefix, uint32_t n, uint64_t g)
-{
-    uint32_t lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) / 2;
-        if (__ldg(prefix + mid) <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
 __device__ __forceinline__ int32_t fix_mul(int32_t a, int32_t b) { return (int32_t)(((int64_t)a * b) >> 13); }
 __device__ __forceinline__ int32_t wadd(int32_t a, int32_t b) { return (int32_t)((uint32_t)a + (uint32_t)b); }
 __device__ __forceinline__ int32_t wsub(int32_t a, int32_t b) { return (int32_t)((uint32_t)a - (uint32_t)b); }
@@ -238,7 +224,7 @@ __global__ void __launch_bounds__(kIdctThreads) k_jdec_idct(const JdecFile *__re
     const uint32_t lane = threadIdx.x & 7;
     const unsigned group = 0xFFu << (threadIdx.x & 24);   // the block's 8 lanes: they return together
     if (g >= total) return;
-    const uint32_t f = file_of(blk_prefix, n, g);
+    const uint32_t f = item_of(blk_prefix, n, g);
     const JdecFile &J = F[f];
     uint64_t b = g - __ldg(blk_prefix + f);   // block within the file, component planes in turn
     uint32_t c = 0;
@@ -295,7 +281,7 @@ __global__ void k_jdec_color(const JdecFile *__restrict__ F, const uint64_t *__r
 {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= total) return;
-    const uint32_t f = file_of(px_prefix, n, g);
+    const uint32_t f = item_of(px_prefix, n, g);
     const JdecFile &J = F[f];
     const uint64_t i = g - __ldg(px_prefix + f), W = J.width, y = i / W, x = i % W;
     const uint8_t *p0 = planes + J.plane[0];
@@ -353,11 +339,10 @@ void describe_pass(Layout &L, const PassSizes &s, JdecPass &P)
     P.planes = L.take<uint8_t>(s.blocks * 64);
 }
 
-// Device scratch of one pass: more files go in further passes; a file larger than this goes alone.  The scratch
-// bound is the only one: every file is charged at least kJdecFileTables, so a pass holds fewer than 65 536 files.
-constexpr uint64_t kJdecPassBytes = (uint64_t)1 << 30;
+// A file's device scratch in a pass.  Scratch is what ends a JPEG pass: every file is charged at least
+// kJdecFileTables, so a pass holds fewer than kDecodePassFiles files.
 constexpr uint64_t kJdecFileTables = 8 * 2048;   // a file's tables, values, order and prefix entries, rounded up
-static_assert(kJdecPassBytes / (kJdecFileTables + sizeof(JdecFile)) < (1u << 16), "a pass's file count stays small");
+static_assert(kDecodePassBytes / (kJdecFileTables + sizeof(JdecFile)) < kDecodePassFiles, "passes end by scratch");
 
 uint64_t file_scratch(const JdecParsed &p)
 {
@@ -366,15 +351,11 @@ uint64_t file_scratch(const JdecParsed &p)
 
 }  // namespace
 
-int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const uint8_t *const *data, uint32_t n,
-                       const uint64_t *out_off, uint8_t *d_out)
+int launch_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const uint8_t *const *data, uint32_t n,
+                  const uint64_t *out_off, uint8_t *d_out, DecodeStatus *)
 {
-    for (uint32_t p0 = 0; p0 < n;) {
-        // the pass: files p0 .. p1-1
-        uint32_t p1 = p0;
-        uint64_t need = 0;
-        while (p1 < n && (p1 == p0 || need + file_scratch(*files[p1]) <= kJdecPassBytes))
-            need += file_scratch(*files[p1++]);
+    for (uint32_t p0 = 0, p1; p0 < n; p0 = p1) {
+        p1 = pass_end(files, p0, n, file_scratch);
         const uint32_t m = p1 - p0;
         PassSizes s;
         s.n = m;
@@ -385,13 +366,8 @@ int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const
             s.bytes += f.entropy_len;
             s.blocks += f.blocks();
         }
-        // the uploaded part, built on the host in the device's layout
         JdecPass H;
-        Layout count;
-        describe_pass(count, s, H);
-        std::vector<uint8_t> host(H.up);
-        Layout HL(host.data());
-        describe_pass(HL, s, H);
+        const std::vector<uint8_t> host = host_image(s, H);
         uint32_t t = 0;
         uint64_t v = 0, by = 0, blk = 0, plane = 0, px = 0;
         for (uint32_t i = 0; i < m; ++i) {
@@ -439,13 +415,8 @@ int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const
         }
         H.blk_prefix[m] = blk;
         H.px_prefix[m] = px;
-        std::iota(H.order, H.order + m, 0u);
-        std::stable_sort(H.order, H.order + m, [&](uint32_t a, uint32_t b) {
-            return H.files[a].src_len > H.files[b].src_len;
-        });
         JdecPass D;
-        PIXO_TRY(bind(ctx, ctx->d_jdec, [&](Layout &L) { describe_pass(L, s, D); }));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(D.files, host.data(), H.up, cudaMemcpyHostToDevice, ctx->stream));
+        PIXO_TRY(upload_pass(ctx, ctx->d_jdec, s, H, host, D));
         if (s.blocks) PIXO_CUDA(ctx, cudaMemsetAsync(D.coef, 0, s.blocks * 128, ctx->stream));
         PIXO_TRY(launch(ctx, k_jdec_scan, dim3(m), dim3(32), 0, D.files, D.tabs, D.vals, D.bytes, D.order, D.coef,
                         D.stored));
@@ -455,7 +426,6 @@ int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const
         if (px)
             PIXO_TRY(launch(ctx, k_jdec_color, dim3((unsigned)((px + 255) / 256)), dim3(256), 0, D.files, D.px_prefix,
                             m, px, D.planes, d_out));
-        p0 = p1;
     }
     return 0;
 }

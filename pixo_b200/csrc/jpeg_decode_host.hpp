@@ -6,8 +6,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include <string>
 #include <vector>
+
+#include "decode_host.hpp"
 
 namespace pixo {
 
@@ -35,38 +36,37 @@ struct JdecFile {
     alignas(16) uint16_t quant[3][64];            // the components' quantisation tables, zig-zag order
 };
 
-// Error kinds of decode_jpeg (src/error.rs): what jdec_parse returns
-enum JdecStatus { kJdecOk = 0, kJdecInvalid = 1, kJdecUnsupported = 2 };
-
 // A file after its headers, up to the first SOS
 struct JdecParsed {
-    int status = kJdecOk;
-    std::string msg;   // pixo's message for the error, without the Display prefix
+    DecodeStatus status;
     uint32_t width = 0, height = 0, ncomp = 0, restart = 0, max_h = 1, max_v = 1;
     uint8_t h[3] = {}, v[3] = {}, q[3] = {}, dc[3] = {}, ac[3] = {};
     uint16_t quant[4][64] = {};
     JdecHuff tab[8] = {};                  // DC 0-3, AC 4-7; `values` indexes vals[i]
     std::vector<uint8_t> vals[8];
     size_t entropy = 0, entropy_len = 0;   // the scan's bytes in the file
+    uint32_t out_ct = 0;                   // pixo_b200 colour type of the decoded frame: Gray or RGB
     uint32_t mcu_w() const { return (width + max_h * 8 - 1) / (max_h * 8); }
     uint32_t mcu_h() const { return (height + max_v * 8 - 1) / (max_v * 8); }
     uint64_t plane_w(int c) const { return (uint64_t)mcu_w() * h[c] * 8; }
     uint64_t plane_h(int c) const { return (uint64_t)mcu_h() * v[c] * 8; }
     uint64_t blocks() const;          // all components' blocks
     uint64_t out_bytes() const { return (uint64_t)width * height * (ncomp == 1 ? 1 : 3); }
+    bool producible() const { return true; }   // every file that parses has its frame decoded
 };
 
 // Parses data as JpegDecoder::decode does up to the scan (src/decode/jpeg.rs:214-484), with pixo's errors in
 // pixo's order, and finds the scan's entropy range (find_entropy_end, :653-671)
-void jdec_parse(const uint8_t *data, size_t len, JdecParsed &p);
+void parse(const uint8_t *data, size_t len, JdecParsed &p);
 size_t jdec_entropy_end(const uint8_t *data, size_t len);
 
 }  // namespace pixo
 
 struct pixo_b200_ctx;
 namespace pixo {
-// Decodes n parsed files (all kJdecOk) on the context's stream: file i's frame to d_out + out_off[i], packed Gray or
-// RGB.  data[i] is the file; its scan's bytes are copied out before the call returns.  Passes of bounded scratch.
-int launch_jpeg_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const uint8_t *const *data, uint32_t n,
-                       const uint64_t *out_off, uint8_t *d_out);
+// Decodes n parsed files (all without error) on the context's stream: file i's frame to d_out + out_off[i], packed
+// Gray or RGB.  data[i] is the file; its scan's bytes are copied out before the call returns.  Passes of bounded
+// scratch.  res is never written: every error of decode_jpeg is decided on the host.
+int launch_decode(pixo_b200_ctx *ctx, const JdecParsed *const *files, const uint8_t *const *data, uint32_t n,
+                  const uint64_t *out_off, uint8_t *d_out, DecodeStatus *res);
 }  // namespace pixo

@@ -10,10 +10,8 @@
 // The host waits once per pass and resolves each file's error in pixo's order.
 #include <string.h>
 
-#include <algorithm>
-#include <numeric>
-
 #include "common.cuh"
+#include "decode_host.hpp"
 #include "png_decode_host.hpp"
 
 namespace pixo {
@@ -74,39 +72,6 @@ constexpr uint32_t ADLER_MOD = 65521;
 
 // ---- k_png_crc -------------------------------------------------------------------------------------------
 
-__device__ uint32_t d_mulmod(uint32_t a, uint32_t b)
-{
-    uint32_t p = 0;
-    for (uint32_t m = 1u << 31; m; m >>= 1) {
-        if (a & m) p ^= b;
-        b = b & 1 ? (b >> 1) ^ 0xEDB88320u : b >> 1;
-    }
-    return p;
-}
-
-__device__ uint32_t d_shift(uint32_t reg, uint64_t nbytes)
-{
-    uint32_t x2n = 1u << 30, f = 1u << 31;
-    for (int k = 0; k < 3; ++k) x2n = d_mulmod(x2n, x2n);
-    for (; nbytes; nbytes >>= 1) {
-        if (nbytes & 1) f = d_mulmod(x2n, f);
-        x2n = d_mulmod(x2n, x2n);
-    }
-    return d_mulmod(f, reg);
-}
-
-// the item of a pass's prefix sums (prefix[0] = 0, prefix[n] = total) that holds g
-__device__ uint32_t item_of(const uint64_t *__restrict__ prefix, uint32_t n, uint64_t g)
-{
-    uint32_t lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) / 2;
-        if (__ldg(prefix + mid) <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
 // One thread per piece of kCrcPiece bytes of a chunk: the register over the piece from 0, shifted over the bytes
 // after it in the chunk, XORed into the chunk's word.  The host starts that word at the register over "IDAT" shifted
 // over the whole payload, inverted and XORed with the stored CRC, so it ends 0 exactly when the CRC matches.
@@ -130,7 +95,7 @@ __global__ void __launch_bounds__(256) k_png_crc(const PdecChunk *__restrict__ C
     const uint8_t *p = bytes + K.src + start;
     uint32_t reg = 0;
     for (uint64_t i = 0; i < n; ++i) reg = (reg >> 8) ^ tab[(reg ^ __ldg(p + i)) & 0xFF];
-    atomicXor(acc + c, d_shift(reg, K.len - start - n));
+    atomicXor(acc + c, crc32_shift(reg, K.len - start - n));
 }
 
 // ---- k_png_inflate ---------------------------------------------------------------------------------------
@@ -705,62 +670,51 @@ void describe_pass(Layout &L, const PassSizes &s, PdecPass &P)
     P.scratch = L.take<uint8_t>(s.scratch);
 }
 
-constexpr uint64_t kPdecPassBytes = (uint64_t)1 << 30;
-constexpr uint32_t kPdecPassFiles = 1u << 16;
-
+// A file's device scratch in a pass
 uint64_t file_scratch(const PdecParsed &p)
 {
     return p.idat_total + p.scratch() + p.idat_len.size() * 28 + (p.height / 32 + 1) * 12 + 1024 + sizeof(PdecFile) +
            sizeof(PdecRecord) + 64;
 }
 
-void resolve(const PdecParsed &p, const PdecRecord &r, PdecResult &res)
+// The file's status from its record: clear, pixo's error, or PIXO_B200_ERR_CUDA for a fault
+void resolve(const PdecParsed &p, const PdecRecord &r, DecodeStatus &res)
 {
-    char buf[160];
-    res.kind = kPdecInvalid;
     switch (r.code) {
     case kOk:
-        if (p.ctype == 3 && !p.has_plte) { res.msg = "Decode error: missing PLTE chunk"; return; }
-        res.kind = kPdecOk;
-        res.msg.clear();
+        if (p.ctype == 3 && !p.has_plte) decode_fail(res, kInvalidDecode, "missing PLTE chunk");
+        else res = DecodeStatus();
         return;
-    case kCrc: res.msg = "Decode error: CRC mismatch in IDAT chunk"; return;
-    case kEos: res.msg = "Decode error: unexpected end of stream"; return;
-    case kReservedBlock: res.msg = "Decode error: reserved block type"; return;
-    case kLenNlen: res.msg = "Decode error: stored block LEN/NLEN mismatch"; return;
-    case kEmptyTable: res.msg = "Decode error: empty Huffman table"; return;
-    case kBadCode: res.msg = "Decode error: invalid Huffman code"; return;
-    case kRepeatAtStart: res.msg = "Decode error: repeat code at start"; return;
-    case kTooManyLengths: res.msg = "Decode error: too many code lengths"; return;
-    case kBadLitLen: snprintf(buf, sizeof buf, "Decode error: invalid literal/length code: %u", r.arg); break;
-    case kBadDistCode: res.msg = "Decode error: invalid distance code"; return;
-    case kDistTooFar: res.msg = "Decode error: distance too far back"; return;
+    case kCrc: decode_fail(res, kInvalidDecode, "CRC mismatch in IDAT chunk"); return;
+    case kEos: decode_fail(res, kInvalidDecode, "unexpected end of stream"); return;
+    case kReservedBlock: decode_fail(res, kInvalidDecode, "reserved block type"); return;
+    case kLenNlen: decode_fail(res, kInvalidDecode, "stored block LEN/NLEN mismatch"); return;
+    case kEmptyTable: decode_fail(res, kInvalidDecode, "empty Huffman table"); return;
+    case kBadCode: decode_fail(res, kInvalidDecode, "invalid Huffman code"); return;
+    case kRepeatAtStart: decode_fail(res, kInvalidDecode, "repeat code at start"); return;
+    case kTooManyLengths: decode_fail(res, kInvalidDecode, "too many code lengths"); return;
+    case kBadLitLen: decode_fail(res, kInvalidDecode, "invalid literal/length code: %u", r.arg); return;
+    case kBadDistCode: decode_fail(res, kInvalidDecode, "invalid distance code"); return;
+    case kDistTooFar: decode_fail(res, kInvalidDecode, "distance too far back"); return;
     case kAdler:
-        snprintf(buf, sizeof buf, "Decode error: Adler32 mismatch: expected %08X, got %08X", r.stored_adler, r.adler);
-        break;
-    case kSize:
-        snprintf(buf, sizeof buf, "Decode error: decompressed size mismatch: expected %llu, got %llu",
-                 (unsigned long long)p.expected, (unsigned long long)r.produced);
-        break;
-    case kFilter: snprintf(buf, sizeof buf, "Decode error: invalid filter type: %u", r.arg); break;
-    default:
-        res.kind = -1;
-        res.msg = "k_png_inflate: a file produced more than its scratch bound";
+        decode_fail(res, kInvalidDecode, "Adler32 mismatch: expected %08X, got %08X", r.stored_adler, r.adler);
         return;
+    case kSize:
+        decode_fail(res, kInvalidDecode, "decompressed size mismatch: expected %llu, got %llu",
+                    (unsigned long long)p.expected, (unsigned long long)r.produced);
+        return;
+    case kFilter: decode_fail(res, kInvalidDecode, "invalid filter type: %u", r.arg); return;
+    default: decode_fail(res, PIXO_B200_ERR_CUDA, "k_png_inflate: a file produced more than its scratch bound"); return;
     }
-    res.msg = buf;
 }
 
 }  // namespace
 
-int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const uint8_t *const *data, uint32_t n,
-                      const uint64_t *out_off, uint8_t *d_out, PdecResult *res)
+int launch_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const uint8_t *const *data, uint32_t n,
+                  const uint64_t *out_off, uint8_t *d_out, DecodeStatus *res)
 {
-    for (uint32_t p0 = 0; p0 < n;) {
-        uint32_t p1 = p0;
-        uint64_t need = 0;
-        while (p1 < n && p1 - p0 < kPdecPassFiles && (p1 == p0 || need + file_scratch(*files[p1]) <= kPdecPassBytes))
-            need += file_scratch(*files[p1++]);
+    for (uint32_t p0 = 0, p1; p0 < n; p0 = p1) {
+        p1 = pass_end(files, p0, n, file_scratch);
         const uint32_t m = p1 - p0;
         PassSizes s;
         s.n = m;
@@ -775,11 +729,7 @@ int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const 
             s.groups += (f.height + 31) / 32;
         }
         PdecPass H;
-        Layout count;
-        describe_pass(count, s, H);
-        std::vector<uint8_t> host(H.up);
-        Layout HL(host.data());
-        describe_pass(HL, s, H);
+        const std::vector<uint8_t> host = host_image(s, H);
         uint64_t by = 0, scr = 0, pieces = 0, groups = 0, ctas = 0;
         uint32_t c = 0, pal = 0;
         bool expand = false;
@@ -836,12 +786,8 @@ int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const 
         H.piece_prefix[c] = pieces;
         H.group_prefix[m] = groups;
         H.cta_prefix[m] = ctas;
-        std::iota(H.order, H.order + m, 0u);
-        std::stable_sort(H.order, H.order + m,
-                         [&](uint32_t a, uint32_t b) { return H.files[a].src_len > H.files[b].src_len; });
         PdecPass D;
-        PIXO_TRY(bind(ctx, ctx->d_pdec, [&](Layout &L) { describe_pass(L, s, D); }));
-        PIXO_CUDA(ctx, cudaMemcpyAsync(D.files, host.data(), H.up, cudaMemcpyHostToDevice, ctx->stream));
+        PIXO_TRY(upload_pass(ctx, ctx->d_pdec, s, H, host, D));
         PIXO_CUDA(ctx, cudaMemsetAsync(D.ctl, 0, 16, ctx->stream));
         PIXO_CUDA(ctx, cudaMemsetAsync(D.progress, 0, groups * 4, ctx->stream));
         if (pieces)
@@ -864,10 +810,10 @@ int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const 
         if (ctl[2] & 1u)
             return set_error(ctx, PIXO_B200_ERR_CUDA, "k_png_unfilter: a row group's wait for the rows above timed out");
         for (uint32_t i = 0; i < m; ++i) {
-            resolve(*files[p0 + i], rec[i], res[p0 + i]);
-            if (res[p0 + i].kind < 0) return set_error(ctx, PIXO_B200_ERR_CUDA, "%s", res[p0 + i].msg.c_str());
+            DecodeStatus &r = res[p0 + i];
+            resolve(*files[p0 + i], rec[i], r);
+            if (r.code == PIXO_B200_ERR_CUDA) return set_error(ctx, r.code, "%s", r.msg.c_str());
         }
-        p0 = p1;
     }
     return 0;
 }

@@ -4,11 +4,7 @@
 // (png_decode.cu).
 #include "png_decode_host.hpp"
 
-#include <stdarg.h>
-#include <stdio.h>
 #include <string.h>
-
-#include "../../include/pixo_b200.h"
 
 namespace pixo {
 
@@ -26,17 +22,6 @@ struct CrcTable {
     }
 };
 const CrcTable kCrc;
-
-// a * b modulo the CRC polynomial, bit 31 holding x^0 (the reflected order the register uses)
-uint32_t crc_mulmod(uint32_t a, uint32_t b)
-{
-    uint32_t p = 0;
-    for (uint32_t m = 1u << 31; m; m >>= 1) {
-        if (a & m) p ^= b;
-        b = b & 1 ? (b >> 1) ^ 0xEDB88320u : b >> 1;
-    }
-    return p;
-}
 
 uint32_t be32(const uint8_t *p) { return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | p[3]; }
 
@@ -81,19 +66,6 @@ std::string utf8_lossy(const uint8_t *s, size_t n)
     return out;
 }
 
-int fail(PdecParsed &p, int kind, const char *fmt, ...)
-{
-    char buf[256];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
-    va_end(ap);
-    p.kind = kind;
-    p.msg = kind == kPdecInvalid ? std::string("Decode error: ") + buf
-          : kind == kPdecUnsupported ? std::string("Unsupported: ") + buf : std::string(buf);
-    return kind;
-}
-
 const char *ctype_name(uint8_t c)
 {
     switch (c) {
@@ -113,23 +85,12 @@ uint32_t crc32_update(uint32_t reg, const uint8_t *p, size_t n)
     return reg;
 }
 
-uint32_t crc32_shift(uint32_t reg, uint64_t nbytes)
-{
-    // x^(8 * nbytes) by squaring: x2n holds x^(2^k) for the bits of 8 * nbytes
-    uint32_t x2n = 1u << 30, f = 1u << 31;   // x^1, x^0
-    for (int k = 0; k < 3; ++k) x2n = crc_mulmod(x2n, x2n);
-    for (; nbytes; nbytes >>= 1) {
-        if (nbytes & 1) f = crc_mulmod(x2n, f);
-        x2n = crc_mulmod(x2n, x2n);
-    }
-    return crc_mulmod(f, reg);
-}
-
-void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_crc)
+// The walk and the checks after it, false for a file refused; with check_idat_crc the IDAT CRCs are checked as well
+static bool walk(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_crc)
 {
     p = PdecParsed();
     static const uint8_t kSig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
-    if (len < 8 || memcmp(data, kSig, 8) != 0) { fail(p, kPdecInvalid, "not a PNG file"); return; }
+    if (len < 8 || memcmp(data, kSig, 8) != 0) return decode_fail(p.status, kInvalidDecode, "not a PNG file");
     bool have_ihdr = false, seen_iend = false;
     uint8_t comp = 0, filt = 0, interlace = 0;
     size_t pos = 8;
@@ -137,24 +98,20 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
         const uint64_t length = be32(data + pos);
         const uint8_t *type = data + pos + 4;
         const uint64_t start = pos + 8, end = start + length, crc_end = end + 4;
-        if (crc_end > len) { fail(p, kPdecInvalid, "truncated PNG chunk"); return; }
+        if (crc_end > len) return decode_fail(p.status, kInvalidDecode, "truncated PNG chunk");
         const uint8_t *d = data + start;
         const uint32_t stored = be32(data + end);
         const bool idat = memcmp(type, "IDAT", 4) == 0;
         if (!idat || check_idat_crc) {
             const uint32_t crc = crc32_update(crc32_update(0xFFFFFFFFu, type, 4), d, length) ^ 0xFFFFFFFFu;
-            if (crc != stored) {
-                fail(p, kPdecInvalid, "CRC mismatch in %s chunk", utf8_lossy(type, 4).c_str());
-                return;
-            }
+            if (crc != stored)
+                return decode_fail(p.status, kInvalidDecode, "CRC mismatch in %s chunk", utf8_lossy(type, 4).c_str());
         }
         if (memcmp(type, "IHDR", 4) == 0) {
-            if (length != 13) { fail(p, kPdecInvalid, "invalid IHDR length"); return; }
+            if (length != 13) return decode_fail(p.status, kInvalidDecode, "invalid IHDR length");
             const uint8_t ct = d[9];
-            if (ct != 0 && ct != 2 && ct != 3 && ct != 4 && ct != 6) {
-                fail(p, kPdecInvalid, "invalid PNG color type: %u", ct);
-                return;
-            }
+            if (ct != 0 && ct != 2 && ct != 3 && ct != 4 && ct != 6)
+                return decode_fail(p.status, kInvalidDecode, "invalid PNG color type: %u", ct);
             have_ihdr = true;
             p.width = be32(d);
             p.height = be32(d + 4);
@@ -164,7 +121,7 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
             filt = d[11];
             interlace = d[12];
         } else if (memcmp(type, "PLTE", 4) == 0) {
-            if (length % 3 != 0) { fail(p, kPdecInvalid, "invalid PLTE length"); return; }
+            if (length % 3 != 0) return decode_fail(p.status, kInvalidDecode, "invalid PLTE length");
             p.has_plte = true;
             p.plte.assign(d, d + length);
         } else if (memcmp(type, "tRNS", 4) == 0) {
@@ -180,19 +137,17 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
         }
         pos = crc_end;
     }
-    if (!seen_iend) { fail(p, kPdecInvalid, "missing IEND chunk"); return; }
-    if (!have_ihdr) { fail(p, kPdecInvalid, "missing IHDR chunk"); return; }
-    if (p.width == 0 || p.height == 0) {
-        fail(p, kPdecDimensions, "Invalid image dimensions: %ux%u", p.width, p.height);
-        return;
-    }
-    if (p.width > (1u << 24) || p.height > (1u << 24)) {
-        fail(p, kPdecTooLarge, "Image %ux%u exceeds maximum dimension %u", p.width, p.height, 1u << 24);
-        return;
-    }
-    if (comp != 0) { fail(p, kPdecInvalid, "unsupported compression method"); return; }
-    if (filt != 0) { fail(p, kPdecInvalid, "unsupported filter method"); return; }
-    if (interlace != 0) { fail(p, kPdecUnsupported, "Adam7 interlaced images not supported"); return; }
+    if (!seen_iend) return decode_fail(p.status, kInvalidDecode, "missing IEND chunk");
+    if (!have_ihdr) return decode_fail(p.status, kInvalidDecode, "missing IHDR chunk");
+    if (p.width == 0 || p.height == 0)
+        return decode_fail(p.status, PIXO_B200_ERR_INVALID_DIMENSIONS, "Invalid image dimensions: %ux%u", p.width,
+                           p.height);
+    if (p.width > (1u << 24) || p.height > (1u << 24))
+        return decode_fail(p.status, PIXO_B200_ERR_IMAGE_TOO_LARGE, "Image %ux%u exceeds maximum dimension %u", p.width,
+                           p.height, 1u << 24);
+    if (comp != 0) return decode_fail(p.status, kInvalidDecode, "unsupported compression method");
+    if (filt != 0) return decode_fail(p.status, kInvalidDecode, "unsupported filter method");
+    if (interlace != 0) return decode_fail(p.status, kUnsupportedDecode, "Adam7 interlaced images not supported");
     const uint8_t bd = p.depth;
     bool ok;
     switch (p.ctype) {
@@ -200,11 +155,9 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
     case 3: ok = bd == 1 || bd == 2 || bd == 4 || bd == 8; break;
     default: ok = bd == 8 || bd == 16; break;
     }
-    if (!ok) {
-        fail(p, kPdecInvalid, "invalid bit depth %u for color type %s", bd, ctype_name(p.ctype));
-        return;
-    }
-    if (p.idat_total == 0) { fail(p, kPdecInvalid, "no IDAT data"); return; }
+    if (!ok)
+        return decode_fail(p.status, kInvalidDecode, "invalid bit depth %u for color type %s", bd, ctype_name(p.ctype));
+    if (p.idat_total == 0) return decode_fail(p.status, kInvalidDecode, "no IDAT data");
     const uint64_t w = p.width;
     static const uint32_t kChannels[7] = {1, 0, 3, 1, 2, 0, 4};
     const uint32_t ch = kChannels[p.ctype];
@@ -217,13 +170,14 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
     }
     p.expected = (uint64_t)p.height * (1 + p.sb);
     // the zlib header: the IDAT payloads concatenated, as inflate_zlib_with_size sees them
-    if (p.idat_total < 6) { fail(p, kPdecInvalid, "zlib stream too short"); return; }
+    if (p.idat_total < 6) return decode_fail(p.status, kInvalidDecode, "zlib stream too short");
     uint8_t hdr[2];
     for (size_t c = 0, k = 0; c < p.idat_off.size() && k < 2; ++c)
         for (uint32_t j = 0; j < p.idat_len[c] && k < 2; ++j) hdr[k++] = data[p.idat_off[c] + j];
-    if ((hdr[0] & 0x0F) != 8) { fail(p, kPdecInvalid, "invalid zlib compression method"); return; }
-    if ((((uint32_t)hdr[0] << 8) | hdr[1]) % 31 != 0) { fail(p, kPdecInvalid, "invalid zlib header checksum"); return; }
-    if (hdr[1] & 0x20) { fail(p, kPdecUnsupported, "preset dictionary not supported"); return; }
+    if ((hdr[0] & 0x0F) != 8) return decode_fail(p.status, kInvalidDecode, "invalid zlib compression method");
+    if ((((uint32_t)hdr[0] << 8) | hdr[1]) % 31 != 0)
+        return decode_fail(p.status, kInvalidDecode, "invalid zlib header checksum");
+    if (hdr[1] & 0x20) return decode_fail(p.status, kUnsupportedDecode, "preset dictionary not supported");
     // the frame decode_png returns
     bool alpha = false;
     for (uint8_t a : p.trns) alpha |= a != 0xFF;
@@ -237,6 +191,12 @@ void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_
         p.out_channels = alpha ? 4 : 3;
         break;
     }
+    return true;
+}
+
+void parse(const uint8_t *data, size_t len, PdecParsed &p)
+{
+    if (!walk(data, len, p, false)) walk(data, len, p, true);
 }
 
 }  // namespace pixo

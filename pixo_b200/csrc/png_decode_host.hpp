@@ -6,25 +6,45 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include <string>
 #include <vector>
+
+#include "decode_host.hpp"
+#include "png_host.hpp"   // PIXO_HOST_DEVICE
 
 namespace pixo {
 
-// Error kinds of decode_png (src/error.rs)
-enum PdecKind { kPdecOk = 0, kPdecInvalid = 1, kPdecUnsupported = 2, kPdecDimensions = 3, kPdecTooLarge = 4 };
-
 // The CRC-32 of PNG chunks (reflected 0xEDB88320).  crc32_update runs the register over bytes without the final
 // inversion; crc32_shift(r, n) is the register r advanced over n zero bytes, so that the register over A || B
-// from any start s is crc32_shift(reg(s, A), |B|) ^ reg(0, B).
+// from any start s is crc32_shift(reg(s, A), |B|) ^ reg(0, B).  k_png_crc combines its pieces with crc32_shift.
 uint32_t crc32_update(uint32_t reg, const uint8_t *p, size_t n);
-uint32_t crc32_shift(uint32_t reg, uint64_t nbytes);
+
+// a * b modulo the CRC polynomial, bit 31 holding x^0 (the reflected order the register uses)
+PIXO_HOST_DEVICE inline uint32_t crc_mulmod(uint32_t a, uint32_t b)
+{
+    uint32_t p = 0;
+    for (uint32_t m = 1u << 31; m; m >>= 1) {
+        if (a & m) p ^= b;
+        b = b & 1 ? (b >> 1) ^ 0xEDB88320u : b >> 1;
+    }
+    return p;
+}
+
+PIXO_HOST_DEVICE inline uint32_t crc32_shift(uint32_t reg, uint64_t nbytes)
+{
+    // x^(8 * nbytes) by squaring: x2n holds x^(2^k) for the bits of 8 * nbytes
+    uint32_t x2n = 1u << 30, f = 1u << 31;   // x^1, x^0
+    for (int k = 0; k < 3; ++k) x2n = crc_mulmod(x2n, x2n);
+    for (; nbytes; nbytes >>= 1) {
+        if (nbytes & 1) f = crc_mulmod(x2n, f);
+        x2n = crc_mulmod(x2n, x2n);
+    }
+    return crc_mulmod(f, reg);
+}
 
 // One file after the host's share of decode_png (src/decode/png.rs:101-263 and the zlib header of
 // inflate_zlib_with_size, src/decode/inflate.rs:294-320)
 struct PdecParsed {
-    int kind = kPdecOk;
-    std::string msg;            // pixo's Display text of the error
+    DecodeStatus status;
     uint32_t width = 0, height = 0;
     uint8_t depth = 0, ctype = 0;   // IHDR bit depth and PNG colour type (0, 2, 3, 4, 6)
     bool has_plte = false;
@@ -50,21 +70,18 @@ struct PdecParsed {
     bool direct() const { return depth == 8 && ctype != 3; }
 };
 
-// Everything decode_png decides before it inflates, IDAT CRCs excepted: p.kind is kPdecOk when the file reaches
-// the DEFLATE data.  With check_idat_crc the IDAT CRCs are checked here as well, each at its place in the walk.
-void pdec_parse(const uint8_t *data, size_t len, PdecParsed &p, bool check_idat_crc);
+// Everything decode_png decides before it inflates: p.status is clear when the file reaches the DEFLATE data.  The
+// IDAT CRCs are left to the device, except in a file refused here: that one is walked again with them checked, each
+// at its place in the walk, so that an IDAT chunk that fails before the error found is reported first, as in pixo.
+void parse(const uint8_t *data, size_t len, PdecParsed &p);
 
 }  // namespace pixo
 
 struct pixo_b200_ctx;
 namespace pixo {
-// What the device decided for one file: 0, or the first failure in pixo's order after the host's checks
-struct PdecResult {
-    int kind;          // PdecKind
-    std::string msg;
-};
-// Decodes n parsed files (all kPdecOk) on the context's stream: file i's frame to d_out + out_off[i].  data[i] is
-// the file.  Waits for the device once per pass and fills res[i].  Passes of bounded scratch.
-int launch_png_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const uint8_t *const *data, uint32_t n,
-                      const uint64_t *out_off, uint8_t *d_out, PdecResult *res);
+// Decodes n parsed files (all without error) on the context's stream: file i's frame to d_out + out_off[i].  data[i]
+// is the file.  Waits for the device once per pass and sets res[i] to what the device decided: clear, or the first
+// failure in pixo's order after the host's checks.  Passes of bounded scratch.
+int launch_decode(pixo_b200_ctx *ctx, const PdecParsed *const *files, const uint8_t *const *data, uint32_t n,
+                  const uint64_t *out_off, uint8_t *d_out, DecodeStatus *res);
 }  // namespace pixo

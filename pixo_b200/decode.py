@@ -63,25 +63,25 @@ class DecodedBatch:
     errors: list
 
 
-def decode_jpeg_batch_dev(files, ctx: Context | None = None, align: int = 256) -> DecodedBatch:
-    """Decodes the files into one device tensor (pixo_b200_jpeg_decode_to_device); the decode is queued on the
-    context's stream when this returns, and the tensor belongs to that stream (work on another stream must wait for
-    it, e.g. through ctx.sync()).  Each frame starts on an `align`-byte boundary."""
+def _batch_dev(blobs, info, entry_point, ctx, align, failed_text) -> DecodedBatch:
+    """Decodes the blobs into one device tensor through entry_point (pixo_b200_*_decode_to_device).  info(b) gives
+    (width, height, color_type, producible); only a producible file gets a slot.  A file the call fails has geometry
+    None, and PixoError(status, failed_text) where info raised no error."""
     import torch
     ctx = ctx or default_context()
-    blobs = [_bytes(f) for f in files]
     geoms, errors, offsets, total = [], [], [], 0
     for b in blobs:
         try:
-            w, h, ct = jpeg_info(b)
+            w, h, ct, producible = info(b)
             geoms.append((w, h, ct))
             errors.append(None)
         except _lib.PixoError as e:
             geoms.append(None)
             errors.append(e)
+            producible = False
         offsets.append(total)
-        if geoms[-1]:
-            total += -(-geoms[-1][0] * geoms[-1][1] * ColorType(geoms[-1][2]).bytes_per_pixel() // align) * align
+        if producible:
+            total += -(-w * h * ColorType(ct).bytes_per_pixel() // align) * align
     # allocated on the stream that writes it: torch's caching allocator then neither hands the memory out while the
     # decode is still writing it nor lets the decode write memory that earlier work on another stream still reads
     dev = torch.device("cuda", ctx.device)
@@ -94,12 +94,21 @@ def decode_jpeg_batch_dev(files, ctx: Context | None = None, align: int = 256) -
     lens = (C.c_size_t * max(n, 1))(*[len(b) for b in blobs])
     offs = (C.c_size_t * max(n, 1))(*offsets)
     status = (C.c_int32 * max(n, 1))()
-    _lib.check(ctx.handle, _lib.load().pixo_b200_jpeg_decode_to_device(
-        ctx.handle, C.cast(ptrs, C.c_void_p), lens, n, frames.data_ptr(), offs, status))
+    _lib.check(ctx.handle, entry_point(ctx.handle, C.cast(ptrs, C.c_void_p), lens, n, frames.data_ptr(), offs, status))
     for i in range(n):
-        if status[i] and errors[i] is None:
-            errors[i] = _lib.PixoError(status[i], "invalid argument")
+        if status[i]:
+            geoms[i] = None
+            if errors[i] is None:
+                errors[i] = _lib.PixoError(status[i], failed_text)
     return DecodedBatch(frames, offsets, geoms, errors)
+
+
+def decode_jpeg_batch_dev(files, ctx: Context | None = None, align: int = 256) -> DecodedBatch:
+    """Decodes the files into one device tensor (pixo_b200_jpeg_decode_to_device); the decode is queued on the
+    context's stream when this returns, and the tensor belongs to that stream (work on another stream must wait for
+    it, e.g. through ctx.sync()).  Each frame starts on an `align`-byte boundary."""
+    return _batch_dev([_bytes(f) for f in files], lambda b: (*jpeg_info(b), True),
+                      _lib.load().pixo_b200_jpeg_decode_to_device, ctx, align, "invalid argument")
 
 
 @dataclasses.dataclass
@@ -143,37 +152,5 @@ def decode_png_batch_dev(files, ctx: Context | None = None, align: int = 256) ->
     once per pass, so every file's status is known when it returns; the frames are written in the context's stream
     order, and the tensor belongs to that stream.  Each frame starts on an `align`-byte boundary.  A file whose rows
     (height * (1 + scanline bytes)) are more than its IDAT data can produce is certain to fail and gets no slot."""
-    import torch
-    ctx = ctx or default_context()
-    blobs = [_bytes(f) for f in files]
-    geoms, errors, offsets, total = [], [], [], 0
-    for b in blobs:
-        try:
-            w, h, ct, producible = _png_info(b)
-            geoms.append((w, h, ct))
-            errors.append(None)
-        except _lib.PixoError as e:
-            geoms.append(None)
-            errors.append(e)
-            producible = False
-        offsets.append(total)
-        if producible:
-            total += -(-w * h * ColorType(ct).bytes_per_pixel() // align) * align
-    dev = torch.device("cuda", ctx.device)
-    sp = _lib.load().pixo_b200_ctx_stream(ctx.handle)
-    stream = torch.cuda.ExternalStream(sp, device=dev) if sp else torch.cuda.default_stream(dev)
-    with torch.cuda.stream(stream):
-        frames = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
-    n = len(blobs)
-    ptrs = (C.c_char_p * max(n, 1))(*blobs)
-    lens = (C.c_size_t * max(n, 1))(*[len(b) for b in blobs])
-    offs = (C.c_size_t * max(n, 1))(*offsets)
-    status = (C.c_int32 * max(n, 1))()
-    _lib.check(ctx.handle, _lib.load().pixo_b200_png_decode_to_device(
-        ctx.handle, C.cast(ptrs, C.c_void_p), lens, n, frames.data_ptr(), offs, status))
-    for i in range(n):
-        if status[i]:
-            geoms[i] = None
-            if errors[i] is None:
-                errors[i] = _lib.PixoError(status[i], "png decode failed")
-    return DecodedBatch(frames, offsets, geoms, errors)
+    return _batch_dev([_bytes(f) for f in files], _png_info, _lib.load().pixo_b200_png_decode_to_device, ctx, align,
+                      "png decode failed")

@@ -379,8 +379,9 @@ def test_jpeg_guarded_offsets_with_bad_files(ctx):
     check_guarded(host, offs, status, want, codes)
 
 
-# launch_jpeg_decode (jpeg_decode.cu) charges each file blocks * 192 + its entropy bytes + sizeof(JdecFile) +
-# kJdecFileTables of scratch (file_scratch) and closes a pass before the file that would take it past 1 GiB
+# The JPEG launcher (jpeg_decode.cu) charges each file blocks * 192 + its entropy bytes + sizeof(JdecFile) +
+# kJdecFileTables of scratch (file_scratch), and the pass driver (pass_end, decode_host.hpp) closes a pass before the
+# file that would take it past 1 GiB
 JDEC_PASS_BYTES = 1 << 30
 JDEC_FILE_BYTES = 576 + 8 * 2048
 
