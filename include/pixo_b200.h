@@ -68,7 +68,8 @@ typedef enum {
     PIXO_B200_ERR_CUDA = 10,               /* CUDA runtime/driver failure (no device, launch) */
     PIXO_B200_ERR_OOM = 11,                /* device or pinned allocation failed */
     PIXO_B200_ERR_INVALID_DECODE = 12,     /* Error::InvalidDecode: malformed or corrupt input to a decoder */
-    PIXO_B200_ERR_UNSUPPORTED_DECODE = 13  /* Error::UnsupportedDecode: valid input a decoder does not handle */
+    PIXO_B200_ERR_UNSUPPORTED_DECODE = 13, /* Error::UnsupportedDecode: valid input a decoder does not handle */
+    PIXO_B200_ERR_INVALID_COMPRESSION_LEVEL = 14  /* Error::InvalidCompressionLevel: a level outside 1-9 */
 } pixo_b200_status;
 
 /* pixo::ColorType repr(u8) — src/color.rs:8-18 */
@@ -733,6 +734,27 @@ int pixo_b200_png_decode_to_device(pixo_b200_ctx *ctx, const uint8_t *const *fil
 int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t *out);
 /* device buffer; result written to d_out (device u32), asynchronous */
 int pixo_b200_adler32_dev(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t len, uint32_t *d_out);
+
+/* Replaces compress::deflate::deflate_zlib_packed (src/compress/deflate.rs:1074) at levels 1-9: the zlib stream
+ * pixo writes for `data`, byte for byte (one DEFLATE block, stored, fixed or dynamic, as compress_packed_zlib
+ * chooses).  A level outside 1-9 returns PIXO_B200_ERR_INVALID_COMPRESSION_LEVEL ("Invalid compression level {n}:
+ * must be 1-9", pixo's png::encode check).  *out_len receives the stream's length; when it exceeds out_cap the call
+ * returns PIXO_B200_ERR_OUTPUT_TOO_SMALL and writes nothing.  Inputs of 2^31 bytes or more (beyond pixo's i32
+ * positions) return PIXO_B200_ERR_UNSUPPORTED. */
+int pixo_b200_deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t level, uint8_t *out,
+                           size_t out_cap, size_t *out_len);
+/* n device streams, stream i at d_streams + i * stride, lens[i] bytes (host array), each to its slot at
+ * d_out + i * out_cap_each.  out_lens[i] and status[i] (host arrays) receive each stream's length and 0, or
+ * PIXO_B200_ERR_OUTPUT_TOO_SMALL for a stream longer than its slot, which is then left untouched.  Streams are
+ * parsed one warp each, longest first, in passes of about 1 GiB of token scratch (a longer stream goes alone); the
+ * call waits once per pass for the symbol counts and for the pass's coding, and returns with the work done.  Level
+ * and length errors as pixo_b200_deflate_zlib, before anything is launched; null arrays or d_out return
+ * PIXO_B200_ERR_INVALID_ARGUMENT, and a stream longer than stride in a batch of more than one returns
+ * PIXO_B200_ERR_INVALID_DATA_LENGTH.  Named like pixo_b200_png_decode_to_device, not `_dev`: it takes host arrays and
+ * waits for the device before it returns, where the `_dev` calls are the stream-ordered ones listed above. */
+int pixo_b200_deflate_zlib_on_device(pixo_b200_ctx *ctx, const uint8_t *d_streams, size_t stride, const size_t *lens,
+                                     uint32_t n, uint32_t level, uint8_t *d_out, size_t out_cap_each,
+                                     size_t *out_lens, int32_t *status);
 
 #ifdef __cplusplus
 }

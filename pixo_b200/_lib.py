@@ -25,6 +25,7 @@ ERR_INVALID_QUALITY, ERR_INVALID_DIMENSIONS, ERR_IMAGE_TOO_LARGE, ERR_UNSUPPORTE
 ERR_INVALID_DATA_LENGTH, ERR_INVALID_RESTART, ERR_INVALID_ARGUMENT, ERR_OUTPUT_TOO_SMALL = 5, 6, 7, 8
 ERR_UNSUPPORTED, ERR_CUDA, ERR_OOM = 9, 10, 11
 ERR_INVALID_DECODE, ERR_UNSUPPORTED_DECODE = 12, 13
+ERR_INVALID_COMPRESSION_LEVEL = 14
 
 # every symbol include/pixo_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
@@ -140,6 +141,9 @@ SYMBOLS = {
     "pixo_b200_resize_weights": (C.c_int, [C.c_uint32, C.c_uint32, vp, vp, vp, vp, C.c_size_t, szp]),
     "pixo_b200_adler32": (C.c_int, [vp, vp, C.c_size_t, u32p]),
     "pixo_b200_adler32_dev": (C.c_int, [vp, vp, C.c_size_t, vp]),
+    "pixo_b200_deflate_zlib": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, vp, C.c_size_t, szp]),
+    "pixo_b200_deflate_zlib_on_device": (C.c_int, [vp, vp, C.c_size_t, szp, C.c_uint32, C.c_uint32, vp, C.c_size_t, szp,
+                                             C.POINTER(C.c_int32)]),
 }
 
 

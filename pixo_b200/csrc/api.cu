@@ -2048,6 +2048,57 @@ int pixo_b200_adler32(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint3
     return 0;
 }
 
+// ---- DEFLATE ---------------------------------------------------------------------------------
+
+// png::encode's first check (src/png/mod.rs:442-447)
+static int check_level(pixo_b200_ctx *ctx, uint32_t level)
+{
+    if (level < 1 || level > 9)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_COMPRESSION_LEVEL, "Invalid compression level %u: must be 1-9", level);
+    return 0;
+}
+
+// Named as pixo_b200_png_decode_to_device is, not `_dev`: like the decoders' batch call it takes host arrays (lens,
+// out_lens, status) and waits for the device before it returns, where the `_dev` calls are the stream-ordered ones
+int pixo_b200_deflate_zlib_on_device(pixo_b200_ctx *ctx, const uint8_t *d_streams, size_t stride, const size_t *lens,
+                                     uint32_t n, uint32_t level, uint8_t *d_out, size_t out_cap_each,
+                                     size_t *out_lens, int32_t *status)
+{
+    if (!ctx) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null context");
+    PIXO_TRY(check_level(ctx, level));
+    if (n && (!lens || !out_lens || !status || !d_out || !d_streams))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
+    // streams of a batch may not overlap: stream i is read at d_streams + i * stride
+    for (uint32_t i = 0; n > 1 && i < n; i++)
+        if (lens[i] > stride)
+            return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: stream %u is %zu bytes, stride %zu",
+                             i, lens[i], stride);
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return deflate_zlib(ctx, d_streams, stride, lens, n, (int)level, d_out, out_cap_each, out_lens, status);
+}
+
+int pixo_b200_deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, uint32_t level, uint8_t *out,
+                           size_t out_cap, size_t *out_len)
+{
+    if (!ctx) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null context");
+    PIXO_TRY(check_level(ctx, level));
+    if (!out_len || (!data && len) || (!out && out_cap))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null argument");
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    // the longest stream pixo writes: stored blocks, 5 bytes per 65 535, with the zlib header and Adler-32
+    const size_t most = 2 + len + (len / 65535 + 1) * 5 + 4;
+    uint8_t *d_data, *d_zout;
+    PIXO_TRY(bind(ctx, ctx->d_in, [&](Layout &L) { d_data = L.take(len + 16), d_zout = L.take(most); }));
+    DrainOnError drain(ctx);
+    if (len) PIXO_TRY(h2d_copy(ctx, d_data, data, len, ctx->stream));
+    int32_t st = 0;
+    PIXO_TRY(deflate_zlib(ctx, d_data, 0, &len, 1, (int)level, d_zout, most, out_len, &st));
+    drain.armed = false;
+    if (*out_len > out_cap)
+        return set_error(ctx, PIXO_B200_ERR_OUTPUT_TOO_SMALL, "output capacity %zu below %zu", out_cap, *out_len);
+    return d2h_copy_sync(ctx, out, d_zout, *out_len, ctx->stream);
+}
+
 // ---- resize --------------------------------------------------------------------------------
 
 // the wasm binding's enum checks (src/wasm.rs:55-67,156-166), then resize_impl's (src/resize.rs:205-250)

@@ -206,6 +206,7 @@ struct pixo_b200_ctx {
     pixo::DevBuf d_resize, d_resize_tmp;   // resize: Lanczos3 weight tables; the u8 intermediate (bounded)
     pixo::DevBuf d_jdec;                   // JPEG decode: a pass's records, tables and scans, coefficients, planes
     pixo::DevBuf d_pdec;                   // PNG decode: a pass's records, chunks and streams, rings, inflated rows
+    pixo::DevBuf d_lz, d_zemit;            // DEFLATE: a pass's streams, tokens and hash state; its coded streams
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn
@@ -330,6 +331,9 @@ int png_quantize_filter(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_str
 // 1 Bilinear, 2 Lanczos3
 int launch_resize(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, uint32_t n, uint32_t sw, uint32_t sh,
                   uint32_t dw, uint32_t dh, uint32_t bpp, uint32_t algorithm, uint8_t *d_dst, size_t dst_stride);
+// pixo_b200_deflate_zlib_on_device after validation (png_deflate.cu): level 1-9, host lens / out_lens / status
+int deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *d_streams, size_t stride, const size_t *lens, uint32_t n, int level,
+                 uint8_t *d_out, size_t out_cap_each, size_t *out_lens, int32_t *status);
 
 struct FrameGeometry;
 struct HuffTables;
