@@ -14,9 +14,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libpixo_b200.so")
-SOURCES = ["api.cu", "jpeg_transform.cu", "jpeg_trellis.cu", "jpeg_entropy.cu", "jpeg_progressive.cu", "png_filter.cu", "png_reduce.cu", "png_quantize.cu",
+SOURCES = ["api.cu", "api_jpeg.cu", "api_png.cu", "api_decode.cu", "jpeg_transform.cu", "jpeg_trellis.cu", "jpeg_entropy.cu", "jpeg_progressive.cu", "png_filter.cu", "png_reduce.cu", "png_quantize.cu",
            "resize.cu", "jpeg_decode.cu", "png_decode.cu", "png_deflate.cu", "jpeg_host.cpp", "jpeg_decode_host.cpp", "png_decode_host.cpp", "png_host.cpp", "resize_host.cpp"]
-HEADERS = ["common.cuh", "decode_host.hpp", "jpeg_host.hpp", "jpeg_decode_host.hpp", "png_decode_host.hpp", "png_host.hpp", "resize_host.hpp", os.path.join("..", "..", "include", "pixo_b200.h")]
+HEADERS = ["api.hpp", "common.cuh", "decode_host.hpp", "jpeg_host.hpp", "jpeg_decode_host.hpp", "png_decode_host.hpp", "png_host.hpp", "resize_host.hpp", os.path.join("..", "..", "include", "pixo_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -381,7 +381,7 @@ int launch_splice_bounded(pixo_b200_ctx *ctx, const SegPlan &sp, uint8_t *seg_sc
 // progressive scans (jpeg_progressive.cu)
 bool prog_tables(const uint8_t bits[4][16], const uint8_t *const vals[4], ProgTables *T);
 // The 7 scans of n whole frames into *dst (the coefficients, DHT blocks and trellis status of an encode come from
-// api.cu's progressive_coefficients).  Tables and the raw strings:
+// api_jpeg.cu's progressive_coefficients).  Tables and the raw strings:
 //  - d_dht: frame i's from its DHT block at d_dht + i * kDhtBytes, queued without a wait; a frame's raw string
 //    is as long as its slot (dst->cap + 16 bytes), and a frame whose raw bytes exceed dst->cap is left out
 //    (overflow bit 0).  d_trellis_status (or null) is folded into the frames' flags.
