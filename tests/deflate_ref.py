@@ -243,6 +243,22 @@ def lz77(data: bytes, level: int):
     return p.parse(), p.ev
 
 
+def is_high_entropy_data(data: bytes):
+    """is_high_entropy_data (deflate.rs:1108-1145): (fires, collisions).  Streams under 4 096 bytes never fire; the
+    first min(n, 8 192) bytes' 4-grams are hashed into 4 096 slots, and the bail fires when the share of 4-grams whose
+    slot was already taken is below 5 %, divided in f32 (`collisions as f32 / total as f32 < 0.05`)."""
+    import numpy as np
+    if len(data) < 4096:
+        return False, 0
+    sample = bytes(data[:8192])
+    seen, coll = set(), 0
+    for i in range(len(sample) - 3):
+        h = ((int.from_bytes(sample[i:i + 4], "little") * 0x1E35A7BD) & M32) >> 20 & 4095
+        coll += h in seen
+        seen.add(h)
+    return bool(np.float32(coll) / np.float32(len(sample) - 3) < np.float32(0.05)), coll
+
+
 # ---- build_codes with Rust's BinaryHeap<Reverse<Node>> ---------------------------------------------------------
 
 def _key(node):

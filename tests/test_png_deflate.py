@@ -87,8 +87,9 @@ def test_code_lengths_are_limited_and_tie_sensitive():
 
 
 def test_high_entropy_bail_never_fires_on_the_samples():
-    """is_high_entropy_data needs fewer than 5 % repeated 4-gram hashes; 8 189 4-grams in 4 096 slots repeat at
-    least 4 093 times, so from 4 312 bytes on it cannot fire.  Random data near 4 096 bytes does not reach it either."""
+    """is_high_entropy_data needs fewer than 5 % repeated 4-gram hashes; n - 3 4-grams in 4 096 slots repeat at
+    least n - 4 099 times, so from 4 315 bytes on it cannot fire.  Random data near 4 096 bytes does not reach it
+    either (test_deflate_edges.py builds streams that do)."""
     rng = np.random.default_rng(3)
     for n in (4096, 4200, 4311, 8192, 100000):
         assert not pd.high_entropy(rng.integers(0, 256, n, dtype=np.uint8).tobytes()), n
