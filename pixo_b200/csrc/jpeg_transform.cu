@@ -255,8 +255,8 @@ struct QPairTab {
 // held as row pairs R[i][c] = (v[2i][c], v[2i+1][c]); writes 64 int16 (8 x 16 B).
 //   x / d      : q0 = x*r; q = fma(fma(q0, -d, x), r, q0) == RN(x/d)     (tools/verify_div.c)
 //   round      : w = RZ(q + 0.5); m = floor(sign(q) * w) via fma.rm with 1.5*2^23;
-//                result = m for q >= 0, ~m for q < 0  == round-half-away(q)  (tests prove it
-//                bit-for-bit against the oracle; derivation in DESIGN.md)
+//                result = m for q >= 0, ~m for q < 0  == round-half-away(q)  (derivation in DESIGN.md;
+//                tests/test_transform_edges_gpu.py runs ties, their neighbours and 0.49999997)
 // `out` is the block's 128-byte slot in a warp-private shared-memory stage; its eight 16-byte
 // chunks are written at chunk index (k ^ swz) so that the lanes of a quarter warp hit distinct
 // banks (the caller then copies the stage out with fully coalesced 512-byte warp stores).
