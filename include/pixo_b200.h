@@ -29,6 +29,8 @@
  *      jpeg_band_entropy_dev, jpeg_band_splice_dev, jpeg_band_dev_progressive_summary,
  *      jpeg_band_dev_progressive, jpeg_band_dev_progressive_splice, png_reduce_filter_dev,
  *      png_quantize_filter_dev.
+ *    The `_on_device` calls (deflate_zlib_on_device, png_encode_on_device) and the decoders' `_to_device` calls
+ *    take host arrays for their per-item results and wait for the device before they return.
  *    The others take host pointers and return after the result is in `out`.
  *  - every function returns a pixo_b200_status (0 = ok).  pixo_b200_last_error(ctx) gives the
  *    message a Rust shim would wrap in Error::CompressionError(String) (src/error.rs:41).
@@ -755,6 +757,55 @@ int pixo_b200_deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, 
 int pixo_b200_deflate_zlib_on_device(pixo_b200_ctx *ctx, const uint8_t *d_streams, size_t stride, const size_t *lens,
                                      uint32_t n, uint32_t level, uint8_t *d_out, size_t out_cap_each,
                                      size_t *out_lens, int32_t *status);
+
+/* ---- whole PNG files ---------------------------------------------------------------------- */
+
+/* PngOptions::optimal_compression (pixo's max preset).  Accepted only by the two encode calls, which refuse it. */
+#define PIXO_B200_PNG_OPTIMAL_COMPRESSION 0x4000u
+
+/* Replaces pixo::png::encode_into (src/png/mod.rs:437-630, and encode_indexed_into :1814-1886 for frames that
+ * quantise) at pixo's fast and balanced presets: one host image -> one complete PNG file in `out`, byte for byte
+ * pixo's (the default, parallel build's filter choice).  strategy_and_flags, max_colors and palette / palette_len
+ * mean what they mean for pixo_b200_png_quantize_filter: without a QUANTIZE flag the frame takes the reduction path,
+ * and without a REDUCE flag either it is only filtered (preset 0).  compression_level: PngOptions::compression_level,
+ * the DEFLATE level (pixo_b200_deflate_zlib).  The file is the signature, IHDR, PLTE and tRNS when the frame has a
+ * palette (a quantised frame's tRNS trimmed as pixo trims it), the zlib stream in IDAT chunks of 256 KiB, and IEND.
+ * pixo's strip_metadata has no flag: pixo never writes tEXt, zTXt, iTXt or tIME, so on its own output
+ * strip_metadata_chunks changes nothing.  Errors in pixo's order, before anything is launched: a level outside 1-9
+ * PIXO_B200_ERR_INVALID_COMPRESSION_LEVEL; then pixo_b200_png_quantize_filter's checks (dimensions, size above 2^24,
+ * colour type, flags, AUTO with FORCE, max_colors, the palette, data_len); then PIXO_B200_PNG_OPTIMAL_COMPRESSION
+ * returns PIXO_B200_ERR_UNSUPPORTED.  A filtered stream of 2^31 bytes or more returns PIXO_B200_ERR_UNSUPPORTED;
+ * more than 8192 sampled colours without a palette returns it as pixo_b200_png_quantize_filter does.  *out_len
+ * receives the file's length; above out_cap the call returns PIXO_B200_ERR_OUTPUT_TOO_SMALL and writes nothing.
+ * The checks need no context: with ctx NULL they run in the same order, and a call that passes them returns
+ * PIXO_B200_ERR_INVALID_ARGUMENT ("ctx is null"). */
+int pixo_b200_png_encode(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width, uint32_t height,
+                         uint32_t color_type, uint32_t strategy_and_flags, uint32_t compression_level,
+                         uint32_t max_colors, const uint8_t *palette, uint32_t palette_len,
+                         uint8_t *out, size_t out_cap, size_t *out_len);
+
+/* n device frames of one geometry (frame i at d_data + i*in_stride) -> n complete PNG files, file i in the slot at
+ * d_out + i*out_cap_each, any byte alignment.  palettes / palette_lens (HOST memory, optional) and info (optional,
+ * n entries) as pixo_b200_png_quantize_filter_dev.  out_lens[i] and status[i] (host arrays) receive each file's
+ * length and 0; the length is known before anything is written, so a slot too small gets
+ * PIXO_B200_ERR_OUTPUT_TOO_SMALL, keeps the length it needs in out_lens[i], and is left untouched.  A frame whose
+ * filtered stream is 2^31 bytes or more gets PIXO_B200_ERR_UNSUPPORTED (out_lens[i] 0) and an untouched slot; the
+ * other frames are still written.  Checks as pixo_b200_png_encode, with in_stride below a frame in a batch of more
+ * than one PIXO_B200_ERR_INVALID_DATA_LENGTH, and input frames overlapping the output slots
+ * PIXO_B200_ERR_INVALID_ARGUMENT, all before anything is launched.  The frames go in passes whose unreduced
+ * filtered streams total about 1 GiB (a larger frame goes alone), on the context's stream: the filter stage
+ * (pixo_b200_png_quantize_filter_dev's launches), DEFLATE (pixo_b200_deflate_zlib_on_device's: k_lz77 and
+ * k_deflate_emit per pass of its own), then k_png_idat (the zlib streams into their IDAT chunks with each chunk's
+ * CRC-32, in 4 KiB pieces over many CTAs) and k_png_idat_finish (the small chunks, the CRCs and IEND) when the pass
+ * writes a file.  The call waits for the device once per stage and pass and returns with every file written.  A
+ * frame that quantises with more than 8192 sampled colours and no palette fails the call with
+ * PIXO_B200_ERR_UNSUPPORTED, as pixo_b200_png_quantize_filter_dev; files of earlier passes may then have been
+ * written.  The extra scratch is the pass's unreduced filtered streams and their stored-block zlib bounds. */
+int pixo_b200_png_encode_on_device(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
+                                   uint32_t width, uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                   uint32_t compression_level, uint32_t max_colors, const uint8_t *palettes,
+                                   const uint32_t *palette_lens, uint8_t *d_out, size_t out_cap_each,
+                                   size_t *out_lens, int32_t *status, pixo_b200_png_reduced *info);
 
 #ifdef __cplusplus
 }

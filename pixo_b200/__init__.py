@@ -2,7 +2,7 @@
 
 Python mirror of the reference's public API for this path:
   pixo_b200.jpeg  <->  pixo::jpeg   (encode, encode_into, JpegOptions, Subsampling)
-  pixo_b200.png   <->  pixo::png    (filter::apply_filters*, FilterStrategy, PngOptions) and
+  pixo_b200.png   <->  pixo::png    (encode, encode_into, filter::apply_filters*, FilterStrategy, PngOptions) and
                        pixo::compress::adler32
   pixo_b200.resize <-> pixo::resize (resize, resize_into, ResizeOptions, ResizeAlgorithm)
   pixo_b200.decode <-> pixo::decode (decode_jpeg, JpegImage, decode_png, PngImage)

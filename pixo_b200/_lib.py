@@ -144,6 +144,11 @@ SYMBOLS = {
     "pixo_b200_deflate_zlib": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, vp, C.c_size_t, szp]),
     "pixo_b200_deflate_zlib_on_device": (C.c_int, [vp, vp, C.c_size_t, szp, C.c_uint32, C.c_uint32, vp, C.c_size_t, szp,
                                              C.POINTER(C.c_int32)]),
+    "pixo_b200_png_encode": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                       C.c_uint32, vp, C.c_uint32, vp, C.c_size_t, szp]),
+    "pixo_b200_png_encode_on_device": (C.c_int, [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                 C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp, C.c_size_t, szp,
+                                                 C.POINTER(C.c_int32), vp]),
 }
 
 

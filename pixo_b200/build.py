@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libpixo_b200.so")
 SOURCES = ["api.cu", "api_jpeg.cu", "api_png.cu", "api_decode.cu", "jpeg_transform.cu", "jpeg_trellis.cu", "jpeg_entropy.cu", "jpeg_progressive.cu", "png_filter.cu", "png_reduce.cu", "png_quantize.cu",
-           "resize.cu", "jpeg_decode.cu", "png_decode.cu", "png_deflate.cu", "jpeg_host.cpp", "jpeg_decode_host.cpp", "png_decode_host.cpp", "png_host.cpp", "resize_host.cpp"]
+           "resize.cu", "jpeg_decode.cu", "png_decode.cu", "png_deflate.cu", "png_encode.cu", "jpeg_host.cpp", "jpeg_decode_host.cpp", "png_decode_host.cpp", "png_host.cpp", "resize_host.cpp"]
 HEADERS = ["api.hpp", "common.cuh", "decode_host.hpp", "jpeg_host.hpp", "jpeg_decode_host.hpp", "png_decode_host.hpp", "png_host.hpp", "resize_host.hpp", os.path.join("..", "..", "include", "pixo_b200.h")]
 
 NVCC_FLAGS = [

@@ -291,6 +291,106 @@ int pixo_b200_deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *data, size_t len, 
     });
 }
 
+// ---- whole PNG files -------------------------------------------------------------------------
+
+// encode_into's checks in pixo's order (src/png/mod.rs:437-467): the level, then those of the quantise entry points
+// with OPTIMAL_COMPRESSION taken as a known flag
+static int validate_png_encode(pixo_b200_ctx *ctx, uint32_t width, uint32_t height, uint32_t color_type,
+                               uint32_t strategy_and_flags, uint32_t level, uint32_t max_colors)
+{
+    PIXO_TRY(check_level(ctx, level));
+    return validate_png_quantize(ctx, width, height, color_type, strategy_and_flags & ~PIXO_B200_PNG_OPTIMAL_COMPRESSION,
+                                 max_colors);
+}
+
+// The longest file of a frame: a stored-block zlib stream (2 + n + (n / 65535 + 1) * 5 + 4 bytes, the most pixo
+// writes for n bytes) in IDAT chunks of 256 KiB, with the signature, IHDR and IEND; either of the unreduced rows, or,
+// for RGB and RGBA, of 8-bit palette indices with the largest PLTE and tRNS
+static uint64_t png_file_bound(uint32_t width, uint32_t height, uint32_t color_type)
+{
+    auto file = [](uint64_t n, uint64_t small) {
+        const uint64_t zb = 2 + n + (n / 65535 + 1) * 5 + 4;
+        return 8 + 25 + small + zb + 12 * ((zb + 262143) / 262144) + 12;
+    };
+    const uint64_t plain = file((uint64_t)height * ((uint64_t)width * (color_type + 1) + 1), 0);
+    if (color_type != PIXO_B200_RGB && color_type != PIXO_B200_RGBA) return plain;
+    return std::max(plain, file((uint64_t)height * ((uint64_t)width + 1), (12 + 768) + (12 + 256)));
+}
+
+static int refuse_optimal(pixo_b200_ctx *ctx, uint32_t strategy_and_flags)
+{
+    if (strategy_and_flags & PIXO_B200_PNG_OPTIMAL_COMPRESSION)
+        return set_error(ctx, PIXO_B200_ERR_UNSUPPORTED, "optimal_compression (pixo's max preset) is not built");
+    return 0;
+}
+
+int pixo_b200_png_encode_on_device(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n_images,
+                                   uint32_t width, uint32_t height, uint32_t color_type, uint32_t strategy_and_flags,
+                                   uint32_t compression_level, uint32_t max_colors, const uint8_t *palettes,
+                                   const uint32_t *palette_lens, uint8_t *d_out, size_t out_cap_each,
+                                   size_t *out_lens, int32_t *status, pixo_b200_png_reduced *info)
+{
+    // the checks run before the context is needed, so that they are pixo's whether or not a device is present
+    PIXO_TRY(validate_png_encode(ctx, width, height, color_type, strategy_and_flags, compression_level, max_colors));
+    if (n_images && (!d_data || !d_out || !out_lens || !status))
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if (palettes && !palette_lens) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "palettes without palette_lens");
+    for (uint32_t i = 0; palettes && i < n_images; ++i)
+        if (palette_lens[i] > 256)
+            return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "palette_lens[%u] = %u not in 0..256", i, palette_lens[i]);
+    const size_t in_bytes = (size_t)width * height * (color_type + 1);
+    if (n_images > 1 && in_stride < in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, in_stride);
+    PIXO_TRY(refuse_optimal(ctx, strategy_and_flags));
+    if (n_images == 0) return ctx ? 0 : set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    // the frames are read in passes while earlier passes' files are written
+    const uintptr_t i0 = (uintptr_t)d_data, i1 = i0 + (size_t)(n_images - 1) * in_stride + in_bytes;
+    const uintptr_t o0 = (uintptr_t)d_out, o1 = o0 + (size_t)n_images * out_cap_each;
+    if (i0 < o1 && o0 < i1)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "the input frames and the output slots overlap");
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    PIXO_CUDA(ctx, cudaSetDevice(ctx->device));
+    return png_encode(ctx, d_data, in_stride, n_images, width, height, color_type, strategy_and_flags,
+                      (int)compression_level, max_colors, palettes, palettes ? palette_lens : nullptr, d_out,
+                      out_cap_each, out_lens, status, info);
+}
+
+int pixo_b200_png_encode(pixo_b200_ctx *ctx, const uint8_t *data, size_t data_len, uint32_t width, uint32_t height,
+                         uint32_t color_type, uint32_t strategy_and_flags, uint32_t compression_level,
+                         uint32_t max_colors, const uint8_t *palette, uint32_t palette_len,
+                         uint8_t *out, size_t out_cap, size_t *out_len)
+{
+    PIXO_TRY(validate_png_encode(ctx, width, height, color_type, strategy_and_flags, compression_level, max_colors));
+    if (!data || !out_len || (!out && out_cap)) return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    if ((palette == nullptr) != (palette_len == 0) || palette_len > 256)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_ARGUMENT, "a given palette has 1..256 entries (palette_len %u)", palette_len);
+    const size_t in_bytes = (size_t)width * height * (color_type + 1);
+    if (data_len != in_bytes)
+        return set_error(ctx, PIXO_B200_ERR_INVALID_DATA_LENGTH, "Invalid data length: expected %zu bytes, got %zu",
+                         in_bytes, data_len);
+    PIXO_TRY(refuse_optimal(ctx, strategy_and_flags));
+    if (!ctx) return set_error(nullptr, PIXO_B200_ERR_INVALID_ARGUMENT, "ctx is null");
+    uint8_t pal256[1024];
+    if (palette) memcpy(pal256, palette, (size_t)palette_len * 4);
+    const size_t cap = png_file_bound(width, height, color_type);
+    uint8_t *d_file;
+    auto outputs = [&](Layout &L) { d_file = L.take(cap); };
+    return stage_host_call(ctx, data, in_bytes, outputs, [&](const uint8_t *d_in, HostResults &back) {
+        size_t len = 0;
+        int32_t st = 0;
+        pixo_b200_png_reduced r;
+        PIXO_TRY(pixo_b200_png_encode_on_device(ctx, d_in, in_bytes, 1, width, height, color_type, strategy_and_flags,
+                                                compression_level, max_colors, palette ? pal256 : nullptr,
+                                                palette ? &palette_len : nullptr, d_file, cap, &len, &st, &r));
+        if (st)   // the slot holds the largest file, so only the stream's length can refuse the frame
+            return set_error(ctx, st, "the filtered stream is %llu bytes: streams of 2^31 bytes or more are beyond "
+                             "pixo's i32 positions", (unsigned long long)height * (r.row_bytes + 1));
+        back = {{{out, d_file, len, out_len, out_cap}}};
+        return 0;
+    });
+}
+
 // ---- resize --------------------------------------------------------------------------------
 
 // the wasm binding's enum checks (src/wasm.rs:55-67,156-166), then resize_impl's (src/resize.rs:205-250)

@@ -207,6 +207,8 @@ struct pixo_b200_ctx {
     pixo::DevBuf d_jdec;                   // JPEG decode: a pass's records, tables and scans, coefficients, planes
     pixo::DevBuf d_pdec;                   // PNG decode: a pass's records, chunks and streams, rings, inflated rows
     pixo::DevBuf d_lz, d_zemit;            // DEFLATE: a pass's streams, tokens and hash state; its coded streams
+    pixo::DevBuf d_png_filt, d_png_z;      // PNG encode: a pass's filtered streams; their zlib streams
+    pixo::DevBuf d_png_box;                // PNG encode: a pass's container upload (files, CRC words, small chunks)
     pixo::PinnedBuf h_in, h_out, h_misc, h_red, h_quant;
     pixo::PinnedBuf h_trellis, h_prog;     // the trellis status; the progressive scans' bit counts / lengths
     pixo::PinnedBuf h_resize[2];           // Lanczos3 weight tables on their way to d_resize, in turn
@@ -334,6 +336,12 @@ int launch_resize(pixo_b200_ctx *ctx, const uint8_t *d_src, size_t src_stride, u
 // pixo_b200_deflate_zlib_on_device after validation (png_deflate.cu): level 1-9, host lens / out_lens / status
 int deflate_zlib(pixo_b200_ctx *ctx, const uint8_t *d_streams, size_t stride, const size_t *lens, uint32_t n, int level,
                  uint8_t *d_out, size_t out_cap_each, size_t *out_lens, int32_t *status);
+// pixo_b200_png_encode_on_device after validation (png_encode.cu): n frames -> n whole PNG files, host arrays;
+// info may be null.  Waits for the device.
+int png_encode(pixo_b200_ctx *ctx, const uint8_t *d_data, size_t in_stride, uint32_t n, uint32_t width,
+               uint32_t height, uint32_t color_type, uint32_t strategy_and_flags, int level, uint32_t max_colors,
+               const uint8_t *palettes, const uint32_t *palette_lens, uint8_t *d_out, size_t out_cap_each,
+               size_t *out_lens, int32_t *status, pixo_b200_png_reduced *info);
 
 struct FrameGeometry;
 struct HuffTables;

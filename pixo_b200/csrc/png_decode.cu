@@ -80,11 +80,7 @@ __global__ void __launch_bounds__(256) k_png_crc(const PdecChunk *__restrict__ C
                                                  uint32_t *__restrict__ acc)
 {
     __shared__ uint32_t tab[256];
-    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) {
-        uint32_t c = i;
-        for (int k = 0; k < 8; ++k) c = c & 1 ? (c >> 1) ^ 0xEDB88320u : c >> 1;
-        tab[i] = c;
-    }
+    crc32_table(tab);
     __syncthreads();
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= npieces) return;
@@ -92,9 +88,7 @@ __global__ void __launch_bounds__(256) k_png_crc(const PdecChunk *__restrict__ C
     const PdecChunk K = C[c];
     const uint64_t start = (g - __ldg(piece_prefix + c)) * kCrcPiece;
     const uint64_t n = min((uint64_t)kCrcPiece, K.len - start);
-    const uint8_t *p = bytes + K.src + start;
-    uint32_t reg = 0;
-    for (uint64_t i = 0; i < n; ++i) reg = (reg >> 8) ^ tab[(reg ^ __ldg(p + i)) & 0xFF];
+    const uint32_t reg = crc32_piece(tab, bytes + K.src + start, n);
     atomicXor(acc + c, crc32_shift(reg, K.len - start - n));
 }
 

@@ -41,6 +41,26 @@ PIXO_HOST_DEVICE inline uint32_t crc32_shift(uint32_t reg, uint64_t nbytes)
     return crc_mulmod(f, reg);
 }
 
+#ifdef __CUDACC__
+// The pieces of a chunk's CRC-32 on the device (k_png_crc checks them, k_png_idat writes them): the CTA fills the
+// 256-entry table in shared memory (a __syncthreads must follow), then a thread runs the register over its piece.
+__device__ __forceinline__ void crc32_table(uint32_t *tab)
+{
+    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) {
+        uint32_t c = i;
+        for (int k = 0; k < 8; ++k) c = c & 1 ? (c >> 1) ^ 0xEDB88320u : c >> 1;
+        tab[i] = c;
+    }
+}
+
+__device__ __forceinline__ uint32_t crc32_piece(const uint32_t *tab, const uint8_t *__restrict__ p, uint64_t n)
+{
+    uint32_t reg = 0;
+    for (uint64_t i = 0; i < n; ++i) reg = (reg >> 8) ^ tab[(reg ^ __ldg(p + i)) & 0xFF];
+    return reg;
+}
+#endif
+
 // One file after the host's share of decode_png (src/decode/png.rs:101-263 and the zlib header of
 // inflate_zlib_with_size, src/decode/inflate.rs:294-320)
 struct PdecParsed {

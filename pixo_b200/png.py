@@ -7,6 +7,8 @@
                                                  apply_filters_with_row_bytes, src/png/mod.rs:521-568,683-1147
   quantize_and_filter[_dev]                      encode_into's quantisation branch (quantize_image ->
                                                  encode_indexed_into) or the above, src/png/mod.rs:469-511
+  encode / encode_into / encode_on_device        png::encode / encode_into, whole files at the fast and balanced
+                                                 presets, src/png/mod.rs:437-630
 """
 from __future__ import annotations
 
@@ -39,6 +41,8 @@ REDUCE_PALETTE = 0x400  # PIXO_B200_PNG_REDUCE_PALETTE
 QUANTIZE_AUTO = 0x800  # PIXO_B200_PNG_QUANTIZE_AUTO
 QUANTIZE_FORCE = 0x1000  # PIXO_B200_PNG_QUANTIZE_FORCE
 DITHER = 0x2000  # PIXO_B200_PNG_DITHER
+OPTIMAL_COMPRESSION = 0x4000  # PIXO_B200_PNG_OPTIMAL_COMPRESSION (the encode calls refuse it)
+IDAT_CHUNK = 256 * 1024  # write_idat_chunks' chunk size, src/png/mod.rs:606-616
 
 
 class QuantizationMode(enum.IntEnum):
@@ -50,7 +54,7 @@ class QuantizationMode(enum.IntEnum):
 
 @dataclasses.dataclass
 class PngOptions:
-    """The fields of pixo::png::PngOptions (src/png/mod.rs:41-118) the filter stage reads."""
+    """The fields of pixo::png::PngOptions (src/png/mod.rs:41-118) the library reads."""
     width: int = 0
     height: int = 0
     color_type: ColorType = ColorType.Rgba
@@ -62,14 +66,19 @@ class PngOptions:
     quantization_mode: QuantizationMode = QuantizationMode.Off
     max_colors: int = 256
     dithering: bool = False
+    compression_level: int = 2          # the DEFLATE level, 1-9 (encode* only)
+    optimal_compression: bool = False   # pixo's max preset; the encode calls refuse it
 
     @classmethod
     def from_preset(cls, width: int, height: int, preset: int) -> "PngOptions":
         """PngOptions::from_preset (src/png/mod.rs:129-197): 0 fast, 2 max, anything else balanced."""
         if preset == 0:
-            return cls(width, height, ColorType.Rgba, FilterStrategy.AdaptiveFast, False, False, False)
-        st = FilterStrategy.Bigrams if preset == 2 else FilterStrategy.Adaptive
-        return cls(width, height, ColorType.Rgba, st, True, True, True)
+            return cls(width, height, ColorType.Rgba, FilterStrategy.AdaptiveFast, False, False, False,
+                       compression_level=2)
+        if preset == 2:
+            return cls(width, height, ColorType.Rgba, FilterStrategy.Bigrams, True, True, True,
+                       compression_level=9, optimal_compression=True)
+        return cls(width, height, ColorType.Rgba, FilterStrategy.Adaptive, True, True, True, compression_level=6)
 
     @classmethod
     def from_preset_with_lossless(cls, width: int, height: int, preset: int, lossless: bool) -> "PngOptions":
@@ -232,15 +241,7 @@ def quantize_and_filter_dev(d_data, in_stride, n_images, options: PngOptions, d_
     n_images = int(n_images)
     infos = (_Reduced * max(n_images, 1))()
     p = lambda t: None if t is None else int(t.data_ptr())
-    pals, lens = None, None
-    if palettes is not None:
-        pals = np.zeros((max(n_images, 1), 256, 4), np.uint8)
-        lens = np.zeros(max(n_images, 1), np.uint32)
-        for i, q in enumerate(palettes):
-            if q is not None:
-                q = np.asarray(q, np.uint8).reshape(-1, 4)
-                pals[i, :len(q)] = q
-                lens[i] = len(q)
+    pals, lens = _palette_table(palettes, n_images)
     _lib.check(ctx.handle, _lib.load().pixo_b200_png_quantize_filter_dev(
         ctx.handle, p(d_data), int(in_stride), n_images, int(options.width), int(options.height),
         int(options.color_type), options.strategy_word(), int(options.max_colors),
@@ -252,3 +253,84 @@ def quantize_and_filter_dev(d_data, in_stride, n_images, options: PngOptions, d_
 def adler32_combine(adler_a: int, adler_b: int, len_b: int) -> int:
     """Adler-32 of A ++ B from the two checksums and len(B)."""
     return int(_lib.load().pixo_b200_adler32_combine(int(adler_a), int(adler_b), int(len_b)))
+
+
+def _palette_table(palettes, n_images):
+    """n_images x 256 x 4 palettes and their lengths for the batch calls (None: every frame designs its own)."""
+    if palettes is None:
+        return None, None
+    pals = np.zeros((max(n_images, 1), 256, 4), np.uint8)
+    lens = np.zeros(max(n_images, 1), np.uint32)
+    for i, q in enumerate(palettes):
+        if q is not None:
+            q = np.asarray(q, np.uint8).reshape(-1, 4)
+            pals[i, :len(q)] = q
+            lens[i] = len(q)
+    return pals, lens
+
+
+def _encode_word(options: PngOptions) -> int:
+    return options.strategy_word() | (OPTIMAL_COMPRESSION if options.optimal_compression else 0)
+
+
+def encode_capacity(width: int, height: int, color_type) -> int:
+    """The largest file pixo_b200_png_encode* can write for a frame of this geometry: a stored-block zlib stream (the
+    most pixo writes for n bytes) in IDAT chunks of 256 KiB with the signature, IHDR and IEND, either of the unreduced
+    filtered rows or, for RGB and RGBA, of 8-bit palette indices with the largest PLTE and tRNS."""
+    def file(n, small):
+        zb = 2 + n + (n // 65535 + 1) * 5 + 4
+        return 8 + 25 + small + zb + 12 * -(-zb // IDAT_CHUNK) + 12
+    ct, w, h = ColorType(color_type), int(width), int(height)
+    plain = file(h * (w * ct.bytes_per_pixel() + 1), 0)
+    return plain if ct not in (ColorType.Rgb, ColorType.Rgba) else max(plain, file(h * (w + 1), 780 + 268))
+
+
+def encode(data, options: PngOptions, palette=None, ctx: Context | None = None) -> bytes:
+    """png::encode (src/png/mod.rs:424-435): the whole PNG file pixo writes for `data` with `options` at the fast
+    and balanced presets, byte for byte.  palette: optional (n, 4) RGBA median-cut palette for a frame that
+    quantises (pixo's truncation case).  See pixo_b200_png_encode."""
+    out = bytearray()
+    encode_into(out, data, options, palette, ctx)
+    return bytes(out)
+
+
+def encode_into(output: bytearray, data, options: PngOptions, palette=None, ctx: Context | None = None) -> None:
+    """png::encode_into (src/png/mod.rs:437-630): output is cleared, then holds the file."""
+    ctx = ctx or default_context()
+    output.clear()
+    d = _as_u8(data)
+    w, h = int(options.width), int(options.height)
+    cap = encode_capacity(w, h, options.color_type) if w and h else 0
+    out = np.empty(max(cap, 1), np.uint8)
+    n = C.c_size_t()
+    pal = None if palette is None else np.ascontiguousarray(palette, np.uint8).reshape(-1, 4)
+    rc = _lib.load().pixo_b200_png_encode(
+        ctx.handle, d.ctypes.data if d.size else None, d.size, w, h, int(options.color_type), _encode_word(options),
+        int(options.compression_level), int(options.max_colors), None if pal is None else pal.ctypes.data,
+        0 if pal is None else len(pal), out.ctypes.data, cap, C.byref(n))
+    _lib.check(ctx.handle, rc)
+    output += out[:n.value].tobytes()
+
+
+def encode_on_device(d_data, in_stride, n_images, options: PngOptions, d_out, out_cap_each, palettes=None,
+                     ctx: Context | None = None):
+    """n device frames (anything with .data_ptr()) of options' geometry -> n whole PNG files, file i in the device
+    slot at d_out + i * out_cap_each.  palettes: optional list of n_images entries, each None or an (n, 4) RGBA
+    palette.  Returns (lengths, status, infos): numpy arrays of each file's length and its status (0,
+    ERR_OUTPUT_TOO_SMALL with the length it needs, or ERR_UNSUPPORTED for a filtered stream of 2^31 bytes or more;
+    the slot is then untouched), and the ReducedImage of each frame.  Waits for the device: see
+    pixo_b200_png_encode_on_device."""
+    ctx = ctx or default_context()
+    n_images = int(n_images)
+    infos = (_Reduced * max(n_images, 1))()
+    out_lens = np.zeros(max(n_images, 1), np.uint64)
+    status = np.zeros(max(n_images, 1), np.int32)
+    pals, lens = _palette_table(palettes, n_images)
+    p = lambda t: None if t is None else int(t.data_ptr())
+    szp = C.POINTER(C.c_size_t)
+    _lib.check(ctx.handle, _lib.load().pixo_b200_png_encode_on_device(
+        ctx.handle, p(d_data), int(in_stride), n_images, int(options.width), int(options.height),
+        int(options.color_type), _encode_word(options), int(options.compression_level), int(options.max_colors),
+        None if pals is None else pals.ctypes.data, None if lens is None else lens.ctypes.data, p(d_out),
+        int(out_cap_each), out_lens.ctypes.data_as(szp), status.ctypes.data_as(C.POINTER(C.c_int32)), infos))
+    return out_lens[:n_images], status[:n_images], [ReducedImage._from_c(infos[i]) for i in range(n_images)]
