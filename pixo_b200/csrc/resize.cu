@@ -9,6 +9,7 @@
 // kResizeScratch bytes: frames that fit go through together, a larger frame is done in bands of
 // destination rows (and, where one row's taps alone exceed the cap, in column chunks).  The weight tables
 // come from the host (resize_host.cpp): pixo's sinf is not CUDA's.
+#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
@@ -22,6 +23,14 @@ namespace {
 
 constexpr size_t kResizeScratch = (size_t)256 << 20;
 constexpr int kThreads = 128;
+
+// The intermediate's cap in bytes.  PIXO_B200_RESIZE_SCRATCH, read on each call, replaces it (test hook: a
+// small cap drives small frames through the row bands, the column chunks and the frame passes).
+size_t scratch_cap()
+{
+    if (const char *e = getenv("PIXO_B200_RESIZE_SCRATCH")) return std::max<size_t>(1, strtoull(e, nullptr, 10));
+    return kResizeScratch;
+}
 
 __device__ __forceinline__ uint8_t to_u8(float v)
 {
@@ -291,11 +300,12 @@ int launch_lanczos(pixo_b200_ctx *ctx, const uint8_t *src, size_t src_stride, ui
     const uint64_t *ho = T.ho, *vo = T.vo;
     const float *hw = T.hw, *vw = T.vw;
 
-    const std::vector<Band> bands = lanczos_bands(v, sh, dw, dh, BPP, kResizeScratch);
+    const size_t cap = scratch_cap();
+    const std::vector<Band> bands = lanczos_bands(v, sh, dw, dh, BPP, cap);
     size_t most = 1;  // intermediate bytes of the largest band
     for (const Band &b : bands) most = std::max(most, (size_t)(b.re - b.rs) * b.cw * BPP);
     // frames per pass: as many whole intermediates as the cap holds (only when one band covers the frame)
-    const uint32_t per_pass = bands.size() == 1 ? (uint32_t)std::min<size_t>({n, 65535, std::max<size_t>(1, kResizeScratch / most)}) : 1;
+    const uint32_t per_pass = bands.size() == 1 ? (uint32_t)std::min<size_t>({n, 65535, std::max<size_t>(1, cap / most)}) : 1;
     const size_t tstride = Layout::round(most);
     PIXO_TRY(ctx->d_resize_tmp.ensure(ctx, tstride * per_pass));
     uint8_t *tmp = reinterpret_cast<uint8_t *>(ctx->d_resize_tmp.ptr);
